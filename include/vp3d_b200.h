@@ -370,6 +370,31 @@ int vp3d_semi_loss_fwd_bwd(const float* pos, const float* traj, const float* tar
                            int32_t linear, int32_t terms, float* losses, float* dpos, float* dtraj,
                            void* scratch, size_t scratch_bytes, void* stream);
 
+/* ---- evaluation metrics (run.py:674-704, common/loss.py:11-17, :27-89) ------------------------
+ * The four per-sequence means run.py's evaluate() computes, in one launch.  pred:
+ * [copies][frames][joints][3] (copies 1 or 2); target: [frames][joints][3]; both fp32, device.
+ * With copies == 2 the prediction is first flip-averaged as run.py:677-680 does:
+ * avg = (pred[0] + mirror(pred[1])) * 0.5, mirror = negate x and read joint j from mirror_src[j]
+ * (the map generators.mirror_source() builds; NULL = no joint swap, the trajectory model's case
+ * at run.py:678).  `averaged` ([frames][joints][3] or NULL) receives avg, bit-identical to the
+ * torch expression (return_predictions, run.py:682-683).  means[k] (device doubles) receives:
+ *   [0] VP3D_EVAL_MPJPE     mean ||avg - target||                              loss.py:11-17
+ *   [1] VP3D_EVAL_P_MPJPE   the same after per-frame similarity Procrustes     loss.py:27-66
+ *   [2] VP3D_EVAL_N_MPJPE   the same after per-frame least-squares scale       loss.py:68-78
+ *   [3] VP3D_EVAL_VELOCITY  mean ||diff(avg) - diff(target)|| along frames     loss.py:80-89
+ * for the metrics selected in `which` (others are written as 0).  Per-frame algebra and every sum
+ * are fp64 and in a fixed order: reproducible.  which == 0 only writes `averaged` (target, means and
+ * scratch may then be NULL).  joints <= 32; frames == 0 is a no-op.  `scratch`: device memory of
+ * vp3d_pose_errors_scratch_bytes(frames) bytes. */
+#define VP3D_EVAL_MPJPE 1
+#define VP3D_EVAL_P_MPJPE 2
+#define VP3D_EVAL_N_MPJPE 4
+#define VP3D_EVAL_VELOCITY 8
+size_t vp3d_pose_errors_scratch_bytes(int64_t frames);
+int vp3d_pose_errors(const float* pred, int32_t copies, const int32_t* mirror_src, const float* target,
+                     int64_t frames, int32_t joints, int32_t which, float* averaged, double* means,
+                     void* scratch, size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,13 +5,17 @@
     same GPU (fp32 with TF32 convolutions = PyTorch default, TF32 off, bf16 autocast), for the
     eval forward of BASELINE configs[1] and the training step of configs[2];
   * this repo's eval forward in all three precision modes and its Optimized1f training step
-    (forward + backward + Adam(amsgrad) as in run.py:252, 409-420).
+    (forward + backward + Adam(amsgrad) as in run.py:252, 409-420);
+  * `--what metrics`: the final evaluation of run.py (run.py:652-721) on a Human3.6M-test-sized
+    workload, the fused metrics kernel (videopose3d_b200.metrics) against the path run.py runs
+    (torch mpjpe / n_mpjpe with .item(), .cpu(), NumPy p_mpjpe / mean_velocity_error of the staged
+    reference), for the metrics alone and for the whole evaluate() with test-time augmentation.
 
 The cuDNN baseline is built here from plain torch.nn modules following common/model.py:85-138 /
 151-197 (it is a measurement target, not the product and not the oracle).  CUDA-event timing,
 10 warm-up + N timed iterations, cudnn.benchmark on, GPU-resident synthetic inputs.
 
-    python tools/bench_extra.py [--iters 30] [--what eval,train] > gpurun_out/extra.jsonl
+    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics] > extra.jsonl
 """
 import argparse
 import json
@@ -87,13 +91,157 @@ def emit(**kw):
     print(json.dumps(kw), flush=True)
 
 
+def card():
+    """Name and power limit of the GPU, read in the run that measures."""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                              "-i", os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0]],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, limit = [v.strip() for v in out.split(",")[:2]]
+    except Exception:
+        name, limit = torch.cuda.get_device_name(0), "not read"
+    return {"gpu": name, "power_limit": limit}
+
+
+def host_time(fn, reps):
+    """Median wall time (s) of fn(), each rep ending in a device synchronise."""
+    import time
+    ts = []
+    for _ in range(reps):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        ts.append(time.perf_counter() - t0)
+    return sorted(ts)[len(ts) // 2]
+
+
+def bench_metrics(dev, reps):
+    """run.py's final evaluation (run.py:652-721, called per action at :825-861): 240 test sequences
+    of 1000-4000 frames (about the Human3.6M S9/S11 test split), J = 17, test-time augmentation on."""
+    import numpy as np
+    from videopose3d_b200 import metrics
+    from videopose3d_b200.generators import UnchunkedGenerator
+    sys.path.insert(0, ROOT)
+    from oracle import stage_ref
+    info = card()
+    left, right = [4, 5, 6, 11, 12, 13], [1, 2, 3, 14, 15, 16]
+    lens = np.random.RandomState(0).randint(1000, 4001, 240)
+    frames = int(lens.sum())
+    g = torch.Generator().manual_seed(0)
+    preds = [(torch.randn(2, n, J, 3, generator=g) * 0.25).to(dev) for n in lens]
+    batches = [(torch.randn(2, n, J, 3, generator=g) * 0.25).to(dev) for n in lens]
+    ref = stage_ref.reference_dir()
+    ref_loss = None
+    if ref is not None:
+        sys.path.insert(0, ref)
+        import common.loss as ref_loss
+
+    def runpy_metrics(pred, batch):
+        """run.py:674-704 with the reference's metrics; returns (frames weight, 4 errors)."""
+        pred = pred.clone()
+        pred[1, :, :, 0] *= -1
+        pred[1, :, left + right] = pred[1, :, right + left]
+        pred = torch.mean(pred, dim=0, keepdim=True)
+        inputs_3d = batch.clone()
+        inputs_3d[:, :, 0] = 0
+        inputs_3d = inputs_3d[:1]
+        w = inputs_3d.shape[0] * inputs_3d.shape[1]
+        e1 = ref_loss.mpjpe(pred, inputs_3d).item()
+        e3 = ref_loss.n_mpjpe(pred, inputs_3d).item()
+        inputs = inputs_3d.cpu().numpy().reshape(-1, J, 3)
+        p = pred.cpu().numpy().reshape(-1, J, 3)
+        return w, (e1, ref_loss.p_mpjpe(p, inputs), e3, ref_loss.mean_velocity_error(p, inputs))
+
+    def fused_metrics(pred, batch):
+        tgt = batch[:1].clone()
+        tgt[:, :, 0] = 0
+        return metrics.pose_errors(pred, tgt, left, right, return_averaged=False)[0]
+
+    def run_fused():
+        acc = None
+        for pred, batch in zip(preds, batches):
+            m = fused_metrics(pred, batch) * pred.shape[1]
+            acc = m if acc is None else acc + m
+        return (acc / frames * 1000).tolist()
+
+    ref_mm = {}
+
+    def run_ref():
+        acc = np.zeros(4)
+        for pred, batch in zip(preds, batches):
+            w, e = runpy_metrics(pred, batch)
+            acc += w * np.array(e)
+        ref_mm["metrics"] = (acc / frames * 1000).tolist()
+
+    run_fused()
+    t_fused = host_time(run_fused, reps)
+    res = dict(what="eval_metrics", sequences=len(lens), frames=frames, joints=J, tta=True, **info,
+               fused_s=t_fused, fused_frames_per_s=frames / t_fused, fused_mm=run_fused())
+    if ref_loss is not None:
+        for p, b in zip(preds[:4], batches[:4]):
+            runpy_metrics(p, b)
+        t_ref = host_time(run_ref, 1)
+        res.update(reference_s=t_ref, reference_frames_per_s=frames / t_ref, reference_mm=ref_mm["metrics"],
+                   speedup=t_ref / t_fused)
+    else:
+        res.update(reference_s="not measured", reference_frames_per_s="not measured")
+    emit(**res)
+
+    # the whole evaluate(): model forward (fp16 inference) + flip average + metrics, per sequence
+    del preds
+    torch.cuda.empty_cache()
+    model = vp.TemporalModel(J, F, J, filter_widths=ARC, channels=C).to(dev).eval()
+    pad = model.receptive_field() // 2
+    rng = np.random.RandomState(1)
+    p2 = [rng.uniform(-1, 1, (n, J, F)).astype(np.float32) for n in lens]
+    p3 = [rng.normal(0, 0.25, (n, J, 3)).astype(np.float32) for n in lens]
+    gen = UnchunkedGenerator(None, p3, p2, pad=pad, causal_shift=0, augment=True, kps_left=left,
+                             kps_right=right, joints_left=left, joints_right=right, device=dev)
+
+    def eval_fused():
+        return metrics.evaluate(model, gen, left, right)
+
+    def eval_ref():
+        acc, n = np.zeros(4), 0
+        with torch.no_grad():
+            for _, batch, batch_2d in gen.next_epoch():
+                w, e = runpy_metrics(model(batch_2d), batch)
+                acc += w * np.array(e)
+                n += w
+        ref_mm["evaluate"] = (acc / n * 1000).tolist()
+
+    def forward_only():
+        with torch.no_grad():
+            for _, _, batch_2d in gen.next_epoch():
+                model(batch_2d)
+
+    forward_only()
+    t_fwd = host_time(forward_only, reps)
+    t_eval = host_time(eval_fused, reps)
+    res = dict(what="evaluate_tta", sequences=len(lens), frames=frames, arc=ARC, channels=C,
+               precision=model.precision, **info, forward_only_s=t_fwd, fused_s=t_eval,
+               fused_mm=eval_fused())
+    if ref_loss is not None:
+        t_ref = host_time(eval_ref, 1)
+        res.update(reference_s=t_ref, reference_mm=ref_mm["evaluate"], speedup=t_ref / t_eval,
+                   metrics_share_of_reference=(t_ref - t_fwd) / t_ref)
+    else:
+        res.update(reference_s="not measured")
+    emit(**res)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--what", default="eval,train")
+    ap.add_argument("--reps", type=int, default=3, help="timed repetitions of the metrics arms")
     args = ap.parse_args()
     what = set(args.what.split(","))
     dev = torch.device("cuda:0")
+    if "metrics" in what:
+        bench_metrics(dev, args.reps)
     torch.backends.cudnn.benchmark = True
     g = torch.Generator().manual_seed(0)
     x = (torch.rand(N, T, J, F, generator=g) * 2 - 1).to(dev)

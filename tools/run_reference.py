@@ -10,8 +10,11 @@ symbols `run.py` picks up with `from common.model import *` (run.py:21), `from c
 (:22) and `optim.Adam` (:252, 264) by this package's drop-ins, then executes run.py as `__main__`.
 No file of the reference is modified.
   model   TemporalModel, TemporalModelOptimized1f -> videopose3d_b200 (CUDA only)
-  loss    mpjpe, weighted_mpjpe                   -> fused kernels (the NumPy metrics p_mpjpe /
-          n_mpjpe / mean_velocity_error stay the reference's)
+  loss    mpjpe, weighted_mpjpe                   -> fused kernels
+  metrics n_mpjpe, p_mpjpe, mean_velocity_error   -> the evaluation kernel (csrc/eval_metrics.cu).
+          run.py hands p_mpjpe / mean_velocity_error NumPy arrays (run.py:697-704): the shims
+          upload them (a few hundred kB per sequence), run the kernel and return a float, in place
+          of the per-frame LAPACK SVDs
   optim   torch.optim.Adam                        -> FusedAdam
   generators  ChunkedGenerator, UnchunkedGenerator -> device-resident generators.  run.py turns
           every batch into a tensor with `torch.from_numpy(batch.astype('float32'))` followed by
@@ -41,7 +44,7 @@ def main():
     ap.add_argument("--swap", default="model")
     args = ap.parse_args(own)
     swaps = set(filter(None, args.swap.split(",")))
-    unknown = swaps - {"model", "loss", "optim", "generators"}
+    unknown = swaps - {"model", "loss", "optim", "generators", "metrics"}
     if unknown:
         raise SystemExit(f"unknown --swap entries: {sorted(unknown)}")
     if args.reference is None:
@@ -72,6 +75,8 @@ def main():
         torch.optim.Adam = FusedAdam
     if "generators" in swaps:
         _swap_generators()
+    if "metrics" in swaps:
+        _swap_metrics()
     sys.argv = [script] + passthrough
     runpy.run_path(script, run_name="__main__")
 
@@ -119,6 +124,25 @@ def _swap_generators():
         return a.tensor if isinstance(a, _DeviceBatch) else real_from_numpy(a)
 
     torch.from_numpy = from_numpy
+
+
+def _swap_metrics():
+    import numpy as np
+    import torch
+    import common.loss as ref_loss
+    from videopose3d_b200 import metrics as M
+
+    def on_device(a):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).cuda()
+
+    def p_mpjpe(predicted, target):
+        return M.p_mpjpe(on_device(predicted), on_device(target)).item()
+
+    def mean_velocity_error(predicted, target):
+        return M.mean_velocity_error(on_device(predicted), on_device(target)).item()
+
+    ref_loss.n_mpjpe = M.n_mpjpe
+    ref_loss.p_mpjpe, ref_loss.mean_velocity_error = p_mpjpe, mean_velocity_error
 
 
 if __name__ == "__main__":
