@@ -258,6 +258,9 @@ typedef struct {
    * lo_row_end == 0 means every row. */
   int lo_row_begin;
   int lo_row_end;
+  /* elements between the A planes; 0 = samples * a_rows * a_ld (A is exactly its planes).  Set when
+   * the A rows are a window into a larger buffer, such as a streaming history ring. */
+  long long a_plane_stride;
 } vp3d_conv_desc;
 
 int vp3d_conv_gemm(const vp3d_conv_desc* d, void* stream);
@@ -394,6 +397,37 @@ size_t vp3d_pose_errors_scratch_bytes(int64_t frames);
 int vp3d_pose_errors(const float* pred, int32_t copies, const int32_t* mirror_src, const float* target,
                      int64_t frames, int32_t joints, int32_t which, float* averaged, double* means,
                      void* scratch, size_t scratch_bytes, void* stream);
+
+/* ---- streaming inference (common/model.py:63-77, 126-138 applied incrementally) ---------------
+ * A session of S stream slots pushes k <= K new frames per slot at a time and gets back the output
+ * frames they complete.  Per slot the concatenated outputs equal vp3d_forward_eval on the sequence
+ * edge-padded as UnchunkedGenerator pads it (common/generators.py:216-238, run.py:186-193): pad +
+ * causal_shift copies of the first frame in front, pad - causal_shift copies of the last behind.
+ * Every conv layer keeps its input history in a time-major device ring inside the caller's state
+ * buffer; a push costs the new frames' share of the FLOPs.  TemporalModel (VP3D_VARIANT_DILATED,
+ * dense or not) in any precision but MIXED; the plan's packed eval weights are read at every push.
+ *
+ * vp3d_stream_lookahead: output frame t of a slot is returned by the push that delivers its input
+ * frame t + lookahead (lookahead = pad - causal_shift: 0 for a causal model).
+ * vp3d_stream_state_bytes: device bytes of a session's state (0 for an invalid or too large size).
+ * vp3d_stream_init: registers `state` (device memory of at least state_bytes) with the plan and
+ * clears it: every slot idle, all history dropped (also the way to reset a session).
+ * vp3d_stream_push: x is (S, k, J_in, F) fp32; start_mask (S bytes, device, or NULL = none): slot
+ * s begins a new sequence whose first frame is x[s, 0] (its history becomes the edge padding of
+ * that frame, the other slots continue undisturbed); y receives (S, k, J_out, 3) fp32 and frame
+ * (S, k) int64 the frame number within each slot's current sequence of every y row, -1 for rows
+ * that are no frame (look-ahead warm-up, idle slot).  Asynchronous, no host synchronisation.
+ * vp3d_stream_finish: emits the last `lookahead` frames of every slot by repeating each slot's
+ * newest frame (the generator's end padding) into y (S, lookahead, J_out, 3) / frame (S,
+ * lookahead), then marks every slot idle.
+ * vp3d_stream_release: forgets `state` (the caller frees the memory). */
+int vp3d_stream_lookahead(const vp3d_plan* plan);
+size_t vp3d_stream_state_bytes(const vp3d_plan* plan, int S, int K);
+int vp3d_stream_init(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, void* stream);
+int vp3d_stream_push(vp3d_plan* plan, void* state, const float* x, int k, const uint8_t* start_mask,
+                     float* y, int64_t* frame, void* stream);
+int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
+int vp3d_stream_release(vp3d_plan* plan, void* state);
 
 #ifdef __cplusplus
 }

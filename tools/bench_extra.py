@@ -6,6 +6,8 @@
     eval forward of BASELINE configs[1] and the training step of configs[2];
   * this repo's eval forward in all three precision modes and its Optimized1f training step
     (forward + backward + Adam(amsgrad) as in run.py:252, 409-420);
+  * `--what stream`: streaming sessions (videopose3d_b200.streaming) against a user recomputing the
+    receptive-field window per new frame, per-push latency over >= 500 pushes (see bench_stream);
   * `--what metrics`: the final evaluation of run.py (run.py:652-721) on a Human3.6M-test-sized
     workload, the fused metrics kernel (videopose3d_b200.metrics) against the path run.py runs
     (torch mpjpe / n_mpjpe with .item(), .cpu(), NumPy p_mpjpe / mean_velocity_error of the staged
@@ -15,13 +17,14 @@ The cuDNN baseline is built here from plain torch.nn modules following common/mo
 151-197 (it is a measurement target, not the product and not the oracle).  CUDA-event timing,
 10 warm-up + N timed iterations, cudnn.benchmark on, GPU-resident synthetic inputs.
 
-    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics] > extra.jsonl
+    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics,stream] > extra.jsonl
 """
 import argparse
 import json
 import os
 import sys
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -232,14 +235,80 @@ def bench_metrics(dev, reps):
     emit(**res)
 
 
+def stream_flops_per_frame(fw, C, c_in, c_out):
+    """Executed FLOPs per output frame, from shapes: (streaming session, dependency-cone forward of
+    one receptive field).  A session computes one new row per layer; the cone forward (model(x)
+    with T = RF) computes L_0 = RF / w_0 expand rows and L_i = L_{i-1} / w_i rows in block i."""
+    rf = 1
+    for w in fw:
+        rf *= w
+    stream = 2 * c_in * fw[0] * C + sum(2 * C * C * (w + 1) for w in fw[1:]) + 2 * C * c_out
+    rows = rf // fw[0]
+    cone = rows * 2 * c_in * fw[0] * C
+    for w in fw[1:]:
+        rows //= w
+        cone += rows * 2 * C * C * (w + 1)
+    cone += rows * 2 * C * c_out
+    return stream, cone
+
+
+def bench_stream(dev, pushes):
+    """Per-push latency of a streaming session at arc 3^5, C = 1024, fp16, against the baseline a
+    real-time user has without it: model(window) on the last receptive field of every stream
+    (N = S * k windows, T = RF, the dependency-cone schedule), alternated with the session in the
+    same loop.  CUDA events around every push / baseline call; no L2 flush in between (a live
+    stream keeps its weights hot)."""
+    torch.manual_seed(0)
+    m = vp.TemporalModel(J, F, J, filter_widths=ARC, channels=C).to(dev).eval().set_precision("fp16")
+    rf = m.receptive_field()
+    st_fl, cone_fl = stream_flops_per_frame(ARC, C, J * F, J * 3)
+    info = card()
+    for S, k in ((1, 1), (16, 1), (256, 1), (1024, 1), (256, 16)):
+        sess = m.streaming(streams=S, max_frames=k)
+        xs = (torch.rand(S, k, J, F, device=dev) * 2 - 1)
+        win = (torch.rand(S * k, rf, J, F, device=dev) * 2 - 1)
+        with torch.no_grad():
+            sess.push(xs, start=[True] * S)
+            for _ in range(50):
+                sess.push(xs)
+                m(win)
+        torch.cuda.synchronize()
+        ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(pushes)]
+        with torch.no_grad():
+            for e in ev:
+                e[0].record()
+                sess.push(xs)
+                e[1].record()
+                e[2].record()
+                m(win)
+                e[3].record()
+        torch.cuda.synchronize()
+        t_s = np.sort([e[0].elapsed_time(e[1]) for e in ev])
+        t_b = np.sort([e[2].elapsed_time(e[3]) for e in ev])
+        p99 = lambda t: float(t[min(len(t) - 1, int(np.ceil(0.99 * len(t))) - 1)])
+        med_s, med_b = float(np.median(t_s)), float(np.median(t_b))
+        emit(what="stream_push", streams=S, k=k, precision="fp16", arc=ARC, channels=C,
+             pushes=pushes, push_ms_median=med_s, push_ms_p99=p99(t_s),
+             frames_per_s=S * k / med_s * 1e3, push_launches=sess.last_launch_count(),
+             baseline_ms_median=med_b, baseline_ms_p99=p99(t_b),
+             baseline_frames_per_s=S * k / med_b * 1e3, speedup_median=med_b / med_s,
+             mflop_per_frame_stream=st_fl / 1e6, mflop_per_frame_baseline=cone_fl / 1e6,
+             stream_tflops=st_fl * S * k / med_s / 1e9, l2_flush="none", **info)
+        del sess, xs, win
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--what", default="eval,train")
     ap.add_argument("--reps", type=int, default=3, help="timed repetitions of the metrics arms")
+    ap.add_argument("--pushes", type=int, default=500, help="timed pushes per streaming config")
     args = ap.parse_args()
     what = set(args.what.split(","))
     dev = torch.device("cuda:0")
+    if "stream" in what:
+        bench_stream(dev, args.pushes)
     if "metrics" in what:
         bench_metrics(dev, args.reps)
     torch.backends.cudnn.benchmark = True

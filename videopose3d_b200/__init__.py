@@ -4,7 +4,8 @@ Public surface = the reference's ``common/model.py`` classes; everything else st
 """
 from .temporal_model import TemporalModel, TemporalModelBase, TemporalModelOptimized1f
 from .data_parallel import GradientReducer, broadcast_buffers
+from .streaming import StreamingSession
 
 __all__ = ["TemporalModelBase", "TemporalModel", "TemporalModelOptimized1f", "GradientReducer",
-           "broadcast_buffers"]
+           "broadcast_buffers", "StreamingSession"]
 __version__ = "0.1.0"

@@ -149,6 +149,7 @@ class ConvDesc(ctypes.Structure):
         ("bnb_layer", ctypes.c_int),
         ("lo_row_begin", ctypes.c_int),
         ("lo_row_end", ctypes.c_int),
+        ("a_plane_stride", ctypes.c_longlong),
     ]
 
 
@@ -217,6 +218,16 @@ SIGNATURES = {
                                         ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32,
                                         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "vp3d_stream_lookahead": (ctypes.c_int, [ctypes.c_void_p]),
+    "vp3d_stream_state_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]),
+    "vp3d_stream_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                        ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "vp3d_stream_push": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                        ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                        ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                          ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
 }
 
 _lib = None

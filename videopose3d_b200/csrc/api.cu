@@ -145,7 +145,9 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
 
   CUtensorMap ma, mw;
   const uint64_t a_rows = d->a_rows, a_ld = d->a_ld;
-  const uint64_t plane_stride = (uint64_t)d->samples * a_rows * a_ld;
+  // (an explicit plane stride when the A rows are a window into a larger buffer, e.g. a history ring)
+  const uint64_t plane_stride = d->a_plane_stride > 0 ? (uint64_t)d->a_plane_stride
+                                                      : (uint64_t)d->samples * a_rows * a_ld;
   VP3D_TRY(make_map_4d(&ma, d->a, a_ld, a_rows, a_ld, d->samples, a_rows * a_ld, a_planes,
                        plane_stride, kBlockM));
   ConvGemmArgs g;

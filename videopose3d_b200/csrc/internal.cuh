@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <map>
 #include <vector>
 
 #include "../../include/vp3d_b200.h"
@@ -53,6 +54,15 @@ struct PackedConv {
 };
 
 struct TrainState;  // train_api.cu
+
+// stream.cu: host side of one streaming session (vp3d_stream_init); the rings live in the
+// caller's device state buffer
+struct StreamHost {
+  int S = 0, K = 0;
+  long long q = 0;        // frames pushed since vp3d_stream_init (all slots advance together)
+  long long prev_q = 0;   // q before the last push
+  int prev_k = 0;         // frames of the last push (their ring rows still need their mirror copy)
+};
 
 // step_ops.cu: Adam / AMSGrad update of conv weights that also refreshes their bf16 packs
 struct AdamPackItem {
@@ -109,6 +119,8 @@ struct vp3d_plan {
   size_t prof_used = 0;                  // events consumed since the last read
   // training-mode state (transposed weight packs, per-layer BN vectors, dropout config)
   vp3d::TrainState* train = nullptr;
+  // streaming sessions of this plan, keyed by their device state buffer
+  std::map<const void*, vp3d::StreamHost> streams;
 };
 
 namespace vp3d {

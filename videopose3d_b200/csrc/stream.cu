@@ -1,0 +1,551 @@
+// Streaming (frame-by-frame) inference of TemporalModel: common/model.py:63-77, 126-138 applied
+// incrementally, with the edge padding of common/generators.py:216-238 done in place.
+//
+// A session holds S stream slots that advance in lockstep.  Every conv layer with history (the
+// expand conv and the first conv of every residual block) keeps its INPUT in a time-major ring,
+//   [plane][frame position][stream][ld]      (ld = padded channels of that input)
+// so that tap j of the k*S new output rows is one contiguous block of k*S ring rows, a fixed
+// dilation*S rows after tap j-1: exactly the flat geometry of conv_gemm_kernel (tap_row_step =
+// dilation*S, M = k*S rows).  The residual of block i is a row offset into the same window.
+//
+// Ring maintenance (mirrored rings).  Ring l needs H_l = (taps-1)*dilation = 2*pad_l frames of
+// history next to the k <= K new ones.  It has R_l = H_l + K + 1 frame positions, stored twice
+// (positions [0, R) and [R, 2R) hold the same frames): frame t lives at t mod R and t mod R + R.
+// The window of a push that starts at frame q is then always the contiguous span
+// [w0, w0 + H + k) with w0 = (q - H) mod R, whatever q is.  New frames are written once by the
+// GEMM epilogue (ring 0: by the input kernel, which writes both copies) and mirrored into the
+// other half by the input kernel of the NEXT push, before any GEMM reads them.  Per push and ring
+// this copies exactly the k*S new rows: O(k*S*C) per layer, no periodic compaction.
+//
+// Start of a sequence.  Every layer maps a constant input sequence to a constant sequence, so the
+// history of a slot that starts with frame x0 (np.pad 'edge' of the generator) is one vector per
+// ring, v_l(x0).  The v-pass computes it with the same GEMM kernel and every tap reading the same
+// row (tap_row_step = 0), which is the very sum (pair -> tap -> k-block order, same operands) the
+// offline forward evaluates on an edge-padded stretch; the broadcast kernel then writes it into
+// the history positions of the starting slots only.
+#include <cuda_fp16.h>
+
+#include "internal.cuh"
+#include "launch.cuh"
+
+namespace vp3d {
+
+namespace {
+
+constexpr int kMaxRings = VP3D_MAX_WIDTHS;   // ring 0 = network input, ring i = block i input
+
+struct StreamRing {
+  __nv_bfloat16* base;   // plane 0, position 0
+  long long plane;       // elements per plane (2R * S * ld)
+  int ld, H, R;
+  int w0;                // first window position of the current push
+  int prev_w0, prev_k;   // window start and new frames of the previous push (prev_k = 0: none)
+};
+
+struct StreamLayout {
+  int rings = 0;
+  int H[kMaxRings], R[kMaxRings], ld[kMaxRings];
+  long long plane[kMaxRings];   // elements per ring plane
+  size_t ring[kMaxRings];       // byte offsets
+  size_t count = 0, active = 0, h = 0, xlast = 0, ybuf = 0, total = 0;
+  size_t v[kMaxRings];          // v_l(x0) of rings 1..nb: [plane][S][C]
+};
+
+StreamLayout stream_layout(const vp3d_plan* p, int S, int K) {
+  StreamLayout L;
+  L.rings = p->nb + 1;
+  const int planes = p->planes;
+  size_t off = 0;
+  L.count = off; off = align_up(off + (size_t)S * 8, 1024);
+  L.active = off; off = align_up(off + (size_t)S, 1024);
+  for (int l = 0; l < L.rings; ++l) {
+    L.H[l] = 2 * p->pad[l];
+    L.R[l] = L.H[l] + K + 1;
+    L.ld[l] = l == 0 ? p->c_in_pad : p->C;
+    L.plane[l] = 2LL * L.R[l] * S * L.ld[l];
+    L.ring[l] = off;
+    off = align_up(off + (size_t)L.plane[l] * planes * 2, 1024);
+  }
+  const size_t act = (size_t)planes * K * S * p->C * 2;
+  L.h = off; off = align_up(off + act, 1024);
+  L.xlast = off; off = align_up(off + act, 1024);
+  L.v[0] = 0;
+  for (int l = 1; l < L.rings; ++l) {
+    L.v[l] = off;
+    off = align_up(off + (size_t)planes * S * p->C * 2, 1024);
+  }
+  L.ybuf = off; off = align_up(off + (size_t)K * S * p->c_out_raw * 4, 1024);
+  L.total = off + 1024;   // slack for aligning the caller's pointer
+  return L;
+}
+
+inline int pos_mod(long long a, int m) { return (int)(((a % m) + m) % m); }
+__device__ __forceinline__ int pos_mod_dev(int a, int m) { return ((a % m) + m) % m; }
+// the other copy of a ring position in [0, 2R)
+__device__ __forceinline__ int mirror_pos(int a, int R) { return a < R ? a + R : a - R; }
+
+__device__ __forceinline__ __nv_bfloat16 to_f16_bits(float v) {
+  // the input pack's fp16 format (pack.cu): saturate, round to nearest
+  v = fminf(fmaxf(v, -65504.0f), 65504.0f);
+  return __ushort_as_bfloat16(__half_as_ushort(__float2half_rn(v)));
+}
+
+struct StepArgs {
+  StreamRing ring[kMaxRings];
+  int rings, planes, f16, S, k, c_raw;
+  const float* x;          // (S, k, c_raw) fp32, or null: repeat each slot's newest frame (finish)
+  const uint8_t* start;    // (S,) or null
+  long long* count;        // frames of the current sequence pushed so far, per slot
+  uint8_t* active;         // 1 while the slot holds a sequence
+  long long* frame;        // (S, frame_ld) int64
+  int frame_ld, frame_off, lookahead;
+};
+
+// One launch at the head of every push:
+//   * frame bookkeeping: a starting slot resets its frame counter; output row f of slot s is frame
+//     count + f - lookahead of its sequence, or -1 (warm-up of the look-ahead, idle slot);
+//   * the input pack: fp32 (S, k, J*F) -> 16-bit ring-0 rows (both copies), zero-padded channels,
+//     rounded exactly as the offline input pack rounds (hi / lo split for bf16x3, saturating fp16);
+//     in finish mode the slot's newest packed frame is repeated instead (the generator's end
+//     padding, generators.py:216-238);
+//   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb.
+__global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long nthr = (long long)gridDim.x * blockDim.x;
+  for (long long s = tid; s < a.S; s += nthr) {
+    long long c = a.count[s];
+    uint8_t act = a.active[s];
+    if (a.start && a.start[s]) { c = 0; act = 1; }
+    for (int f = 0; f < a.k; ++f) {
+      const long long idx = c + f - a.lookahead;
+      a.frame[s * a.frame_ld + a.frame_off + f] = (act && idx >= 0) ? idx : -1;
+    }
+    a.count[s] = c + a.k;
+    a.active[s] = act;
+  }
+
+  const StreamRing& r0 = a.ring[0];
+  const int pairs = r0.ld >> 1;
+  const long long n_pack = (long long)a.k * a.S * pairs;
+  const int src_pos = pos_mod_dev(r0.w0 + r0.H - 1, r0.R);
+  for (long long i = tid; i < n_pack; i += nthr) {
+    const int cp = (int)(i % pairs);
+    const long long row = i / pairs;          // f * S + s
+    const int s = (int)(row % a.S), f = (int)(row / a.S);
+    const int pos = r0.w0 + r0.H + f;
+    const long long d0 = ((long long)pos * a.S + s) * r0.ld + 2 * cp;
+    const long long d1 = ((long long)mirror_pos(pos, r0.R) * a.S + s) * r0.ld + 2 * cp;
+    if (a.x) {
+      const float* src = a.x + ((long long)s * a.k + f) * a.c_raw;
+      const int c0 = 2 * cp;
+      const float v0 = c0 < a.c_raw ? __ldg(src + c0) : 0.0f;
+      const float v1 = c0 + 1 < a.c_raw ? __ldg(src + c0 + 1) : 0.0f;
+      __nv_bfloat162 hi, lo;
+      if (a.f16) {
+        hi.x = to_f16_bits(v0);
+        hi.y = to_f16_bits(v1);
+      } else {
+        hi.x = __float2bfloat16_rn(v0);
+        hi.y = __float2bfloat16_rn(v1);
+        lo.x = __float2bfloat16_rn(v0 - __bfloat162float(hi.x));
+        lo.y = __float2bfloat16_rn(v1 - __bfloat162float(hi.y));
+      }
+      *reinterpret_cast<__nv_bfloat162*>(r0.base + d0) = hi;
+      *reinterpret_cast<__nv_bfloat162*>(r0.base + d1) = hi;
+      if (a.planes == 2) {
+        *reinterpret_cast<__nv_bfloat162*>(r0.base + r0.plane + d0) = lo;
+        *reinterpret_cast<__nv_bfloat162*>(r0.base + r0.plane + d1) = lo;
+      }
+    } else {
+      const long long sr = ((long long)src_pos * a.S + s) * r0.ld + 2 * cp;
+      for (int pl = 0; pl < a.planes; ++pl) {
+        const uint32_t v = *reinterpret_cast<const uint32_t*>(r0.base + pl * r0.plane + sr);
+        *reinterpret_cast<uint32_t*>(r0.base + pl * r0.plane + d0) = v;
+        *reinterpret_cast<uint32_t*>(r0.base + pl * r0.plane + d1) = v;
+      }
+    }
+  }
+
+#pragma unroll
+  for (int l = 1; l < kMaxRings; ++l) {   // (unrolled: the ring table stays in parameter space)
+    const StreamRing& r = a.ring[l];
+    if (l >= a.rings || r.prev_k == 0) continue;
+    const long long per_frame = (long long)a.S * r.ld / 8;   // 16-byte vectors
+    const long long n = (long long)a.planes * r.prev_k * per_frame;
+    for (long long i = tid; i < n; i += nthr) {
+      const long long e = i % per_frame;
+      const long long q = i / per_frame;
+      const int f = (int)(q % r.prev_k), pl = (int)(q / r.prev_k);
+      const int pos = r.prev_w0 + r.H + f;
+      const uint4* src = reinterpret_cast<const uint4*>(r.base + pl * r.plane +
+                                                        (long long)pos * a.S * r.ld) + e;
+      uint4* dst = reinterpret_cast<uint4*>(r.base + pl * r.plane +
+                                            (long long)mirror_pos(pos, r.R) * a.S * r.ld) + e;
+      *dst = *src;
+    }
+  }
+}
+
+struct BcastArgs {
+  StreamRing ring[kMaxRings];
+  const __nv_bfloat16* src[kMaxRings];   // [plane][S][ld] rows v_l(x0)
+  long long src_plane[kMaxRings];
+  int rings, planes, S;
+  const uint8_t* start;
+};
+
+// Start of a sequence: history positions [w0, w0 + H) of every ring (both copies) of the starting
+// slots receive that slot's v_l(x0).
+__global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a) {
+  pdl_entry();
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long nthr = (long long)gridDim.x * blockDim.x;
+  for (int l = 0; l < a.rings; ++l) {
+    const StreamRing& r = a.ring[l];
+    const int vec = r.ld / 8;
+    const long long n = (long long)a.planes * r.H * a.S * vec;
+    for (long long i = tid; i < n; i += nthr) {
+      const int e = (int)(i % vec);
+      long long q = i / vec;
+      const int s = (int)(q % a.S);
+      q /= a.S;
+      if (!a.start[s]) continue;
+      const int j = (int)(q % r.H), pl = (int)(q / r.H);
+      const uint4 v = *(reinterpret_cast<const uint4*>(a.src[l] + pl * a.src_plane[l] +
+                                                       (long long)s * r.ld) + e);
+      const int pos = r.w0 + j;
+      __nv_bfloat16* pbase = r.base + pl * r.plane;
+      *(reinterpret_cast<uint4*>(pbase + ((long long)pos * a.S + s) * r.ld) + e) = v;
+      *(reinterpret_cast<uint4*>(pbase + ((long long)mirror_pos(pos, r.R) * a.S + s) * r.ld) + e) = v;
+    }
+  }
+}
+
+// Shrink output rows are time-major (f * S + s); y is (S, y_frames, c_out) at frame offset f_off.
+__global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, float* y, int S, int k,
+                                                            int c_out, int y_frames, int f_off) {
+  pdl_entry();
+  const long long n = (long long)k * S * c_out;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % c_out);
+    const long long r = i / c_out;
+    const int s = (int)(r % S), f = (int)(r / S);
+    y[((long long)s * y_frames + f_off + f) * c_out + c] = ybuf[i];
+  }
+}
+
+inline int grid_for(long long work) {
+  long long b = (work + 255) / 256;
+  if (b < 1) b = 1;
+  if (b > 132 * 8) b = 132 * 8;
+  return (int)b;
+}
+
+}  // namespace
+
+// run.py:186-193 pads pad + causal_shift frames in front and pad - causal_shift behind, with
+// causal_shift = pad for a causal model (every block's shift, in frames, adds up to pad)
+int stream_lookahead(const vp3d_plan* p) {
+  return p->cfg.causal ? 0 : (vp3d_receptive_field(p) - 1) / 2;
+}
+
+// One push of k frames (x null: k copies of every slot's newest frame).  y receives rows
+// [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, frame the matching (S, y_frames) entries.
+static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
+                       const uint8_t* start, float* y, int y_frames, int f_off, long long* frame,
+                       cudaStream_t stream) {
+  const int S = h.S, K = h.K, C = p->C, planes = p->planes;
+  const StreamLayout L = stream_layout(p, S, K);
+  int launches = 0;
+
+  StepArgs a;
+  memset(&a, 0, sizeof(a));
+  StreamRing ring[kMaxRings];
+  for (int l = 0; l < L.rings; ++l) {
+    StreamRing& r = ring[l];
+    r.base = reinterpret_cast<__nv_bfloat16*>(base + L.ring[l]);
+    r.plane = L.plane[l];
+    r.ld = L.ld[l];
+    r.H = L.H[l];
+    r.R = L.R[l];
+    r.w0 = pos_mod(h.q - r.H, r.R);
+    r.prev_w0 = pos_mod(h.prev_q - r.H, r.R);
+    r.prev_k = h.prev_k;
+    a.ring[l] = r;
+  }
+  a.rings = L.rings;
+  a.planes = planes;
+  a.f16 = p->f16;
+  a.S = S;
+  a.k = k;
+  a.c_raw = p->c_in_raw;
+  a.x = x;
+  a.start = start;
+  a.count = reinterpret_cast<long long*>(base + L.count);
+  a.active = base + L.active;
+  a.frame = frame;
+  a.frame_ld = y_frames;
+  a.frame_off = f_off;
+  a.lookahead = stream_lookahead(p);
+  {
+    long long work = (long long)k * S * (p->c_in_pad / 2);
+    for (int l = 1; l < L.rings; ++l) work += (long long)planes * h.prev_k * S * C / 8;
+    if (work < S) work = S;
+    // a plain launch: the first kernel of a push may follow a weight re-pack, which the GEMMs'
+    // early weight loads must not overlap
+    stream_input_kernel<<<grid_for(work), 256, 0, stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    ++launches;
+  }
+
+  __nv_bfloat16* hbuf = reinterpret_cast<__nv_bfloat16*>(base + L.h);
+  __nv_bfloat16* xlast = reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
+  const long long act_plane = (long long)K * S * C;
+  const long long v_plane = (long long)S * C;
+  auto vbuf = [&](int l) { return reinterpret_cast<__nv_bfloat16*>(base + L.v[l]); };
+  // window of ring l: frame positions [w0, w0 + H + k); new frames start at w0 + H
+  auto window = [&](int l) { return ring[l].base + (long long)ring[l].w0 * S * ring[l].ld; };
+  auto new_rows = [&](int l) {
+    return ring[l].base + (long long)(ring[l].w0 + ring[l].H) * S * ring[l].ld;
+  };
+  const int* fw = p->cfg.filter_widths;
+
+  vp3d_conv_desc d;
+  auto common = [&](vp3d_conv_desc& q) {
+    memset(&q, 0, sizeof(q));
+    q.a_planes = planes;
+    q.precision = p->f16 ? VP3D_PRECISION_FP16
+                         : (planes == 2 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16);
+    q.out_planes = planes;
+    q.res_planes = planes;
+    q.samples = 1;
+    q.per_sample_tiles = 0;
+  };
+  auto set_out = [&](vp3d_conv_desc& q, int layer_out, bool vpass) {
+    // layer_out = i: X_i, the output of block i (0 = expand)
+    q.out_ld = C;
+    if (vpass) {
+      q.out = vbuf(layer_out + 1);
+      q.out_plane_stride = v_plane;
+    } else if (layer_out < p->nb) {
+      q.out = new_rows(layer_out + 1);
+      q.out_plane_stride = ring[layer_out + 1].plane;
+    } else {
+      q.out = xlast;
+      q.out_plane_stride = act_plane;
+    }
+  };
+
+  if (start && p->nb >= 1) {
+    // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i), every tap on the same row
+    common(d);
+    d.a = new_rows(0); d.a_plane_stride = ring[0].plane; d.a_rows = S; d.a_ld = p->c_in_pad;
+    d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+    d.tap_row_step = 0; d.out_rows = S;
+    d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
+    set_out(d, 0, true);
+    VP3D_TRY(run_conv(&d, stream));
+    ++launches;
+    for (int i = 1; i < p->nb; ++i) {
+      const PackedConv& c0 = p->conv[2 * (i - 1)];
+      const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
+      common(d);
+      d.a = vbuf(i); d.a_plane_stride = v_plane; d.a_rows = S; d.a_ld = C;
+      d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
+      d.tap_row_step = 0; d.out_rows = S;
+      d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
+      d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
+      VP3D_TRY(run_conv(&d, stream));
+      common(d);
+      d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = S; d.a_ld = C;
+      d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = S;
+      d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
+      d.res = vbuf(i); d.res_plane_stride = v_plane; d.res_ld = C; d.res_row_step = 1;
+      d.res_row_off = 0;
+      set_out(d, i, true);
+      VP3D_TRY(run_conv(&d, stream));
+      launches += 2;
+    }
+  }
+  if (start) {
+    BcastArgs b;
+    memset(&b, 0, sizeof(b));
+    long long work = 0;
+    for (int l = 0; l < L.rings; ++l) {
+      b.ring[l] = ring[l];
+      if (l == 0) {
+        b.src[0] = new_rows(0);   // the starting slot's first frame, just packed
+        b.src_plane[0] = ring[0].plane;
+      } else {
+        b.src[l] = vbuf(l);
+        b.src_plane[l] = v_plane;
+      }
+      work += (long long)planes * ring[l].H * S * ring[l].ld / 8;
+    }
+    b.rings = L.rings;
+    b.planes = planes;
+    b.S = S;
+    b.start = start;
+    CUDA_TRY(launch_pdl(stream_broadcast_kernel, dim3(grid_for(work)), dim3(256), 0, stream, b));
+    ++launches;
+  }
+
+  // ---- the push: expand (model.py:127), residual blocks (:129-135), shrink (:137)
+  common(d);
+  d.a = window(0); d.a_plane_stride = ring[0].plane; d.a_rows = (ring[0].H + k) * S;
+  d.a_ld = p->c_in_pad;
+  d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+  d.tap_row_step = S; d.out_rows = k * S;
+  d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
+  set_out(d, 0, false);
+  VP3D_TRY(run_conv(&d, stream));
+  ++launches;
+  for (int i = 1; i <= p->nb; ++i) {
+    const PackedConv& c0 = p->conv[2 * (i - 1)];
+    const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
+    common(d);
+    d.a = window(i); d.a_plane_stride = ring[i].plane; d.a_rows = (ring[i].H + k) * S; d.a_ld = C;
+    d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
+    d.tap_row_step = p->dilation[i] * S; d.out_rows = k * S;
+    d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
+    d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
+    VP3D_TRY(run_conv(&d, stream));
+    common(d);
+    d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = k * S; d.a_ld = C;
+    d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = k * S;
+    d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
+    // residual: the centre tap (causal: the newest) of the block input window, model.py:130-132
+    d.res = window(i); d.res_plane_stride = ring[i].plane; d.res_ld = C; d.res_row_step = 1;
+    d.res_row_off = (p->pad[i] + p->shift_dil[i]) * S;
+    set_out(d, i, false);
+    VP3D_TRY(run_conv(&d, stream));
+    launches += 2;
+  }
+  // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1)
+  const bool direct = y_frames == 1 || S == 1;
+  float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
+  common(d);
+  d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * S; d.a_ld = C;
+  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad; d.out_rows = k * S;
+  d.scale = p->shrink.scale; d.shift = p->shrink.shift; d.relu = 0;
+  d.out_f32 = direct ? y + (long long)f_off * p->c_out_raw : ybuf;
+  d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
+  VP3D_TRY(run_conv(&d, stream));
+  ++launches;
+  if (!direct) {
+    CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
+                        dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
+                        f_off));
+    ++launches;
+  }
+  h.prev_q = h.q;
+  h.prev_k = k;
+  h.q += k;
+  p->last_launches = launches;
+  return VP3D_OK;
+}
+
+static int stream_supported(const vp3d_plan* p, const char* what) {
+  if (p->cfg.variant != VP3D_VARIANT_DILATED)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: streaming needs the TemporalModel (dilated) variant",
+                what);
+  if (p->cfg.precision == VP3D_PRECISION_MIXED)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'mixed' is not supported for streaming", what);
+  return VP3D_OK;
+}
+
+static uint8_t* aligned_state(void* state) {
+  return reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(state), 1024));
+}
+
+}  // namespace vp3d
+
+using namespace vp3d;
+
+#define VP3D_EXPORT extern "C" __attribute__((visibility("default")))
+
+VP3D_EXPORT int vp3d_stream_lookahead(const vp3d_plan* p) {
+  if (!p) return fail(VP3D_ERR_INVALID, "stream_lookahead: null plan");
+  return stream_lookahead(p);
+}
+
+VP3D_EXPORT size_t vp3d_stream_state_bytes(const vp3d_plan* p, int S, int K) {
+  if (!p || S < 1 || K < 1 || (long long)S * (K + 2LL * vp3d_receptive_field(p)) > 0x7fffffffLL)
+    return 0;
+  return stream_layout(p, S, K).total;
+}
+
+VP3D_EXPORT int vp3d_stream_init(vp3d_plan* p, void* state, size_t state_bytes, int S, int K,
+                                 void* stream) {
+  if (S < 1 || K < 1)
+    return fail(VP3D_ERR_INVALID, "stream_init: streams (%d) and max_frames (%d) must be >= 1", S, K);
+  if (!p) return fail(VP3D_ERR_INVALID, "stream_init: null plan");
+  if (!state) return fail(VP3D_ERR_INVALID, "stream_init: null state");
+  VP3D_TRY(stream_supported(p, "stream_init"));
+  const size_t need = vp3d_stream_state_bytes(p, S, K);
+  if (need == 0) return fail(VP3D_ERR_UNSUPPORTED, "stream_init: %d streams x %d frames is too large", S, K);
+  if (state_bytes < need)
+    return fail(VP3D_ERR_WORKSPACE, "stream_init: state too small: %zu < %zu", state_bytes, need);
+  StreamHost h;
+  h.S = S;
+  h.K = K;
+  p->streams[state] = h;
+  CUDA_TRY(cudaMemsetAsync(aligned_state(state), 0, need - 1024, static_cast<cudaStream_t>(stream)));
+  return VP3D_OK;
+}
+
+VP3D_EXPORT int vp3d_stream_release(vp3d_plan* p, void* state) {
+  if (!p || !state) return fail(VP3D_ERR_INVALID, "stream_release: null argument");
+  p->streams.erase(state);
+  return VP3D_OK;
+}
+
+static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost** out) {
+  auto it = p->streams.find(state);
+  if (it == p->streams.end())
+    return fail(VP3D_ERR_STATE, "%s: state was not initialised with vp3d_stream_init", what);
+  *out = &it->second;
+  return VP3D_OK;
+}
+
+VP3D_EXPORT int vp3d_stream_push(vp3d_plan* p, void* state, const float* x, int k,
+                                 const uint8_t* start_mask, float* y, int64_t* frame,
+                                 void* stream) {
+  if (!state) return fail(VP3D_ERR_INVALID, "stream_push: null state");
+  if (k < 1) return fail(VP3D_ERR_INVALID, "stream_push: k must be >= 1 (got %d)", k);
+  if (!p) return fail(VP3D_ERR_INVALID, "stream_push: null plan");
+  if (!x || !y || !frame) return fail(VP3D_ERR_INVALID, "stream_push: null x, y or frame");
+  StreamHost* h = nullptr;
+  VP3D_TRY(stream_lookup(p, state, "stream_push", &h));
+  if (k > h->K)
+    return fail(VP3D_ERR_INVALID, "stream_push: k = %d frames exceeds max_frames = %d", k, h->K);
+  if (!p->conv_packed || !p->bn_packed)
+    return fail(VP3D_ERR_STATE, "stream_push: vp3d_set_weights has not been called");
+  return stream_step(p, aligned_state(state), *h, x, k, start_mask, y, k, 0,
+                     reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
+}
+
+VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t* frame,
+                                   void* stream) {
+  if (!state) return fail(VP3D_ERR_INVALID, "stream_finish: null state");
+  if (!p) return fail(VP3D_ERR_INVALID, "stream_finish: null plan");
+  StreamHost* h = nullptr;
+  VP3D_TRY(stream_lookup(p, state, "stream_finish", &h));
+  if (!p->conv_packed || !p->bn_packed)
+    return fail(VP3D_ERR_STATE, "stream_finish: vp3d_set_weights has not been called");
+  const int la = stream_lookahead(p);
+  if (la > 0 && (!y || !frame)) return fail(VP3D_ERR_INVALID, "stream_finish: null y or frame");
+  uint8_t* base = aligned_state(state);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int launches = 0;
+  for (int off = 0; off < la; off += h->K) {
+    const int k = la - off < h->K ? la - off : h->K;
+    VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, y, la, off,
+                         reinterpret_cast<long long*>(frame), s));
+    launches += p->last_launches;
+  }
+  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K).active, 0, h->S, s));
+  p->last_launches = launches;
+  return VP3D_OK;
+}

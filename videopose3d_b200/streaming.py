@@ -1,0 +1,244 @@
+"""Streaming (frame-by-frame) inference of a TemporalModel: one 3-D pose per new 2-D frame.
+
+The reference's causal models exist for real-time use (DOCUMENTATION.md: causal convolutions are
+"suitable for real-time applications"), but ``model(x)`` recomputes a whole receptive field per
+output frame.  A session keeps every conv layer's past activations in device rings and computes only
+the new frames' share (``include/vp3d_b200.h``, vp3d_stream_*):
+
+    sess = model.streaming(streams=S, max_frames=K)   # TemporalModel in eval()
+    y, frame = sess.push(x, start=None)   # x: (S, k, J_in, F) CUDA fp32, 1 <= k <= K
+    y, frame = sess.finish()              # the look-ahead tail of every slot; slots become idle
+    sess.reset()                          # drop all history
+
+Per slot, the outputs of frames 0..T-1 of a sequence are exactly ``model(xp)`` with ``xp`` the
+sequence padded as run.py's UnchunkedGenerator pads it (run.py:186-193, common/generators.py:
+216-238): ``np.pad(x, (pad + shift, pad - shift), 'edge')``, pad = (RF - 1) // 2, shift = pad
+for a causal model and 0 otherwise.  Output frame t comes back in the push that delivers input frame
+t + lookahead (lookahead = pad - shift, 0 for a causal model); ``frame`` numbers every returned row
+within its slot's sequence and is -1 for rows that are no frame yet.
+"""
+import weakref
+
+import numpy as np
+import torch
+
+from . import _capi
+
+
+def lookahead(model):
+    """Input frames a session needs past output frame t before it can return t: pad - shift with
+    shift = pad for a causal model (run.py:186-193)."""
+    return 0 if model._causal else (model.receptive_field() - 1) // 2
+
+
+def ring_history(filter_widths, dense=False):
+    """Frames of history each ring keeps next to the new ones: ring 0 holds the network input (the
+    expand conv's w0 - 1 frames), ring i the input of residual block i (its first conv spans
+    (w_i - 1) * dilation_i = 2 * pad_i frames; the same for the dense ablation).  They add up to
+    receptive_field - 1."""
+    hist = [filter_widths[0] - 1]
+    d = filter_widths[0]
+    for w in filter_widths[1:]:
+        hist.append((w - 1) * d)
+        d *= w
+    return hist
+
+
+def ring_bytes_per_stream(model, max_frames, planes=1):
+    """Device bytes of history one stream slot occupies (both mirror halves, every plane)."""
+    fw = model.filter_widths
+    c_in = -(-model.num_joints_in * model.in_features // 64) * 64
+    c = -(-model._channels // 64) * 64
+    total = 0
+    for i, h in enumerate(ring_history(fw)):
+        total += 2 * (h + max_frames + 1) * (c_in if i == 0 else c) * 2 * planes
+    return total
+
+
+class FrameBook:
+    """Host model of the frame bookkeeping the session's input kernel does on the device (used by
+    the tests): per slot a frame counter and an active flag."""
+
+    def __init__(self, streams, lookahead):
+        self.count = np.zeros(streams, np.int64)
+        self.active = np.zeros(streams, bool)
+        self.lookahead = lookahead
+
+    def push(self, k, start=None):
+        if start is not None:
+            start = np.asarray(start, bool)
+            self.count[start] = 0
+            self.active[start] = True
+        idx = self.count[:, None] + np.arange(k)[None, :] - self.lookahead
+        frame = np.where(self.active[:, None] & (idx >= 0), idx, -1)
+        self.count += k
+        return frame
+
+    def finish(self):
+        frame = self.push(self.lookahead) if self.lookahead else \
+            np.zeros((len(self.count), 0), np.int64)
+        self.active[:] = False
+        return frame
+
+
+def _param_versions(model):
+    conv, bn = model._param_tensors()
+    return (tuple((t.data_ptr(), t._version) for t in conv),
+            tuple((t.data_ptr(), t._version) for t in bn), model._stats_epoch)
+
+
+def check_push_input(x, streams, max_frames, joints, features):
+    """The validation push() applies to x (raises like the model's forward does)."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("push expects a torch tensor")
+    if not x.is_cuda:
+        raise RuntimeError("videopose3d_b200 streaming runs on CUDA (sm_90a) tensors only; "
+                           "there is no CPU fallback")
+    if x.dtype != torch.float32:
+        raise TypeError(f"expected a float32 input, got {x.dtype}")
+    if x.dim() != 4 or x.shape[0] != streams or x.shape[2] != joints or x.shape[3] != features:
+        raise ValueError(f"expected x of shape ({streams}, k, {joints}, {features}), "
+                         f"got {tuple(x.shape)}")
+    k = int(x.shape[1])
+    if not 1 <= k <= max_frames:
+        raise ValueError(f"push of {k} frames: k must be in [1, max_frames = {max_frames}]")
+    return k
+
+
+class StreamingSession:
+    """S stream slots running a TemporalModel frame by frame (see the module docstring).  Create it
+    with ``model.streaming(streams, max_frames)``."""
+
+    def __init__(self, model, streams, max_frames):
+        from .temporal_model import TemporalModel
+        if type(model)._variant != TemporalModel._variant:
+            raise NotImplementedError(
+                "streaming needs a TemporalModel; a TemporalModelOptimized1f state_dict loads into "
+                "TemporalModel(..., same arguments) unchanged -- stream that model instead")
+        if model.precision == "mixed":
+            raise NotImplementedError(
+                "precision 'mixed' cannot stream: its per-layer split choice depends on the "
+                "sequence length; use 'fp16', 'bf16' or 'bf16x3'")
+        if model.training:
+            raise RuntimeError("streaming is an eval-mode computation: call model.eval() first")
+        streams, max_frames = int(streams), int(max_frames)
+        if streams < 1 or max_frames < 1:
+            raise ValueError("streams and max_frames must be >= 1")
+        device = model.expand_conv.weight.device
+        if device.type != "cuda":
+            raise RuntimeError("streaming needs the model on a CUDA device; there is no CPU fallback")
+        self.model = model
+        self.streams = streams
+        self.max_frames = max_frames
+        self.precision = model.precision
+        self.device = device
+        self.lookahead = lookahead(model)
+        lib = _capi.load()
+        with torch.cuda.device(device):
+            self._plan = self._model_plan()
+            nbytes = lib.vp3d_stream_state_bytes(self._plan, streams, max_frames)
+            if nbytes == 0:
+                raise ValueError(f"{streams} streams x {max_frames} frames is too large a session")
+            self._state = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self._finalizer = weakref.finalize(self, _release, self._plan, self._state.data_ptr(),
+                                           model._plans)
+        self.reset()
+
+    def _model_plan(self):
+        # the model's plan of this precision (same packed eval weights as model(x)); the model's
+        # current-plan bookkeeping is left as it was
+        m = self.model
+        saved = (m._plan, m._plan_key)
+        try:
+            return m._get_plan(self.device, self.precision)
+        finally:
+            m._plan, m._plan_key = saved
+
+    def reset(self):
+        """Drop all history: every slot idle, weights re-read at the next push."""
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _capi.check(_capi.load().vp3d_stream_init(self._plan, self._state.data_ptr(),
+                                                      self._state.numel(), self.streams,
+                                                      self.max_frames, stream), "vp3d_stream_init")
+        self._versions = None
+        return self
+
+    def _prepare(self):
+        m = self.model
+        if m.training:
+            raise RuntimeError("the model is in train() mode: streaming is an eval-mode computation")
+        current = _param_versions(m)
+        if self._versions is not None and current != self._versions:
+            raise RuntimeError("the model's parameters changed since this session started; call "
+                               "reset() before pushing again (old and new weights never mix)")
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        saved = (m._plan, m._plan_key)
+        try:
+            plan = m._get_plan(self.device, self.precision)
+            m._sync_weights(plan, stream)
+        finally:
+            m._plan, m._plan_key = saved
+        self._versions = _param_versions(m)
+        return stream
+
+    def _start_mask(self, start):
+        if start is None:
+            return None
+        if isinstance(start, torch.Tensor):
+            if start.shape != (self.streams,):
+                raise ValueError(f"start must have shape ({self.streams},)")
+            if start.device != self.device:
+                raise RuntimeError("start must be on the session's device (or a list)")
+            return start.to(torch.uint8).contiguous()
+        start = [bool(v) for v in start]
+        if len(start) != self.streams:
+            raise ValueError(f"start must list {self.streams} slots")
+        if not any(start):
+            return None
+        return torch.tensor(start, dtype=torch.uint8).to(self.device)
+
+    def push(self, x, start=None):
+        """Push k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64)."""
+        k = check_push_input(x, self.streams, self.max_frames, self.model.num_joints_in,
+                             self.model.in_features)
+        if x.device != self.device:
+            raise RuntimeError("input and parameters are on different devices")
+        x = x.contiguous()
+        mask = self._start_mask(start)
+        y = torch.empty((self.streams, k, self.model.num_joints_out, 3), dtype=torch.float32,
+                        device=self.device)
+        frame = torch.empty((self.streams, k), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            stream = self._prepare()
+            _capi.check(_capi.load().vp3d_stream_push(
+                self._plan, self._state.data_ptr(), x.data_ptr(), k,
+                None if mask is None else mask.data_ptr(), y.data_ptr(), frame.data_ptr(), stream),
+                "vp3d_stream_push")
+        return y, frame
+
+    def finish(self):
+        """Emit the last `lookahead` frames of every slot (its last frame repeated, as the
+        generator's end padding does), then mark every slot idle."""
+        la = self.lookahead
+        y = torch.empty((self.streams, la, self.model.num_joints_out, 3), dtype=torch.float32,
+                        device=self.device)
+        frame = torch.empty((self.streams, la), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            stream = self._prepare()
+            _capi.check(_capi.load().vp3d_stream_finish(self._plan, self._state.data_ptr(),
+                                                        y.data_ptr(), frame.data_ptr(), stream),
+                        "vp3d_stream_finish")
+        return y, frame
+
+    def last_launch_count(self):
+        """Kernels the last push (or finish) launched."""
+        return _capi.load().vp3d_last_launch_count(self._plan)
+
+
+def _release(plan, state_ptr, plans):
+    # `plans` keeps the model's plan store (and with it the plan) alive until the session is gone
+    try:
+        _capi.load().vp3d_stream_release(plan, state_ptr)
+    except Exception:  # pragma: no cover - interpreter shutdown
+        pass

@@ -510,6 +510,13 @@ class TemporalModelBase(nn.Module):
     def last_launch_count(self):
         return 0 if self._plan is None else _capi.load().vp3d_last_launch_count(self._plan)
 
+    def streaming(self, streams, max_frames=1):
+        """A StreamingSession (videopose3d_b200.streaming) of `streams` slots that takes up to
+        `max_frames` new frames per slot and push, and returns each output frame as soon as its
+        input has arrived.  Not in the reference."""
+        from .streaming import StreamingSession
+        return StreamingSession(self, streams, max_frames)
+
 
 class _TrainFunction(torch.autograd.Function):
     """Training-mode forward/backward through the C ABI (vp3d_forward_train / vp3d_backward).
