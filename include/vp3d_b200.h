@@ -420,10 +420,28 @@ int vp3d_pose_errors(const float* pred, int32_t copies, const int32_t* mirror_sr
  * vp3d_stream_finish: emits the last `lookahead` frames of every slot by repeating each slot's
  * newest frame (the generator's end padding) into y (S, lookahead, J_out, 3) / frame (S,
  * lookahead), then marks every slot idle.
- * vp3d_stream_release: forgets `state` (the caller frees the memory). */
+ * vp3d_stream_release: forgets `state` (the caller frees the memory).
+ *
+ * Test-time flip augmentation (VP3D_STREAM_AUGMENT, the default of run.py, common/arguments.py:43):
+ * vp3d_stream_state_bytes_ex / vp3d_stream_init_ex with flags = VP3D_STREAM_AUGMENT give every slot
+ * a second, mirrored copy, as UnchunkedGenerator(augment=True) appends it (common/generators.py:
+ * 223-237: x negated, input joint j read from kps_src[j]), run in the same launches (rows [S, 2S) of
+ * every ring; the state is about twice as large).  Push and finish then return, per slot, the flip
+ * average of run.py:674-680, bit-identical to it: (plain + mirror(mirrored)) * 0.5 with mirror =
+ * negate x and read output joint j from joints_src[j].  kps_src: HOST int32 array of J_in entries
+ * (the map generators.mirror_source(J_in, kps_left, kps_right) builds), required with AUGMENT;
+ * joints_src: HOST int32 array of J_out entries, or NULL = negate x only (the trajectory model,
+ * run.py:678).  init_ex checks every entry is in [0, J) and copies the maps into the state, so a push
+ * still makes no host-to-device copy.  Unknown flag bits, and maps without AUGMENT, are errors.
+ * vp3d_stream_state_bytes / vp3d_stream_init are the _ex calls with flags = 0 and no maps; push,
+ * finish and release take either kind of session, with x, start_mask, y and frame shaped by S. */
+#define VP3D_STREAM_AUGMENT 1
 int vp3d_stream_lookahead(const vp3d_plan* plan);
 size_t vp3d_stream_state_bytes(const vp3d_plan* plan, int S, int K);
 int vp3d_stream_init(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, void* stream);
+size_t vp3d_stream_state_bytes_ex(const vp3d_plan* plan, int S, int K, int flags);
+int vp3d_stream_init_ex(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, int flags,
+                        const int32_t* kps_src, const int32_t* joints_src, void* stream);
 int vp3d_stream_push(vp3d_plan* plan, void* state, const float* x, int k, const uint8_t* start_mask,
                      float* y, int64_t* frame, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);

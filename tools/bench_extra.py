@@ -8,6 +8,9 @@
     (forward + backward + Adam(amsgrad) as in run.py:252, 409-420);
   * `--what stream`: streaming sessions (videopose3d_b200.streaming) against a user recomputing the
     receptive-field window per new frame, per-push latency over >= 500 pushes (see bench_stream);
+  * `--what stream_tta`: the same with test-time flip augmentation -- an augmented session against a
+    plain session of twice the slots and against model(windows) + metrics.flip_average (see
+    bench_stream_tta);
   * `--what metrics`: the final evaluation of run.py (run.py:652-721) on a Human3.6M-test-sized
     workload, the fused metrics kernel (videopose3d_b200.metrics) against the path run.py runs
     (torch mpjpe / n_mpjpe with .item(), .cpu(), NumPy p_mpjpe / mean_velocity_error of the staged
@@ -17,7 +20,7 @@ The cuDNN baseline is built here from plain torch.nn modules following common/mo
 151-197 (it is a measurement target, not the product and not the oracle).  CUDA-event timing,
 10 warm-up + N timed iterations, cudnn.benchmark on, GPU-resident synthetic inputs.
 
-    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics,stream] > extra.jsonl
+    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics,stream,stream_tta] > extra.jsonl
 """
 import argparse
 import json
@@ -298,6 +301,75 @@ def bench_stream(dev, pushes):
         torch.cuda.empty_cache()
 
 
+def bench_stream_tta(dev, pushes):
+    """Streaming with test-time flip augmentation (run.py's default), same model, configs and loop
+    as bench_stream.  Three arms alternate in one loop, CUDA events around each:
+      * the augmented session, S slots (plain + mirrored rows in the same launches, flip average on
+        the device);
+      * a plain session with 2S slots: the same GEMM rows, so the difference is the cost of
+        mirroring and averaging;
+      * what a TTA user has without it: model(windows) on the S*k plain and S*k mirrored
+        receptive-field windows, then metrics.flip_average."""
+    from videopose3d_b200 import metrics
+    left, right = [4, 5, 6, 11, 12, 13], [1, 2, 3, 14, 15, 16]
+    lists = dict(kps_left=left, kps_right=right, joints_left=left, joints_right=right)
+    torch.manual_seed(0)
+    m = vp.TemporalModel(J, F, J, filter_widths=ARC, channels=C).to(dev).eval().set_precision("fp16")
+    rf = m.receptive_field()
+    st_fl, cone_fl = stream_flops_per_frame(ARC, C, J * F, J * 3)
+    info = card()
+    p99 = lambda t: float(t[min(len(t) - 1, int(np.ceil(0.99 * len(t))) - 1)])  # noqa: E731
+    for S, k in ((1, 1), (16, 1), (256, 1), (1024, 1), (256, 16)):
+        aug = m.streaming(streams=S, max_frames=k, augment=True, **lists)
+        plain = m.streaming(streams=2 * S, max_frames=k)
+        xs = (torch.rand(S, k, J, F, device=dev) * 2 - 1)
+        x2 = (torch.rand(2 * S, k, J, F, device=dev) * 2 - 1)
+        win = (torch.rand(2 * S * k, rf, J, F, device=dev) * 2 - 1)   # [plain; mirrored] windows
+
+        def baseline():
+            return metrics.flip_average(m(win).view(2, S * k, J, 3), left, right)
+
+        arms = (("augmented", lambda: aug.push(xs)), ("plain_2S", lambda: plain.push(x2)),
+                ("model_windows_flip_average", baseline))
+        with torch.no_grad():
+            aug.push(xs, start=[True] * S)
+            plain.push(x2, start=[True] * 2 * S)
+            for _ in range(50):
+                for _, fn in arms:
+                    fn()
+        torch.cuda.synchronize()
+        ev = [[(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+               for _ in arms] for _ in range(pushes)]
+        with torch.no_grad():
+            for n, e in enumerate(ev):
+                for j in range(len(arms)):   # rotated, so that no arm always follows the same one
+                    i = (j + n) % len(arms)
+                    e[i][0].record()
+                    arms[i][1]()
+                    e[i][1].record()
+            # the sessions share the model's plan and its launch counter: read it after each call
+            launches = {}
+            for (name, fn), count in zip(arms, (aug.last_launch_count, plain.last_launch_count,
+                                                lambda: m.last_launch_count() + 1)):
+                fn()
+                launches[name] = count()
+        torch.cuda.synchronize()
+        res = dict(what="stream_tta_push", streams=S, k=k, precision="fp16", arc=ARC, channels=C,
+                   pushes=pushes, l2_flush="none", **info)
+        for i, (name, _) in enumerate(arms):
+            t = np.sort([e[i][0].elapsed_time(e[i][1]) for e in ev])
+            med = float(np.median(t))
+            res[name] = dict(ms_median=med, ms_p99=p99(t), frames_per_s=S * k / med * 1e3,
+                             launches=launches[name],
+                             mflop_per_frame=2 * (cone_fl if i == 2 else st_fl) / 1e6)
+        res["augmented_over_plain_2S"] = res["augmented"]["ms_median"] / res["plain_2S"]["ms_median"]
+        res["speedup_over_windows"] = (res["model_windows_flip_average"]["ms_median"]
+                                       / res["augmented"]["ms_median"])
+        emit(**res)
+        del aug, plain, xs, x2, win
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -309,6 +381,8 @@ def main():
     dev = torch.device("cuda:0")
     if "stream" in what:
         bench_stream(dev, args.pushes)
+    if "stream_tta" in what:
+        bench_stream_tta(dev, args.pushes)
     if "metrics" in what:
         bench_metrics(dev, args.reps)
     torch.backends.cudnn.benchmark = True

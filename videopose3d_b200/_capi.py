@@ -22,6 +22,7 @@ VP3D_PACK_BN_EVAL = 2
 VP3D_PACK_CONV_T = 4
 VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
+VP3D_STREAM_AUGMENT = 1
 
 _LIB_NAME = "libvp3d_b200.so"
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_lib", _LIB_NAME)
@@ -222,6 +223,11 @@ SIGNATURES = {
     "vp3d_stream_state_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]),
     "vp3d_stream_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
                                         ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "vp3d_stream_state_bytes_ex": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                     ctypes.c_int]),
+    "vp3d_stream_init_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_push": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_void_p]),

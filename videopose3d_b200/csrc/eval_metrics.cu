@@ -43,8 +43,7 @@ __device__ __forceinline__ double warp_sum(double v) {  // butterfly: every lane
   return v;
 }
 
-// Flip-averaged prediction of joint j of frame f, rounded as torch rounds
-// `torch.mean(stack(p0, mirror(p1)), dim=0)`: one fp32 add, then the exact * 0.5.
+// Flip-averaged prediction of joint j of frame f (flip_average, internal.cuh).
 __device__ __forceinline__ void load_avg(const EvalArgs& a, long long f, int j, float* out) {
   const float* p0 = a.pred + (f * a.J + j) * 3;
   if (a.copies == 1) {
@@ -53,9 +52,9 @@ __device__ __forceinline__ void load_avg(const EvalArgs& a, long long f, int j, 
   }
   const int s = a.mirror_src ? a.mirror_src[j] : j;
   const float* p1 = a.pred + ((a.frames + f) * a.J + s) * 3;
-  out[0] = __fmul_rn(__fadd_rn(p0[0], -p1[0]), 0.5f);
-  out[1] = __fmul_rn(__fadd_rn(p0[1], p1[1]), 0.5f);
-  out[2] = __fmul_rn(__fadd_rn(p0[2], p1[2]), 0.5f);
+  out[0] = flip_average(p0[0], p1[0], 0);
+  out[1] = flip_average(p0[1], p1[1], 1);
+  out[2] = flip_average(p0[2], p1[2], 2);
 }
 
 // One Jacobi rotation zeroing A[p][q] of the symmetric 4x4 A, accumulated into the columns of V.

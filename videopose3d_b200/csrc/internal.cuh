@@ -53,12 +53,22 @@ struct PackedConv {
   float* shift = nullptr;
 };
 
+// One coordinate of the test-time flip average (run.py:677-680): p0 from the plain copy, p1 from the
+// mirrored copy (its joints already swapped back), axis 0 negated back.  Rounded as torch rounds
+// `torch.mean(stack(p0, mirror(p1)), dim=0)`: one fp32 add, then the exact * 0.5.  The one
+// definition of run.py's averaging, shared by eval_metrics.cu and stream.cu.
+__device__ __forceinline__ float flip_average(float p0, float p1, int axis) {
+  return __fmul_rn(__fadd_rn(p0, axis == 0 ? -p1 : p1), 0.5f);
+}
+
 struct TrainState;  // train_api.cu
 
 // stream.cu: host side of one streaming session (vp3d_stream_init); the rings live in the
 // caller's device state buffer
 struct StreamHost {
-  int S = 0, K = 0;
+  int S = 0, K = 0;       // logical stream slots, max frames per push
+  int flags = 0;          // VP3D_STREAM_* of vp3d_stream_init_ex
+  bool joint_src = false; // AUGMENT: an output joint map is stored in the state (else negate x only)
   long long q = 0;        // frames pushed since vp3d_stream_init (all slots advance together)
   long long prev_q = 0;   // q before the last push
   int prev_k = 0;         // frames of the last push (their ring rows still need their mirror copy)

@@ -23,6 +23,14 @@
 // row (tap_row_step = 0), which is the very sum (pair -> tap -> k-block order, same operands) the
 // offline forward evaluates on an edge-padded stretch; the broadcast kernel then writes it into
 // the history positions of the starting slots only.
+//
+// Test-time flip augmentation (VP3D_STREAM_AUGMENT).  Slot s runs two physical rows: row s the
+// plain copy, row S + s the mirrored one (common/generators.py:223-237), in every ring and buffer,
+// so every layer is the same flat GEMM over P = 2S rows.  Only the frame bookkeeping and the
+// output stay logical: the output kernel writes the flip average of rows s and S + s (run.py:
+// 674-680).  The offline forward never mixes samples, so each physical row is the offline forward
+// of its own padded sequence; the mirrored row's start history is v_l(mirror(x0)), the edge padding
+// of the mirrored sequence.
 #include <cuda_fp16.h>
 
 #include "internal.cuh"
@@ -36,7 +44,7 @@ constexpr int kMaxRings = VP3D_MAX_WIDTHS;   // ring 0 = network input, ring i =
 
 struct StreamRing {
   __nv_bfloat16* base;   // plane 0, position 0
-  long long plane;       // elements per plane (2R * S * ld)
+  long long plane;       // elements per plane (2R * P * ld, P physical rows per position)
   int ld, H, R;
   int w0;                // first window position of the current push
   int prev_w0, prev_k;   // window start and new frames of the previous push (prev_k = 0: none)
@@ -48,13 +56,18 @@ struct StreamLayout {
   long long plane[kMaxRings];   // elements per ring plane
   size_t ring[kMaxRings];       // byte offsets
   size_t count = 0, active = 0, h = 0, xlast = 0, ybuf = 0, total = 0;
-  size_t v[kMaxRings];          // v_l(x0) of rings 1..nb: [plane][S][C]
+  size_t v[kMaxRings];          // v_l(x0) of rings 1..nb: [plane][P][C]
+  size_t kps = 0, jsrc = 0;     // AUGMENT: int32 mirror maps [J_in], [J_out]
 };
 
-StreamLayout stream_layout(const vp3d_plan* p, int S, int K) {
+// rows every ring, activation and output buffer holds per frame position
+inline int physical_rows(int S, int flags) { return flags & VP3D_STREAM_AUGMENT ? 2 * S : S; }
+
+StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   StreamLayout L;
   L.rings = p->nb + 1;
   const int planes = p->planes;
+  const int P = physical_rows(S, flags);
   size_t off = 0;
   L.count = off; off = align_up(off + (size_t)S * 8, 1024);
   L.active = off; off = align_up(off + (size_t)S, 1024);
@@ -62,19 +75,23 @@ StreamLayout stream_layout(const vp3d_plan* p, int S, int K) {
     L.H[l] = 2 * p->pad[l];
     L.R[l] = L.H[l] + K + 1;
     L.ld[l] = l == 0 ? p->c_in_pad : p->C;
-    L.plane[l] = 2LL * L.R[l] * S * L.ld[l];
+    L.plane[l] = 2LL * L.R[l] * P * L.ld[l];
     L.ring[l] = off;
     off = align_up(off + (size_t)L.plane[l] * planes * 2, 1024);
   }
-  const size_t act = (size_t)planes * K * S * p->C * 2;
+  const size_t act = (size_t)planes * K * P * p->C * 2;
   L.h = off; off = align_up(off + act, 1024);
   L.xlast = off; off = align_up(off + act, 1024);
   L.v[0] = 0;
   for (int l = 1; l < L.rings; ++l) {
     L.v[l] = off;
-    off = align_up(off + (size_t)planes * S * p->C * 2, 1024);
+    off = align_up(off + (size_t)planes * P * p->C * 2, 1024);
   }
-  L.ybuf = off; off = align_up(off + (size_t)K * S * p->c_out_raw * 4, 1024);
+  L.ybuf = off; off = align_up(off + (size_t)K * P * p->c_out_raw * 4, 1024);
+  if (flags & VP3D_STREAM_AUGMENT) {
+    L.kps = off; off = align_up(off + (size_t)p->cfg.num_joints_in * 4, 1024);
+    L.jsrc = off; off = align_up(off + (size_t)p->cfg.num_joints_out * 4, 1024);
+  }
   L.total = off + 1024;   // slack for aligning the caller's pointer
   return L;
 }
@@ -92,8 +109,9 @@ __device__ __forceinline__ __nv_bfloat16 to_f16_bits(float v) {
 
 struct StepArgs {
   StreamRing ring[kMaxRings];
-  int rings, planes, f16, S, k, c_raw;
+  int rings, planes, f16, S, P, k, c_raw, feat;
   const float* x;          // (S, k, c_raw) fp32, or null: repeat each slot's newest frame (finish)
+  const int* kps;          // AUGMENT: [J_in] mirror source of every input joint; null: no rows >= S
   const uint8_t* start;    // (S,) or null
   long long* count;        // frames of the current sequence pushed so far, per slot
   uint8_t* active;         // 1 while the slot holds a sequence
@@ -101,15 +119,26 @@ struct StepArgs {
   int frame_ld, frame_off, lookahead;
 };
 
+// Channel c of the mirrored input frame (generators.py:235-237) is source channel *src, negated when
+// *neg: feature 0 negated, joint j read from kps[j].  Negation is exact, so the pack below rounds it
+// as the offline pack rounds the generator's mirrored batch.
+__device__ __forceinline__ void mirror_channel(int c, const StepArgs& a, int* src, bool* neg) {
+  if (c >= a.c_raw) return;
+  const int j = c / a.feat, e = c - j * a.feat;
+  *src = __ldg(a.kps + j) * a.feat + e;
+  *neg = e == 0;
+}
+
 // One launch at the head of every push:
 //   * frame bookkeeping: a starting slot resets its frame counter; output row f of slot s is frame
 //     count + f - lookahead of its sequence, or -1 (warm-up of the look-ahead, idle slot);
 //   * the input pack: fp32 (S, k, J*F) -> 16-bit ring-0 rows (both copies), zero-padded channels,
 //     rounded exactly as the offline input pack rounds (hi / lo split for bf16x3, saturating fp16);
-//     in finish mode the slot's newest packed frame is repeated instead (the generator's end
+//     with AUGMENT every frame is packed twice, plain into row s and mirrored into row S + s; in
+//     finish mode each physical row's newest packed frame is repeated instead (the generator's end
 //     padding, generators.py:216-238);
 //   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb.
-__global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
+__global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) {
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nthr = (long long)gridDim.x * blockDim.x;
   for (long long s = tid; s < a.S; s += nthr) {
@@ -126,20 +155,30 @@ __global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
 
   const StreamRing& r0 = a.ring[0];
   const int pairs = r0.ld >> 1;
-  const long long n_pack = (long long)a.k * a.S * pairs;
+  const long long n_pack = (long long)a.k * a.P * pairs;
   const int src_pos = pos_mod_dev(r0.w0 + r0.H - 1, r0.R);
   for (long long i = tid; i < n_pack; i += nthr) {
     const int cp = (int)(i % pairs);
-    const long long row = i / pairs;          // f * S + s
-    const int s = (int)(row % a.S), f = (int)(row / a.S);
+    const long long row = i / pairs;          // f * P + r
+    const int r = (int)(row % a.P), f = (int)(row / a.P);
     const int pos = r0.w0 + r0.H + f;
-    const long long d0 = ((long long)pos * a.S + s) * r0.ld + 2 * cp;
-    const long long d1 = ((long long)mirror_pos(pos, r0.R) * a.S + s) * r0.ld + 2 * cp;
+    const long long d0 = ((long long)pos * a.P + r) * r0.ld + 2 * cp;
+    const long long d1 = ((long long)mirror_pos(pos, r0.R) * a.P + r) * r0.ld + 2 * cp;
     if (a.x) {
+      const bool mirrored = r >= a.S;
+      const int s = mirrored ? r - a.S : r;
       const float* src = a.x + ((long long)s * a.k + f) * a.c_raw;
       const int c0 = 2 * cp;
-      const float v0 = c0 < a.c_raw ? __ldg(src + c0) : 0.0f;
-      const float v1 = c0 + 1 < a.c_raw ? __ldg(src + c0 + 1) : 0.0f;
+      int i0 = c0, i1 = c0 + 1;   // source channels
+      bool n0 = false, n1 = false;
+      if (mirrored) {
+        mirror_channel(c0, a, &i0, &n0);
+        mirror_channel(c0 + 1, a, &i1, &n1);
+      }
+      float v0 = c0 < a.c_raw ? __ldg(src + i0) : 0.0f;
+      float v1 = c0 + 1 < a.c_raw ? __ldg(src + i1) : 0.0f;
+      if (n0) v0 = -v0;
+      if (n1) v1 = -v1;
       __nv_bfloat162 hi, lo;
       if (a.f16) {
         hi.x = to_f16_bits(v0);
@@ -157,7 +196,7 @@ __global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
         *reinterpret_cast<__nv_bfloat162*>(r0.base + r0.plane + d1) = lo;
       }
     } else {
-      const long long sr = ((long long)src_pos * a.S + s) * r0.ld + 2 * cp;
+      const long long sr = ((long long)src_pos * a.P + r) * r0.ld + 2 * cp;
       for (int pl = 0; pl < a.planes; ++pl) {
         const uint32_t v = *reinterpret_cast<const uint32_t*>(r0.base + pl * r0.plane + sr);
         *reinterpret_cast<uint32_t*>(r0.base + pl * r0.plane + d0) = v;
@@ -170,7 +209,7 @@ __global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
   for (int l = 1; l < kMaxRings; ++l) {   // (unrolled: the ring table stays in parameter space)
     const StreamRing& r = a.ring[l];
     if (l >= a.rings || r.prev_k == 0) continue;
-    const long long per_frame = (long long)a.S * r.ld / 8;   // 16-byte vectors
+    const long long per_frame = (long long)a.P * r.ld / 8;   // 16-byte vectors
     const long long n = (long long)a.planes * r.prev_k * per_frame;
     for (long long i = tid; i < n; i += nthr) {
       const long long e = i % per_frame;
@@ -178,9 +217,9 @@ __global__ void __launch_bounds__(256) stream_input_kernel(const StepArgs a) {
       const int f = (int)(q % r.prev_k), pl = (int)(q / r.prev_k);
       const int pos = r.prev_w0 + r.H + f;
       const uint4* src = reinterpret_cast<const uint4*>(r.base + pl * r.plane +
-                                                        (long long)pos * a.S * r.ld) + e;
+                                                        (long long)pos * a.P * r.ld) + e;
       uint4* dst = reinterpret_cast<uint4*>(r.base + pl * r.plane +
-                                            (long long)mirror_pos(pos, r.R) * a.S * r.ld) + e;
+                                            (long long)mirror_pos(pos, r.R) * a.P * r.ld) + e;
       *dst = *src;
     }
   }
@@ -190,12 +229,12 @@ struct BcastArgs {
   StreamRing ring[kMaxRings];
   const __nv_bfloat16* src[kMaxRings];   // [plane][S][ld] rows v_l(x0)
   long long src_plane[kMaxRings];
-  int rings, planes, S;
+  int rings, planes, S, P;
   const uint8_t* start;
 };
 
 // Start of a sequence: history positions [w0, w0 + H) of every ring (both copies) of the starting
-// slots receive that slot's v_l(x0).
+// slots' physical rows (row r belongs to slot r mod S) receive that row's v_l(x0).
 __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a) {
   pdl_entry();
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -203,27 +242,31 @@ __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a
   for (int l = 0; l < a.rings; ++l) {
     const StreamRing& r = a.ring[l];
     const int vec = r.ld / 8;
-    const long long n = (long long)a.planes * r.H * a.S * vec;
+    const long long n = (long long)a.planes * r.H * a.P * vec;
     for (long long i = tid; i < n; i += nthr) {
       const int e = (int)(i % vec);
       long long q = i / vec;
-      const int s = (int)(q % a.S);
-      q /= a.S;
-      if (!a.start[s]) continue;
+      const int row = (int)(q % a.P);
+      q /= a.P;
+      if (!a.start[row < a.S ? row : row - a.S]) continue;
       const int j = (int)(q % r.H), pl = (int)(q / r.H);
       const uint4 v = *(reinterpret_cast<const uint4*>(a.src[l] + pl * a.src_plane[l] +
-                                                       (long long)s * r.ld) + e);
+                                                       (long long)row * r.ld) + e);
       const int pos = r.w0 + j;
       __nv_bfloat16* pbase = r.base + pl * r.plane;
-      *(reinterpret_cast<uint4*>(pbase + ((long long)pos * a.S + s) * r.ld) + e) = v;
-      *(reinterpret_cast<uint4*>(pbase + ((long long)mirror_pos(pos, r.R) * a.S + s) * r.ld) + e) = v;
+      *(reinterpret_cast<uint4*>(pbase + ((long long)pos * a.P + row) * r.ld) + e) = v;
+      *(reinterpret_cast<uint4*>(pbase + ((long long)mirror_pos(pos, r.R) * a.P + row) * r.ld) + e) = v;
     }
   }
 }
 
-// Shrink output rows are time-major (f * S + s); y is (S, y_frames, c_out) at frame offset f_off.
+// Shrink output rows are time-major; y is (S, y_frames, c_out) at frame offset f_off.  Plain: rows
+// f * S + s are copied.  augment: rows f * 2S + s (plain) and f * 2S + S + s (mirrored) are
+// flip-averaged (run.py:674-680), output joint j of the mirrored row read from joint_src[j]
+// (null: no joint swap, the trajectory model).
 __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, float* y, int S, int k,
-                                                            int c_out, int y_frames, int f_off) {
+                                                            int c_out, int y_frames, int f_off,
+                                                            int augment, const int* joint_src) {
   pdl_entry();
   const long long n = (long long)k * S * c_out;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
@@ -231,7 +274,16 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
     const int c = (int)(i % c_out);
     const long long r = i / c_out;
     const int s = (int)(r % S), f = (int)(r / S);
-    y[((long long)s * y_frames + f_off + f) * c_out + c] = ybuf[i];
+    float v;
+    if (augment) {
+      const int j = c / 3, e = c - 3 * j;
+      const int js = joint_src ? __ldg(joint_src + j) : j;
+      const float* row0 = ybuf + ((long long)f * 2 * S + s) * c_out;
+      v = flip_average(row0[c], row0[(long long)S * c_out + js * 3 + e], e);
+    } else {
+      v = ybuf[i];
+    }
+    y[((long long)s * y_frames + f_off + f) * c_out + c] = v;
   }
 }
 
@@ -252,11 +304,14 @@ int stream_lookahead(const vp3d_plan* p) {
 
 // One push of k frames (x null: k copies of every slot's newest frame).  y receives rows
 // [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, frame the matching (S, y_frames) entries.
+// The GEMMs run over P physical rows per frame (S, or 2S with AUGMENT).
 static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
                        const uint8_t* start, float* y, int y_frames, int f_off, long long* frame,
                        cudaStream_t stream) {
   const int S = h.S, K = h.K, C = p->C, planes = p->planes;
-  const StreamLayout L = stream_layout(p, S, K);
+  const bool aug = h.flags & VP3D_STREAM_AUGMENT;
+  const int P = physical_rows(S, h.flags);
+  const StreamLayout L = stream_layout(p, S, K, h.flags);
   int launches = 0;
 
   StepArgs a;
@@ -278,9 +333,12 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.planes = planes;
   a.f16 = p->f16;
   a.S = S;
+  a.P = P;
   a.k = k;
   a.c_raw = p->c_in_raw;
+  a.feat = p->cfg.in_features;
   a.x = x;
+  a.kps = aug ? reinterpret_cast<const int*>(base + L.kps) : nullptr;
   a.start = start;
   a.count = reinterpret_cast<long long*>(base + L.count);
   a.active = base + L.active;
@@ -289,8 +347,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.frame_off = f_off;
   a.lookahead = stream_lookahead(p);
   {
-    long long work = (long long)k * S * (p->c_in_pad / 2);
-    for (int l = 1; l < L.rings; ++l) work += (long long)planes * h.prev_k * S * C / 8;
+    long long work = (long long)k * P * (p->c_in_pad / 2);
+    for (int l = 1; l < L.rings; ++l) work += (long long)planes * h.prev_k * P * C / 8;
     if (work < S) work = S;
     // a plain launch: the first kernel of a push may follow a weight re-pack, which the GEMMs'
     // early weight loads must not overlap
@@ -301,13 +359,13 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
 
   __nv_bfloat16* hbuf = reinterpret_cast<__nv_bfloat16*>(base + L.h);
   __nv_bfloat16* xlast = reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
-  const long long act_plane = (long long)K * S * C;
-  const long long v_plane = (long long)S * C;
+  const long long act_plane = (long long)K * P * C;
+  const long long v_plane = (long long)P * C;
   auto vbuf = [&](int l) { return reinterpret_cast<__nv_bfloat16*>(base + L.v[l]); };
   // window of ring l: frame positions [w0, w0 + H + k); new frames start at w0 + H
-  auto window = [&](int l) { return ring[l].base + (long long)ring[l].w0 * S * ring[l].ld; };
+  auto window = [&](int l) { return ring[l].base + (long long)ring[l].w0 * P * ring[l].ld; };
   auto new_rows = [&](int l) {
-    return ring[l].base + (long long)(ring[l].w0 + ring[l].H) * S * ring[l].ld;
+    return ring[l].base + (long long)(ring[l].w0 + ring[l].H) * P * ring[l].ld;
   };
   const int* fw = p->cfg.filter_widths;
 
@@ -340,9 +398,9 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   if (start && p->nb >= 1) {
     // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i), every tap on the same row
     common(d);
-    d.a = new_rows(0); d.a_plane_stride = ring[0].plane; d.a_rows = S; d.a_ld = p->c_in_pad;
+    d.a = new_rows(0); d.a_plane_stride = ring[0].plane; d.a_rows = P; d.a_ld = p->c_in_pad;
     d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
-    d.tap_row_step = 0; d.out_rows = S;
+    d.tap_row_step = 0; d.out_rows = P;
     d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
     set_out(d, 0, true);
     VP3D_TRY(run_conv(&d, stream));
@@ -351,15 +409,15 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
       const PackedConv& c0 = p->conv[2 * (i - 1)];
       const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
       common(d);
-      d.a = vbuf(i); d.a_plane_stride = v_plane; d.a_rows = S; d.a_ld = C;
+      d.a = vbuf(i); d.a_plane_stride = v_plane; d.a_rows = P; d.a_ld = C;
       d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
-      d.tap_row_step = 0; d.out_rows = S;
+      d.tap_row_step = 0; d.out_rows = P;
       d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
       d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
       VP3D_TRY(run_conv(&d, stream));
       common(d);
-      d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = S; d.a_ld = C;
-      d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = S;
+      d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = P; d.a_ld = C;
+      d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = P;
       d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
       d.res = vbuf(i); d.res_plane_stride = v_plane; d.res_ld = C; d.res_row_step = 1;
       d.res_row_off = 0;
@@ -381,11 +439,12 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
         b.src[l] = vbuf(l);
         b.src_plane[l] = v_plane;
       }
-      work += (long long)planes * ring[l].H * S * ring[l].ld / 8;
+      work += (long long)planes * ring[l].H * P * ring[l].ld / 8;
     }
     b.rings = L.rings;
     b.planes = planes;
     b.S = S;
+    b.P = P;
     b.start = start;
     CUDA_TRY(launch_pdl(stream_broadcast_kernel, dim3(grid_for(work)), dim3(256), 0, stream, b));
     ++launches;
@@ -393,10 +452,10 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
 
   // ---- the push: expand (model.py:127), residual blocks (:129-135), shrink (:137)
   common(d);
-  d.a = window(0); d.a_plane_stride = ring[0].plane; d.a_rows = (ring[0].H + k) * S;
+  d.a = window(0); d.a_plane_stride = ring[0].plane; d.a_rows = (ring[0].H + k) * P;
   d.a_ld = p->c_in_pad;
   d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
-  d.tap_row_step = S; d.out_rows = k * S;
+  d.tap_row_step = P; d.out_rows = k * P;
   d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
   set_out(d, 0, false);
   VP3D_TRY(run_conv(&d, stream));
@@ -405,29 +464,30 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     const PackedConv& c0 = p->conv[2 * (i - 1)];
     const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
     common(d);
-    d.a = window(i); d.a_plane_stride = ring[i].plane; d.a_rows = (ring[i].H + k) * S; d.a_ld = C;
+    d.a = window(i); d.a_plane_stride = ring[i].plane; d.a_rows = (ring[i].H + k) * P; d.a_ld = C;
     d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
-    d.tap_row_step = p->dilation[i] * S; d.out_rows = k * S;
+    d.tap_row_step = p->dilation[i] * P; d.out_rows = k * P;
     d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
     d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
     VP3D_TRY(run_conv(&d, stream));
     common(d);
-    d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = k * S; d.a_ld = C;
-    d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = k * S;
+    d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
+    d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = k * P;
     d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
     // residual: the centre tap (causal: the newest) of the block input window, model.py:130-132
     d.res = window(i); d.res_plane_stride = ring[i].plane; d.res_ld = C; d.res_row_step = 1;
-    d.res_row_off = (p->pad[i] + p->shift_dil[i]) * S;
+    d.res_row_off = (p->pad[i] + p->shift_dil[i]) * P;
     set_out(d, i, false);
     VP3D_TRY(run_conv(&d, stream));
     launches += 2;
   }
-  // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1)
-  const bool direct = y_frames == 1 || S == 1;
+  // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
+  // AUGMENT: the flip average always takes the output kernel)
+  const bool direct = !aug && (y_frames == 1 || S == 1);
   float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
   common(d);
-  d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * S; d.a_ld = C;
-  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad; d.out_rows = k * S;
+  d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
+  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad; d.out_rows = k * P;
   d.scale = p->shrink.scale; d.shift = p->shrink.shift; d.relu = 0;
   d.out_f32 = direct ? y + (long long)f_off * p->c_out_raw : ybuf;
   d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
@@ -436,7 +496,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   if (!direct) {
     CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
                         dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
-                        f_off));
+                        f_off, (int)aug,
+                        h.joint_src ? (const int*)(base + L.jsrc) : (const int*)nullptr));
     ++launches;
   }
   h.prev_q = h.q;
@@ -470,29 +531,78 @@ VP3D_EXPORT int vp3d_stream_lookahead(const vp3d_plan* p) {
   return stream_lookahead(p);
 }
 
-VP3D_EXPORT size_t vp3d_stream_state_bytes(const vp3d_plan* p, int S, int K) {
-  if (!p || S < 1 || K < 1 || (long long)S * (K + 2LL * vp3d_receptive_field(p)) > 0x7fffffffLL)
+VP3D_EXPORT size_t vp3d_stream_state_bytes_ex(const vp3d_plan* p, int S, int K, int flags) {
+  if (!p || S < 1 || K < 1 || (flags & ~VP3D_STREAM_AUGMENT) ||
+      (long long)physical_rows(S, flags) * (K + 2LL * vp3d_receptive_field(p)) > 0x7fffffffLL)
     return 0;
-  return stream_layout(p, S, K).total;
+  return stream_layout(p, S, K, flags).total;
+}
+
+VP3D_EXPORT size_t vp3d_stream_state_bytes(const vp3d_plan* p, int S, int K) {
+  return vp3d_stream_state_bytes_ex(p, S, K, 0);
+}
+
+static int check_mirror_map(const int32_t* map, int n, const char* what, const char* name) {
+  for (int j = 0; j < n; ++j)
+    if (map[j] < 0 || map[j] >= n)
+      return fail(VP3D_ERR_INVALID, "%s: %s[%d] = %d is not a joint index in [0, %d)", what, name, j,
+                  map[j], n);
+  return VP3D_OK;
+}
+
+static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state_bytes, int S,
+                       int K, int flags, const int32_t* kps_src, const int32_t* joints_src,
+                       void* stream) {
+  if (S < 1 || K < 1)
+    return fail(VP3D_ERR_INVALID, "%s: streams (%d) and max_frames (%d) must be >= 1", what, S, K);
+  if (flags & ~VP3D_STREAM_AUGMENT)
+    return fail(VP3D_ERR_INVALID, "%s: unknown flags 0x%x", what, (unsigned)flags);
+  const bool aug = flags & VP3D_STREAM_AUGMENT;
+  if (!aug && (kps_src || joints_src))
+    return fail(VP3D_ERR_INVALID, "%s: mirror maps given without VP3D_STREAM_AUGMENT", what);
+  if (aug && !kps_src)
+    return fail(VP3D_ERR_INVALID, "%s: VP3D_STREAM_AUGMENT needs kps_src", what);
+  if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
+  if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
+  VP3D_TRY(stream_supported(p, what));
+  const int j_in = p->cfg.num_joints_in, j_out = p->cfg.num_joints_out;
+  if (aug) {
+    VP3D_TRY(check_mirror_map(kps_src, j_in, what, "kps_src"));
+    if (joints_src) VP3D_TRY(check_mirror_map(joints_src, j_out, what, "joints_src"));
+  }
+  const size_t need = vp3d_stream_state_bytes_ex(p, S, K, flags);
+  if (need == 0) return fail(VP3D_ERR_UNSUPPORTED, "%s: %d streams x %d frames is too large", what, S, K);
+  if (state_bytes < need)
+    return fail(VP3D_ERR_WORKSPACE, "%s: state too small: %zu < %zu", what, state_bytes, need);
+  StreamHost h;
+  h.S = S;
+  h.K = K;
+  h.flags = flags;
+  h.joint_src = aug && joints_src;
+  p->streams[state] = h;
+  uint8_t* base = aligned_state(state);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemsetAsync(base, 0, need - 1024, s));
+  if (aug) {
+    // the maps live in the state from here on: pushes read them on the device
+    const StreamLayout L = stream_layout(p, S, K, flags);
+    CUDA_TRY(cudaMemcpyAsync(base + L.kps, kps_src, (size_t)j_in * 4, cudaMemcpyHostToDevice, s));
+    if (joints_src)
+      CUDA_TRY(cudaMemcpyAsync(base + L.jsrc, joints_src, (size_t)j_out * 4, cudaMemcpyHostToDevice, s));
+  }
+  return VP3D_OK;
+}
+
+VP3D_EXPORT int vp3d_stream_init_ex(vp3d_plan* p, void* state, size_t state_bytes, int S, int K,
+                                    int flags, const int32_t* kps_src, const int32_t* joints_src,
+                                    void* stream) {
+  return stream_init("stream_init_ex", p, state, state_bytes, S, K, flags, kps_src, joints_src,
+                     stream);
 }
 
 VP3D_EXPORT int vp3d_stream_init(vp3d_plan* p, void* state, size_t state_bytes, int S, int K,
                                  void* stream) {
-  if (S < 1 || K < 1)
-    return fail(VP3D_ERR_INVALID, "stream_init: streams (%d) and max_frames (%d) must be >= 1", S, K);
-  if (!p) return fail(VP3D_ERR_INVALID, "stream_init: null plan");
-  if (!state) return fail(VP3D_ERR_INVALID, "stream_init: null state");
-  VP3D_TRY(stream_supported(p, "stream_init"));
-  const size_t need = vp3d_stream_state_bytes(p, S, K);
-  if (need == 0) return fail(VP3D_ERR_UNSUPPORTED, "stream_init: %d streams x %d frames is too large", S, K);
-  if (state_bytes < need)
-    return fail(VP3D_ERR_WORKSPACE, "stream_init: state too small: %zu < %zu", state_bytes, need);
-  StreamHost h;
-  h.S = S;
-  h.K = K;
-  p->streams[state] = h;
-  CUDA_TRY(cudaMemsetAsync(aligned_state(state), 0, need - 1024, static_cast<cudaStream_t>(stream)));
-  return VP3D_OK;
+  return stream_init("stream_init", p, state, state_bytes, S, K, 0, nullptr, nullptr, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_release(vp3d_plan* p, void* state) {
@@ -545,7 +655,7 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
                          reinterpret_cast<long long*>(frame), s));
     launches += p->last_launches;
   }
-  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K).active, 0, h->S, s));
+  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K, h->flags).active, 0, h->S, s));
   p->last_launches = launches;
   return VP3D_OK;
 }

@@ -16,6 +16,17 @@ sequence padded as run.py's UnchunkedGenerator pads it (run.py:186-193, common/g
 for a causal model and 0 otherwise.  Output frame t comes back in the push that delivers input frame
 t + lookahead (lookahead = pad - shift, 0 for a causal model); ``frame`` numbers every returned row
 within its slot's sequence and is -1 for rows that are no frame yet.
+
+Test-time flip augmentation, run.py's default (common/arguments.py:43):
+
+    sess = model.streaming(streams=S, max_frames=K, augment=True,
+                           kps_left=kl, kps_right=kr, joints_left=jl, joints_right=jr)
+
+runs every slot twice in the same launches, plain and mirrored as UnchunkedGenerator(augment=True)
+mirrors it (common/generators.py:223-237), and returns the flip average of run.py:674-680: per slot
+bit-identical to ``metrics.flip_average(model(b), jl, jr)[0]`` with ``b`` the generator's (2, T +
+2 pad, J, F) batch.  The trajectory model (num_joints_out = 1) takes no joints lists (negate x only,
+run.py:678).
 """
 import weakref
 
@@ -23,6 +34,7 @@ import numpy as np
 import torch
 
 from . import _capi
+from .generators import mirror_source
 
 
 def lookahead(model):
@@ -44,15 +56,52 @@ def ring_history(filter_widths, dense=False):
     return hist
 
 
-def ring_bytes_per_stream(model, max_frames, planes=1):
-    """Device bytes of history one stream slot occupies (both mirror halves, every plane)."""
+def ring_bytes_per_stream(model, max_frames, planes=1, augment=False):
+    """Device bytes of history one stream slot occupies (both mirror halves, every plane; twice that
+    with augment: the slot's mirrored copy has rings of its own)."""
     fw = model.filter_widths
     c_in = -(-model.num_joints_in * model.in_features // 64) * 64
     c = -(-model._channels // 64) * 64
     total = 0
     for i, h in enumerate(ring_history(fw)):
         total += 2 * (h + max_frames + 1) * (c_in if i == 0 else c) * 2 * planes
-    return total
+    return 2 * total if augment else total
+
+
+def _check_pair(left, right, n, what):
+    if (left is None) != (right is None):
+        raise ValueError(f"{what}_left and {what}_right go together: give both or neither")
+    if left is None:
+        return
+    for j in list(left) + list(right):
+        if not 0 <= int(j) < n:
+            raise ValueError(f"{what} index {j} is out of range for {n} joints")
+
+
+def augment_maps(model, augment, kps_left=None, kps_right=None, joints_left=None,
+                 joints_right=None):
+    """The (kps_src, joints_src) int32 mirror maps of a session (generators.mirror_source), or
+    (None, None) without augmentation; joints_src is None for the trajectory model.  Raises
+    ValueError for lists that are missing, unpaired, out of range, or given with augment=False."""
+    lists = (kps_left, kps_right, joints_left, joints_right)
+    if not augment:
+        if any(v is not None for v in lists):
+            raise ValueError("kps_left / kps_right / joints_left / joints_right are only used with "
+                             "augment=True")
+        return None, None
+    j_in, j_out = model.num_joints_in, model.num_joints_out
+    _check_pair(kps_left, kps_right, j_in, "kps")
+    _check_pair(joints_left, joints_right, j_out, "joints")
+    if kps_left is None:
+        raise ValueError("augment=True needs kps_left/kps_right (and joints_left/joints_right "
+                         "unless num_joints_out == 1)")
+    if joints_left is None and j_out > 1:
+        raise ValueError("augment=True needs joints_left/joints_right for a model with "
+                         f"num_joints_out = {j_out}: only the trajectory model (num_joints_out == 1) "
+                         "skips the joint swap (run.py:678)")
+    kps = mirror_source(j_in, kps_left, kps_right)
+    joints = None if joints_left is None else mirror_source(j_out, joints_left, joints_right)
+    return kps, joints
 
 
 class FrameBook:
@@ -107,9 +156,11 @@ def check_push_input(x, streams, max_frames, joints, features):
 
 class StreamingSession:
     """S stream slots running a TemporalModel frame by frame (see the module docstring).  Create it
-    with ``model.streaming(streams, max_frames)``."""
+    with ``model.streaming(streams, max_frames)``; ``augment=True`` with the left / right lists of
+    UnchunkedGenerator returns the test-time flip average instead."""
 
-    def __init__(self, model, streams, max_frames):
+    def __init__(self, model, streams, max_frames, augment=False, kps_left=None, kps_right=None,
+                 joints_left=None, joints_right=None):
         from .temporal_model import TemporalModel
         if type(model)._variant != TemporalModel._variant:
             raise NotImplementedError(
@@ -124,6 +175,11 @@ class StreamingSession:
         streams, max_frames = int(streams), int(max_frames)
         if streams < 1 or max_frames < 1:
             raise ValueError("streams and max_frames must be >= 1")
+        # host-side int32 maps; vp3d_stream_init_ex copies them into the session state
+        self._kps_src, self._joints_src = augment_maps(model, augment, kps_left, kps_right,
+                                                       joints_left, joints_right)
+        self.augment = bool(augment)
+        self._flags = _capi.VP3D_STREAM_AUGMENT if self.augment else 0
         device = model.expand_conv.weight.device
         if device.type != "cuda":
             raise RuntimeError("streaming needs the model on a CUDA device; there is no CPU fallback")
@@ -136,7 +192,7 @@ class StreamingSession:
         lib = _capi.load()
         with torch.cuda.device(device):
             self._plan = self._model_plan()
-            nbytes = lib.vp3d_stream_state_bytes(self._plan, streams, max_frames)
+            nbytes = lib.vp3d_stream_state_bytes_ex(self._plan, streams, max_frames, self._flags)
             if nbytes == 0:
                 raise ValueError(f"{streams} streams x {max_frames} frames is too large a session")
             self._state = torch.empty(nbytes, dtype=torch.uint8, device=device)
@@ -156,11 +212,13 @@ class StreamingSession:
 
     def reset(self):
         """Drop all history: every slot idle, weights re-read at the next push."""
+        host_ptr = lambda a: None if a is None else a.ctypes.data  # noqa: E731
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            _capi.check(_capi.load().vp3d_stream_init(self._plan, self._state.data_ptr(),
-                                                      self._state.numel(), self.streams,
-                                                      self.max_frames, stream), "vp3d_stream_init")
+            _capi.check(_capi.load().vp3d_stream_init_ex(
+                self._plan, self._state.data_ptr(), self._state.numel(), self.streams,
+                self.max_frames, self._flags, host_ptr(self._kps_src), host_ptr(self._joints_src),
+                stream), "vp3d_stream_init_ex")
         self._versions = None
         return self
 
