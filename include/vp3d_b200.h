@@ -417,9 +417,28 @@ int vp3d_pose_errors(const float* pred, int32_t copies, const int32_t* mirror_sr
  * that frame, the other slots continue undisturbed); y receives (S, k, J_out, 3) fp32 and frame
  * (S, k) int64 the frame number within each slot's current sequence of every y row, -1 for rows
  * that are no frame (look-ahead warm-up, idle slot).  Asynchronous, no host synchronisation.
+ * vp3d_stream_push_ex: vp3d_stream_push with three optional DEVICE arrays (vp3d_stream_push is
+ * push_ex with all three NULL: the same bits and launches as before them):
+ *   end (S int32, or NULL): end[s] = n in [0, k] ends slot s's sequence after frame n - 1 of this
+ *     push (length = frames pushed before + n); -1 = it continues.  From then on the slot is fed the
+ *     generator's end padding, its last real frame repeated (common/generators.py:216-238,
+ *     run.py:186-193: pad - causal_shift copies behind), x[s, f >= n] is never read, and frame
+ *     length - 1 comes out `lookahead` frames later (in the same push for a causal model); the push
+ *     that returns it leaves the slot idle.  Rows past the end get frame -1.  end is ignored for an
+ *     idle slot and for a sequence that has already ended; start_mask on a slot that is still
+ *     draining begins the new sequence and drops the undelivered tail; start with end = 0 leaves the
+ *     slot idle.  Values outside [-1, k] are read as -1 (a device array is not checked on the host).
+ *     No extra launch.
+ *   x_rows (S int64, or NULL): x is a flat (rows, J_in, F) fp32 store; frame f of slot s is row
+ *     x_rows[s] + f, read only for f < n of an active slot whose sequence has not ended.
+ *   y_rows (S int64, or NULL): y is a flat (rows, J_out, 3) fp32 buffer; the returned frame t of
+ *     slot s (frame >= 0) is written to row y_rows[s] + t, rows of frame -1 are not written.  frame
+ *     (S, k) is still written and is required.  The output kernel then always runs (one launch
+ *     more where a push would shrink straight into y).
  * vp3d_stream_finish: emits the last `lookahead` frames of every slot by repeating each slot's
  * newest frame (the generator's end padding) into y (S, lookahead, J_out, 3) / frame (S,
- * lookahead), then marks every slot idle.
+ * lookahead), then marks every slot idle.  A slot whose sequence ended in an earlier push returns
+ * what is left of its tail, and -1 after that.
  * vp3d_stream_release: forgets `state` (the caller frees the memory).
  *
  * Test-time flip augmentation (VP3D_STREAM_AUGMENT, the default of run.py, common/arguments.py:43):
@@ -444,6 +463,9 @@ int vp3d_stream_init_ex(vp3d_plan* plan, void* state, size_t state_bytes, int S,
                         const int32_t* kps_src, const int32_t* joints_src, void* stream);
 int vp3d_stream_push(vp3d_plan* plan, void* state, const float* x, int k, const uint8_t* start_mask,
                      float* y, int64_t* frame, void* stream);
+int vp3d_stream_push_ex(vp3d_plan* plan, void* state, const float* x, int k,
+                        const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
+                        const int64_t* y_rows, float* y, int64_t* frame, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 int vp3d_stream_release(vp3d_plan* plan, void* state);
 

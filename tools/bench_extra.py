@@ -11,6 +11,9 @@
   * `--what stream_tta`: the same with test-time flip augmentation -- an augmented session against a
     plain session of twice the slots and against model(windows) + metrics.flip_average (see
     bench_stream_tta);
+  * `--what stream_seq`: the 240 sequences of the metrics workload through a session's predict()
+    (sequences ending on their own slot, longest first) against what metrics.evaluate runs, one
+    padded TTA batch per sequence (see bench_stream_seq);
   * `--what metrics`: the final evaluation of run.py (run.py:652-721) on a Human3.6M-test-sized
     workload, the fused metrics kernel (videopose3d_b200.metrics) against the path run.py runs
     (torch mpjpe / n_mpjpe with .item(), .cpu(), NumPy p_mpjpe / mean_velocity_error of the staged
@@ -20,7 +23,7 @@ The cuDNN baseline is built here from plain torch.nn modules following common/mo
 151-197 (it is a measurement target, not the product and not the oracle).  CUDA-event timing,
 10 warm-up + N timed iterations, cudnn.benchmark on, GPU-resident synthetic inputs.
 
-    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics,stream,stream_tta] > extra.jsonl
+    python tools/bench_extra.py [--iters 30] [--what eval,train,seq,metrics,stream,stream_tta,stream_seq] > extra.jsonl
 """
 import argparse
 import json
@@ -370,6 +373,90 @@ def bench_stream_tta(dev, pushes):
         torch.cuda.empty_cache()
 
 
+def offline_flops(fw, C, c_in, c_out, t_in):
+    """Executed FLOPs of the offline dilated forward on one padded sequence of t_in frames."""
+    rows = t_in - (fw[0] - 1)
+    fl = rows * 2 * c_in * fw[0] * C
+    d = fw[0]
+    for w in fw[1:]:
+        rows -= (w - 1) * d
+        fl += rows * 2 * C * C * (w + 1)
+        d *= w
+    return fl + rows * 2 * C * c_out
+
+
+def bench_stream_seq(dev, reps):
+    """The metrics workload's 240 sequences (lengths RandomState(0).randint(1000, 4001), J = 17) at
+    arc 3^5, C = 1024, fp16, test-time augmentation, two ways:
+      (a) what metrics.evaluate runs: per sequence model(b) on the padded (2, T + 2 pad, J, F) batch
+          of the device UnchunkedGenerator, then metrics.flip_average;
+      (b) sess.predict(seqs) of an augmented session at a few (S, K), the session reused.
+    Wall time ending in a device synchronise (median of `reps`, after one warm-up), frames/s,
+    launches, FLOPs executed (from shapes: (b) counts every row a push computes, drain frames and
+    idle slots included, and the start v-passes), session state bytes, and whether all 240 outputs
+    of every arm are bit-identical to (a)'s."""
+    from videopose3d_b200 import metrics
+    from videopose3d_b200.generators import UnchunkedGenerator
+    from videopose3d_b200.streaming import predict_schedule
+    left, right = [4, 5, 6, 11, 12, 13], [1, 2, 3, 14, 15, 16]
+    lists = dict(kps_left=left, kps_right=right, joints_left=left, joints_right=right)
+    info = card()
+    lens = np.random.RandomState(0).randint(1000, 4001, 240)
+    frames = int(lens.sum())
+    torch.manual_seed(0)
+    m = vp.TemporalModel(J, F, J, filter_widths=ARC, channels=C).to(dev).eval().set_precision("fp16")
+    pad = (m.receptive_field() - 1) // 2
+    la = vp.streaming.lookahead(m)
+    rng = np.random.RandomState(1)
+    p2 = [rng.uniform(-1, 1, (n, J, F)).astype(np.float32) for n in lens]
+    seqs = [torch.from_numpy(x).to(dev) for x in p2]
+    gen = UnchunkedGenerator(None, None, p2, pad=pad, causal_shift=0, augment=True, kps_left=left,
+                             kps_right=right, device=dev)
+    batches = [b for _, _, b in gen.next_epoch()]
+    outs = {}
+
+    def per_sequence():
+        with torch.no_grad():
+            outs["a"] = [metrics.flip_average(m(b), left, right)[0] for b in batches]
+
+    per_sequence()
+    t_a = host_time(per_sequence, reps)
+    launches_a = 0
+    for b in batches:
+        with torch.no_grad():
+            m(b)
+        launches_a += m.last_launch_count() + 1   # + the flip average
+    fl_a = sum(2 * offline_flops(ARC, C, J * F, J * 3, int(n) + 2 * pad) for n in lens)
+    rows = [dict(arm="model_per_sequence_flip_average", seconds=t_a, frames_per_s=frames / t_a,
+                 launches=launches_a, tflop_executed=fl_a / 1e12, tflops=fl_a / t_a / 1e12)]
+    st_fl, _ = stream_flops_per_frame(ARC, C, J * F, J * 3)
+    v_fl = st_fl - 2 * C * J * 3        # a start's v-pass: every layer but the shrink, one row
+    for S, K in ((240, 16), (128, 32), (64, 64)):
+        sess = m.streaming(streams=S, max_frames=K, augment=True, **lists)
+        got = {}
+
+        def run():
+            with torch.no_grad():
+                got["b"] = sess.predict(seqs)
+
+        run()
+        t_b = host_time(run, reps)
+        pushes = predict_schedule(lens, S, K, la)
+        P = 2 * S
+        fl_b = sum(p["k"] * P * st_fl + (P * v_fl if p["start"].any() else 0) for p in pushes)
+        equal = all(torch.equal(a, b) for a, b in zip(outs["a"], got["b"]))
+        rows.append(dict(arm="predict", streams=S, max_frames=K, seconds=t_b,
+                         frames_per_s=frames / t_b, launches=sess.last_predict_launches,
+                         pushes=len(pushes), tflop_executed=fl_b / 1e12, tflops=fl_b / t_b / 1e12,
+                         state_bytes=sess._state.numel(), bit_equal_to_per_sequence=equal,
+                         speedup_over_per_sequence=t_a / t_b))
+        del sess, got
+        torch.cuda.empty_cache()
+    for r in rows:
+        emit(what="stream_seq", sequences=len(lens), frames=frames, arc=ARC, channels=C,
+             precision="fp16", tta=True, **info, **r)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -383,6 +470,8 @@ def main():
         bench_stream(dev, args.pushes)
     if "stream_tta" in what:
         bench_stream_tta(dev, args.pushes)
+    if "stream_seq" in what:
+        bench_stream_seq(dev, args.reps)
     if "metrics" in what:
         bench_metrics(dev, args.reps)
     torch.backends.cudnn.benchmark = True

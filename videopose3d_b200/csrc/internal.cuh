@@ -72,6 +72,7 @@ struct StreamHost {
   long long q = 0;        // frames pushed since vp3d_stream_init (all slots advance together)
   long long prev_q = 0;   // q before the last push
   int prev_k = 0;         // frames of the last push (their ring rows still need their mirror copy)
+  int parity = 0;         // bookkeeping buffer the next push reads (the pushes alternate the two)
 };
 
 // step_ops.cu: Adam / AMSGrad update of conv weights that also refreshes their bf16 packs

@@ -31,6 +31,13 @@
 // 674-680).  The offline forward never mixes samples, so each physical row is the offline forward
 // of its own padded sequence; the mirrored row's start history is v_l(mirror(x0)), the edge padding
 // of the mirrored sequence.
+//
+// End of a sequence (vp3d_stream_push_ex's `end`).  A slot whose sequence ended is fed the
+// generator's end padding, its last real frame repeated (common/generators.py:216-238), until frame
+// length - 1 has come out lookahead frames later; then it is idle.  The per-slot bookkeeping (count,
+// active, length) is double-buffered by push parity: the input kernel reads buffer `parity` and
+// writes buffer `parity ^ 1`, so the pack, which depends on the bookkeeping of its slot, reads only
+// values no block of the same launch writes, whatever order the blocks run in.
 #include <cuda_fp16.h>
 
 #include "internal.cuh"
@@ -55,7 +62,8 @@ struct StreamLayout {
   int H[kMaxRings], R[kMaxRings], ld[kMaxRings];
   long long plane[kMaxRings];   // elements per ring plane
   size_t ring[kMaxRings];       // byte offsets
-  size_t count = 0, active = 0, h = 0, xlast = 0, ybuf = 0, total = 0;
+  size_t count = 0, active = 0, length = 0;   // per-slot bookkeeping, [2][S] (push parity)
+  size_t h = 0, xlast = 0, ybuf = 0, total = 0;
   size_t v[kMaxRings];          // v_l(x0) of rings 1..nb: [plane][P][C]
   size_t kps = 0, jsrc = 0;     // AUGMENT: int32 mirror maps [J_in], [J_out]
 };
@@ -69,8 +77,9 @@ StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   const int planes = p->planes;
   const int P = physical_rows(S, flags);
   size_t off = 0;
-  L.count = off; off = align_up(off + (size_t)S * 8, 1024);
-  L.active = off; off = align_up(off + (size_t)S, 1024);
+  L.count = off; off = align_up(off + (size_t)2 * S * 8, 1024);
+  L.active = off; off = align_up(off + (size_t)2 * S, 1024);
+  L.length = off; off = align_up(off + (size_t)2 * S * 8, 1024);
   for (int l = 0; l < L.rings; ++l) {
     L.H[l] = 2 * p->pad[l];
     L.R[l] = L.H[l] + K + 1;
@@ -111,10 +120,18 @@ struct StepArgs {
   StreamRing ring[kMaxRings];
   int rings, planes, f16, S, P, k, c_raw, feat;
   const float* x;          // (S, k, c_raw) fp32, or null: repeat each slot's newest frame (finish)
+  const long long* x_rows; // (S,) or null: x is a flat (rows, c_raw) store, frame f of slot s at
+                           // row x_rows[s] + f
   const int* kps;          // AUGMENT: [J_in] mirror source of every input joint; null: no rows >= S
   const uint8_t* start;    // (S,) or null
-  long long* count;        // frames of the current sequence pushed so far, per slot
-  uint8_t* active;         // 1 while the slot holds a sequence
+  const int* end;          // (S,) or null: the sequence ends after frame end[s] - 1 of this push
+  // per slot, the buffer of this push's parity (read) and of the next one (written):
+  const long long* count_in;    // frames of the current sequence pushed so far
+  const uint8_t* active_in;     // 1 while the slot holds a sequence (also while it drains)
+  const long long* length_in;   // length of the ended sequence, -1 while it is open
+  long long* count_out;
+  uint8_t* active_out;
+  long long* length_out;
   long long* frame;        // (S, frame_ld) int64
   int frame_ld, frame_off, lookahead;
 };
@@ -129,28 +146,58 @@ __device__ __forceinline__ void mirror_channel(int c, const StepArgs& a, int* sr
   *neg = e == 0;
 }
 
+// end[s] of this push, values outside [-1, k] read as -1 (a device array cannot be checked on the host)
+__device__ __forceinline__ int slot_end(const StepArgs& a, int s) {
+  if (!a.end) return -1;
+  const int e = a.end[s];
+  return e < -1 || e > a.k ? -1 : e;
+}
+
+// Frames of this push that row r packs from x: k for an open sequence, end[s] for one that ends in
+// this push, 0 once it has ended or in finish mode (the newest packed frame is repeated instead).
+// An idle slot packs its dense x as it always has; row-addressed x is not read for it.  Only
+// pre-push values are read: the bookkeeping loop of the same launch writes the other buffer.
+__device__ __forceinline__ int packed_frames(const StepArgs& a, int s) {
+  if (!a.x) return 0;
+  const bool st = a.start && a.start[s];
+  if (!st && !a.active_in[s]) return a.x_rows ? 0 : a.k;
+  if (!st && a.length_in[s] >= 0) return 0;
+  const int e = slot_end(a, s);
+  return e >= 0 ? e : a.k;
+}
+
 // One launch at the head of every push:
-//   * frame bookkeeping: a starting slot resets its frame counter; output row f of slot s is frame
-//     count + f - lookahead of its sequence, or -1 (warm-up of the look-ahead, idle slot);
+//   * frame bookkeeping: a starting slot resets its frame counter; an `end` fixes the sequence's
+//     length; output row f of slot s is frame idx = count + f - lookahead of its sequence when
+//     0 <= idx < length, else -1 (warm-up of the look-ahead, idle slot, frames past the end); a slot
+//     whose frame length - 1 has come out becomes idle;
 //   * the input pack: fp32 (S, k, J*F) -> 16-bit ring-0 rows (both copies), zero-padded channels,
 //     rounded exactly as the offline input pack rounds (hi / lo split for bf16x3, saturating fp16);
 //     with AUGMENT every frame is packed twice, plain into row s and mirrored into row S + s; in
-//     finish mode each physical row's newest packed frame is repeated instead (the generator's end
-//     padding, generators.py:216-238);
+//     finish mode, and for the frames of a slot after its sequence's end, each physical row's last
+//     real frame is repeated instead (the generator's end padding, generators.py:216-238): packed
+//     from x[s, end - 1] in the push that ends it, the newest ring-0 position after that;
 //   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb.
 __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) {
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nthr = (long long)gridDim.x * blockDim.x;
   for (long long s = tid; s < a.S; s += nthr) {
-    long long c = a.count[s];
-    uint8_t act = a.active[s];
-    if (a.start && a.start[s]) { c = 0; act = 1; }
+    long long c = a.count_in[s], len = a.length_in[s];
+    uint8_t act = a.active_in[s];
+    if (a.start && a.start[s]) { c = 0; act = 1; len = -1; }
+    const int e = slot_end(a, (int)s);
+    if (act && len < 0 && e >= 0) len = c + e;
     for (int f = 0; f < a.k; ++f) {
       const long long idx = c + f - a.lookahead;
-      a.frame[s * a.frame_ld + a.frame_off + f] = (act && idx >= 0) ? idx : -1;
+      a.frame[s * a.frame_ld + a.frame_off + f] =
+          (act && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
     }
-    a.count[s] = c + a.k;
-    a.active[s] = act;
+    c += a.k;
+    // idle once frame length - 1 is out (at once for a sequence without frames: start with end 0)
+    if (act && len >= 0 && (c - a.lookahead >= len || len == 0)) act = 0;
+    a.count_out[s] = c;
+    a.active_out[s] = act;
+    a.length_out[s] = len;
   }
 
   const StreamRing& r0 = a.ring[0];
@@ -164,10 +211,13 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
     const int pos = r0.w0 + r0.H + f;
     const long long d0 = ((long long)pos * a.P + r) * r0.ld + 2 * cp;
     const long long d1 = ((long long)mirror_pos(pos, r0.R) * a.P + r) * r0.ld + 2 * cp;
-    if (a.x) {
-      const bool mirrored = r >= a.S;
-      const int s = mirrored ? r - a.S : r;
-      const float* src = a.x + ((long long)s * a.k + f) * a.c_raw;
+    const bool mirrored = r >= a.S;
+    const int s = mirrored ? r - a.S : r;
+    const int n = packed_frames(a, s);
+    if (n > 0) {
+      // frames past the end repeat x[s, n - 1], rounded as every pack is: the bits of a ring copy
+      const long long xrow = (a.x_rows ? __ldg(a.x_rows + s) : (long long)s * a.k) + min(f, n - 1);
+      const float* src = a.x + xrow * a.c_raw;
       const int c0 = 2 * cp;
       int i0 = c0, i1 = c0 + 1;   // source channels
       bool n0 = false, n1 = false;
@@ -260,13 +310,17 @@ __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a
   }
 }
 
-// Shrink output rows are time-major; y is (S, y_frames, c_out) at frame offset f_off.  Plain: rows
-// f * S + s are copied.  augment: rows f * 2S + s (plain) and f * 2S + S + s (mirrored) are
-// flip-averaged (run.py:674-680), output joint j of the mirrored row read from joint_src[j]
-// (null: no joint swap, the trajectory model).
+// Shrink output rows are time-major; y is (S, y_frames, c_out) at frame offset f_off, or with
+// y_rows a flat (rows, c_out) buffer that receives the returned frame t of slot s at row
+// y_rows[s] + t (rows whose frame is -1 are not written).  Plain: rows f * S + s are copied.
+// augment: rows f * 2S + s (plain) and f * 2S + S + s (mirrored) are flip-averaged (run.py:674-680),
+// output joint j of the mirrored row read from joint_src[j] (null: no joint swap, the trajectory
+// model).
 __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, float* y, int S, int k,
                                                             int c_out, int y_frames, int f_off,
-                                                            int augment, const int* joint_src) {
+                                                            int augment, const int* joint_src,
+                                                            const long long* frame,
+                                                            const long long* y_rows) {
   pdl_entry();
   const long long n = (long long)k * S * c_out;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
@@ -274,6 +328,12 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
     const int c = (int)(i % c_out);
     const long long r = i / c_out;
     const int s = (int)(r % S), f = (int)(r / S);
+    long long dst = ((long long)s * y_frames + f_off + f) * c_out + c;
+    if (y_rows) {
+      const long long t = frame[(long long)s * y_frames + f_off + f];
+      if (t < 0) continue;
+      dst = (__ldg(y_rows + s) + t) * c_out + c;
+    }
     float v;
     if (augment) {
       const int j = c / 3, e = c - 3 * j;
@@ -283,7 +343,7 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
     } else {
       v = ybuf[i];
     }
-    y[((long long)s * y_frames + f_off + f) * c_out + c] = v;
+    y[dst] = v;
   }
 }
 
@@ -303,10 +363,12 @@ int stream_lookahead(const vp3d_plan* p) {
 }
 
 // One push of k frames (x null: k copies of every slot's newest frame).  y receives rows
-// [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, frame the matching (S, y_frames) entries.
-// The GEMMs run over P physical rows per frame (S, or 2S with AUGMENT).
+// [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, or with y_rows the rows y_rows[s] + frame
+// of a flat one; frame the matching (S, y_frames) entries.  The GEMMs run over P physical rows per
+// frame (S, or 2S with AUGMENT).
 static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
-                       const uint8_t* start, float* y, int y_frames, int f_off, long long* frame,
+                       const uint8_t* start, const int* end, const long long* x_rows,
+                       const long long* y_rows, float* y, int y_frames, int f_off, long long* frame,
                        cudaStream_t stream) {
   const int S = h.S, K = h.K, C = p->C, planes = p->planes;
   const bool aug = h.flags & VP3D_STREAM_AUGMENT;
@@ -338,10 +400,21 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.c_raw = p->c_in_raw;
   a.feat = p->cfg.in_features;
   a.x = x;
+  a.x_rows = x_rows;
   a.kps = aug ? reinterpret_cast<const int*>(base + L.kps) : nullptr;
   a.start = start;
-  a.count = reinterpret_cast<long long*>(base + L.count);
-  a.active = base + L.active;
+  a.end = end;
+  {
+    const int in = h.parity, out = h.parity ^ 1;
+    long long* count = reinterpret_cast<long long*>(base + L.count);
+    long long* length = reinterpret_cast<long long*>(base + L.length);
+    a.count_in = count + (size_t)in * S;
+    a.count_out = count + (size_t)out * S;
+    a.active_in = base + L.active + (size_t)in * S;
+    a.active_out = base + L.active + (size_t)out * S;
+    a.length_in = length + (size_t)in * S;
+    a.length_out = length + (size_t)out * S;
+  }
   a.frame = frame;
   a.frame_ld = y_frames;
   a.frame_off = f_off;
@@ -482,8 +555,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     launches += 2;
   }
   // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
-  // AUGMENT: the flip average always takes the output kernel)
-  const bool direct = !aug && (y_frames == 1 || S == 1);
+  // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs)
+  const bool direct = !aug && !y_rows && (y_frames == 1 || S == 1);
   float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
   common(d);
   d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
@@ -497,9 +570,11 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
                         dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
                         f_off, (int)aug,
-                        h.joint_src ? (const int*)(base + L.jsrc) : (const int*)nullptr));
+                        h.joint_src ? (const int*)(base + L.jsrc) : (const int*)nullptr,
+                        (const long long*)frame, y_rows));
     ++launches;
   }
+  h.parity ^= 1;
   h.prev_q = h.q;
   h.prev_k = k;
   h.q += k;
@@ -583,6 +658,8 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
   uint8_t* base = aligned_state(state);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(base, 0, need - 1024, s));
+  // every sequence open (length -1) in both bookkeeping buffers
+  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, S, K, flags).length, 0xff, (size_t)2 * S * 8, s));
   if (aug) {
     // the maps live in the state from here on: pushes read them on the device
     const StreamLayout L = stream_layout(p, S, K, flags);
@@ -619,21 +696,41 @@ static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost
   return VP3D_OK;
 }
 
+static int stream_push(const char* what, vp3d_plan* p, void* state, const float* x, int k,
+                       const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
+                       const int64_t* y_rows, float* y, int64_t* frame, void* stream) {
+  if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
+  if (k < 1) return fail(VP3D_ERR_INVALID, "%s: k must be >= 1 (got %d)", what, k);
+  if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
+  if (y_rows && !frame)
+    return fail(VP3D_ERR_INVALID, "%s: y_rows needs frame (the row of every output is its frame)",
+                what);
+  if (!x || !y || !frame) return fail(VP3D_ERR_INVALID, "%s: null x, y or frame", what);
+  StreamHost* h = nullptr;
+  VP3D_TRY(stream_lookup(p, state, what, &h));
+  if (k > h->K)
+    return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
+  if (!p->conv_packed || !p->bn_packed)
+    return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
+  return stream_step(p, aligned_state(state), *h, x, k, start_mask, end,
+                     reinterpret_cast<const long long*>(x_rows),
+                     reinterpret_cast<const long long*>(y_rows), y, k, 0,
+                     reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
+}
+
+VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, int k,
+                                    const uint8_t* start_mask, const int32_t* end,
+                                    const int64_t* x_rows, const int64_t* y_rows, float* y,
+                                    int64_t* frame, void* stream) {
+  return stream_push("stream_push_ex", p, state, x, k, start_mask, end, x_rows, y_rows, y, frame,
+                     stream);
+}
+
 VP3D_EXPORT int vp3d_stream_push(vp3d_plan* p, void* state, const float* x, int k,
                                  const uint8_t* start_mask, float* y, int64_t* frame,
                                  void* stream) {
-  if (!state) return fail(VP3D_ERR_INVALID, "stream_push: null state");
-  if (k < 1) return fail(VP3D_ERR_INVALID, "stream_push: k must be >= 1 (got %d)", k);
-  if (!p) return fail(VP3D_ERR_INVALID, "stream_push: null plan");
-  if (!x || !y || !frame) return fail(VP3D_ERR_INVALID, "stream_push: null x, y or frame");
-  StreamHost* h = nullptr;
-  VP3D_TRY(stream_lookup(p, state, "stream_push", &h));
-  if (k > h->K)
-    return fail(VP3D_ERR_INVALID, "stream_push: k = %d frames exceeds max_frames = %d", k, h->K);
-  if (!p->conv_packed || !p->bn_packed)
-    return fail(VP3D_ERR_STATE, "stream_push: vp3d_set_weights has not been called");
-  return stream_step(p, aligned_state(state), *h, x, k, start_mask, y, k, 0,
-                     reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
+  return stream_push("stream_push", p, state, x, k, start_mask, nullptr, nullptr, nullptr, y, frame,
+                     stream);
 }
 
 VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t* frame,
@@ -651,11 +748,13 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
   int launches = 0;
   for (int off = 0; off < la; off += h->K) {
     const int k = la - off < h->K ? la - off : h->K;
-    VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, y, la, off,
+    VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, nullptr, nullptr, nullptr, y, la, off,
                          reinterpret_cast<long long*>(frame), s));
     launches += p->last_launches;
   }
-  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K, h->flags).active, 0, h->S, s));
+  // every slot idle in the buffer the next push reads
+  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K, h->flags).active +
+                               (size_t)h->parity * h->S, 0, h->S, s));
   p->last_launches = launches;
   return VP3D_OK;
 }

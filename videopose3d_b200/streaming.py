@@ -6,9 +6,10 @@ output frame.  A session keeps every conv layer's past activations in device rin
 the new frames' share (``include/vp3d_b200.h``, vp3d_stream_*):
 
     sess = model.streaming(streams=S, max_frames=K)   # TemporalModel in eval()
-    y, frame = sess.push(x, start=None)   # x: (S, k, J_in, F) CUDA fp32, 1 <= k <= K
+    y, frame = sess.push(x, start=None, end=None)   # x: (S, k, J_in, F) CUDA fp32, 1 <= k <= K
     y, frame = sess.finish()              # the look-ahead tail of every slot; slots become idle
     sess.reset()                          # drop all history
+    ys = sess.predict([x0, x1, ...])      # whole (T_i, J_in, F) sequences, scheduled over the slots
 
 Per slot, the outputs of frames 0..T-1 of a sequence are exactly ``model(xp)`` with ``xp`` the
 sequence padded as run.py's UnchunkedGenerator pads it (run.py:186-193, common/generators.py:
@@ -16,6 +17,12 @@ sequence padded as run.py's UnchunkedGenerator pads it (run.py:186-193, common/g
 for a causal model and 0 otherwise.  Output frame t comes back in the push that delivers input frame
 t + lookahead (lookahead = pad - shift, 0 for a causal model); ``frame`` numbers every returned row
 within its slot's sequence and is -1 for rows that are no frame yet.
+
+``end[s] = n`` (0 <= n <= k) ends slot s's sequence after frame n - 1 of the push: from then on the
+slot is fed its last frame repeated (the generator's end padding), its last `lookahead` frames come
+out over the following pushes while the other slots go on, and the slot is idle once the last one is
+out.  ``predict`` uses this to run a list of sequences of any lengths through the slots, longest
+first, each slot taking the next sequence once the previous one has drained.
 
 Test-time flip augmentation, run.py's default (common/arguments.py:43):
 
@@ -106,21 +113,34 @@ def augment_maps(model, augment, kps_left=None, kps_right=None, joints_left=None
 
 class FrameBook:
     """Host model of the frame bookkeeping the session's input kernel does on the device (used by
-    the tests): per slot a frame counter and an active flag."""
+    the tests and by predict's scheduler): per slot a frame counter, an active flag and the length of
+    an ended sequence (-1 while it is open)."""
 
     def __init__(self, streams, lookahead):
         self.count = np.zeros(streams, np.int64)
         self.active = np.zeros(streams, bool)
+        self.length = np.full(streams, -1, np.int64)
         self.lookahead = lookahead
 
-    def push(self, k, start=None):
+    def push(self, k, start=None, end=None):
         if start is not None:
             start = np.asarray(start, bool)
             self.count[start] = 0
             self.active[start] = True
+            self.length[start] = -1
+        if end is not None:
+            end = np.asarray(end, np.int64)
+            end = np.where((end < -1) | (end > k), -1, end)   # as the device reads it
+            ends = self.active & (self.length < 0) & (end >= 0)
+            self.length[ends] = self.count[ends] + end[ends]
         idx = self.count[:, None] + np.arange(k)[None, :] - self.lookahead
-        frame = np.where(self.active[:, None] & (idx >= 0), idx, -1)
+        length = self.length[:, None]
+        frame = np.where(self.active[:, None] & (idx >= 0) & ((length < 0) | (idx < length)), idx, -1)
         self.count += k
+        # idle once frame length - 1 is out (at once for a sequence without frames)
+        done = self.active & (self.length >= 0) & ((self.count - self.lookahead >= self.length)
+                                                   | (self.length == 0))
+        self.active[done] = False
         return frame
 
     def finish(self):
@@ -128,6 +148,70 @@ class FrameBook:
             np.zeros((len(self.count), 0), np.int64)
         self.active[:] = False
         return frame
+
+
+def predict_schedule(lengths, streams, max_frames, lookahead):
+    """The pushes StreamingSession.predict makes for sequences of `lengths` frames: a list of dicts
+    with k and the per-slot arrays start (bool), end (int32), x_rows and y_rows (int64), rows
+    counted in the concatenation of the sequences (input and output alike).
+
+    Sequences go longest first (ties: input order) to the slots that are free; a slot is free in
+    the push after the one that returned its previous sequence's last frame.  Pushes carry
+    max_frames frames, fewer only once no sequence waits and the remaining drains are shorter."""
+    lengths = [int(n) for n in lengths]
+    if any(n < 1 for n in lengths):
+        raise ValueError("every sequence needs at least one frame")
+    S, K = int(streams), int(max_frames)
+    order = sorted(range(len(lengths)), key=lambda i: (-lengths[i], i))
+    offset = np.concatenate([[0], np.cumsum(lengths, dtype=np.int64)])
+    book = FrameBook(S, lookahead)
+    seq = np.full(S, -1, np.int64)     # sequence each slot holds
+    fed = np.zeros(S, np.int64)        # its frames pushed so far
+    pushes, q = [], 0
+    while True:
+        start = np.zeros(S, bool)
+        for s in range(S):
+            if not book.active[s] and q < len(order):
+                seq[s], fed[s], start[s] = order[q], 0, True
+                q += 1
+        busy = book.active | start
+        if not busy.any():
+            return pushes
+        if q < len(order):
+            k = K
+        else:
+            count = np.where(start, 0, book.count)
+            need = max(lengths[seq[s]] + lookahead - int(count[s]) for s in np.nonzero(busy)[0])
+            k = min(K, need)
+        end = np.full(S, -1, np.int32)
+        x_rows = np.zeros(S, np.int64)
+        y_rows = np.zeros(S, np.int64)
+        for s in np.nonzero(busy)[0]:
+            i = seq[s]
+            rest = lengths[i] - fed[s]
+            if rest > 0:
+                x_rows[s] = offset[i] + fed[s]
+                if rest <= k:
+                    end[s] = rest
+                fed[s] += min(rest, k)
+            y_rows[s] = offset[i]
+        book.push(k, start, end)
+        pushes.append(dict(k=k, start=start, end=end, x_rows=x_rows, y_rows=y_rows))
+
+
+def _check_sequence(x, joints, features, device):
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("predict expects a list of torch tensors")
+    if not x.is_cuda:
+        raise RuntimeError("videopose3d_b200 streaming runs on CUDA (sm_90a) tensors only; "
+                           "there is no CPU fallback")
+    if x.dtype != torch.float32:
+        raise TypeError(f"expected float32 sequences, got {x.dtype}")
+    if x.dim() != 3 or x.shape[1] != joints or x.shape[2] != features or x.shape[0] < 1:
+        raise ValueError(f"expected sequences of shape (T >= 1, {joints}, {features}), "
+                         f"got {tuple(x.shape)}")
+    if x.device != device:
+        raise RuntimeError("input and parameters are on different devices")
 
 
 def _param_versions(model):
@@ -189,6 +273,7 @@ class StreamingSession:
         self.precision = model.precision
         self.device = device
         self.lookahead = lookahead(model)
+        self.last_predict_launches = 0   # kernels the last predict() launched
         lib = _capi.load()
         with torch.cuda.device(device):
             self._plan = self._model_plan()
@@ -240,44 +325,135 @@ class StreamingSession:
         self._versions = _param_versions(m)
         return stream
 
-    def _start_mask(self, start):
+    def _slot_tensor(self, v, name):
+        if v.shape != (self.streams,):
+            raise ValueError(f"{name} must have shape ({self.streams},)")
+        if v.device != self.device:
+            raise RuntimeError(f"{name} must be on the session's device (or a list)")
+
+    def _start_list(self, start):
+        """None, a device tensor, or the validated host list of bools."""
         if start is None:
             return None
         if isinstance(start, torch.Tensor):
-            if start.shape != (self.streams,):
-                raise ValueError(f"start must have shape ({self.streams},)")
-            if start.device != self.device:
-                raise RuntimeError("start must be on the session's device (or a list)")
-            return start.to(torch.uint8).contiguous()
+            self._slot_tensor(start, "start")
+            return start
         start = [bool(v) for v in start]
         if len(start) != self.streams:
             raise ValueError(f"start must list {self.streams} slots")
+        return start
+
+    def _end_list(self, end, k, start):
+        """None, a device tensor, or the validated host list of ints in [-1, k]."""
+        if end is None:
+            return None
+        if isinstance(end, torch.Tensor):
+            self._slot_tensor(end, "end")
+            if end.dtype != torch.int32:
+                raise TypeError(f"end must be an int32 tensor, got {end.dtype}")
+            return end
+        end = [int(v) for v in end]
+        if len(end) != self.streams:
+            raise ValueError(f"end must list {self.streams} slots")
+        for s, e in enumerate(end):
+            if not -1 <= e <= k:
+                raise ValueError(f"end[{s}] = {e} is outside [-1, k = {k}]")
+            if e == 0 and isinstance(start, list) and start[s]:
+                raise ValueError(f"slot {s} starts and ends with end = 0: a sequence without frames")
+        return end
+
+    def _start_mask(self, start):
+        start = self._start_list(start)
+        if start is None:
+            return None
+        if isinstance(start, torch.Tensor):
+            return start.to(torch.uint8).contiguous()
         if not any(start):
             return None
         return torch.tensor(start, dtype=torch.uint8).to(self.device)
 
-    def push(self, x, start=None):
-        """Push k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64)."""
+    def push(self, x, start=None, end=None):
+        """Push k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64).
+
+        start: S bools (list or device tensor), slots that begin a new sequence with x[s, 0].
+        end: S ints in [-1, k] (list or CUDA int32 tensor), end[s] = n >= 0 ends slot s's sequence
+        after frame n - 1 of this push (x[s, n:] is not read), -1 = it continues.  Values of a
+        device tensor outside [-1, k] count as -1."""
         k = check_push_input(x, self.streams, self.max_frames, self.model.num_joints_in,
                              self.model.in_features)
         if x.device != self.device:
             raise RuntimeError("input and parameters are on different devices")
+        start = self._start_list(start)
+        end = self._end_list(end, k, start)   # host lists are checked before any device work
         x = x.contiguous()
         mask = self._start_mask(start)
+        if isinstance(end, list):
+            end = torch.tensor(end, dtype=torch.int32).to(self.device) if max(end) >= 0 else None
+        elif end is not None:
+            end = end.contiguous()
         y = torch.empty((self.streams, k, self.model.num_joints_out, 3), dtype=torch.float32,
                         device=self.device)
         frame = torch.empty((self.streams, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
             stream = self._prepare()
-            _capi.check(_capi.load().vp3d_stream_push(
+            _capi.check(_capi.load().vp3d_stream_push_ex(
                 self._plan, self._state.data_ptr(), x.data_ptr(), k,
-                None if mask is None else mask.data_ptr(), y.data_ptr(), frame.data_ptr(), stream),
-                "vp3d_stream_push")
+                None if mask is None else mask.data_ptr(), None if end is None else end.data_ptr(),
+                None, None, y.data_ptr(), frame.data_ptr(), stream), "vp3d_stream_push_ex")
         return y, frame
+
+    def predict(self, sequences):
+        """Run whole sequences through the slots: a list of CUDA fp32 (T_i, J_in, F) tensors, T_i >= 1,
+        in; the list of their (T_i, J_out, 3) outputs (views into one buffer) out, in input order,
+        each equal to the offline forward on the edge-padded sequence (the flip average with
+        augment=True).  The session is reset first and left idle.
+
+        The schedule (predict_schedule) follows from the lengths alone, so nothing is read back from
+        the device: one host-to-device copy of the whole schedule, then one push per step, each
+        reading its frames from and writing its outputs to rows of the two flat buffers."""
+        seqs = list(sequences)
+        J, F = self.model.num_joints_in, self.model.in_features
+        for x in seqs:
+            _check_sequence(x, J, F, self.device)
+        lengths = [int(x.shape[0]) for x in seqs]
+        pushes = predict_schedule(lengths, self.streams, self.max_frames, self.lookahead)
+        self.reset()
+        self.last_predict_launches = 0
+        if not seqs:
+            return []
+        S, n = self.streams, len(pushes)
+        # one row per push: x_rows | y_rows (int64) | end (int32) | start (uint8), 8-byte aligned
+        row = -(-(20 * S + S) // 8) * 8
+        host = np.zeros((n, row), np.uint8)
+        for i, p in enumerate(pushes):
+            host[i, :8 * S] = p["x_rows"].view(np.uint8)
+            host[i, 8 * S:16 * S] = p["y_rows"].view(np.uint8)
+            host[i, 16 * S:20 * S] = p["end"].view(np.uint8)
+            host[i, 20 * S:21 * S] = p["start"]
+        with torch.cuda.device(self.device):
+            sched = torch.from_numpy(host).pin_memory().to(self.device, non_blocking=True)
+            xs = torch.cat(seqs)
+            y = torch.empty((sum(lengths), self.model.num_joints_out, 3), dtype=torch.float32,
+                            device=self.device)
+            frame = torch.empty((S, self.max_frames), dtype=torch.int64, device=self.device)
+            lib = _capi.load()
+            base = sched.data_ptr()
+            for i, p in enumerate(pushes):
+                stream = self._prepare()
+                b = base + i * row
+                _capi.check(lib.vp3d_stream_push_ex(
+                    self._plan, self._state.data_ptr(), xs.data_ptr(), p["k"],
+                    b + 20 * S if p["start"].any() else None,
+                    b + 16 * S if (p["end"] >= 0).any() else None,
+                    b, b + 8 * S, y.data_ptr(), frame.data_ptr(), stream), "vp3d_stream_push_ex")
+                self.last_predict_launches += lib.vp3d_last_launch_count(self._plan)
+        offset = np.concatenate([[0], np.cumsum(lengths)])
+        return [y[int(offset[i]):int(offset[i + 1])] for i in range(len(seqs))]
 
     def finish(self):
         """Emit the last `lookahead` frames of every slot (its last frame repeated, as the
-        generator's end padding does), then mark every slot idle."""
+        generator's end padding does), then mark every slot idle.  A slot whose sequence ended
+        earlier returns what is left of its tail, -1 after that."""
         la = self.lookahead
         y = torch.empty((self.streams, la, self.model.num_joints_out, 3), dtype=torch.float32,
                         device=self.device)
