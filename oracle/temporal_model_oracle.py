@@ -152,10 +152,12 @@ def forward_numpy(sd, x, filter_widths, causal=False, dense=False, strided=False
 # torch.nn.functional restatement (what the reference runs on a CPU) — also the timed CPU baseline
 # ---------------------------------------------------------------------------------------------
 def forward_torch(sd, x, filter_widths, causal=False, dense=False, strided=False, training=False,
-                  momentum=0.1, update_stats=False, dropout=0.0):
+                  momentum=0.1, update_stats=False, dropout=0.0, masks=None):
     """sd: dict of torch tensors (state_dict layout); x: torch (N, T, J, F).  Same math through
     F.conv1d / F.batch_norm in x's dtype on x's device.  `dropout` > 0 applies torch's dropout
     after every ReLU in training mode (model.py:127, 134-135); the default is the identity.
+    `masks` ({layer: (N * frames, channels)}, layers numbered as in train_emulation.model_masks)
+    instead multiplies given dropout masks in at the same places.
     Differentiable: tensors in `sd` that require grad receive gradients."""
     import torch
     import torch.nn.functional as F
@@ -172,11 +174,13 @@ def forward_torch(sd, x, filter_widths, causal=False, dense=False, strided=False
         return F.batch_norm(t, rm, rv, sd[prefix + ".weight"], sd[prefix + ".bias"], training,
                             momentum, EPS)
 
-    def act(t):
+    def act(t, layer):
         t = F.relu(t)
+        if masks is not None:
+            return t * masks[layer].to(t).reshape(N, t.shape[2], t.shape[1]).permute(0, 2, 1)
         return F.dropout(t, dropout, True) if (training and dropout > 0.0) else t
 
-    h = act(bn(F.conv1d(h, sd["expand_conv.weight"], stride=fw[0] if strided else 1), "expand_bn"))
+    h = act(bn(F.conv1d(h, sd["expand_conv.weight"], stride=fw[0] if strided else 1), "expand_bn"), 0)
     for i in range(len(fw) - 1):
         w = fw[i + 1]
         if strided:
@@ -187,8 +191,8 @@ def forward_torch(sd, x, filter_widths, causal=False, dense=False, strided=False
             pad, sh = a["pad"][i + 1], a["shift"][i + 1]
             res = h[:, :, pad + sh: h.shape[2] - pad + sh]
             z = F.conv1d(h, sd[f"layers_conv.{2 * i}.weight"], dilation=a["dilation"][i + 1])
-        z = act(bn(z, f"layers_bn.{2 * i}"))
-        z = act(bn(F.conv1d(z, sd[f"layers_conv.{2 * i + 1}.weight"]), f"layers_bn.{2 * i + 1}"))
+        z = act(bn(z, f"layers_bn.{2 * i}"), 2 * i + 1)
+        z = act(bn(F.conv1d(z, sd[f"layers_conv.{2 * i + 1}.weight"]), f"layers_bn.{2 * i + 1}"), 2 * i + 2)
         h = res + z
     y = F.conv1d(h, sd["shrink.weight"], sd["shrink.bias"])
     return y.permute(0, 2, 1).reshape(N, -1, sd["shrink.weight"].shape[0] // 3, 3)

@@ -32,8 +32,13 @@ def pack_weight(w, n_pad, k_pad, planes):
 def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_pad, *,
               per_sample_tiles, tap_row_step, tap_col_step, out_rows, precision=0, scale=None,
               shift=None, relu=False, res=None, res_rows_per_sample=0, res_row_step=1, res_row_off=0,
-              res_sample_div=0, out_planes=1, out_f32_cols=None, stats=None):
-    """Launch vp3d_conv_gemm; returns (out_bf16_planes or None, out_f32 or None)."""
+              res_sample_div=0, res_col_begin=0, res_cols=0, res_check_rows=0, out_planes=1,
+              out_f32_cols=None, stats=None, bnb_z=None, bnb_scale=None, bnb_shift=None,
+              bnb_mean=None, bnb_invstd=None, bnb_sums=None, bnb_c=0, bnb_p=0.0, bnb_seed=0,
+              bnb_layer=0):
+    """Launch vp3d_conv_gemm; returns (out_bf16_planes or None, out_f32 or None).
+    bnb_*: the fused BatchNorm-backward reductions (see vp3d_conv_desc); bnb_z is a bf16 tensor
+    with the output's [rows][n_pad] view, the vectors fp32 [bnb_c], bnb_sums fp32 [slabs][2][n_pad]."""
     lib = _capi.load()
     dev = a_planes_t.device
     total_rows = samples * out_rows if per_sample_tiles else out_rows
@@ -52,6 +57,13 @@ def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_
         d.res_plane_stride = res[0].numel(); d.res_ld = res.shape[-1]
         d.res_rows_per_sample = res_rows_per_sample; d.res_row_step = res_row_step
         d.res_row_off = res_row_off; d.res_sample_div = res_sample_div
+        d.res_col_begin = res_col_begin; d.res_cols = res_cols; d.res_check_rows = res_check_rows
+    if bnb_z is not None:
+        d.bnb_z = bnb_z.data_ptr()
+        d.bnb_scale = bnb_scale.data_ptr(); d.bnb_shift = bnb_shift.data_ptr()
+        d.bnb_mean = bnb_mean.data_ptr(); d.bnb_invstd = bnb_invstd.data_ptr()
+        d.bnb_sums = bnb_sums.data_ptr(); d.bnb_c = bnb_c; d.bnb_p = bnb_p
+        d.bnb_seed = bnb_seed; d.bnb_layer = bnb_layer
     out = out32 = None
     if out_f32_cols is None:
         out = torch.full((out_planes, total_rows, n_pad), float("nan"),
@@ -79,13 +91,13 @@ def expected_conv(a_val, w_val, *, samples, a_rows, taps, k_per_tap, per_sample_
     if per_sample_tiles:
         acc = torch.zeros(samples, out_rows, n_pad, dtype=torch.float64, device=a_val.device)
         for tap in range(taps):
-            r0 = tap * tap_row_step
             c0 = tap * tap_col_step
-            rows = a3[:, r0:r0 + out_rows, c0:c0 + k_per_tap]
-            if rows.shape[1] < out_rows:  # TMA zero fill past the end of the sample
-                pad = torch.zeros(samples, out_rows - rows.shape[1], k_per_tap, dtype=torch.float64,
-                                  device=a_val.device)
-                rows = torch.cat([rows, pad], dim=1)
+            # output row t reads input row t + tap*tap_row_step (either sign); TMA zero-fills the
+            # rows outside the sample
+            src = torch.arange(out_rows, device=a_val.device) + tap * tap_row_step
+            ok = (src >= 0) & (src < a_rows)
+            rows = torch.zeros(samples, out_rows, k_per_tap, dtype=torch.float64, device=a_val.device)
+            rows[:, ok] = a3[:, src[ok], c0:c0 + k_per_tap]
             acc += rows @ w_val[tap].T
         return acc.reshape(samples * out_rows, n_pad)
     acc = torch.zeros(out_rows, n_pad, dtype=torch.float64, device=a_val.device)

@@ -4,8 +4,9 @@ running-stat update, backward for every parameter) against goldens produced by t
 
 Gates (SURVEY.md §8d G1): bf16x3 (fp32-faithful) mode: max|new - ref| / max|ref| <= 1e-3 on the
 output, every parameter gradient and the post-step running statistics.  bf16 mode: <= 5e-2.
-Dropout (p > 0) is statistically equal to torch's, not bitwise: checked through keep-rate /
-determinism properties and a directional finite-difference check of the gradients."""
+Dropout (p > 0) is statistically equal to torch's, not bitwise: checked here through keep-rate /
+determinism properties and a directional finite-difference check of the gradients, and in
+tests/test_gpu_train_dropout.py against references that replay the kernels' own masks."""
 import numpy as np
 import pytest
 import torch
@@ -109,20 +110,35 @@ def test_gradients_accumulate_and_eval_sees_new_stats(cuda_device):
 
 
 def test_dropout_statistics_and_determinism(cuda_device):
-    meta, sd, x, _, _ = load_golden("opt_333_c128_train")
+    _dropout_statistics_and_determinism(cuda_device, "bf16x3")
+
+
+def test_bf16_dropout_statistics_and_determinism(cuda_device):
+    """The default precision: BatchNorm-backward sums fused into the data-gradient GEMMs."""
+    _dropout_statistics_and_determinism(cuda_device, "bf16")
+
+
+def _dropout_statistics_and_determinism(cuda_device, precision):
+    meta, sd, x, _, new = load_golden("opt_333_c128_train")
     xg = x.to(cuda_device)
-    m = _build(meta, sd, cuda_device, "bf16x3", dropout=0.25)
-    torch.manual_seed(11)
-    y1 = m(xg).detach()
-    torch.manual_seed(11)
-    y2 = m(xg).detach()
-    torch.manual_seed(12)
-    y3 = m(xg).detach()
-    # same torch seed -> same dropout masks (BN batch sums use fp32 atomics: not bit-reproducible)
+    gy = torch.from_numpy(new["gy"]).to(cuda_device)
+    m = _build(meta, sd, cuda_device, precision, dropout=0.25)
+
+    def step(seed):
+        m.zero_grad(set_to_none=True)
+        torch.manual_seed(seed)
+        y = m(xg)
+        (y * gy).sum().backward()
+        return y.detach(), {k: prm.grad.clone() for k, prm in m.named_parameters()}
+    (y1, g1), (y2, g2), (y3, _) = step(11), step(11), step(12)
+    # same torch seed -> same dropout masks, and every reduction (batch statistics, BatchNorm-backward
+    # sums, weight-gradient partials) runs in a fixed order: bit-identical output and gradients
+    assert torch.equal(y1, y2)
+    for k in g1:
+        assert torch.equal(g1[k], g2[k]), k
     scale = float(y1.abs().max())
-    assert float((y1 - y2).abs().max()) <= 1e-4 * scale
     assert float((y1 - y3).abs().max()) >= 1e-2 * scale, "different seed -> different masks"
-    m0 = _build(meta, sd, cuda_device, "bf16x3", dropout=0.0)
+    m0 = _build(meta, sd, cuda_device, precision, dropout=0.0)
     y0 = m0(xg).detach()
     assert torch.isfinite(y1).all()
     # dropout perturbs but does not bias the activations grossly
@@ -376,13 +392,30 @@ def test_cfg3_shape_default_bf16_training_is_close_and_reproducible(cuda_device)
 
 
 def test_dropout_keep_rate_scale_and_mask_consistency(cuda_device):
+    _dropout_keep_rate_scale_and_mask(cuda_device, "bf16x3", "TemporalModel", 64)
+
+
+@pytest.mark.parametrize("precision,cls,C", [
+    (pr, cl, c) for pr in ("bf16x3", "bf16") for cl in ("TemporalModel", "TemporalModelOptimized1f")
+    for c in (64, 100) if (pr, cl, c) != ("bf16x3", "TemporalModel", 64)])
+def test_dropout_keep_rate_and_mask_across_precisions_models_and_padding(cuda_device, precision, cls, C):
+    """The same checks in the default bf16 precision (layer 0's BatchNorm-backward sums come from the
+    shrink GEMM's fused epilogue), for the strided model, and with C = 100 on 128 padded channels."""
+    _dropout_keep_rate_scale_and_mask(cuda_device, precision, cls, C)
+
+
+def _dropout_keep_rate_scale_and_mask(cuda_device, precision, cls, C):
     """SURVEY §8d gate G3 on the kernels' own output.  arc [3] (no residual block) with a shrink
     layer that copies the first 51 channels makes the dropout output observable:
     y[..., c] = drop(relu(bn(expand(x))))[..., c].  Against the same step with p = 0: every value is
-    either dropped (0) or scaled by exactly 1/(1-p) = 4/3; the kept fraction is 0.75 +- 3 sigma; and
-    the backward uses the same mask (d sum(y) / d beta_c = 4/3 x #kept positive rows)."""
-    C, J, N, T, p = 64, 17, 64, 50, 0.25
+    either dropped (0) or scaled by exactly 1/(1-p) = 4/3; the units dropped are exactly those the
+    mask of oracle/train_emulation.dropout_mask drops (C = 100 runs on 128 padded channels); the kept
+    fraction is 0.75 +- 3 sigma; and the backward uses the same mask (d sum(y) / d beta_c = 4/3 x
+    #kept positive rows -- in bf16 through the BatchNorm-backward sums fused into the shrink's
+    data-gradient GEMM)."""
+    J, N, T, p = 17, 64, 50, 0.25
     from oracle import temporal_model_oracle as orc
+    from oracle import train_emulation as emu
     sd = orc.make_state_dict(J, 2, J, [3], C, seed=77)
     sd["shrink.weight"] = torch.zeros(51, C, 1)
     sd["shrink.weight"][torch.arange(51), torch.arange(51), 0] = 1.0
@@ -390,9 +423,9 @@ def test_dropout_keep_rate_scale_and_mask_consistency(cuda_device):
     x = orc.make_input(N, T, J, 2, seed=78).to(cuda_device)
     outs = {}
     for prob in (0.0, p):
-        m = vp.TemporalModel(J, 2, J, filter_widths=[3], dropout=prob, channels=C)
+        m = getattr(vp, cls)(J, 2, J, filter_widths=[3], dropout=prob, channels=C)
         m.load_state_dict(sd)
-        m = m.to(cuda_device).train().set_train_precision("bf16x3")
+        m = m.to(cuda_device).train().set_train_precision(precision)
         torch.manual_seed(5)
         y = m(x)
         y.sum().backward()
@@ -401,8 +434,14 @@ def test_dropout_keep_rate_scale_and_mask_consistency(cuda_device):
     yp, dbeta = outs[p]
     pos = y0 > 1e-4                                   # rows where ReLU passed a value
     kept = pos & (yp != 0)
+    mask = emu.model_masks(emu.step_seed(5), [3], N, T, C, p, dilated=cls == "TemporalModel")[0]
+    assert mask.shape[0] == y0.shape[0]
+    assert torch.equal(pos & (yp == 0), pos & (mask[:, :51] == 0).to(cuda_device))
     ratio = yp[kept] / y0[kept]
-    assert float((ratio - 4.0 / 3.0).abs().max()) <= 1e-3      # scale 1/(1-p), nothing in between
+    # scale 1/(1-p), nothing in between (bf16 storage: both values rounded, each by up to half an
+    # ulp = 2^-8 relative)
+    tol = 1e-3 if precision == "bf16x3" else 4.0 / 3.0 * 2 ** -7
+    assert float((ratio - 4.0 / 3.0).abs().max()) <= tol
     assert float(yp[~pos].abs().max()) <= 2e-4                 # dropout never creates values
     n = int(pos.sum())
     rate = float(kept.sum()) / n
