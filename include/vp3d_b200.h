@@ -110,6 +110,9 @@ int vp3d_total_causal_shift(const vp3d_plan* plan);
 #define VP3D_PACK_CONV 1
 #define VP3D_PACK_BN_EVAL 2
 #define VP3D_PACK_CONV_T 4 /* transposed conv weights for the data-gradient GEMMs (training only) */
+/* transposed expand-conv weights for the input gradient of vp3d_backward_ex (training plans only;
+ * not refreshed by vp3d_adam_step_packed: re-pack after every change of expand_conv.weight) */
+#define VP3D_PACK_EXPAND_T 8
 int vp3d_set_weights(vp3d_plan* plan, const vp3d_weights* w, int what, void* stream);
 
 /* Output frames for an input of T frames: T - receptive_field + 1 for the dilated variant
@@ -167,6 +170,19 @@ int vp3d_forward_train(vp3d_plan* plan, const float* x, float* y, int N, int T, 
                        const float* bn_momentum, float dropout_p, unsigned long long seed,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* vp3d_forward_train with flags.  VP3D_TRAIN_FROZEN_BN: every BatchNorm is the fixed affine of its
+ * running statistics (the eval-mode fold of VP3D_PACK_BN_EVAL: scale = w / sqrt(running_var + 1e-5),
+ * shift = b - running_mean * scale), as model.eval() computes it; running statistics are neither
+ * read for an update nor written, bn_momentum may be NULL and dropout_p must be 0.  The matching
+ * vp3d_backward_ex then differentiates that forward: dZ = scale * dY without batch-statistics terms,
+ * d weight = sum dY * (z - running_mean) / sqrt(running_var + 1e-5), d bias = sum dY -- autograd
+ * through the reference's module in eval() mode.  flags == 0 is vp3d_forward_train. */
+#define VP3D_TRAIN_FROZEN_BN 1
+int vp3d_forward_train_ex(vp3d_plan* plan, const float* x, float* y, int N, int T,
+                          const vp3d_weights* w, const float* bn_momentum, float dropout_p,
+                          unsigned long long seed, int flags, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
 /* Replaces autograd's backward through the model (run.py:394, 418): dy is (N, T_out, J_out, 3) fp32;
  * writes every parameter gradient.  Uses the activations saved by the last vp3d_forward_train. */
 int vp3d_backward(vp3d_plan* plan, const float* dy, const vp3d_grads* grads, void* workspace,
@@ -181,6 +197,19 @@ int vp3d_backward(vp3d_plan* plan, const float* dy, const vp3d_grads* grads, voi
 typedef void (*vp3d_stage_fn)(int stage, void* user);
 int vp3d_backward_staged(vp3d_plan* plan, const float* dy, const vp3d_grads* grads, void* workspace,
                          size_t workspace_bytes, void* stream, vp3d_stage_fn stage_done, void* user);
+
+/* vp3d_backward_staged with optional outputs (stage_done may be NULL):
+ *   grads == NULL: no parameter gradients -- no weight-gradient GEMMs, no shrink-bias sum, and after
+ *     a VP3D_TRAIN_FROZEN_BN forward no BatchNorm-backward reductions: only the data-gradient chain
+ *     runs (test-time refinement of the input through a frozen model).
+ *   dx != NULL: the input gradient dL/dx, an fp32 DEVICE buffer shaped like the forward's x
+ *     (N, T, J_in, F); it is overwritten entirely, with zeros for frames no output depends on.
+ *     Needs the transposed expand pack (vp3d_set_weights with VP3D_PACK_EXPAND_T) of the current
+ *     expand_conv.weight.
+ * At least one of grads / dx must be given.  vp3d_backward_staged is _ex with dx = NULL. */
+int vp3d_backward_ex(vp3d_plan* plan, const float* dy, const vp3d_grads* grads, float* dx,
+                     void* workspace, size_t workspace_bytes, void* stream, vp3d_stage_fn stage_done,
+                     void* user);
 
 /* Number of kernels the last forward on this plan launched (for bench.py's gpu_launches). */
 int vp3d_last_launch_count(const vp3d_plan* plan);

@@ -20,6 +20,8 @@ VP3D_PRECISION_FP16 = 3
 VP3D_PACK_CONV = 1
 VP3D_PACK_BN_EVAL = 2
 VP3D_PACK_CONV_T = 4
+VP3D_PACK_EXPAND_T = 8
+VP3D_TRAIN_FROZEN_BN = 1
 VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
@@ -188,6 +190,14 @@ SIGNATURES = {
     "vp3d_backward_staged": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Grads),
                                             ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
                                             ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_forward_train_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_int, ctypes.c_int, ctypes.POINTER(Weights),
+                                             ctypes.POINTER(ctypes.c_float), ctypes.c_float,
+                                             ctypes.c_ulonglong, ctypes.c_int, ctypes.c_void_p,
+                                             ctypes.c_size_t, ctypes.c_void_p]),
+    "vp3d_backward_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Grads),
+                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_last_launch_count": (ctypes.c_int, [ctypes.c_void_p]),
     "vp3d_profile_launch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "vp3d_profile_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),

@@ -487,6 +487,9 @@ extern "C" __attribute__((visibility("default"))) int vp3d_set_weights(vp3d_plan
     return fail(VP3D_ERR_UNSUPPORTED, "fp16 plans are inference-only (train with bf16 / bf16x3)");
   if (what & VP3D_PACK_CONV_T)
     VP3D_TRY(train_pack_transposed(p, w, stream, (what & VP3D_PACK_CONV) != 0));
+  if ((what & VP3D_PACK_EXPAND_T) && p->f16)
+    return fail(VP3D_ERR_UNSUPPORTED, "fp16 plans are inference-only (train with bf16 / bf16x3)");
+  if (what & VP3D_PACK_EXPAND_T) VP3D_TRY(train_pack_expand_t(p, w, stream));
   return VP3D_OK;
 }
 

@@ -143,4 +143,5 @@ int strided_trim(const vp3d_plan* p, int* L);
 void train_state_destroy(TrainState* t);
 int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream,
                           bool also_forward);
+int train_pack_expand_t(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream);
 }  // namespace vp3d

@@ -198,7 +198,8 @@ cudaError_t launch_pack_conv_weight(const float* w, __nv_bfloat16* out, int plan
 __global__ void bn_fold_kernel(const float* __restrict__ gamma, const float* __restrict__ beta,
                                const float* __restrict__ mean, const float* __restrict__ var,
                                float eps, float* __restrict__ scale, float* __restrict__ shift,
-                               int c, int c_pad) {
+                               int c, int c_pad, float* __restrict__ mean_out,
+                               float* __restrict__ invstd_out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c_pad) return;
   float s = 0.0f, b = 0.0f;
@@ -208,13 +209,17 @@ __global__ void bn_fold_kernel(const float* __restrict__ gamma, const float* __r
   }
   scale[i] = s;
   shift[i] = b;
+  if (mean_out) {
+    mean_out[i] = i < c ? mean[i] : 0.0f;
+    invstd_out[i] = i < c ? 1.0f / sqrtf(var[i] + eps) : 0.0f;
+  }
 }
 
 cudaError_t launch_bn_fold(const float* gamma, const float* beta, const float* mean,
                            const float* var, float eps, float* scale, float* shift, int c,
-                           int c_pad, cudaStream_t stream) {
+                           int c_pad, cudaStream_t stream, float* mean_out, float* invstd_out) {
   bn_fold_kernel<<<(c_pad + 255) / 256, 256, 0, stream>>>(gamma, beta, mean, var, eps, scale, shift,
-                                                          c, c_pad);
+                                                          c, c_pad, mean_out, invstd_out);
   return cudaGetLastError();
 }
 

@@ -40,10 +40,13 @@ cudaError_t launch_pack_conv_weight(const float* w, __nv_bfloat16* out, int plan
                                     cudaStream_t stream, int f16 = 0);
 
 // Eval-mode BatchNorm1d (model.py:32,117,119; eps = 1e-5) as y = x*scale + shift.
-// gamma/beta/mean/var: [c]; scale/shift: [c_pad] (padding: scale 0, shift 0).
+// gamma/beta/mean/var: [c]; scale/shift: [c_pad] (padding: scale 0, shift 0).  mean_out /
+// invstd_out (both or neither, [c_pad]) also receive running_mean and 1/sqrt(var + eps), padding 0:
+// the frozen-BatchNorm training forward needs them for its backward.
 cudaError_t launch_bn_fold(const float* gamma, const float* beta, const float* mean,
                            const float* var, float eps, float* scale, float* shift, int c,
-                           int c_pad, cudaStream_t stream);
+                           int c_pad, cudaStream_t stream, float* mean_out = nullptr,
+                           float* invstd_out = nullptr);
 
 // shrink bias (model.py:33): scale = 1, shift = bias, padded with zeros.
 cudaError_t launch_bias_affine(const float* bias, float* scale, float* shift, int c, int c_pad,

@@ -10,7 +10,14 @@
 // Backward, per layer top-down: BN/ReLU/Dropout backward (bn_bwd_reduce + bn_bwd_apply -> dZ,
 // dgamma, dbeta), weight gradient dW = dZ^T * X (MN-major wgmma GEMM, split over rows),
 // data gradient G_prev = dZ * W^T through the same conv GEMM kernel on transposed weight packs,
-// with the skip-connection gradient added in the epilogue.
+// with the skip-connection gradient added in the epilogue.  On request (vp3d_backward_ex with dx)
+// the chain ends with the expand conv's data gradient dX = dZ0 * W0^T, written as fp32 in x's layout.
+//
+// Frozen BatchNorm (vp3d_forward_train_ex with VP3D_TRAIN_FROZEN_BN, the eval-mode backward):
+// every BatchNorm is the fixed affine of its running statistics (the eval fold, bn_fold), running
+// statistics are left alone and no batch-statistics slabs are written; the backward then applies
+// dZ = scale * dY without the batch-statistics terms, and dgamma / dbeta come from the same sums
+// with the running mean / invstd.
 //
 // Both layouts are covered: strided (TemporalModelOptimized1f, the model run.py trains with by
 // default, run.py:172-175) and dilated (TemporalModel, run.py:176-180: per-sample tiles, transposed
@@ -28,6 +35,10 @@ struct TrainState {
   __nv_bfloat16* conv_t[VP3D_MAX_LAYERS] = {};  // [planes][taps][C][C], out[tap][ci][co]
   __nv_bfloat16* shrink_t = nullptr;            // [planes][1][C][c_out_pad128]
   bool packed_t = false;
+  // transposed expand pack for the input gradient (VP3D_PACK_EXPAND_T): dilated [planes][w0][c_in_pad][C],
+  // strided tap-merged [planes][1][k0_pad][C] (row tap*c_in + ci)
+  __nv_bfloat16* expand_t = nullptr;
+  bool packed_expand_t = false;
   float* vec = nullptr;       // per BN layer l: scale, shift, mean, invstd, stats[2C], sums[2C]
   size_t vec_floats = 0;
   float* shrink_affine = nullptr;  // scale / shift of the shrink bias [2 * c_out_pad]
@@ -38,6 +49,7 @@ struct TrainState {
   int L[VP3D_MAX_WIDTHS] = {};
   float dropout_p = 0.0f;
   uint64_t seed = 0;
+  bool frozen_bn = false;
   bool have_forward = false;
   std::vector<void*> allocs;
 };
@@ -72,6 +84,11 @@ int ensure_train_state(vp3d_plan* p) {
   }
   VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->shrink_t),
                    (size_t)p->planes * p->C * c_out_pad128(p) * 2));
+  {
+    const size_t rows_dil = (size_t)p->cfg.filter_widths[0] * p->c_in_pad;
+    const size_t rows = rows_dil > (size_t)p->k0_pad ? rows_dil : (size_t)p->k0_pad;
+    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->expand_t), (size_t)p->planes * rows * p->C * 2));
+  }
   t->vec_floats = (size_t)(2 * p->nb + 1) * 8 * p->C;
   VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->vec), t->vec_floats * sizeof(float)));
   VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->shrink_affine), 2 * p->c_out_pad * sizeof(float)));
@@ -101,6 +118,8 @@ struct TrainLayout {
   size_t partial_bytes = 0;
   size_t slab = 0;         // per-slab statistics partials of the GEMM epilogues (fp32)
   size_t slab_floats = 0;
+  size_t dx_stage = 0;     // strided model with T % w0 != 0: fp32 [N * L0][w0 * c_in] input gradient
+                           // before the copy that opens each sample's tail (else unused)
   size_t total = 0;
   long long rows[VP3D_MAX_WIDTHS] = {};  // rows[i] = N * L[i]
 };
@@ -155,6 +174,8 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
     w.slab_floats = need + 1024;
     w.slab = take(w.slab_floats * sizeof(float));
   }
+  if (strided && T != p->cfg.filter_widths[0] * L[0])
+    w.dx_stage = take((size_t)w.rows[0] * p->cfg.filter_widths[0] * p->c_in_raw * sizeof(float));
   w.total = off + 1024;
   return w;
 }
@@ -254,6 +275,21 @@ int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stre
   return VP3D_OK;
 }
 
+int train_pack_expand_t(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream) {
+  if (!w->expand_conv_weight) return fail(VP3D_ERR_INVALID, "set_weights: missing expand_conv.weight");
+  VP3D_TRY(ensure_train_state(p));
+  TrainState* t = p->train;
+  const int w0 = p->cfg.filter_widths[0];
+  if (p->cfg.variant == VP3D_VARIANT_STRIDED)
+    CUDA_TRY(launch_pack_conv_weight_t(w->expand_conv_weight, t->expand_t, p->planes, p->c_real,
+                                       p->c_in_raw, w0, p->k0_pad, p->C, stream, nullptr, 0, 0, 1));
+  else
+    CUDA_TRY(launch_pack_conv_weight_t(w->expand_conv_weight, t->expand_t, p->planes, p->c_real,
+                                       p->c_in_raw, w0, p->c_in_pad, p->C, stream));
+  t->packed_expand_t = true;
+  return VP3D_OK;
+}
+
 }  // namespace vp3d
 
 using namespace vp3d;
@@ -268,11 +304,31 @@ VP3D_API size_t vp3d_train_workspace_bytes(const vp3d_plan* p, int N, int T) {
   return train_layout(p, N, T, L).total;
 }
 
+VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N, int T,
+                                   const vp3d_weights* w, const float* bn_momentum, float dropout_p,
+                                   unsigned long long seed, int flags, void* ws, size_t ws_bytes,
+                                   void* stream_);
+
 VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, int T,
                                 const vp3d_weights* w, const float* bn_momentum, float dropout_p,
                                 unsigned long long seed, void* ws, size_t ws_bytes, void* stream_) {
-  if (!p || !x || !y || !w || !bn_momentum)
+  if (!bn_momentum) return fail(VP3D_ERR_INVALID, "forward_train: null argument");
+  return vp3d_forward_train_ex(p, x, y, N, T, w, bn_momentum, dropout_p, seed, 0, ws, ws_bytes,
+                               stream_);
+}
+
+VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N, int T,
+                                   const vp3d_weights* w, const float* bn_momentum, float dropout_p,
+                                   unsigned long long seed, int flags, void* ws, size_t ws_bytes,
+                                   void* stream_) {
+  if (flags & ~VP3D_TRAIN_FROZEN_BN)
+    return fail(VP3D_ERR_INVALID, "forward_train: unknown flags 0x%x", flags);
+  const bool frozen = (flags & VP3D_TRAIN_FROZEN_BN) != 0;
+  if (!p || !x || !y || !w || (!bn_momentum && !frozen))
     return fail(VP3D_ERR_INVALID, "forward_train: null argument");
+  if (frozen && dropout_p != 0.0f)
+    return fail(VP3D_ERR_INVALID, "forward_train: VP3D_TRAIN_FROZEN_BN (the eval-mode forward) "
+                "runs without dropout; dropout p must be 0");
   const bool strided = p->cfg.variant == VP3D_VARIANT_STRIDED;
   if (N < 1) return fail(VP3D_ERR_INVALID, "forward_train: batch must be >= 1");
   if (dropout_p < 0.0f || dropout_p >= 1.0f)
@@ -301,7 +357,8 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
   uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
   auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
   const int C = p->C, pl = p->planes;
-  t->N = N; t->T = T; t->dropout_p = dropout_p; t->seed = seed; t->have_forward = false;
+  t->N = N; t->T = T; t->dropout_p = dropout_p; t->seed = seed; t->frozen_bn = frozen;
+  t->have_forward = false;
   for (int i = 0; i <= p->nb; ++i) t->L[i] = L[i];
   int launches = 0;
 
@@ -329,11 +386,16 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
     const int per_sample_rows = stats_per_sample_rows;
     const int tps = per_sample_rows ? (per_sample_rows + 127) / 128 : 0;
     const int slabs = per_sample_rows ? N * tps * 4 : (int)((rows + 127) / 128) * 4;
-    CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
-                                      per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
-                                      bnp[1], const_cast<float*>(bnp[2]), const_cast<float*>(bnp[3]),
-                                      bn_momentum[layer], 1e-5f, v.scale, v.shift, v.mean, v.invstd,
-                                      C, p->c_real, t->red_scratch, t->red_counter, stream));
+    if (frozen) {  // the eval fold of the running statistics, plus the mean / invstd backward reads
+      CUDA_TRY(launch_bn_fold(bnp[0], bnp[1], bnp[2], bnp[3], 1e-5f, v.scale, v.shift, p->c_real, C,
+                              stream, v.mean, v.invstd));
+    } else {
+      CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
+                                        per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
+                                        bnp[1], const_cast<float*>(bnp[2]), const_cast<float*>(bnp[3]),
+                                        bn_momentum[layer], 1e-5f, v.scale, v.shift, v.mean, v.invstd,
+                                        C, p->c_real, t->red_scratch, t->red_counter, stream));
+    }
     CUDA_TRY(launch_bn_apply(z, rows * C, out, rows * C, pl, rows, C, v.scale, v.shift,
                              drop_cfg(t, layer), res, res_plane, map, stream));
     launches += 2;
@@ -358,7 +420,7 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
   }
   ++launches;
   d.out = bf(wl.z[0]); d.out_plane_stride = wl.rows[0] * C; d.out_ld = C;
-  d.stats = slab_part;
+  d.stats = frozen ? nullptr : slab_part;
   stats_per_sample_rows = d.per_sample_tiles ? d.out_rows : 0;
   VP3D_TRY(run_conv(&d, stream));
   ++launches;
@@ -378,7 +440,7 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
       d.per_sample_tiles = 1; d.tap_row_step = p->dilation[i]; d.out_rows = L[i];
     }
     d.out = bf(wl.z[l1]); d.out_plane_stride = rows * C; d.out_ld = C;
-    d.stats = slab_part;
+    d.stats = frozen ? nullptr : slab_part;
     stats_per_sample_rows = d.per_sample_tiles ? d.out_rows : 0;
     VP3D_TRY(run_conv(&d, stream));
     ++launches;
@@ -389,7 +451,7 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
     d.w = p->conv[2 * (i - 1) + 1].w; d.taps = 1; d.k_per_tap = C; d.n_pad = C;
     d.out_rows = (int)rows;
     d.out = bf(wl.z[l2]); d.out_plane_stride = rows * C; d.out_ld = C;
-    d.stats = slab_part;
+    d.stats = frozen ? nullptr : slab_part;
     stats_per_sample_rows = 0;
     VP3D_TRY(run_conv(&d, stream));
     ++launches;
@@ -413,25 +475,41 @@ VP3D_API int vp3d_forward_train(vp3d_plan* p, const float* x, float* y, int N, i
   return VP3D_OK;
 }
 
-static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, void* ws,
+static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, float* dx, void* ws,
                          size_t ws_bytes, void* stream_, vp3d_stage_fn stage_done, void* user);
 
 VP3D_API int vp3d_backward(vp3d_plan* p, const float* dy, const vp3d_grads* g, void* ws,
                            size_t ws_bytes, void* stream_) {
-  return backward_impl(p, dy, g, ws, ws_bytes, stream_, nullptr, nullptr);
+  if (!g) return fail(VP3D_ERR_INVALID, "backward: null argument");
+  return backward_impl(p, dy, g, nullptr, ws, ws_bytes, stream_, nullptr, nullptr);
 }
 
 VP3D_API int vp3d_backward_staged(vp3d_plan* p, const float* dy, const vp3d_grads* g, void* ws,
                                   size_t ws_bytes, void* stream_, vp3d_stage_fn stage_done,
                                   void* user) {
-  return backward_impl(p, dy, g, ws, ws_bytes, stream_, stage_done, user);
+  if (!g) return fail(VP3D_ERR_INVALID, "backward: null argument");
+  return backward_impl(p, dy, g, nullptr, ws, ws_bytes, stream_, stage_done, user);
 }
 
-static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, void* ws,
+VP3D_API int vp3d_backward_ex(vp3d_plan* p, const float* dy, const vp3d_grads* g, float* dx, void* ws,
+                              size_t ws_bytes, void* stream_, vp3d_stage_fn stage_done, void* user) {
+  if (!g && !dx) return fail(VP3D_ERR_INVALID, "backward: neither parameter nor input gradients asked for");
+  return backward_impl(p, dy, g, dx, ws, ws_bytes, stream_, stage_done, user);
+}
+
+// g == nullptr: no parameter gradients (no weight-gradient GEMMs, no shrink-bias sum, and under
+// frozen BatchNorm no BatchNorm-backward reductions either); dx == nullptr: no input gradient.
+static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, float* dx, void* ws,
                          size_t ws_bytes, void* stream_, vp3d_stage_fn stage_done, void* user) {
-  if (!p || !dy || !g) return fail(VP3D_ERR_INVALID, "backward: null argument");
+  if (!p || !dy) return fail(VP3D_ERR_INVALID, "backward: null argument");
   TrainState* t = p->train;
   if (!t || !t->have_forward) return fail(VP3D_ERR_STATE, "backward: no training forward to match");
+  if (dx && !t->packed_expand_t)
+    return fail(VP3D_ERR_STATE, "backward: the input gradient needs the transposed expand pack "
+                "(vp3d_set_weights with VP3D_PACK_EXPAND_T)");
+  const bool want_w = g != nullptr;
+  const bool frozen = t->frozen_bn;
+  const bool need_sums = want_w || !frozen;   // BatchNorm-backward reductions
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int N = t->N, C = p->C, Cr = p->c_real, pl = p->planes;   // padded / real channels
   const int* L = t->L;
@@ -443,12 +521,14 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
   auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
   float* partial = reinterpret_cast<float*>(base + wl.partial);
   float* slab_part = reinterpret_cast<float*>(base + wl.slab);
-  if (!g->expand_conv_weight || !g->shrink_weight || !g->shrink_bias || !g->expand_bn[0] ||
-      !g->expand_bn[1])
-    return fail(VP3D_ERR_INVALID, "backward: missing gradient buffer");
-  for (int l = 0; l < 2 * p->nb; ++l)
-    if (!g->layers_conv_weight[l] || !g->layers_bn[l][0] || !g->layers_bn[l][1])
-      return fail(VP3D_ERR_INVALID, "backward: missing gradient buffer for layer %d", l);
+  if (want_w) {
+    if (!g->expand_conv_weight || !g->shrink_weight || !g->shrink_bias || !g->expand_bn[0] ||
+        !g->expand_bn[1])
+      return fail(VP3D_ERR_INVALID, "backward: missing gradient buffer");
+    for (int l = 0; l < 2 * p->nb; ++l)
+      if (!g->layers_conv_weight[l] || !g->layers_bn[l][0] || !g->layers_bn[l][1])
+        return fail(VP3D_ERR_INVALID, "backward: missing gradient buffer for layer %d", l);
+  }
   int launches = 0;
   const int co128 = c_out_pad128(p);
   const long long rows_top = wl.rows[p->nb];
@@ -469,7 +549,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
   // geometry of the slab partials the last fused GEMM left behind (consumed by the next bn_bwd)
   int bnb_slabs = 0, bnb_ld = 0;
   auto fuse_bnb = [&](vp3d_conv_desc& q, int layer) {
-    if (!fuse) return;
+    if (!fuse || !need_sums) return;
     const LayerVec v = layer_vec(p, layer);
     q.bnb_z = bf(wl.z[layer]);
     q.bnb_scale = v.scale; q.bnb_shift = v.shift; q.bnb_mean = v.mean; q.bnb_invstd = v.invstd;
@@ -484,7 +564,9 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
                     float* dgamma, float* dbeta) -> int {
     const LayerVec v = layer_vec(p, layer);
     const DropoutCfg dc = drop_cfg(t, layer);
-    if (!fuse) {
+    if (!need_sums) {
+      // frozen BatchNorm without parameter gradients: dZ = scale * dY needs no reduction
+    } else if (!fuse) {
       CUDA_TRY(launch_bn_bwd_reduce(gin, rows * C, z, rows * C, pl, rows, C, v.scale, v.shift,
                                     v.mean, v.invstd, dc, slab_part, wl.slab_floats, v.sums,
                                     t->red_scratch, t->red_counter, stream));
@@ -500,8 +582,9 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
       ++launches;
     }
     CUDA_TRY(launch_bn_bwd_apply(gin, rows * C, z, rows * C, bf(wl.dz), rows * C, pl, rows, C,
-                                 v.scale, v.shift, v.mean, v.invstd, dc, v.sums, dgamma, dbeta,
-                                 p->c_real, stream));
+                                 v.scale, v.shift, v.mean, v.invstd, dc,
+                                 need_sums ? v.sums : nullptr, want_w ? dgamma : nullptr,
+                                 want_w ? dbeta : nullptr, p->c_real, stream, frozen ? 1 : 0));
     ++launches;
     return VP3D_OK;
   };
@@ -509,16 +592,17 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
   // ---- shrink backward: y = X_nb * Wsh^T + b
   CUDA_TRY(launch_pack_input(dy, bf(wl.dyp), pl, 1, (int)rows_top, p->c_out_raw, (int)rows_top, 1, 1,
                              co128, rows_top * co128, stream));
-  CUDA_TRY(launch_col_sum_f32(dy, rows_top, p->c_out_raw, slab_part, wl.slab_floats, g->shrink_bias,
-                              t->red_scratch, t->red_counter, stream));
-  launches += 3;
-  {
+  ++launches;
+  if (want_w) {
+    CUDA_TRY(launch_col_sum_f32(dy, rows_top, p->c_out_raw, slab_part, wl.slab_floats, g->shrink_bias,
+                                t->red_scratch, t->red_counter, stream));
+    launches += 2;
     WgradCall c;
     c.dz = bf(wl.dyp); c.dz_ld = co128; c.x = bf(wl.x[p->nb]); c.x_ld = C; c.rows = rows_top;
     c.c_out = p->c_out_raw; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->shrink_weight;
     VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+    launches += 2;
   }
-  launches += 2;
   __nv_bfloat16* gb[2] = {bf(wl.g0), bf(wl.g1)};
   int cur = 0;
   common(d);
@@ -537,14 +621,15 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
     const int l1 = 2 * i - 1, l2 = 2 * i;
     const int c1 = 2 * (i - 1), c2 = c1 + 1;
     // second conv (1x1): X_i = res + act(bn(conv2(H_i)))
-    VP3D_TRY(bn_bwd(l2, rows, gb[cur], bf(wl.z[l2]), g->layers_bn[c2][0], g->layers_bn[c2][1]));
-    {
+    VP3D_TRY(bn_bwd(l2, rows, gb[cur], bf(wl.z[l2]), want_w ? g->layers_bn[c2][0] : nullptr,
+                    want_w ? g->layers_bn[c2][1] : nullptr));
+    if (want_w) {
       WgradCall c;
       c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.h[i]); c.x_ld = C; c.rows = rows;
       c.c_out = Cr; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->layers_conv_weight[c2];
       VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+      launches += 2;
     }
-    launches += 2;
     common(d);
     d.a = bf(wl.dz); d.a_rows = (int)rows; d.a_ld = C;
     d.w = t->conv_t[c2]; d.taps = 1; d.k_per_tap = C; d.n_pad = C;
@@ -554,8 +639,9 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
     VP3D_TRY(run_conv(&d, stream));
     ++launches;
     // first conv (w taps, stride w): H_i = act(bn(conv1(X_{i-1})))
-    VP3D_TRY(bn_bwd(l1, rows, gb[cur ^ 1], bf(wl.z[l1]), g->layers_bn[c1][0], g->layers_bn[c1][1]));
-    {
+    VP3D_TRY(bn_bwd(l1, rows, gb[cur ^ 1], bf(wl.z[l1]), want_w ? g->layers_bn[c1][0] : nullptr,
+                    want_w ? g->layers_bn[c1][1] : nullptr));
+    if (want_w) {
       WgradCall c;
       c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.x[i - 1]); c.taps = p->taps[i];
       c.c_out = Cr; c.c_in_cols = Cr; c.c_in = Cr; c.taps_out = p->taps[i];
@@ -567,8 +653,8 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
         c.tap_row_step = p->dilation[i];
       }
       VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+      launches += 2;
     }
-    launches += 2;
     common(d);
     d.w = t->conv_t[c1]; d.k_per_tap = C;
     d.res = gb[cur]; d.res_planes = pl; d.res_plane_stride = rows * C; d.res_ld = C;
@@ -599,9 +685,11 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
     if (stage_done) stage_done(p->nb - i + 1, user);  // all four parameter groups of block i
   }
 
-  // ---- expand backward (no data gradient: the 2-D input needs none, run.py:402-412)
-  VP3D_TRY(bn_bwd(0, wl.rows[0], gb[cur], bf(wl.z[0]), g->expand_bn[0], g->expand_bn[1]));
-  {
+  // ---- expand backward (the data gradient only on request: run.py's 2-D input needs none,
+  // run.py:402-412; a differentiable front end or test-time refinement of x does)
+  VP3D_TRY(bn_bwd(0, wl.rows[0], gb[cur], bf(wl.z[0]), want_w ? g->expand_bn[0] : nullptr,
+                  want_w ? g->expand_bn[1] : nullptr));
+  if (want_w) {
     WgradCall c;
     c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.a0); c.c_out = Cr; c.c_in = p->c_in_raw;
     c.taps_out = fw[0]; c.grad = g->expand_conv_weight;
@@ -612,8 +700,44 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, voi
       c.taps = fw[0]; c.tap_row_step = 1; c.c_in_cols = p->c_in_raw;
     }
     VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+    launches += 2;
   }
-  launches += 2;
+  if (dx) {
+    // dX = dZ0 * W0^T through the conv GEMM, fp32 epilogue straight into x's (N, T, J*F) layout
+    const int cin = p->c_in_raw, T = t->T;
+    common(d);
+    d.a = bf(wl.dz); d.a_ld = C; d.w = t->expand_t; d.k_per_tap = C;
+    d.out_f32 = dx;
+    if (strided) {
+      // G_x[rows0, w0*cin] = dZ0 * W0^T with the tap-merged pack: column tap*cin + ci of row
+      // (n, r) is x[n, r*w0 + tap, ci], i.e. x's own memory order when T = w0 * L0
+      d.taps = 1; d.n_pad = p->k0_pad;
+      d.a_rows = (int)wl.rows[0]; d.out_rows = (int)wl.rows[0];
+      d.out_f32_ld = fw[0] * cin; d.n_valid = fw[0] * cin;
+      const size_t used = (size_t)fw[0] * L[0] * cin;   // floats per sample the output depends on
+      const bool tail = T != fw[0] * L[0];
+      // trailing frames no output depends on: the GEMM writes a staging buffer, one strided copy
+      // moves each sample's rows into place and one strided memset zeroes the tails
+      if (tail) d.out_f32 = reinterpret_cast<float*>(base + wl.dx_stage);
+      VP3D_TRY(run_conv(&d, stream));
+      ++launches;
+      if (tail) {
+        const size_t pitch = (size_t)T * cin * sizeof(float);
+        CUDA_TRY(cudaMemcpy2DAsync(dx, pitch, d.out_f32, used * sizeof(float), used * sizeof(float),
+                                   N, cudaMemcpyDeviceToDevice, stream));
+        CUDA_TRY(cudaMemset2DAsync(dx + used, pitch, 0, pitch - used * sizeof(float), N, stream));
+        launches += 2;
+      }
+    } else {
+      // transposed convolution: dX[n, t] = sum_k dZ0[n, t - k] * W0_k^T; rows outside [0, L0) are
+      // zero-filled by the A tensor map, so every one of the T rows is written
+      d.samples = N; d.a_rows = L[0]; d.per_sample_tiles = 1;
+      d.taps = fw[0]; d.tap_row_step = -1; d.n_pad = p->c_in_pad;
+      d.out_rows = T; d.out_f32_ld = cin; d.n_valid = cin;
+      VP3D_TRY(run_conv(&d, stream));
+      ++launches;
+    }
+  }
   if (stage_done) stage_done(p->nb + 1, user);  // expand_conv / expand_bn
   p->last_launches = launches;
   return VP3D_OK;

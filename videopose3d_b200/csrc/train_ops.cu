@@ -447,7 +447,8 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
 }
 
 // dz = scale*(dY - s1/n - xhat*s2/n) = scale*dY + B*z + D with per-channel
-// B = -scale*invstd*s2/n,  D = -scale*s1/n - B*mean.
+// B = -scale*invstd*s2/n,  D = -scale*s1/n - B*mean.  frozen (BatchNorm on running statistics):
+// B = D = 0, dz = scale*dY; sums may then be null (no dgamma / dbeta wanted).
 __global__ void __launch_bounds__(256)
 bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
                     const __nv_bfloat16* __restrict__ z, long long z_plane,
@@ -455,7 +456,7 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
                     int c, const float* __restrict__ scale, const float* __restrict__ shift,
                     const float* __restrict__ mean, const float* __restrict__ invstd,
                     DropoutCfg drop, const float* __restrict__ sums, float* __restrict__ dgamma,
-                    float* __restrict__ dbeta, int c_real, RowTiling tl) {
+                    float* __restrict__ dbeta, int c_real, int frozen, RowTiling tl) {
   pdl_entry();
   const int cg = threadIdx.x % tl.G, rl = threadIdx.x / tl.G, lanes = 256 / tl.G;
   const int c0 = (blockIdx.x * tl.G + cg) * 8;
@@ -470,11 +471,21 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
     float mu[8], is[8], s1[8], s2[8];
     load_vec8(scale + c0, sc);
     load_vec8(shift + c0, sh);
-    load_vec8(mean + c0, mu);
-    load_vec8(invstd + c0, is);
-    load_vec8(sums + c0, s1);
-    load_vec8(sums + c + c0, s2);
-    if (blockIdx.y == 0 && rl == 0) {
+    if (sums) {
+      load_vec8(sums + c0, s1);
+      load_vec8(sums + c + c0, s2);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s1[j] = s2[j] = 0.0f;
+    }
+    if (frozen) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mu[j] = is[j] = 0.0f;
+    } else {
+      load_vec8(mean + c0, mu);
+      load_vec8(invstd + c0, is);
+    }
+    if (sums && blockIdx.y == 0 && rl == 0) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         if (c0 + j >= c_real) break;   // gradient tensors hold the model's real channel count
@@ -484,8 +495,8 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      B[j] = -sc[j] * is[j] * s2[j] * inv_n;
-      D[j] = -sc[j] * s1[j] * inv_n - B[j] * mu[j];
+      B[j] = frozen ? 0.0f : -sc[j] * is[j] * s2[j] * inv_n;
+      D[j] = frozen ? 0.0f : -sc[j] * s1[j] * inv_n - B[j] * mu[j];
     }
   }
   long long r = r_begin + rl;
@@ -540,14 +551,17 @@ __global__ void col_sum_f32_kernel(const float* __restrict__ x, long long rows, 
 // the writes (co fastest) are coalesced.  Padding entries are written as zeros.
 // If `fwd` is non-null the same pass also writes the forward pack fwd[pl][tap][co][ci] (rows
 // fwd_n_pad, cols fwd_k_pad), so one read of the fp32 master feeds both layouts.
+// merged: one tap-merged slab out[pl][tap*c_in + ci][co] (rows n_pad >= taps*c_in; the last tap
+// writes the padding rows) -- the data gradient of the strided expand conv.
 __global__ void __launch_bounds__(256)
 pack_conv_weight_t_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int planes,
                           int c_out, int c_in, int taps, int n_pad, int k_pad,
-                          __nv_bfloat16* __restrict__ fwd, int fwd_n_pad, int fwd_k_pad) {
+                          __nv_bfloat16* __restrict__ fwd, int fwd_n_pad, int fwd_k_pad,
+                          int merged) {
   __shared__ float sm[32][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
   const int ci0 = blockIdx.x * 32, co0 = blockIdx.y * 32;
-  const long long plane_elems = (long long)taps * n_pad * k_pad;
+  const long long plane_elems = merged ? (long long)n_pad * k_pad : (long long)taps * n_pad * k_pad;
   const long long fwd_plane = (long long)taps * fwd_n_pad * fwd_k_pad;
   for (int tap = 0; tap < taps; ++tap) {
 #pragma unroll
@@ -567,9 +581,11 @@ pack_conv_weight_t_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict
 #pragma unroll
     for (int j = ty; j < 32; j += 8) {
       const int ci = ci0 + j, co = co0 + tx;
-      if (ci < n_pad && co < k_pad) {
+      const int row = merged ? tap * c_in + ci : ci;
+      const bool own = !merged || ci < c_in || tap == taps - 1;
+      if (own && row < n_pad && co < k_pad) {
         const float v = sm[tx][j];
-        const long long o = ((long long)tap * n_pad + ci) * k_pad + co;
+        const long long o = ((long long)(merged ? 0 : tap) * n_pad + row) * k_pad + co;
         const __nv_bfloat16 hi = __float2bfloat16_rn(v);
         out[o] = hi;
         if (planes == 2) out[plane_elems + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
@@ -669,13 +685,14 @@ cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* g, long long g_plane, const
                                 long long rows, int c, const float* scale, const float* shift,
                                 const float* mean, const float* invstd, DropoutCfg drop,
                                 const float* sums, float* dgamma, float* dbeta, int c_real,
-                                cudaStream_t stream) {
+                                cudaStream_t stream, int frozen) {
   if (rows <= 0) return cudaSuccess;
+  if (!sums && !frozen) return cudaErrorInvalidValue;
   dim3 grid;
   const RowTiling tl = row_tiling(rows, c, grid);
   const cudaError_t le = launch_pdl(bn_bwd_apply_kernel, grid, dim3(256), 0, stream, g, g_plane, z, z_plane, dz, dz_plane, planes, rows,
                                                 c, scale, shift, mean, invstd, drop, sums, dgamma,
-                                                dbeta, c_real, tl);
+                                                dbeta, c_real, frozen, tl);
   return le != cudaSuccess ? le : cudaGetLastError();
 }
 
@@ -694,14 +711,16 @@ cudaError_t launch_col_sum_f32(const float* x, long long rows, int c, float* par
 
 cudaError_t launch_pack_conv_weight_t(const float* w, __nv_bfloat16* out, int planes, int c_out,
                                       int c_in, int taps, int n_pad, int k_pad, cudaStream_t stream,
-                                      __nv_bfloat16* fwd, int fwd_n_pad, int fwd_k_pad) {
+                                      __nv_bfloat16* fwd, int fwd_n_pad, int fwd_k_pad, int merged) {
+  if (merged && (fwd || n_pad < taps * c_in)) return cudaErrorInvalidValue;
   int gx = (n_pad + 31) / 32, gy = (k_pad + 31) / 32;
   if (fwd) {  // the grid must also cover the forward pack's padding
     if ((fwd_k_pad + 31) / 32 > gx) gx = (fwd_k_pad + 31) / 32;
     if ((fwd_n_pad + 31) / 32 > gy) gy = (fwd_n_pad + 31) / 32;
   }
   pack_conv_weight_t_kernel<<<dim3(gx, gy), 256, 0, stream>>>(w, out, planes, c_out, c_in, taps,
-                                                              n_pad, k_pad, fwd, fwd_n_pad, fwd_k_pad);
+                                                              n_pad, k_pad, fwd, fwd_n_pad, fwd_k_pad,
+                                                              merged);
   return cudaGetLastError();
 }
 

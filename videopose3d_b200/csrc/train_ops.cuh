@@ -68,13 +68,15 @@ cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* g, long long g_plane, cons
                                  unsigned* counter, cudaStream_t stream);
 
 // dz = scale * (dY - sums[0]/n - xhat * sums[1]/n); also writes dgamma = sums[1], dbeta = sums[0]
-// (done by block 0).  dz: bf16 [planes][rows][c].
+// (done by block 0).  dz: bf16 [planes][rows][c].  frozen != 0 (BatchNorm on running statistics,
+// eval-mode backward): dz = scale * dY, mean / invstd are not read, and sums may be null (then no
+// dgamma / dbeta are written).
 cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* g, long long g_plane, const __nv_bfloat16* z,
                                 long long z_plane, __nv_bfloat16* dz, long long dz_plane, int planes,
                                 long long rows, int c, const float* scale, const float* shift,
                                 const float* mean, const float* invstd, DropoutCfg drop,
                                 const float* sums, float* dgamma, float* dbeta, int c_real,
-                                cudaStream_t stream);
+                                cudaStream_t stream, int frozen = 0);
 
 // out[c] = sum_rows x[row][c] for fp32 x [rows][c] (shrink.bias gradient), via per-64-row partials
 // summed in a fixed order.
@@ -86,9 +88,11 @@ cudaError_t launch_col_sum_f32(const float* x, long long rows, int c, float* par
 // with out[pl][tap][ci][co] = w[co][ci][tap]  (rows = input channels, K = output channels).
 // If fwd != nullptr the same pass also writes the forward pack fwd[pl][tap][co][ci] (rows fwd_n_pad,
 // cols fwd_k_pad): one read of the fp32 master feeds both layouts.
+// merged != 0 (fwd must be null): one slab out[pl][0][tap*c_in + ci][co], rows padded to n_pad >=
+// taps*c_in -- the tap-merged layout of the strided expand conv's data gradient.
 cudaError_t launch_pack_conv_weight_t(const float* w, __nv_bfloat16* out, int planes, int c_out,
                                       int c_in, int taps, int n_pad, int k_pad, cudaStream_t stream,
                                       __nv_bfloat16* fwd = nullptr, int fwd_n_pad = 0,
-                                      int fwd_k_pad = 0);
+                                      int fwd_k_pad = 0, int merged = 0);
 
 }  // namespace vp3d

@@ -373,6 +373,38 @@ class TemporalModelBase(nn.Module):
                     tuple((t.data_ptr(), t._version) for t in bn) + (self._stats_epoch,))
         self._packed[((device.index, self._train_precision), True)] = versions
 
+    def _sync_expand_t(self, plan, stream):
+        """Pack the transposed expand conv for the input gradient when expand_conv.weight changed
+        since this plan last packed it.  Only input-gradient backwards call this, and nothing else
+        marks the pack current (the fused optimizer step does not refresh it), so a version bump
+        of the weight always leads to a re-pack here."""
+        wt = self.expand_conv.weight
+        key = (self._plan_key, "expand_t")
+        seen = (wt.data_ptr(), wt._version)
+        packed = self.__dict__.setdefault("_packed", {})
+        if packed.get(key) == seen:
+            return
+        w = self._weights_struct()
+        _capi.check(_capi.load().vp3d_set_weights(plan, _capi.ctypes.byref(w),
+                                                   _capi.VP3D_PACK_EXPAND_T, stream),
+                    "vp3d_set_weights")
+        packed[key] = seen
+
+    def _grads_struct(self, grads):
+        """vp3d_grads over `grads`, tensors in the order of ``_learnable_tensors``."""
+        nb2 = len(self.layers_conv)
+        g = _capi.Grads()
+        g.expand_conv_weight = grads[0].data_ptr()
+        g.expand_bn[0] = grads[1].data_ptr()
+        g.expand_bn[1] = grads[2].data_ptr()
+        for i in range(nb2):
+            g.layers_conv_weight[i] = grads[3 + i].data_ptr()
+            g.layers_bn[i][0] = grads[3 + nb2 + 2 * i].data_ptr()
+            g.layers_bn[i][1] = grads[3 + nb2 + 2 * i + 1].data_ptr()
+        g.shrink_weight = grads[3 + 3 * nb2].data_ptr()
+        g.shrink_bias = grads[3 + 3 * nb2 + 1].data_ptr()
+        return g
+
     def _get_workspace(self, nbytes, device):
         ws = self._workspace
         if ws is None or ws.device != device or ws.numel() < nbytes:
@@ -399,6 +431,16 @@ class TemporalModelBase(nn.Module):
         return self._forward_eval(x)
 
     def _forward_eval(self, x):
+        params = self._learnable_tensors()
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+            reducer = getattr(self, "_grad_reducer", None)
+            if reducer is not None and reducer.world > 1:
+                raise NotImplementedError("eval-mode gradients are not all-reduced across ranks; "
+                                          "detach the data-parallel reducer or run under no_grad")
+            return _EvalFunction.apply(self, x.contiguous(), *params)
+        return self._eval_launch(x)
+
+    def _eval_launch(self, x):
         lib = _capi.load()
         x = x.contiguous()
         device = x.device
@@ -526,7 +568,9 @@ class _TrainFunction(torch.autograd.Function):
     """Training-mode forward/backward through the C ABI (vp3d_forward_train / vp3d_backward).
 
     The learnable tensors are passed as inputs so that autograd accumulates the returned
-    gradients into ``.grad`` exactly as it does for the reference's nn modules."""
+    gradients into ``.grad`` exactly as it does for the reference's nn modules.  dL/dx is computed
+    when x requires grad (vp3d_backward_ex with the expand conv's data gradient); parameter
+    gradients are skipped when no learnable tensor requires grad."""
 
     @staticmethod
     def forward(ctx, module, x, *params):
@@ -567,6 +611,7 @@ class _TrainFunction(torch.autograd.Function):
         ctx.ws = ws
         ctx.token = module._fwd_token
         ctx.shapes = [tuple(p.shape) for p in params]
+        ctx.x_shape = tuple(x.shape)
         ctx.device = device
         return y
 
@@ -581,6 +626,10 @@ class _TrainFunction(torch.autograd.Function):
         dy = dy.contiguous().float()
         names = [n for n, _ in module.named_parameters()]
         order = module._learnable_names()
+        want_x = ctx.needs_input_grad[1]
+        want_p = ctx.needs_input_grad[2:]
+        if want_x or not any(want_p):
+            return _TrainFunction._backward_ex(ctx, dy, want_x, want_p)
         reducer = getattr(module, "_grad_reducer", None)
         if reducer is not None and reducer.world > 1:
             # one flat buffer laid out in backward-completion order: each stage is a contiguous
@@ -630,6 +679,132 @@ class _TrainFunction(torch.autograd.Function):
         del names
         ctx.ws = None
         return (None, None) + tuple(grads)
+
+    @staticmethod
+    def _backward_ex(ctx, dy, want_x, want_p):
+        """vp3d_backward_ex: the input gradient and / or the parameter gradients (None for those
+        not wanted; with no parameter requiring grad no weight gradient is computed at all)."""
+        module = ctx.module
+        lib = _capi.load()
+        device = ctx.device
+        reducer = getattr(module, "_grad_reducer", None)
+        flat, stage_spans = None, None
+        grads = None
+        if any(want_p):
+            if reducer is not None and reducer.world > 1:
+                _, spans, stage_spans, total = reducer.plan_layout(module)
+                flat = torch.empty(total, dtype=torch.float32, device=device)
+                by_name = {n: flat[spans[n][0]: spans[n][0] + spans[n][1]] for n in spans}
+                grads = [by_name[n].view(s) for n, s in zip(module._learnable_names(), ctx.shapes)]
+            else:
+                grads = [torch.empty(s, dtype=torch.float32, device=device) for s in ctx.shapes]
+        dx = torch.empty(ctx.x_shape, dtype=torch.float32, device=device) if want_x else None
+        g = module._grads_struct(grads) if grads is not None else None
+        errors = []
+
+        def _stage(stage, _user):
+            try:
+                lo, hi = stage_spans[stage]
+                reducer.stage_ready(flat, lo, hi)
+            except Exception as e:  # never raise through the C frame
+                errors.append(e)
+
+        cb = _capi.STAGE_FN(_stage) if flat is not None else None
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            if want_x:
+                module._sync_expand_t(ctx.plan, stream)
+            _capi.check(lib.vp3d_backward_ex(ctx.plan, dy.data_ptr(),
+                                             _capi.ctypes.byref(g) if g is not None else None,
+                                             dx.data_ptr() if dx is not None else None,
+                                             ctx.ws.data_ptr(), ctx.ws.numel(), stream,
+                                             _capi.ctypes.cast(cb, _capi.ctypes.c_void_p)
+                                             if cb is not None else None, None),
+                        "vp3d_backward_ex")
+            if errors:
+                raise errors[0]
+            if flat is not None:
+                reducer.finish(flat)
+        ctx.ws = None
+        out = [None] * len(want_p)
+        if grads is not None:
+            out = [gr if w else None for gr, w in zip(grads, want_p)]
+        return (None, dx) + tuple(out)
+
+
+class _EvalFunction(torch.autograd.Function):
+    """Eval-mode forward inside autograd (model.eval() with x or parameters requiring grad).
+
+    The forward is the plain eval forward (``vp3d_forward_eval``: same kernels, same bits as under
+    ``no_grad``, no workspace kept).  The backward recomputes: a training-geometry forward with
+    BatchNorm frozen to its running statistics (``VP3D_TRAIN_FROZEN_BN``) in the module's train
+    precision, then ``vp3d_backward_ex``.  The gradient is therefore that of the train-precision
+    forward ('bf16' or the fp32-faithful 'bf16x3', ``set_train_precision``), which is the reference's
+    eval-mode backward: BatchNorm is a fixed affine, no dropout, running statistics untouched."""
+
+    @staticmethod
+    def forward(ctx, module, x, *params):
+        y = module._eval_launch(x)
+        ctx.module = module
+        ctx.save_for_backward(x, *params)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        module = ctx.module
+        x = ctx.saved_tensors[0]     # (raises if x or a parameter was modified in place since)
+        want_x = ctx.needs_input_grad[1]
+        want_p = ctx.needs_input_grad[2:]
+        lib = _capi.load()
+        device = x.device
+        N, T = int(x.shape[0]), int(x.shape[1])
+        dy = dy.contiguous().float()
+        with torch.cuda.device(device):
+            plan = module._get_plan(device, module._train_precision)
+            stream = torch.cuda.current_stream(device).cuda_stream
+            module._sync_weights(plan, stream, training=True)
+            if want_x:
+                module._sync_expand_t(plan, stream)
+            t_out = lib.vp3d_output_frames(plan, T)
+            t_used = T
+            if module._variant == _capi.VP3D_VARIANT_STRIDED:
+                # the strided convs ignore trailing frames: recompute on the prefix the output
+                # depends on (exact under frozen BatchNorm, whose affine does not see the batch)
+                t_used = t_out
+                for w in module.filter_widths:
+                    t_used *= int(w)
+            xs = x if t_used == T else x[:, :t_used].contiguous()
+            nbytes = lib.vp3d_train_workspace_bytes(plan, N, t_used)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+            y = torch.empty((N, t_out, module.num_joints_out, 3), dtype=torch.float32, device=device)
+            w = module._weights_struct()
+            _capi.check(lib.vp3d_forward_train_ex(plan, xs.data_ptr(), y.data_ptr(), N, t_used,
+                                                  _capi.ctypes.byref(w), None, 0.0, 0,
+                                                  _capi.VP3D_TRAIN_FROZEN_BN, ws.data_ptr(),
+                                                  ws.numel(), stream), "vp3d_forward_train_ex")
+            # the recompute replaced the plan's saved training state: a pending train-mode
+            # backward of this module must now fail instead of reading it
+            module._fwd_token += 1
+            grads = None
+            if any(want_p):
+                grads = [torch.empty(p.shape, dtype=torch.float32, device=device)
+                         for p in ctx.saved_tensors[1:]]
+            dx = torch.empty((N, t_used) + tuple(x.shape[2:]), dtype=torch.float32,
+                             device=device) if want_x else None
+            g = module._grads_struct(grads) if grads is not None else None
+            _capi.check(lib.vp3d_backward_ex(plan, dy.data_ptr(),
+                                             _capi.ctypes.byref(g) if g is not None else None,
+                                             dx.data_ptr() if dx is not None else None,
+                                             ws.data_ptr(), ws.numel(), stream, None, None),
+                        "vp3d_backward_ex")
+        if dx is not None and t_used != T:
+            full = torch.zeros(x.shape, dtype=torch.float32, device=device)
+            full[:, :t_used] = dx
+            dx = full
+        out = [None] * len(want_p)
+        if grads is not None:
+            out = [gr if w else None for gr, w in zip(grads, want_p)]
+        return (None, dx) + tuple(out)
 
 
 class TemporalModel(TemporalModelBase):
