@@ -294,6 +294,93 @@ typedef struct {
 
 int vp3d_conv_gemm(const vp3d_conv_desc* d, void* stream);
 
+/* Weight gradient of one temporal convolution, the call vp3d_backward makes for every conv layer
+ * (autograd's conv backward-filter):
+ *   grad[(co * c_in + ci) * taps_out + tap] = sum_row dz[row][co] * x[xrow(row, tap)][xcol(tap, ci)]
+ * flat (per_sample = 0): row < rows, xrow = row + tap * tap_row_step,
+ *   xcol = tap * tap_col_step + ci, or tap * c_in + ci when merged (one GEMM over the taps_out * c_in
+ *   columns of the strided expand conv's packed input; taps must then be 1);
+ * per_sample = 1: the sum also runs over the samples, dz row t of sample n pairs with x row
+ *   t + tap * tap_row_step of the same sample.
+ * Operands are bf16 planes (planes 2: hi + lo, the three products hi*hi + lo*hi + hi*lo), fp32
+ * accumulation.  The reduction is split over row ranges into `partial` and the splits are summed in
+ * a fixed order (bit-reproducible); the tile width and the split count follow from the shape and the
+ * SM count as in the training step, fewer splits when `partial` is small, VP3D_ERR_WORKSPACE (and
+ * nothing launched) when it cannot hold one: taps * round_up(c_out, 128) * round_up(c_in_cols, 128)
+ * floats always suffice for one split. */
+typedef struct {
+  const void* dz;     /* bf16 [planes][samples][rows][dz_ld] */
+  int dz_ld;          /* multiple of 64, >= c_out rounded up to 64 */
+  const void* x;      /* bf16 [planes][samples][x_rows][x_ld] (flat: [planes][rows][x_ld]) */
+  int x_ld;           /* multiple of 64 */
+  int planes;         /* 1 or 2 */
+  long long rows;     /* dz rows: per sample when per_sample, else in total */
+  int per_sample;
+  int samples;        /* per_sample only */
+  long long x_rows;   /* x rows per sample (per_sample only) */
+  int taps;           /* GEMM taps (merged: 1) */
+  int tap_row_step;   /* x row offset per tap (dilation), 0 for column taps */
+  int tap_col_step;   /* x column offset per tap (strided layout), else 0 */
+  int c_out;
+  int c_in_cols;      /* x columns one tap's GEMM spans (merged: taps_out * c_in) */
+  int c_in;
+  int taps_out;       /* taps of the gradient tensor (= taps unless merged) */
+  int merged;
+  float* grad;        /* fp32 (c_out, c_in, taps_out), every entry overwritten */
+  float* partial;     /* fp32 scratch */
+  size_t partial_bytes;
+} vp3d_wgrad_desc;
+
+int vp3d_wgrad_gemm(const vp3d_wgrad_desc* d, void* stream);
+
+/* The BatchNorm training passes around the GEMMs (each the launch the training step makes), with
+ * DropoutCfg / RowMap flattened into plain arguments.  Channels c <= 8192.  The ordered reductions
+ * take a caller-owned scratch of 96 * c floats (bn_stats_finalize) or 64 * c floats (the others) and
+ * ceil(c / 32) ticket counters that the caller zeroes once; every launch leaves them zero again.
+ *
+ * vp3d_bn_stats_finalize: part = [slabs][2][c] per-slab sum / sum of squares as the conv GEMM
+ *   epilogue writes them (slab s = rows (s % 4) * 32 .. + 32 of row tile s / 4; dilated: tiles per
+ *   sample, out_rows rows each; flat: out_rows rows in total) -> batch mean, invstd =
+ *   1 / sqrt(var + eps), scale = gamma * invstd, shift = beta - mean * scale; channels [c_real, c)
+ *   get zeros.  running_mean / running_var (both or neither) are updated in place with `momentum`
+ *   and the unbiased variance.
+ * vp3d_ordered_col_sums: out_st[ch] = mul_st[ch] * sum_p sum_f part[p][st][f * c + ch] for
+ *   st < nstat (1 or 2), f < folds; mul_st may be NULL (= 1).
+ * vp3d_bn_apply: x = dropout(relu(z * scale + shift)) [+ res[map(row)]] on bf16 [planes][rows][c]
+ *   (c a multiple of 64), map(r) = (r / res_div) * res_rows_per_sample + (r % res_div) * res_step +
+ *   res_off, or r * res_step + res_off when res_div = 0.  Dropout keyed by (seed, layer, element).
+ * vp3d_bn_bwd_reduce: sums[0][c] = sum dY, sums[1][c] = invstd * sum dY * (z - mean) with
+ *   dY = g * mask * [z * scale + shift > 0]; `partials` holds the per-block partials
+ *   (VP3D_ERR_WORKSPACE when too small).
+ * vp3d_bn_bwd_apply: dz = scale * (dY - sums[0] / rows - (z - mean) * invstd * sums[1] / rows), and
+ *   dbeta = sums[0], dgamma = sums[1] for the first c_real channels (each may be NULL).  frozen:
+ *   dz = scale * dY; mean / invstd are not read and sums may be NULL (then nothing else written). */
+int vp3d_bn_stats_finalize(const float* part, int slabs, int dilated, int out_rows,
+                           int tiles_per_sample, const float* gamma, const float* beta,
+                           float* running_mean, float* running_var, float momentum, float eps,
+                           float* scale, float* shift, float* mean, float* invstd, int c, int c_real,
+                           float* scratch, size_t scratch_floats, unsigned* counter, int counters,
+                           void* stream);
+int vp3d_ordered_col_sums(const float* part, int n_part, int nstat, int ld, int c, int folds,
+                          const float* mul0, const float* mul1, float* out0, float* out1,
+                          float* scratch, size_t scratch_floats, unsigned* counter, int counters,
+                          void* stream);
+int vp3d_bn_apply(const void* z, long long z_plane, void* x, long long x_plane, int planes,
+                  long long rows, int c, const float* scale, const float* shift, float dropout_p,
+                  unsigned long long seed, int layer, const void* res, long long res_plane,
+                  int res_div, int res_rows_per_sample, int res_step, int res_off, void* stream);
+int vp3d_bn_bwd_reduce(const void* g, long long g_plane, const void* z, long long z_plane, int planes,
+                       long long rows, int c, const float* scale, const float* shift,
+                       const float* mean, const float* invstd, float dropout_p,
+                       unsigned long long seed, int layer, float* partials, size_t partial_floats,
+                       float* sums, float* scratch, size_t scratch_floats, unsigned* counter,
+                       int counters, void* stream);
+int vp3d_bn_bwd_apply(const void* g, long long g_plane, const void* z, long long z_plane, void* dz,
+                      long long dz_plane, int planes, long long rows, int c, const float* scale,
+                      const float* shift, const float* mean, const float* invstd, float dropout_p,
+                      unsigned long long seed, int layer, const float* sums, float* dgamma,
+                      float* dbeta, int c_real, int frozen, void* stream);
+
 /* ---- device-resident batch gather (SURVEY §8 row f1) --------------------------------------------
  * Replaces the per-chunk Python loops of the reference generators:
  *   common/generators.py:99-160  ChunkedGenerator.next_epoch   (training windows)

@@ -51,7 +51,7 @@ def test_ctypes_structs_match_the_c_header(tmp_path):
     ct = _capi.ctypes
     pairs = {"vp3d_config": _capi.Config, "vp3d_weights": _capi.Weights, "vp3d_grads": _capi.Grads,
              "vp3d_conv_desc": _capi.ConvDesc, "vp3d_gather_desc": _capi.GatherDesc,
-             "vp3d_adam_tensor": _capi.AdamTensor}
+             "vp3d_adam_tensor": _capi.AdamTensor, "vp3d_wgrad_desc": _capi.WgradDesc}
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "vp3d_b200.h"', 'int main(void) {']
     for cname, cls in pairs.items():
         lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
@@ -240,3 +240,38 @@ def test_copies_and_replicas_never_share_engine_state():
     del clones
     assert len(store) == 1 and destroyed == []             # the original still owns its plan
     assert m.invalidate() is m and m._packed == {}
+
+
+def test_training_operator_entries_validate_before_launching():
+    """vp3d_wgrad_gemm and the BatchNorm-pass entries report bad arguments without touching a device
+    (the pointers below are never dereferenced)."""
+    ct = _capi.ctypes
+    lib = _capi.load()
+    assert lib.vp3d_wgrad_gemm(None, None) == -1
+    d = _capi.WgradDesc()
+    fake = 1 << 20
+    d.dz = d.x = d.grad = d.partial = fake
+    d.dz_ld = d.x_ld = 256
+    d.planes, d.rows, d.taps, d.taps_out = 1, 1000, 3, 3
+    d.c_out = d.c_in = d.c_in_cols = 256
+    d.tap_col_step = 256
+    d.partial_bytes = 3 * 256 * 256 * 4 - 4          # one float short of a single split
+    assert lib.vp3d_wgrad_gemm(ct.byref(d), None) == -4
+    assert b"partial buffer too small" in lib.vp3d_last_error()
+    d.planes = 3
+    assert lib.vp3d_wgrad_gemm(ct.byref(d), None) == -1
+    d.planes, d.merged = 1, 1                          # merged needs taps == 1
+    assert lib.vp3d_wgrad_gemm(ct.byref(d), None) == -1
+    c = 8256
+    args = [fake, 4, 0, 100, 0, fake, fake, None, None, 0.1, 1e-5, fake, fake, fake, fake, c, c,
+            fake, 96 * c, fake, (c + 31) // 32, None]
+    assert lib.vp3d_bn_stats_finalize(*args) == -2     # more than 8192 channels
+    args[15] = args[16] = 1024
+    args[18] = 96 * 1024 - 1                           # scratch one float short
+    assert lib.vp3d_bn_stats_finalize(*args) == -4
+    assert lib.vp3d_ordered_col_sums(fake, 10, 3, 64, 64, 1, None, None, fake, fake, fake, 64 * 64,
+                                     fake, 2, None) == -1
+    assert lib.vp3d_bn_apply(fake, 0, fake, 0, 1, 10, 100, fake, fake, 0.0, 0, 0, None, 0, 0, 0, 0,
+                             0, None) == -1            # channels not a multiple of 64
+    assert lib.vp3d_bn_bwd_apply(fake, 0, fake, 0, fake, 0, 1, 10, 64, fake, fake, None, None, 0.0,
+                                 0, 0, None, None, None, 64, 0, None) == -1   # sums needed unless frozen

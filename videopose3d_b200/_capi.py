@@ -156,6 +156,34 @@ class ConvDesc(ctypes.Structure):
     ]
 
 
+class WgradDesc(ctypes.Structure):
+    """vp3d_wgrad_desc (include/vp3d_b200.h)."""
+    _fields_ = [
+        ("dz", ctypes.c_void_p),
+        ("dz_ld", ctypes.c_int),
+        ("x", ctypes.c_void_p),
+        ("x_ld", ctypes.c_int),
+        ("planes", ctypes.c_int),
+        ("rows", ctypes.c_longlong),
+        ("per_sample", ctypes.c_int),
+        ("samples", ctypes.c_int),
+        ("x_rows", ctypes.c_longlong),
+        ("taps", ctypes.c_int),
+        ("tap_row_step", ctypes.c_int),
+        ("tap_col_step", ctypes.c_int),
+        ("c_out", ctypes.c_int),
+        ("c_in_cols", ctypes.c_int),
+        ("c_in", ctypes.c_int),
+        ("taps_out", ctypes.c_int),
+        ("merged", ctypes.c_int),
+        ("grad", ctypes.c_void_p),
+        ("partial", ctypes.c_void_p),
+        ("partial_bytes", ctypes.c_size_t),
+    ]
+
+
+_P, _I, _LL, _F, _SZ = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_size_t
+
 # name -> (restype, argtypes); also the list the CPU test checks against include/vp3d_b200.h
 SIGNATURES = {
     "vp3d_version": (ctypes.c_int, []),
@@ -203,6 +231,16 @@ SIGNATURES = {
     "vp3d_profile_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
                                          ctypes.POINTER(ctypes.c_int)]),
     "vp3d_conv_gemm": (ctypes.c_int, [ctypes.POINTER(ConvDesc), ctypes.c_void_p]),
+    "vp3d_wgrad_gemm": (ctypes.c_int, [ctypes.POINTER(WgradDesc), ctypes.c_void_p]),
+    "vp3d_bn_stats_finalize": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _F, _F, _P, _P, _P, _P, _I,
+                                    _I, _P, _SZ, _P, _I, _P]),
+    "vp3d_ordered_col_sums": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P, _I, _P]),
+    "vp3d_bn_apply": (_I, [_P, _LL, _P, _LL, _I, _LL, _I, _P, _P, _F, ctypes.c_ulonglong, _I, _P,
+                           _LL, _I, _I, _I, _I, _P]),
+    "vp3d_bn_bwd_reduce": (_I, [_P, _LL, _P, _LL, _I, _LL, _I, _P, _P, _P, _P, _F,
+                                ctypes.c_ulonglong, _I, _P, _SZ, _P, _P, _SZ, _P, _I, _P]),
+    "vp3d_bn_bwd_apply": (_I, [_P, _LL, _P, _LL, _P, _LL, _I, _LL, _I, _P, _P, _P, _P, _F,
+                               ctypes.c_ulonglong, _I, _P, _P, _P, _I, _I, _P]),
     "vp3d_gather_windows": (ctypes.c_int, [ctypes.POINTER(GatherDesc), ctypes.c_void_p]),
     "vp3d_gather_cameras": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p,
                                            ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]),

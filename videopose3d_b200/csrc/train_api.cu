@@ -202,7 +202,9 @@ struct WgradCall {
   float* grad = nullptr;
 };
 
-int run_wgrad(const vp3d_plan* p, const WgradCall& c, float* partial, size_t partial_bytes,
+// planes: 1 (bf16) or 2 (hi + lo, three products per pair of planes).  The tile width and the
+// split count follow from the shape alone; vp3d_wgrad_gemm reaches the same code.
+int run_wgrad(int planes, const WgradCall& c, float* partial, size_t partial_bytes,
               cudaStream_t stream) {
   const int block_n = pick_block_n(round_up(c.c_in_cols, 64));
   WgradArgs a;
@@ -218,7 +220,7 @@ int run_wgrad(const vp3d_plan* p, const WgradCall& c, float* partial, size_t par
   a.n_pad = round_up(c.c_in_cols, block_n);
   a.m_tiles = a.m_pad / 128;
   a.n_tiles = a.n_pad / block_n;
-  a.pairs = p->planes == 2 ? 3 : 1;
+  a.pairs = planes == 2 ? 3 : 1;
   const int items = c.taps * a.m_tiles * a.n_tiles;
   const long long total_kb = (long long)a.kchunks * a.samples;
   int splits = (2 * num_sms() + items - 1) / items;
@@ -234,8 +236,8 @@ int run_wgrad(const vp3d_plan* p, const WgradCall& c, float* partial, size_t par
   CUtensorMap mdz, mx;
   const uint64_t x_rows = c.per_sample ? (uint64_t)c.x_rows : (uint64_t)c.rows;
   VP3D_TRY(make_map_4d(&mdz, c.dz, c.dz_ld, c.rows, c.dz_ld, a.samples, (uint64_t)c.rows * c.dz_ld,
-                       p->planes, (uint64_t)a.samples * c.rows * c.dz_ld, 64));
-  VP3D_TRY(make_map_4d(&mx, c.x, c.x_ld, x_rows, c.x_ld, a.samples, x_rows * c.x_ld, p->planes,
+                       planes, (uint64_t)a.samples * c.rows * c.dz_ld, 64));
+  VP3D_TRY(make_map_4d(&mx, c.x, c.x_ld, x_rows, c.x_ld, a.samples, x_rows * c.x_ld, planes,
                        (uint64_t)a.samples * x_rows * c.x_ld, 64));
   CUDA_TRY(launch_wgrad_gemm(mdz, mx, a, block_n, num_sms(), stream));
   CUDA_TRY(launch_wgrad_reduce(partial, c.grad, splits, c.taps, a.m_pad, a.n_pad, c.c_out, c.c_in,
@@ -600,7 +602,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
     WgradCall c;
     c.dz = bf(wl.dyp); c.dz_ld = co128; c.x = bf(wl.x[p->nb]); c.x_ld = C; c.rows = rows_top;
     c.c_out = p->c_out_raw; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->shrink_weight;
-    VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+    VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
     launches += 2;
   }
   __nv_bfloat16* gb[2] = {bf(wl.g0), bf(wl.g1)};
@@ -627,7 +629,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       WgradCall c;
       c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.h[i]); c.x_ld = C; c.rows = rows;
       c.c_out = Cr; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->layers_conv_weight[c2];
-      VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+      VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
       launches += 2;
     }
     common(d);
@@ -652,7 +654,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
         c.x_ld = C; c.per_sample = 1; c.samples = N; c.rows = L[i]; c.x_rows = L[i - 1];
         c.tap_row_step = p->dilation[i];
       }
-      VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+      VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
       launches += 2;
     }
     common(d);
@@ -699,7 +701,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       c.x_ld = p->c_in_pad; c.per_sample = 1; c.samples = N; c.rows = L[0]; c.x_rows = t->T;
       c.taps = fw[0]; c.tap_row_step = 1; c.c_in_cols = p->c_in_raw;
     }
-    VP3D_TRY(run_wgrad(p, c, partial, wl.partial_bytes, stream));
+    VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
     launches += 2;
   }
   if (dx) {
@@ -800,5 +802,151 @@ VP3D_API int vp3d_adam_step_packed(vp3d_plan* p, const vp3d_weights* w,
                                      p->c_in_raw, w0, p->C, p->k0_pad, 1, stream));
   }
   p->last_launches = (plain.empty() ? 0 : 1) + (packed.empty() ? 0 : 1) + (expand_seen ? 2 : 0);
+  return VP3D_OK;
+}
+
+// ---- operator-level entries (include/vp3d_b200.h): the launch functions the training step uses,
+// with the step's own shape rules, for tests that compare one operator with a reference.
+VP3D_API int vp3d_wgrad_gemm(const vp3d_wgrad_desc* d, void* stream) {
+  if (!d || !d->dz || !d->x || !d->grad || !d->partial)
+    return fail(VP3D_ERR_INVALID, "wgrad_gemm: null argument");
+  if (d->planes != 1 && d->planes != 2) return fail(VP3D_ERR_INVALID, "wgrad_gemm: planes must be 1 or 2");
+  if (d->rows < 1 || d->taps < 1 || d->c_out < 1 || d->c_in < 1 || d->c_in_cols < 1 ||
+      d->taps_out < 1 || (d->per_sample && (d->samples < 1 || d->x_rows < 1)))
+    return fail(VP3D_ERR_INVALID, "wgrad_gemm: empty shape");
+  if (d->merged ? (d->taps != 1 || d->c_in_cols < d->taps_out * d->c_in)
+                : (d->taps != d->taps_out || d->c_in_cols < d->c_in))
+    return fail(VP3D_ERR_INVALID, "wgrad_gemm: taps / columns inconsistent with merged = %d", d->merged);
+  if (d->dz_ld < round_up(d->c_out, 64) || d->dz_ld % 64 || d->x_ld % 64)
+    return fail(VP3D_ERR_INVALID, "wgrad_gemm: row pitches must be multiples of 64 covering the channels");
+  WgradCall c;
+  c.dz = static_cast<const __nv_bfloat16*>(d->dz); c.dz_ld = d->dz_ld;
+  c.x = static_cast<const __nv_bfloat16*>(d->x); c.x_ld = d->x_ld;
+  c.rows = d->rows; c.per_sample = d->per_sample ? 1 : 0; c.samples = d->samples;
+  c.x_rows = d->x_rows; c.taps = d->taps; c.tap_col_step = d->tap_col_step;
+  c.tap_row_step = d->tap_row_step; c.c_out = d->c_out; c.c_in_cols = d->c_in_cols; c.c_in = d->c_in;
+  c.taps_out = d->taps_out; c.merged = d->merged ? 1 : 0; c.grad = d->grad;
+  return run_wgrad(d->planes, c, d->partial, d->partial_bytes, static_cast<cudaStream_t>(stream));
+}
+
+namespace {
+int check_reduce_scratch(const char* what, int c, int per_split, size_t scratch_floats, int counters) {
+  if (c < 1) return fail(VP3D_ERR_INVALID, "%s: channels must be positive", what);
+  if (c > kReduceMaxChannels)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: %d channels, at most %d", what, c, kReduceMaxChannels);
+  if (scratch_floats < (size_t)kReduceMaxSplits * per_split * c || counters < (c + 31) / 32)
+    return fail(VP3D_ERR_WORKSPACE, "%s: scratch of %zu floats / %d counters, %zu / %d needed", what,
+                scratch_floats, counters, (size_t)kReduceMaxSplits * per_split * c, (c + 31) / 32);
+  return VP3D_OK;
+}
+
+int check_rows_c(const char* what, long long rows, int c, int planes) {
+  if (rows < 1 || c < 64 || c % 64) return fail(VP3D_ERR_INVALID, "%s: rows >= 1 and channels a multiple of 64", what);
+  if (planes != 1 && planes != 2) return fail(VP3D_ERR_INVALID, "%s: planes must be 1 or 2", what);
+  return VP3D_OK;
+}
+
+DropoutCfg flat_drop(float p, unsigned long long seed, int layer) {
+  DropoutCfg d;
+  d.p = p;
+  d.seed_lo = (uint32_t)(seed & 0xFFFFFFFFu);
+  d.seed_hi = (uint32_t)(seed >> 32);
+  d.layer = (uint32_t)layer;
+  return d;
+}
+}  // namespace
+
+VP3D_API int vp3d_bn_stats_finalize(const float* part, int slabs, int dilated, int out_rows,
+                                    int tiles_per_sample, const float* gamma, const float* beta,
+                                    float* running_mean, float* running_var, float momentum,
+                                    float eps, float* scale, float* shift, float* mean,
+                                    float* invstd, int c, int c_real, float* scratch,
+                                    size_t scratch_floats, unsigned* counter, int counters,
+                                    void* stream) {
+  if (!part || !gamma || !beta || !scale || !shift || !mean || !invstd || !scratch || !counter ||
+      (!running_mean != !running_var))
+    return fail(VP3D_ERR_INVALID, "bn_stats_finalize: null argument");
+  if (slabs < 1 || out_rows < 1 || c_real < 1 || c_real > c || (dilated && tiles_per_sample < 1))
+    return fail(VP3D_ERR_INVALID, "bn_stats_finalize: bad geometry");
+  VP3D_TRY(check_reduce_scratch("bn_stats_finalize", c, 3, scratch_floats, counters));
+  CUDA_TRY(launch_bn_stats_finalize(part, slabs, dilated ? 1 : 0, out_rows, tiles_per_sample, gamma,
+                                    beta, running_mean, running_var, momentum, eps, scale, shift,
+                                    mean, invstd, c, c_real, scratch, counter,
+                                    static_cast<cudaStream_t>(stream)));
+  return VP3D_OK;
+}
+
+VP3D_API int vp3d_ordered_col_sums(const float* part, int n_part, int nstat, int ld, int c, int folds,
+                                   const float* mul0, const float* mul1, float* out0, float* out1,
+                                   float* scratch, size_t scratch_floats, unsigned* counter,
+                                   int counters, void* stream) {
+  if (!part || !out0 || (nstat == 2 && !out1) || !scratch || !counter)
+    return fail(VP3D_ERR_INVALID, "ordered_col_sums: null argument");
+  if (nstat < 1 || nstat > 2 || n_part < 1 || folds < 1 || ld < folds * c)
+    return fail(VP3D_ERR_INVALID, "ordered_col_sums: bad geometry");
+  VP3D_TRY(check_reduce_scratch("ordered_col_sums", c, 2, scratch_floats, counters));
+  CUDA_TRY(launch_ordered_col_sums(part, n_part, nstat, ld, c, folds, mul0, mul1, out0, out1, scratch,
+                                   counter, static_cast<cudaStream_t>(stream)));
+  return VP3D_OK;
+}
+
+VP3D_API int vp3d_bn_apply(const void* z, long long z_plane, void* x, long long x_plane, int planes,
+                           long long rows, int c, const float* scale, const float* shift,
+                           float dropout_p, unsigned long long seed, int layer, const void* res,
+                           long long res_plane, int res_div, int res_rows_per_sample, int res_step,
+                           int res_off, void* stream) {
+  if (!z || !x || !scale || !shift) return fail(VP3D_ERR_INVALID, "bn_apply: null argument");
+  VP3D_TRY(check_rows_c("bn_apply", rows, c, planes));
+  if (dropout_p < 0.0f || dropout_p >= 1.0f)
+    return fail(VP3D_ERR_INVALID, "bn_apply: dropout p must be in [0, 1)");
+  const RowMap map = {res_div, res_rows_per_sample, res_step, res_off};
+  CUDA_TRY(launch_bn_apply(static_cast<const __nv_bfloat16*>(z), z_plane,
+                           static_cast<__nv_bfloat16*>(x), x_plane, planes, rows, c, scale, shift,
+                           flat_drop(dropout_p, seed, layer), static_cast<const __nv_bfloat16*>(res),
+                           res_plane, map, static_cast<cudaStream_t>(stream)));
+  return VP3D_OK;
+}
+
+VP3D_API int vp3d_bn_bwd_reduce(const void* g, long long g_plane, const void* z, long long z_plane,
+                                int planes, long long rows, int c, const float* scale,
+                                const float* shift, const float* mean, const float* invstd,
+                                float dropout_p, unsigned long long seed, int layer, float* partials,
+                                size_t partial_floats, float* sums, float* scratch,
+                                size_t scratch_floats, unsigned* counter, int counters,
+                                void* stream) {
+  if (!g || !z || !scale || !shift || !mean || !invstd || !partials || !sums || !scratch || !counter)
+    return fail(VP3D_ERR_INVALID, "bn_bwd_reduce: null argument");
+  VP3D_TRY(check_rows_c("bn_bwd_reduce", rows, c, planes));
+  if (dropout_p < 0.0f || dropout_p >= 1.0f)
+    return fail(VP3D_ERR_INVALID, "bn_bwd_reduce: dropout p must be in [0, 1)");
+  VP3D_TRY(check_reduce_scratch("bn_bwd_reduce", c, 2, scratch_floats, counters));
+  const cudaError_t e = launch_bn_bwd_reduce(
+      static_cast<const __nv_bfloat16*>(g), g_plane, static_cast<const __nv_bfloat16*>(z), z_plane,
+      planes, rows, c, scale, shift, mean, invstd, flat_drop(dropout_p, seed, layer), partials,
+      partial_floats, sums, scratch, counter, static_cast<cudaStream_t>(stream));
+  // the one argument error of the launch: per-block partials larger than `partials` (nothing ran)
+  if (e == cudaErrorInvalidValue)
+    return fail(VP3D_ERR_WORKSPACE, "bn_bwd_reduce: %zu partial floats are too few", partial_floats);
+  CUDA_TRY(e);
+  return VP3D_OK;
+}
+
+VP3D_API int vp3d_bn_bwd_apply(const void* g, long long g_plane, const void* z, long long z_plane,
+                               void* dz, long long dz_plane, int planes, long long rows, int c,
+                               const float* scale, const float* shift, const float* mean,
+                               const float* invstd, float dropout_p, unsigned long long seed,
+                               int layer, const float* sums, float* dgamma, float* dbeta,
+                               int c_real, int frozen, void* stream) {
+  if (!g || !z || !dz || !scale || !shift || (!frozen && (!mean || !invstd || !sums)))
+    return fail(VP3D_ERR_INVALID, "bn_bwd_apply: null argument");
+  VP3D_TRY(check_rows_c("bn_bwd_apply", rows, c, planes));
+  if (dropout_p < 0.0f || dropout_p >= 1.0f)
+    return fail(VP3D_ERR_INVALID, "bn_bwd_apply: dropout p must be in [0, 1)");
+  if (c_real < 1 || c_real > c) return fail(VP3D_ERR_INVALID, "bn_bwd_apply: c_real out of range");
+  CUDA_TRY(launch_bn_bwd_apply(static_cast<const __nv_bfloat16*>(g), g_plane,
+                               static_cast<const __nv_bfloat16*>(z), z_plane,
+                               static_cast<__nv_bfloat16*>(dz), dz_plane, planes, rows, c, scale,
+                               shift, mean, invstd, flat_drop(dropout_p, seed, layer), sums, dgamma,
+                               dbeta, c_real, static_cast<cudaStream_t>(stream), frozen ? 1 : 0));
   return VP3D_OK;
 }
