@@ -215,31 +215,33 @@ def test_fused_losses_refuse_cpu_tensors():
         vloss.mpjpe(pred, pred.clone())
 
 
-def test_copies_and_replicas_never_share_engine_state():
-    """copy / deepcopy / pickle / DataParallel replicas start with empty plan stores of their own
+def test_copies_and_replicas_start_with_empty_engine_state():
+    """copy / deepcopy / pickle / DataParallel replicas start with empty engine states of their own
     (a collected copy used to destroy the original's plans), and deepcopy works after a forward
     has created ctypes handles (EMA / best-model patterns)."""
     import copy
     import pickle
-    from videopose3d_b200.temporal_model import _PlanStore
+    from videopose3d_b200.temporal_model import _EngineState
     m = vp.TemporalModelOptimized1f(17, 2, 17, [3, 3], channels=64)
     destroyed = []
-    m._plans._finalizer.detach()
-    m._plans = store = _PlanStore()
-    store._finalizer.detach()
-    store.add((0, "fp16"), _capi.ctypes.c_void_p(1234))   # what a first forward leaves behind
-    m._packed[((0, "fp16"), False)] = "versions"
+    m._engine._finalizer.detach()
+    m._engine = engine = _EngineState()
+    engine._finalizer.detach()
+    # what a first forward leaves behind
+    plan = engine.last = engine.add((0, "fp16"), _capi.ctypes.c_void_p(1234))
+    plan.eval = plan.train = plan.expand_t = "versions"
     clones = [copy.deepcopy(m), copy.copy(m), pickle.loads(pickle.dumps(m)),
               m._replicate_for_data_parallel()]
     for c in clones:
-        assert isinstance(c._plans, _PlanStore) and c._plans is not store and len(c._plans) == 0
-        assert c._packed == {} and c._plan is None
+        assert isinstance(c._engine, _EngineState) and c._engine is not engine
+        assert c._engine.plans == {} and c._plan is None
         assert sorted(c.state_dict()) == sorted(m.state_dict())
     assert torch.equal(clones[0].shrink.weight, m.shrink.weight)
     assert clones[0].shrink.weight.data_ptr() != m.shrink.weight.data_ptr()
     del clones
-    assert len(store) == 1 and destroyed == []             # the original still owns its plan
-    assert m.invalidate() is m and m._packed == {}
+    assert len(engine.plans) == 1 and destroyed == []      # the original still owns its plan
+    assert m.invalidate() is m
+    assert (plan.eval, plan.train, plan.expand_t) == (None, None, None)
 
 
 def test_training_operator_entries_validate_before_launching():

@@ -6,17 +6,19 @@ counterpart; it adds exactly one collective.  BatchNorm statistics stay per-GPU 
 "allreduce on gradients only"); `broadcast_buffers` aligns the running statistics before a
 checkpoint / evaluation, as DistributedDataParallel does.
 
-Overlap: the C backward (`vp3d_backward_staged`) reports, stage by stage, when the kernels producing
-a group of gradients have been enqueued (shrink first, expand last).  All gradients of a step live
-in one flat fp32 buffer laid out in that completion order, so each stage is a contiguous slice whose
-all-reduce is launched on a side stream behind an event while the remaining backward GEMMs run.
+Overlap: the C backward (`vp3d_backward_ex` with a stage callback) reports, stage by stage, when the
+kernels producing a group of gradients have been enqueued (shrink first, expand last).  All
+gradients of a step live in one flat fp32 buffer laid out in that completion order, so each stage is
+a contiguous slice whose all-reduce is launched on a side stream behind an event while the remaining
+backward GEMMs run.
 """
 import torch
 import torch.distributed as dist
 
 
 def stage_order(module):
-    """Parameter names grouped by backward completion stage (see vp3d_backward_staged)."""
+    """Parameter names grouped by backward completion stage (the stage callback of
+    vp3d_backward_ex)."""
     nb = len(module.layers_conv) // 2
     stages = [["shrink.weight", "shrink.bias"]]
     for i in range(nb, 0, -1):

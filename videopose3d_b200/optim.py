@@ -112,8 +112,9 @@ class FusedAdam(torch.optim.Optimizer):
                 for p, st in items:
                     ref = self._owners.get(id(p))
                     m = ref() if ref is not None else _tm.owner_of(p)
-                    if m is not None and self.fuse_repack and m._train_plan_ready(dev):
-                        by_model.setdefault(id(m), (m, []))[1].append((p, st))
+                    plan = m._packed_train_plan(dev) if m is not None and self.fuse_repack else None
+                    if plan is not None:
+                        by_model.setdefault(id(m), (m, plan, []))[2].append((p, st))
                     else:
                         plain.append((p, st))
 
@@ -135,8 +136,7 @@ class FusedAdam(torch.optim.Optimizer):
                         _capi.check(lib.vp3d_adam_step(table_of(plain), len(plain), *hyper, stream),
                                     "vp3d_adam_step")
                         self.last_launches += 1
-                    for m, rows in by_model.values():
-                        plan = m._get_plan(dev, m._train_precision)
+                    for m, plan, rows in by_model.values():
                         w = m._weights_struct()
                         _capi.check(lib.vp3d_adam_step_packed(plan, ctypes.byref(w), table_of(rows),
                                                               len(rows), *hyper, stream),
@@ -145,6 +145,6 @@ class FusedAdam(torch.optim.Optimizer):
                 for p, _ in items:
                     # the kernel wrote through raw pointers: tell autograd / the weight-pack cache
                     torch.autograd.graph.increment_version(p)
-                for m, _ in by_model.values():
-                    m._mark_train_packs_current(dev)   # after the version bumps above
+                for m, plan, _ in by_model.values():
+                    m._mark_train_packs_current(plan)   # after the version bumps above
         return loss

@@ -214,12 +214,6 @@ def _check_sequence(x, joints, features, device):
         raise RuntimeError("input and parameters are on different devices")
 
 
-def _param_versions(model):
-    conv, bn = model._param_tensors()
-    return (tuple((t.data_ptr(), t._version) for t in conv),
-            tuple((t.data_ptr(), t._version) for t in bn), model._stats_epoch)
-
-
 def check_push_input(x, streams, max_frames, joints, features):
     """The validation push() applies to x (raises like the model's forward does)."""
     if not isinstance(x, torch.Tensor):
@@ -275,25 +269,16 @@ class StreamingSession:
         self.lookahead = lookahead(model)
         self.last_predict_launches = 0   # kernels the last predict() launched
         lib = _capi.load()
+        # the model's plan of this precision (same packed eval weights as model(x))
+        self._plan = model._get_plan(device, self.precision)
         with torch.cuda.device(device):
-            self._plan = self._model_plan()
             nbytes = lib.vp3d_stream_state_bytes_ex(self._plan, streams, max_frames, self._flags)
             if nbytes == 0:
                 raise ValueError(f"{streams} streams x {max_frames} frames is too large a session")
             self._state = torch.empty(nbytes, dtype=torch.uint8, device=device)
         self._finalizer = weakref.finalize(self, _release, self._plan, self._state.data_ptr(),
-                                           model._plans)
+                                           model._engine)
         self.reset()
-
-    def _model_plan(self):
-        # the model's plan of this precision (same packed eval weights as model(x)); the model's
-        # current-plan bookkeeping is left as it was
-        m = self.model
-        saved = (m._plan, m._plan_key)
-        try:
-            return m._get_plan(self.device, self.precision)
-        finally:
-            m._plan, m._plan_key = saved
 
     def reset(self):
         """Drop all history: every slot idle, weights re-read at the next push."""
@@ -311,18 +296,13 @@ class StreamingSession:
         m = self.model
         if m.training:
             raise RuntimeError("the model is in train() mode: streaming is an eval-mode computation")
-        current = _param_versions(m)
+        current = m._versions()
         if self._versions is not None and current != self._versions:
             raise RuntimeError("the model's parameters changed since this session started; call "
                                "reset() before pushing again (old and new weights never mix)")
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        saved = (m._plan, m._plan_key)
-        try:
-            plan = m._get_plan(self.device, self.precision)
-            m._sync_weights(plan, stream)
-        finally:
-            m._plan, m._plan_key = saved
-        self._versions = _param_versions(m)
+        m._sync_weights(self._plan, stream)
+        self._versions = current
         return stream
 
     def _slot_tensor(self, v, name):
@@ -470,8 +450,8 @@ class StreamingSession:
         return _capi.load().vp3d_last_launch_count(self._plan)
 
 
-def _release(plan, state_ptr, plans):
-    # `plans` keeps the model's plan store (and with it the plan) alive until the session is gone
+def _release(plan, state_ptr, engine):
+    # `engine` keeps the model's engine state (and with it the plan) alive until the session is gone
     try:
         _capi.load().vp3d_stream_release(plan, state_ptr)
     except Exception:  # pragma: no cover - interpreter shutdown

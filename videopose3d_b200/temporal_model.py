@@ -9,6 +9,7 @@ device pointers to the sm_90a kernels behind the C ABI (``include/vp3d_b200.h``)
 There is no PyTorch/CPU execution path here: without the CUDA library or with CPU tensors
 ``forward`` raises.
 """
+import copy
 import os
 import weakref
 
@@ -36,28 +37,52 @@ def owner_of(param):
     return m
 
 
-class _PlanStore(dict):
-    """(device index, precision) -> plan handle.  Owns the handles: they are destroyed exactly once,
-    when the store itself is collected (weakref.finalize), never by a module that merely shares or
-    copies the reference.  Copies of a module start with an empty store of their own."""
+class _Plan:
+    """A plan handle and the parameter versions (``TemporalModelBase._versions``) each kind of its
+    weight packs was made from, None while never packed: ``eval`` (VP3D_PACK_CONV |
+    VP3D_PACK_BN_EVAL), ``train`` (VP3D_PACK_CONV | VP3D_PACK_CONV_T) and ``expand_t``
+    (VP3D_PACK_EXPAND_T, the expand conv weight's entry only)."""
+
+    __slots__ = ("handle", "eval", "train", "expand_t")
+
+    def __init__(self, handle):
+        self.handle = handle
+        self.eval = self.train = self.expand_t = None
+
+    @property
+    def _as_parameter_(self):
+        # ctypes passes a _Plan to the C ABI as its handle
+        return self.handle
+
+
+class _EngineState:
+    """A module's engine state: its plans by (device index, precision), the plan of its last call
+    (what ``_plan`` and ``last_launch_count`` report), the plan each host-pipeline slot was submitted
+    on, and the eval workspace.  Owns the handles: they are destroyed exactly once, when the state
+    itself is collected (weakref.finalize), never by a module that merely shares or copies the
+    reference.  Copies of a module start with an empty state of their own."""
 
     def __init__(self):
-        super().__init__()
+        self.plans = {}
+        self.last = None
+        self.host_slots = {}
+        self.workspace = None
         self._handles = []
-        self._finalizer = weakref.finalize(self, _PlanStore._destroy, self._handles)
+        self._finalizer = weakref.finalize(self, _EngineState._destroy, self._handles)
 
     def add(self, key, handle):
-        self[key] = handle
+        self.plans[key] = plan = _Plan(handle)
         self._handles.append(handle)
+        return plan
 
     def __deepcopy__(self, memo):
-        return _PlanStore()
+        return _EngineState()
 
     def __copy__(self):
-        return _PlanStore()
+        return _EngineState()
 
     def __reduce__(self):
-        return (_PlanStore, ())
+        return (_EngineState, ())
 
     @staticmethod
     def _destroy(handles):
@@ -113,14 +138,10 @@ class TemporalModelBase(nn.Module):
         self._dense = False
         self._precision = _default_precision()
         self._train_precision = os.environ.get("VP3D_TRAIN_PRECISION", "bf16")
-        self._plan = None
-        self._plan_key = None
-        self._plans = _PlanStore()
-        self._packed = {}
+        self._engine = _EngineState()
         self._stats_epoch = 0      # bumped by every training forward (running stats changed)
         self._fwd_token = 0        # identifies the most recent training forward
         self._grad_reducer = None  # data_parallel.GradientReducer, set by its attach()
-        self._workspace = None
 
     def _build_layers(self, strided):
         """Create the parameter containers with the reference's names, shapes and default init.
@@ -210,38 +231,21 @@ class TemporalModelBase(nn.Module):
     def precision(self):
         return self._precision
 
-    def _reset_engine_state(self):
-        """Forget every derived cache (plans, packed weights, workspace); the next forward rebuilds
-        them.  The plan handles themselves are released when their store is collected."""
-        self._plans = _PlanStore()
-        self._packed = {}
-        self._plan = None
-        self._plan_key = None
-        self._workspace = None
-
     def invalidate(self):
         """Force a re-pack of every parameter on the next forward.  Needed only after edits that
         bypass torch's version counters (``p.data.mul_()``, ``p.data.copy_()``, raw-pointer
         writes): ordinary in-place ops, ``optimizer.step`` and ``load_state_dict`` are detected
         automatically through ``tensor._version``.  Not in the reference."""
-        self._packed = {}
+        for plan in self._engine.plans.values():
+            plan.eval = plan.train = plan.expand_t = None
         return self
 
     # copies / replicas never share engine state with the original (the handles point into one
     # device allocation each; sharing them made a collected copy free the original's plans)
     def __deepcopy__(self, memo):
-        cls = self.__class__
-        new = cls.__new__(cls)
+        new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
-        import copy as _copy
-        skip = ("_plans", "_packed", "_plan", "_plan_key", "_workspace", "_grad_reducer")
-        for k, v in self.__dict__.items():
-            if k in skip:
-                continue
-            new.__dict__[k] = _copy.deepcopy(v, memo)
-        new._reset_engine_state()
-        new._grad_reducer = None
-        new._register_params()
+        new.__setstate__(copy.deepcopy(self.__getstate__(), memo))
         return new
 
     def __copy__(self):
@@ -251,24 +255,24 @@ class TemporalModelBase(nn.Module):
         # nn.Module.__copy__-style shallow copy of the registries
         for k in ("_parameters", "_buffers", "_modules"):
             new.__dict__[k] = self.__dict__[k].copy()
-        new._reset_engine_state()
+        new._engine = _EngineState()
         return new
 
     def __getstate__(self):
         state = self.__dict__.copy()
-        for k in ("_plans", "_packed", "_plan", "_plan_key", "_workspace", "_grad_reducer"):
-            state.pop(k, None)
+        state.pop("_engine", None)
+        state.pop("_grad_reducer", None)
         return state
 
     def __setstate__(self, state):
         super().__setstate__(state)
-        self._reset_engine_state()
+        self._engine = _EngineState()
         self._grad_reducer = None
         self._register_params()
 
     def _replicate_for_data_parallel(self):
         replica = super()._replicate_for_data_parallel()
-        replica._reset_engine_state()
+        replica._engine = _EngineState()
         return replica
 
     def _config(self, precision):
@@ -289,22 +293,32 @@ class TemporalModelBase(nn.Module):
         return cfg
 
     def _get_plan(self, device, precision=None):
-        precision = precision or self._precision
-        key = (device.index, precision)
-        plans = self.__dict__.get("_plans")
-        if plans is None:
-            plans = self._plans = _PlanStore()
-        if key not in plans:
+        """The _Plan of `precision` (default: the eval precision) on `device`, created on first use.
+        A lookup: which plan ``_plan`` reports does not change."""
+        key = (device.index, precision or self._precision)
+        plan = self._engine.plans.get(key)
+        if plan is None:
             lib = _capi.load()
             handle = _capi.ctypes.c_void_p()
-            cfg = self._config(precision)
+            cfg = self._config(key[1])
             with torch.cuda.device(device):
                 _capi.check(lib.vp3d_plan_create(_capi.ctypes.byref(cfg), _capi.ctypes.byref(handle)),
                             "vp3d_plan_create")
-            plans.add(key, handle)
-        self._plan = plans[key]
-        self._plan_key = key
-        return plans[key]
+            plan = self._engine.add(key, handle)
+        return plan
+
+    def _use_plan(self, device, precision):
+        """_get_plan for a call that runs on the plan: it becomes the plan ``_plan`` and
+        ``last_launch_count`` report."""
+        plan = self._engine.last = self._get_plan(device, precision)
+        return plan
+
+    @property
+    def _plan(self):
+        """Handle of the plan of the module's last forward, eval-mode backward or fused optimizer
+        step (None before the first)."""
+        last = self._engine.last
+        return None if last is None else last.handle
 
     def _param_tensors(self):
         """All fp32 tensors of the state_dict in the order of ``vp3d_weights``."""
@@ -331,16 +345,20 @@ class TemporalModelBase(nn.Module):
         w.shrink_bias = self.shrink.bias.data_ptr()
         return w
 
-    def _sync_weights(self, plan, stream, training=False):
-        """Re-pack whatever changed since this plan last saw the parameters (optimizer.step,
-        load_state_dict, in-place edits; the training kernels' running-stat updates are tracked
-        through ``_stats_epoch`` because they bypass torch's version counters)."""
+    def _versions(self):
+        """What the packs are made from: ((data pointer, ``_version``) of every conv weight, the
+        same of every BatchNorm / bias tensor followed by ``_stats_epoch``), tensors in the order of
+        ``_param_tensors``.  The training kernels' running-stat updates are tracked through
+        ``_stats_epoch`` because they bypass torch's version counters."""
         conv, bn = self._param_tensors()
-        versions = (tuple((t.data_ptr(), t._version) for t in conv),
-                    tuple((t.data_ptr(), t._version) for t in bn) + (self._stats_epoch,))
-        packed = self.__dict__.setdefault("_packed", {})
-        key = (self._plan_key, training)
-        seen = packed.get(key)
+        return (tuple((t.data_ptr(), t._version) for t in conv),
+                tuple((t.data_ptr(), t._version) for t in bn) + (self._stats_epoch,))
+
+    def _sync_weights(self, plan, stream, training=False):
+        """Re-pack whatever changed since `plan`'s eval (or training) packs last saw the parameters
+        (optimizer.step, load_state_dict, in-place edits).  Returns whether it packed."""
+        versions = self._versions()
+        seen = plan.train if training else plan.eval
         what = 0
         if seen is None or seen[0] != versions[0]:
             what |= _capi.VP3D_PACK_CONV
@@ -349,46 +367,47 @@ class TemporalModelBase(nn.Module):
         if not training and (seen is None or seen[1] != versions[1]):
             what |= _capi.VP3D_PACK_BN_EVAL
         if not what:
-            return
+            return False
+        conv, bn = self._param_tensors()
         for t in conv + bn:
             if t.dtype != torch.float32 or not t.is_contiguous():
                 raise RuntimeError("parameters must be contiguous float32 tensors")
         w = self._weights_struct()
         _capi.check(_capi.load().vp3d_set_weights(plan, _capi.ctypes.byref(w), what, stream),
                     "vp3d_set_weights")
-        packed[key] = versions
+        if training:
+            plan.train = versions
+        else:
+            plan.eval = versions
+        return True
 
-    # -- hooks for optim.FusedAdam.attach (update + re-pack in one kernel) ---------------------------
-    def _train_plan_ready(self, device):
-        """True when the training plan on `device` already holds packed weights (i.e. a training
-        forward has run): only then can the fused optimizer keep them current."""
-        key = ((device.index, self._train_precision), True)
-        return self.__dict__.get("_packed", {}).get(key) is not None
+    # -- hooks for optim.FusedAdam (update + re-pack in one kernel) -----------------------------------
+    def _packed_train_plan(self, device):
+        """The training plan on `device` if it already holds packed weights (i.e. a training forward
+        has run), else None: only such a plan can the fused optimizer keep current."""
+        plan = self._engine.plans.get((device.index, self._train_precision))
+        return plan if plan is not None and plan.train is not None else None
 
-    def _mark_train_packs_current(self, device):
-        """The fused optimizer step has just re-packed every conv weight of the training plan:
-        record the parameters' new versions so that the next forward does not pack again."""
-        conv, bn = self._param_tensors()
-        versions = (tuple((t.data_ptr(), t._version) for t in conv),
-                    tuple((t.data_ptr(), t._version) for t in bn) + (self._stats_epoch,))
-        self._packed[((device.index, self._train_precision), True)] = versions
+    def _mark_train_packs_current(self, plan):
+        """The fused optimizer step has just re-packed every conv weight of the training plan `plan`:
+        record the parameters' new versions so that the next forward does not pack again.  The step
+        ran on the plan, so it is the one ``last_launch_count`` reports."""
+        plan.train = self._versions()
+        self._engine.last = plan
 
     def _sync_expand_t(self, plan, stream):
         """Pack the transposed expand conv for the input gradient when expand_conv.weight changed
-        since this plan last packed it.  Only input-gradient backwards call this, and nothing else
+        since `plan` last packed it.  Only input-gradient backwards call this, and nothing else
         marks the pack current (the fused optimizer step does not refresh it), so a version bump
         of the weight always leads to a re-pack here."""
-        wt = self.expand_conv.weight
-        key = (self._plan_key, "expand_t")
-        seen = (wt.data_ptr(), wt._version)
-        packed = self.__dict__.setdefault("_packed", {})
-        if packed.get(key) == seen:
+        seen = self._versions()[0][0]   # expand_conv.weight
+        if plan.expand_t == seen:
             return
         w = self._weights_struct()
         _capi.check(_capi.load().vp3d_set_weights(plan, _capi.ctypes.byref(w),
                                                    _capi.VP3D_PACK_EXPAND_T, stream),
                     "vp3d_set_weights")
-        packed[key] = seen
+        plan.expand_t = seen
 
     def _grads_struct(self, grads):
         """vp3d_grads over `grads`, tensors in the order of ``_learnable_tensors``."""
@@ -406,11 +425,11 @@ class TemporalModelBase(nn.Module):
         return g
 
     def _get_workspace(self, nbytes, device):
-        ws = self._workspace
+        ws = self._engine.workspace
         if ws is None or ws.device != device or ws.numel() < nbytes:
-            self._workspace = None
+            self._engine.workspace = None
             ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-            self._workspace = ws
+            self._engine.workspace = ws
         return ws
 
     # ------------------------------------------------------------------ forward
@@ -446,7 +465,7 @@ class TemporalModelBase(nn.Module):
         device = x.device
         N, T = int(x.shape[0]), int(x.shape[1])
         with torch.cuda.device(device):
-            plan = self._get_plan(device)
+            plan = self._use_plan(device, self._precision)
             stream = torch.cuda.current_stream(device).cuda_stream
             self._sync_weights(plan, stream)
             t_out = lib.vp3d_output_frames(plan, T)
@@ -505,7 +524,7 @@ class TemporalModelBase(nn.Module):
             raise RuntimeError("module parameters must be on a CUDA device")
         N, T = int(x_host.shape[0]), int(x_host.shape[1])
         with torch.cuda.device(device):
-            plan = self._get_plan(device)
+            plan = self._use_plan(device, self._precision)
             stream = torch.cuda.current_stream(device)
             self._sync_weights(plan, stream.cuda_stream)
             stream.synchronize()  # packed weights are read by the plan's own stream
@@ -534,19 +553,21 @@ class TemporalModelBase(nn.Module):
         device = self.expand_conv.weight.device
         N, T = int(x_host.shape[0]), int(x_host.shape[1])
         with torch.cuda.device(device):
-            plan = self._get_plan(device)
+            plan = self._use_plan(device, self._precision)
             stream = torch.cuda.current_stream(device)
-            before = self._packed.get((self._plan_key, False))
-            self._sync_weights(plan, stream.cuda_stream)
-            if self._packed.get((self._plan_key, False)) is not before:
+            if self._sync_weights(plan, stream.cuda_stream):
                 stream.synchronize()  # freshly packed weights are read by the plan's own stream
             _capi.check(lib.vp3d_forward_eval_host_submit(plan, x_host.data_ptr(), out.data_ptr(), N,
                                                           T, int(slot)),
                         "vp3d_forward_eval_host_submit")
+        self._engine.host_slots[int(slot)] = plan
         return out
 
     def forward_host_wait(self, slot):
-        _capi.check(_capi.load().vp3d_forward_eval_host_wait(self._plan, int(slot)),
+        """Block until the batch submitted on `slot` is in its `out`, on the plan it was submitted
+        on (calls at other precisions in between do not matter)."""
+        plan = self._engine.host_slots.pop(int(slot), self._engine.last)
+        _capi.check(_capi.load().vp3d_forward_eval_host_wait(plan, int(slot)),
                     "vp3d_forward_eval_host_wait")
 
     def last_launch_count(self):
@@ -564,41 +585,95 @@ class TemporalModelBase(nn.Module):
                                 joints_right=joints_right)
 
 
+def _train_forward(module, plan, x, stream, momenta=None, p_drop=0.0, seed=0, flags=0):
+    """vp3d_forward_train_ex of `module` on `plan` (training packs current); returns y and the
+    workspace that holds the activations its backward reads."""
+    lib = _capi.load()
+    N, T = int(x.shape[0]), int(x.shape[1])
+    t_out = lib.vp3d_output_frames(plan, T)
+    nbytes = lib.vp3d_train_workspace_bytes(plan, N, T)
+    if t_out < 1 or nbytes == 0:
+        raise ValueError(f"input of {T} frames is shorter than the receptive field "
+                         f"({module.receptive_field()})")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    y = torch.empty((N, t_out, module.num_joints_out, 3), dtype=torch.float32, device=x.device)
+    w = module._weights_struct()
+    _capi.check(lib.vp3d_forward_train_ex(plan, x.data_ptr(), y.data_ptr(), N, T,
+                                          _capi.ctypes.byref(w), momenta, p_drop, seed, flags,
+                                          ws.data_ptr(), ws.numel(), stream),
+                "vp3d_forward_train_ex")
+    return y, ws
+
+
+def _backward(module, plan, ws, dy, stream, want_x, dx_shape, want_p, shapes, reducer=None):
+    """The vp3d_backward_ex call of both autograd functions, after a _train_forward on `plan`.
+
+    Parameter gradients, when any is wanted, go to one tensor each, or with a data-parallel
+    `reducer` to its flat buffer, whose stages the stage callback all-reduces while the later
+    stages still compute; dL/dx, when wanted, to a new `dx_shape` tensor.  Returns dx (or None) and
+    the gradients in the order of ``_learnable_tensors``, None for those not wanted."""
+    device = dy.device
+    grads = flat = cb = g = None
+    errors = []
+    if any(want_p):
+        if reducer is not None:
+            # one flat buffer laid out in backward-completion order: each stage is a contiguous
+            # slice that is all-reduced on a side stream while later stages are still computing
+            _, spans, stage_spans, total = reducer.plan_layout(module)
+            flat = torch.empty(total, dtype=torch.float32, device=device)
+            grads = [flat[spans[n][0]: spans[n][0] + spans[n][1]].view(s)
+                     for n, s in zip(module._learnable_names(), shapes)]
+
+            def _stage(stage, _user):
+                try:
+                    lo, hi = stage_spans[stage]
+                    reducer.stage_ready(flat, lo, hi)
+                except Exception as e:  # never raise through the C frame
+                    errors.append(e)
+
+            cb = _capi.STAGE_FN(_stage)
+        else:
+            grads = [torch.empty(s, dtype=torch.float32, device=device) for s in shapes]
+        g = module._grads_struct(grads)
+    dx = torch.empty(dx_shape, dtype=torch.float32, device=device) if want_x else None
+    _capi.check(_capi.load().vp3d_backward_ex(
+        plan, dy.data_ptr(), None if g is None else _capi.ctypes.byref(g),
+        None if dx is None else dx.data_ptr(), ws.data_ptr(), ws.numel(), stream,
+        None if cb is None else _capi.ctypes.cast(cb, _capi.ctypes.c_void_p), None),
+        "vp3d_backward_ex")
+    if errors:
+        raise errors[0]
+    if flat is not None:
+        reducer.finish(flat)
+    if grads is None:
+        return dx, (None,) * len(want_p)
+    return dx, tuple(gr if w else None for gr, w in zip(grads, want_p))
+
+
 class _TrainFunction(torch.autograd.Function):
-    """Training-mode forward/backward through the C ABI (vp3d_forward_train / vp3d_backward).
+    """Training-mode forward/backward through the C ABI (vp3d_forward_train_ex with flags 0 /
+    vp3d_backward_ex).
 
     The learnable tensors are passed as inputs so that autograd accumulates the returned
     gradients into ``.grad`` exactly as it does for the reference's nn modules.  dL/dx is computed
-    when x requires grad (vp3d_backward_ex with the expand conv's data gradient); parameter
-    gradients are skipped when no learnable tensor requires grad."""
+    when x requires grad (the expand conv's data gradient); parameter gradients are skipped when no
+    learnable tensor requires grad.  With a data-parallel reducer of more than one rank attached,
+    the backward's stage callback all-reduces the gradients while it runs."""
 
     @staticmethod
     def forward(ctx, module, x, *params):
-        lib = _capi.load()
         device = x.device
-        N, T = int(x.shape[0]), int(x.shape[1])
         momenta = [module.expand_bn.momentum] + [bn.momentum for bn in module.layers_bn]
         if any(m is None for m in momenta):
             raise NotImplementedError("BatchNorm momentum=None (cumulative average) is not supported")
         p_drop = float(module.drop.p)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())  # CPU generator: torch.manual_seed applies
         with torch.cuda.device(device):
-            plan = module._get_plan(device, module._train_precision)
+            plan = module._use_plan(device, module._train_precision)
             stream = torch.cuda.current_stream(device).cuda_stream
             module._sync_weights(plan, stream, training=True)
-            t_out = lib.vp3d_output_frames(plan, T)
-            nbytes = lib.vp3d_train_workspace_bytes(plan, N, T)
-            if t_out < 1 or nbytes == 0:
-                raise ValueError(f"input of {T} frames is shorter than the receptive field "
-                                 f"({module.receptive_field()})")
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-            y = torch.empty((N, t_out, module.num_joints_out, 3), dtype=torch.float32, device=device)
-            w = module._weights_struct()
             mom = (_capi.ctypes.c_float * len(momenta))(*[float(m) for m in momenta])
-            _capi.check(lib.vp3d_forward_train(plan, x.data_ptr(), y.data_ptr(), N, T,
-                                               _capi.ctypes.byref(w), mom, p_drop, seed,
-                                               ws.data_ptr(), ws.numel(), stream),
-                        "vp3d_forward_train")
+            y, ws = _train_forward(module, plan, x, stream, mom, p_drop, seed)
         # nn.BatchNorm1d bookkeeping that lives outside the kernels
         with torch.no_grad():
             module.expand_bn.num_batches_tracked += 1
@@ -621,115 +696,19 @@ class _TrainFunction(torch.autograd.Function):
         if ctx.token != module._fwd_token:
             raise RuntimeError("only the most recent training forward of a module can be "
                                "back-propagated (one forward per backward, as in run.py)")
-        lib = _capi.load()
-        device = ctx.device
         dy = dy.contiguous().float()
-        names = [n for n, _ in module.named_parameters()]
-        order = module._learnable_names()
         want_x = ctx.needs_input_grad[1]
-        want_p = ctx.needs_input_grad[2:]
-        if want_x or not any(want_p):
-            return _TrainFunction._backward_ex(ctx, dy, want_x, want_p)
         reducer = getattr(module, "_grad_reducer", None)
-        if reducer is not None and reducer.world > 1:
-            # one flat buffer laid out in backward-completion order: each stage is a contiguous
-            # slice that is all-reduced on a side stream while later stages are still computing
-            _, spans, stage_spans, total = reducer.plan_layout(module)
-            flat = torch.empty(total, dtype=torch.float32, device=device)
-            by_name = {n: flat[spans[n][0]: spans[n][0] + spans[n][1]] for n in spans}
-            grads = [by_name[n].view(s) for n, s in zip(order, ctx.shapes)]
-        else:
-            flat, stage_spans = None, None
-            grads = [torch.empty(s, dtype=torch.float32, device=device) for s in ctx.shapes]
-        nb2 = len(module.layers_conv)
-        g = _capi.Grads()
-        g.expand_conv_weight = grads[0].data_ptr()
-        g.expand_bn[0] = grads[1].data_ptr()
-        g.expand_bn[1] = grads[2].data_ptr()
-        for i in range(nb2):
-            g.layers_conv_weight[i] = grads[3 + i].data_ptr()
-            g.layers_bn[i][0] = grads[3 + nb2 + 2 * i].data_ptr()
-            g.layers_bn[i][1] = grads[3 + nb2 + 2 * i + 1].data_ptr()
-        g.shrink_weight = grads[3 + 3 * nb2].data_ptr()
-        g.shrink_bias = grads[3 + 3 * nb2 + 1].data_ptr()
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if flat is None:
-                _capi.check(lib.vp3d_backward(ctx.plan, dy.data_ptr(), _capi.ctypes.byref(g),
-                                              ctx.ws.data_ptr(), ctx.ws.numel(), stream),
-                            "vp3d_backward")
-            else:
-                errors = []
-
-                def _stage(stage, _user):
-                    try:
-                        lo, hi = stage_spans[stage]
-                        reducer.stage_ready(flat, lo, hi)
-                    except Exception as e:  # never raise through the C frame
-                        errors.append(e)
-
-                cb = _capi.STAGE_FN(_stage)
-                _capi.check(lib.vp3d_backward_staged(ctx.plan, dy.data_ptr(), _capi.ctypes.byref(g),
-                                                     ctx.ws.data_ptr(), ctx.ws.numel(), stream,
-                                                     _capi.ctypes.cast(cb, _capi.ctypes.c_void_p),
-                                                     None), "vp3d_backward_staged")
-                if errors:
-                    raise errors[0]
-                reducer.finish(flat)
-        del names
-        ctx.ws = None
-        return (None, None) + tuple(grads)
-
-    @staticmethod
-    def _backward_ex(ctx, dy, want_x, want_p):
-        """vp3d_backward_ex: the input gradient and / or the parameter gradients (None for those
-        not wanted; with no parameter requiring grad no weight gradient is computed at all)."""
-        module = ctx.module
-        lib = _capi.load()
-        device = ctx.device
-        reducer = getattr(module, "_grad_reducer", None)
-        flat, stage_spans = None, None
-        grads = None
-        if any(want_p):
-            if reducer is not None and reducer.world > 1:
-                _, spans, stage_spans, total = reducer.plan_layout(module)
-                flat = torch.empty(total, dtype=torch.float32, device=device)
-                by_name = {n: flat[spans[n][0]: spans[n][0] + spans[n][1]] for n in spans}
-                grads = [by_name[n].view(s) for n, s in zip(module._learnable_names(), ctx.shapes)]
-            else:
-                grads = [torch.empty(s, dtype=torch.float32, device=device) for s in ctx.shapes]
-        dx = torch.empty(ctx.x_shape, dtype=torch.float32, device=device) if want_x else None
-        g = module._grads_struct(grads) if grads is not None else None
-        errors = []
-
-        def _stage(stage, _user):
-            try:
-                lo, hi = stage_spans[stage]
-                reducer.stage_ready(flat, lo, hi)
-            except Exception as e:  # never raise through the C frame
-                errors.append(e)
-
-        cb = _capi.STAGE_FN(_stage) if flat is not None else None
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
+        if reducer is not None and reducer.world <= 1:
+            reducer = None
+        with torch.cuda.device(ctx.device):
+            stream = torch.cuda.current_stream(ctx.device).cuda_stream
             if want_x:
                 module._sync_expand_t(ctx.plan, stream)
-            _capi.check(lib.vp3d_backward_ex(ctx.plan, dy.data_ptr(),
-                                             _capi.ctypes.byref(g) if g is not None else None,
-                                             dx.data_ptr() if dx is not None else None,
-                                             ctx.ws.data_ptr(), ctx.ws.numel(), stream,
-                                             _capi.ctypes.cast(cb, _capi.ctypes.c_void_p)
-                                             if cb is not None else None, None),
-                        "vp3d_backward_ex")
-            if errors:
-                raise errors[0]
-            if flat is not None:
-                reducer.finish(flat)
+            dx, grads = _backward(module, ctx.plan, ctx.ws, dy, stream, want_x,
+                                  ctx.x_shape, ctx.needs_input_grad[2:], ctx.shapes, reducer)
         ctx.ws = None
-        out = [None] * len(want_p)
-        if grads is not None:
-            out = [gr if w else None for gr, w in zip(grads, want_p)]
-        return (None, dx) + tuple(out)
+        return (None, dx) + grads
 
 
 class _EvalFunction(torch.autograd.Function):
@@ -754,57 +733,35 @@ class _EvalFunction(torch.autograd.Function):
         module = ctx.module
         x = ctx.saved_tensors[0]     # (raises if x or a parameter was modified in place since)
         want_x = ctx.needs_input_grad[1]
-        want_p = ctx.needs_input_grad[2:]
-        lib = _capi.load()
-        device = x.device
-        N, T = int(x.shape[0]), int(x.shape[1])
         dy = dy.contiguous().float()
+        device = x.device
+        T = int(x.shape[1])
         with torch.cuda.device(device):
-            plan = module._get_plan(device, module._train_precision)
+            plan = module._use_plan(device, module._train_precision)
             stream = torch.cuda.current_stream(device).cuda_stream
             module._sync_weights(plan, stream, training=True)
             if want_x:
                 module._sync_expand_t(plan, stream)
-            t_out = lib.vp3d_output_frames(plan, T)
             t_used = T
             if module._variant == _capi.VP3D_VARIANT_STRIDED:
                 # the strided convs ignore trailing frames: recompute on the prefix the output
                 # depends on (exact under frozen BatchNorm, whose affine does not see the batch)
-                t_used = t_out
+                t_used = _capi.load().vp3d_output_frames(plan, T)
                 for w in module.filter_widths:
                     t_used *= int(w)
             xs = x if t_used == T else x[:, :t_used].contiguous()
-            nbytes = lib.vp3d_train_workspace_bytes(plan, N, t_used)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-            y = torch.empty((N, t_out, module.num_joints_out, 3), dtype=torch.float32, device=device)
-            w = module._weights_struct()
-            _capi.check(lib.vp3d_forward_train_ex(plan, xs.data_ptr(), y.data_ptr(), N, t_used,
-                                                  _capi.ctypes.byref(w), None, 0.0, 0,
-                                                  _capi.VP3D_TRAIN_FROZEN_BN, ws.data_ptr(),
-                                                  ws.numel(), stream), "vp3d_forward_train_ex")
+            _, ws = _train_forward(module, plan, xs, stream, flags=_capi.VP3D_TRAIN_FROZEN_BN)
             # the recompute replaced the plan's saved training state: a pending train-mode
             # backward of this module must now fail instead of reading it
             module._fwd_token += 1
-            grads = None
-            if any(want_p):
-                grads = [torch.empty(p.shape, dtype=torch.float32, device=device)
-                         for p in ctx.saved_tensors[1:]]
-            dx = torch.empty((N, t_used) + tuple(x.shape[2:]), dtype=torch.float32,
-                             device=device) if want_x else None
-            g = module._grads_struct(grads) if grads is not None else None
-            _capi.check(lib.vp3d_backward_ex(plan, dy.data_ptr(),
-                                             _capi.ctypes.byref(g) if g is not None else None,
-                                             dx.data_ptr() if dx is not None else None,
-                                             ws.data_ptr(), ws.numel(), stream, None, None),
-                        "vp3d_backward_ex")
+            dx, grads = _backward(module, plan, ws, dy, stream, want_x,
+                                  tuple(xs.shape), ctx.needs_input_grad[2:],
+                                  [p.shape for p in ctx.saved_tensors[1:]])
         if dx is not None and t_used != T:
             full = torch.zeros(x.shape, dtype=torch.float32, device=device)
             full[:, :t_used] = dx
             dx = full
-        out = [None] * len(want_p)
-        if grads is not None:
-            out = [gr if w else None for gr, w in zip(grads, want_p)]
-        return (None, dx) + tuple(out)
+        return (None, dx) + grads
 
 
 class TemporalModel(TemporalModelBase):
