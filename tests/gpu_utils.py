@@ -35,15 +35,22 @@ def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_
               res_sample_div=0, res_col_begin=0, res_cols=0, res_check_rows=0, out_planes=1,
               out_f32_cols=None, stats=None, bnb_z=None, bnb_scale=None, bnb_shift=None,
               bnb_mean=None, bnb_invstd=None, bnb_sums=None, bnb_c=0, bnb_p=0.0, bnb_seed=0,
-              bnb_layer=0):
+              bnb_layer=0, out=None, out_f32=None, out_plane_stride=0, a_plane_stride=0,
+              lo_row_begin=0, lo_row_end=0):
     """Launch vp3d_conv_gemm; returns (out_bf16_planes or None, out_f32 or None).
     bnb_*: the fused BatchNorm-backward reductions (see vp3d_conv_desc); bnb_z is a bf16 tensor
-    with the output's [rows][n_pad] view, the vectors fp32 [bnb_c], bnb_sums fp32 [slabs][2][n_pad]."""
+    with the output's [rows][n_pad] view, the vectors fp32 [bnb_c], bnb_sums fp32 [slabs][2][n_pad].
+    out / out_f32: caller-owned outputs ([planes][rows][ld] 16-bit, or [rows][ld] fp32, ld = the
+    row pitch); they are filled with NaN before the launch, like the ones allocated here, so that
+    whatever the kernel leaves unwritten (a lo plane outside [lo_row_begin, lo_row_end)) reads NaN.
+    out_plane_stride / a_plane_stride: 0 = the planes are contiguous."""
     lib = _capi.load()
     dev = a_planes_t.device
     total_rows = samples * out_rows if per_sample_tiles else out_rows
     d = _capi.ConvDesc()
     d.a = a_planes_t.data_ptr(); d.a_planes = a_planes_t.shape[0]
+    d.a_plane_stride = a_plane_stride
+    d.lo_row_begin = lo_row_begin; d.lo_row_end = lo_row_end
     d.samples = samples; d.a_rows = a_rows; d.a_ld = a_ld
     d.w = w_planes_t.data_ptr(); d.taps = taps; d.k_per_tap = k_per_tap; d.n_pad = n_pad
     d.per_sample_tiles = int(per_sample_tiles); d.tap_row_step = tap_row_step
@@ -64,8 +71,16 @@ def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_
         d.bnb_mean = bnb_mean.data_ptr(); d.bnb_invstd = bnb_invstd.data_ptr()
         d.bnb_sums = bnb_sums.data_ptr(); d.bnb_c = bnb_c; d.bnb_p = bnb_p
         d.bnb_seed = bnb_seed; d.bnb_layer = bnb_layer
-    out = out32 = None
-    if out_f32_cols is None:
+    out32 = out_f32
+    if out is not None:
+        out.fill_(float("nan"))
+        d.out = out.data_ptr(); d.out_planes = out.shape[0]
+        d.out_plane_stride = out_plane_stride or out[0].numel(); d.out_ld = out.shape[-1]
+    elif out32 is not None:
+        out32.fill_(float("nan"))
+        d.out_f32 = out32.data_ptr(); d.out_f32_ld = out32.shape[-1]
+        d.n_valid = out_f32_cols or out32.shape[-1]
+    elif out_f32_cols is None:
         out = torch.full((out_planes, total_rows, n_pad), float("nan"),
                          dtype=torch.float16 if precision == 3 else torch.bfloat16, device=dev)
         d.out = out.data_ptr(); d.out_planes = out_planes; d.out_plane_stride = out[0].numel()
