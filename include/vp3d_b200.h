@@ -211,6 +211,33 @@ int vp3d_backward_ex(vp3d_plan* plan, const float* dy, const vp3d_grads* grads, 
                      void* workspace, size_t workspace_bytes, void* stream, vp3d_stage_fn stage_done,
                      void* user);
 
+/* Synchronized BatchNorm for data-parallel training over `world` ranks (replaces
+ * nn.SyncBatchNorm / convert_sync_batchnorm for this model; no reference counterpart: the reference
+ * is single-GPU).  Every following vp3d_forward_train_ex without VP3D_TRAIN_FROZEN_BN, and the
+ * vp3d_backward_ex that matches it (the forward's setting is kept for it), then take each training
+ * BatchNorm's statistics over the rows of all ranks:
+ *   forward: per BatchNorm l = 0 (expand_bn), 1.. 2B (layers_bn[l-1]) this rank writes its
+ *     per-channel (n, mean, M2) into slot `rank` of slots [world][3][C] (C = channels, the other
+ *     slots zero) and calls exchange(l, VP3D_BN_SYNC_FORWARD, slots, 3 * C, user); the slots are
+ *     merged in rank order 0..world-1 and batch mean, variance and the running-statistics update
+ *     (unbiased over the global row count) follow from the merged moments.
+ *   backward: the same with [world][2][C] slots holding this rank's sum dY and invstd * sum dY (z -
+ *     mean), VP3D_BN_SYNC_BACKWARD; dZ uses the rank-ordered sum over ranks and the global row
+ *     count, d weight / d bias this rank's own sums (averaging them over ranks, as the gradient
+ *     all-reduce does, gives the global-batch gradient, as nn.SyncBatchNorm computes it).
+ * exchange runs on the host once the kernel writing this rank's slot is enqueued on the call's
+ * stream; before it returns it must enqueue on that stream an operation that fills every rank's
+ * slot (an element-wise sum of the ranks' zero-padded buffers is exact).  It cannot fail the call:
+ * a host records its own errors, as with vp3d_stage_fn.  The slot buffers belong to the plan; the
+ * workspace sizes do not change.  world = 0 switches synchronisation off (exchange may be NULL);
+ * world = 1 runs the synchronized kernels with one slot and gives the unsynchronized results bit
+ * for bit. */
+#define VP3D_BN_SYNC_FORWARD 0
+#define VP3D_BN_SYNC_BACKWARD 1
+typedef void (*vp3d_bn_exchange_fn)(int layer, int phase, float* slots, int floats_per_rank,
+                                    void* user);
+int vp3d_set_bn_sync(vp3d_plan* plan, int world, int rank, vp3d_bn_exchange_fn exchange, void* user);
+
 /* Number of kernels the last forward on this plan launched (for bench.py's gpu_launches). */
 int vp3d_last_launch_count(const vp3d_plan* plan);
 

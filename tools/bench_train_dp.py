@@ -9,10 +9,16 @@ Adam(amsgrad), one process per GPU over NCCL.
 Rank 0 prints one JSON line: total frames/s (max over ranks of the CUDA-event time), per-step ms,
 and — with --check — the maximum difference between the averaged gradients and a reference average
 computed with a plain all_reduce of per-rank gradients (parity of the staged / overlapped path).
+
+--sync-bn: the step with and without synchronized BatchNorm (GradientReducer(sync_bn=...)),
+alternated --rounds times in one run, with the forward / backward launch counts of each and the
+card's name and power limit.  Also runs on one GPU, where it measures the cost of the synchronized
+kernels alone (one rank: the exchange moves nothing).
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -32,6 +38,8 @@ def main():
     ap.add_argument("--no-overlap", action="store_true")
     ap.add_argument("--check", action="store_true")
     ap.add_argument("--precision", default="bf16")
+    ap.add_argument("--sync-bn", action="store_true")
+    ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -49,6 +57,10 @@ def main():
     g = torch.Generator().manual_seed(1000 + rank)  # each rank its own batches
     x = (torch.rand(N, T, J, F, generator=g) * 2 - 1).to(dev)
     tgt = (torch.randn(N, 1, J, 3, generator=g) * 0.3).to(dev)
+
+    if args.sync_bn:
+        sync_bn_compare(args, m, opt, x, tgt, world, rank, dev)
+        return
 
     check = None
     if args.check and world > 1:
@@ -106,6 +118,68 @@ def main():
             "frames_per_s": N * world * args.steps / (total_ms * 1e-3), "scaling": "weak",
             "grad_allreduce_mb": sum(p.numel() for p in m.parameters()) * 4 / 1e6,
             "staged_vs_plain_allreduce_max_rel": check, "final_loss": float(loss.detach()),
+        }), flush=True)
+    if world > 1:
+        dist.barrier()
+        dist.destroy_process_group()
+
+
+def card():
+    """Name and power limit of the current GPU (read-only query)."""
+    info = {"gpu": torch.cuda.get_device_name()}
+    try:
+        idx = str(torch.cuda.current_device())
+        out = subprocess.run(["nvidia-smi", "-i", idx, "--query-gpu=power.limit",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        info["power_limit"] = out.stdout.strip() or None
+    except (OSError, subprocess.SubprocessError):
+        info["power_limit"] = None
+    return info
+
+
+def sync_bn_compare(args, m, opt, x, tgt, world, rank, dev):
+    reducers = {False: vp.GradientReducer(overlap=not args.no_overlap),
+                True: vp.GradientReducer(overlap=not args.no_overlap, sync_bn=True)}
+    times = {False: [], True: []}
+    launches = {}
+
+    def step():
+        opt.zero_grad()
+        loss = torch.mean(torch.norm(m(x) - tgt, dim=-1))
+        fwd = m.last_launch_count()
+        loss.backward()
+        bwd = m.last_launch_count()
+        opt.step()
+        return fwd, bwd
+
+    for _ in range(args.rounds):
+        for sync in (False, True):
+            reducers[sync].attach(m)
+            for _ in range(args.warmup):
+                launches[sync] = step()
+            if world > 1:
+                dist.barrier()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.steps):
+                step()
+            e1.record()
+            torch.cuda.synchronize()
+            ms = torch.tensor([e0.elapsed_time(e1) / args.steps], dtype=torch.float64, device=dev)
+            if world > 1:
+                dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+            times[sync].append(float(ms[0]))
+    if rank == 0:
+        med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+        print(json.dumps({
+            "what": "train_step_dp_sync_bn", "n_gpus": world, "precision": args.precision,
+            "overlap": not args.no_overlap, "n_per_rank": N, **card(),
+            "ms_per_step": {"plain": med[False], "sync_bn": med[True]},
+            "ms_per_step_rounds": {"plain": times[False], "sync_bn": times[True]},
+            "sync_bn_overhead": med[True] / med[False] - 1.0,
+            "launches_fwd_bwd": {"plain": launches[False], "sync_bn": launches[True]},
+            "bn_exchanges_per_step": reducers[True].exchanges // (args.rounds * (args.warmup + args.steps)),
         }), flush=True)
     if world > 1:
         dist.barrier()

@@ -22,6 +22,7 @@ VP3D_PACK_BN_EVAL = 2
 VP3D_PACK_CONV_T = 4
 VP3D_PACK_EXPAND_T = 8
 VP3D_TRAIN_FROZEN_BN = 1
+VP3D_BN_SYNC_FORWARD, VP3D_BN_SYNC_BACKWARD = 0, 1
 VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
@@ -34,6 +35,9 @@ _LIB_PATH = os.environ.get("VP3D_LIB_PATH", _LIB_PATH)
 
 c_float_p = ctypes.POINTER(ctypes.c_float)
 STAGE_FN = ctypes.CFUNCTYPE(None, ctypes.c_int, ctypes.c_void_p)
+# vp3d_bn_exchange_fn(layer, phase, slots, floats_per_rank, user)
+BN_EXCHANGE_FN = ctypes.CFUNCTYPE(None, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                  ctypes.c_void_p)
 
 
 class Config(ctypes.Structure):
@@ -226,6 +230,8 @@ SIGNATURES = {
     "vp3d_backward_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Grads),
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_set_bn_sync": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                        ctypes.c_void_p]),
     "vp3d_last_launch_count": (ctypes.c_int, [ctypes.c_void_p]),
     "vp3d_profile_launch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "vp3d_profile_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),

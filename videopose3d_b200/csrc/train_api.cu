@@ -51,12 +51,25 @@ struct TrainState {
   uint64_t seed = 0;
   bool frozen_bn = false;
   bool have_forward = false;
+  // synchronized BatchNorm (vp3d_set_bn_sync): the current setting and the one the last forward ran
+  // with, which its backward keeps (world 0 = off)
+  struct BnSync {
+    int world = 0, rank = 0;
+    vp3d_bn_exchange_fn exchange = nullptr;
+    void* user = nullptr;
+  } sync, fwd_sync;
+  // exchange slots, per BN layer l: forward moments at l * cap * 3C ([world][3][C]), backward sums
+  // at (layers * 3 + l * 2) * cap * C ([world][2][C]); cap = ranks the buffer holds (grows only)
+  float* sync_slots = nullptr;
+  int sync_cap = 0;
+  float* sync_n = nullptr;    // per BN layer: global row count of the last synchronized forward
   std::vector<void*> allocs;
 };
 
 void train_state_destroy(TrainState* t) {
   if (!t) return;
   for (void* q : t->allocs) cudaFree(q);
+  if (t->sync_slots) cudaFree(t->sync_slots);
   delete t;
 }
 
@@ -106,6 +119,16 @@ struct LayerVec {
 LayerVec layer_vec(const vp3d_plan* p, int l) {
   float* b = p->train->vec + (size_t)l * 8 * p->C;
   return {b, b + p->C, b + 2 * p->C, b + 3 * p->C, b + 4 * p->C, b + 6 * p->C};
+}
+
+// exchange slots of BN layer l (layout in TrainState::sync_slots)
+float* sync_fwd_slots(const vp3d_plan* p, int l) {
+  const TrainState* t = p->train;
+  return t->sync_slots + (size_t)l * t->sync_cap * 3 * p->C;
+}
+float* sync_bwd_slots(const vp3d_plan* p, int l) {
+  const TrainState* t = p->train;
+  return t->sync_slots + ((size_t)(2 * p->nb + 1) * 3 + (size_t)l * 2) * t->sync_cap * p->C;
 }
 
 // ---------------------------------------------------------------- workspace layout (strided)
@@ -306,6 +329,38 @@ VP3D_API size_t vp3d_train_workspace_bytes(const vp3d_plan* p, int N, int T) {
   return train_layout(p, N, T, L).total;
 }
 
+VP3D_API int vp3d_set_bn_sync(vp3d_plan* p, int world, int rank, vp3d_bn_exchange_fn exchange,
+                              void* user) {
+  if (!p) return fail(VP3D_ERR_INVALID, "set_bn_sync: null plan");
+  if (world < 0 || (world > 0 && (rank < 0 || rank >= world || !exchange)))
+    return fail(VP3D_ERR_INVALID, "set_bn_sync: need 0 <= rank < world and an exchange function "
+                "(world %d, rank %d)", world, rank);
+  if (p->f16) return fail(VP3D_ERR_UNSUPPORTED, "set_bn_sync: fp16 plans are inference-only");
+  VP3D_TRY(ensure_train_state(p));
+  TrainState* t = p->train;
+  if (world == 0) {
+    t->sync = TrainState::BnSync();
+    return VP3D_OK;
+  }
+  if (!t->sync_n)
+    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->sync_n), (VP3D_MAX_LAYERS + 1) * sizeof(float)));
+  if (world > t->sync_cap) {
+    // grows only; a backward still pending across the reallocation stays valid: it zeroes its
+    // slots itself and the forward's global counts live in sync_n
+    const size_t floats = (size_t)(2 * p->nb + 1) * 5 * world * p->C;
+    float* q = nullptr;
+    CUDA_TRY(cudaMalloc(&q, floats * sizeof(float)));
+    if (t->sync_slots) cudaFree(t->sync_slots);
+    t->sync_slots = q;
+    t->sync_cap = world;
+  }
+  t->sync.world = world;
+  t->sync.rank = rank;
+  t->sync.exchange = exchange;
+  t->sync.user = user;
+  return VP3D_OK;
+}
+
 VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N, int T,
                                    const vp3d_weights* w, const float* bn_momentum, float dropout_p,
                                    unsigned long long seed, int flags, void* ws, size_t ws_bytes,
@@ -361,6 +416,9 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
   const int C = p->C, pl = p->planes;
   t->N = N; t->T = T; t->dropout_p = dropout_p; t->seed = seed; t->frozen_bn = frozen;
   t->have_forward = false;
+  // frozen BatchNorm has no batch statistics: nothing to exchange, in this forward or its backward
+  t->fwd_sync = frozen ? TrainState::BnSync() : t->sync;
+  const TrainState::BnSync sync = t->fwd_sync;
   for (int i = 0; i <= p->nb; ++i) t->L[i] = L[i];
   int launches = 0;
 
@@ -391,6 +449,21 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
     if (frozen) {  // the eval fold of the running statistics, plus the mean / invstd backward reads
       CUDA_TRY(launch_bn_fold(bnp[0], bnp[1], bnp[2], bnp[3], 1e-5f, v.scale, v.shift, p->c_real, C,
                               stream, v.mean, v.invstd));
+    } else if (sync.world > 0) {
+      // this rank's moments into its slot, the exchange fills the others, then the rank-ordered
+      // merge and the finalize over the global batch
+      float* slots = sync_fwd_slots(p, layer);
+      CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
+                                        per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
+                                        bnp[1], nullptr, nullptr, 0.0f, 1e-5f, v.scale, v.shift,
+                                        v.mean, v.invstd, C, p->c_real, t->red_scratch,
+                                        t->red_counter, stream, slots, sync.world, sync.rank));
+      sync.exchange(layer, VP3D_BN_SYNC_FORWARD, slots, 3 * C, sync.user);
+      CUDA_TRY(launch_bn_sync_finalize(slots, sync.world, bnp[0], bnp[1], const_cast<float*>(bnp[2]),
+                                       const_cast<float*>(bnp[3]), bn_momentum[layer], 1e-5f,
+                                       v.scale, v.shift, v.mean, v.invstd, C, p->c_real,
+                                       t->sync_n + layer, stream));
+      ++launches;
     } else {
       CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
                                         per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
@@ -534,6 +607,17 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
   int launches = 0;
   const int co128 = c_out_pad128(p);
   const long long rows_top = wl.rows[p->nb];
+  // the forward's synchronized-BatchNorm setting (never set after a frozen-BatchNorm forward)
+  const TrainState::BnSync sync = t->fwd_sync;
+  const bool synced = sync.world > 0;
+  if (synced) {
+    if (!t->sync_slots || sync.world > t->sync_cap)
+      return fail(VP3D_ERR_STATE, "backward: no exchange slots for %d ranks", sync.world);
+    // every rank's slot starts at zero, so that summing the ranks' buffers is an exact gather
+    CUDA_TRY(cudaMemsetAsync(sync_bwd_slots(p, 0), 0,
+                             (size_t)(2 * p->nb + 1) * 2 * t->sync_cap * C * sizeof(float), stream));
+    ++launches;
+  }
 
   vp3d_conv_desc d;
   auto common = [&](vp3d_conv_desc& q) {
@@ -566,11 +650,15 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
                     float* dgamma, float* dbeta) -> int {
     const LayerVec v = layer_vec(p, layer);
     const DropoutCfg dc = drop_cfg(t, layer);
+    // synchronized BatchNorm: this rank's sums go to its exchange slot, v.sums receives the
+    // rank-ordered global sums
+    float* slots = synced ? sync_bwd_slots(p, layer) : nullptr;
+    float* local = synced ? slots + (size_t)sync.rank * 2 * C : v.sums;
     if (!need_sums) {
       // frozen BatchNorm without parameter gradients: dZ = scale * dY needs no reduction
     } else if (!fuse) {
       CUDA_TRY(launch_bn_bwd_reduce(gin, rows * C, z, rows * C, pl, rows, C, v.scale, v.shift,
-                                    v.mean, v.invstd, dc, slab_part, wl.slab_floats, v.sums,
+                                    v.mean, v.invstd, dc, slab_part, wl.slab_floats, local,
                                     t->red_scratch, t->red_counter, stream));
       launches += 2;
     } else {
@@ -579,14 +667,20 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       if ((size_t)bnb_slabs * 2 * bnb_ld > wl.slab_floats)
         return fail(VP3D_ERR_WORKSPACE, "backward: slab partial buffer too small");
       CUDA_TRY(launch_ordered_col_sums(slab_part, bnb_slabs, 2, bnb_ld, C, bnb_ld / C, nullptr,
-                                       v.invstd, v.sums, v.sums + C, t->red_scratch, t->red_counter,
+                                       v.invstd, local, local + C, t->red_scratch, t->red_counter,
                                        stream));
+      ++launches;
+    }
+    if (synced) {
+      sync.exchange(layer, VP3D_BN_SYNC_BACKWARD, slots, 2 * C, sync.user);
+      CUDA_TRY(launch_rank_ordered_sum(slots, sync.world, 2 * C, v.sums, stream));
       ++launches;
     }
     CUDA_TRY(launch_bn_bwd_apply(gin, rows * C, z, rows * C, bf(wl.dz), rows * C, pl, rows, C,
                                  v.scale, v.shift, v.mean, v.invstd, dc,
-                                 need_sums ? v.sums : nullptr, want_w ? dgamma : nullptr,
-                                 want_w ? dbeta : nullptr, p->c_real, stream, frozen ? 1 : 0));
+                                 need_sums ? local : nullptr, want_w ? dgamma : nullptr,
+                                 want_w ? dbeta : nullptr, p->c_real, stream, frozen ? 1 : 0,
+                                 synced ? v.sums : nullptr, synced ? t->sync_n + layer : nullptr));
     ++launches;
     return VP3D_OK;
   };

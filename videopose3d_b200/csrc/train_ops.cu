@@ -115,6 +115,36 @@ __device__ __forceinline__ bool last_block_of_group(unsigned* counter, int split
   return is_last;
 }
 
+// Batch moments of channel ch -> scale, shift, mean, invstd and the running-statistics update
+// (unbiased variance over acc.n rows).  The one epilogue of the local and the rank-merged finalize.
+__device__ __forceinline__ void bn_finalize_channel(const Moments& acc, int ch, int c_real,
+                                                    const float* gamma, const float* beta,
+                                                    float* running_mean, float* running_var,
+                                                    float momentum, float eps, float* scale,
+                                                    float* shift, float* mean_out, float* invstd) {
+  if (ch >= c_real) {   // padding channel (channels not a multiple of 64): identically zero
+    scale[ch] = 0.0f; shift[ch] = 0.0f; mean_out[ch] = 0.0f; invstd[ch] = 0.0f;
+    return;
+  }
+  const double n = (double)acc.n;
+  const double m = (double)acc.mean;
+  double var = n > 0.0 ? (double)acc.m2 / n : 0.0;
+  if (var < 0.0) var = 0.0;
+  const float is = (float)(1.0 / sqrt(var + (double)eps));
+  const float sc = gamma[ch] * is;
+  scale[ch] = sc;
+  shift[ch] = beta[ch] - (float)m * sc;
+  mean_out[ch] = (float)m;
+  invstd[ch] = is;
+  if (running_mean) {
+    const double unbiased = n > 1.0 ? var * n / (n - 1.0) : var;
+    running_mean[ch] = (float)((1.0 - momentum) * running_mean[ch] + momentum * m);
+    running_var[ch] = (float)((1.0 - momentum) * running_var[ch] + momentum * unbiased);
+  }
+}
+
+// moments != null (synchronized BatchNorm): instead of finalizing, store this rank's (n, mean, M2)
+// into slot `rank` of moments [world][3][c] and zeros into every other slot.
 __global__ void __launch_bounds__(256)
 bn_stats_finalize_kernel(const float* __restrict__ part, int slabs, SlabGeom geom, int c,
                          int c_real, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -122,7 +152,8 @@ bn_stats_finalize_kernel(const float* __restrict__ part, int slabs, SlabGeom geo
                          float momentum, float eps, float* __restrict__ scale,
                          float* __restrict__ shift, float* __restrict__ mean_out,
                          float* __restrict__ invstd, float* __restrict__ scratch,
-                         unsigned* __restrict__ counter) {
+                         unsigned* __restrict__ counter, float* __restrict__ moments, int world,
+                         int rank) {
   pdl_entry();
   __shared__ float sm[8][3][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -193,25 +224,52 @@ bn_stats_finalize_kernel(const float* __restrict__ part, int slabs, SlabGeom geo
     return;
   }
   if (!live) return;
-  if (ch >= c_real) {   // padding channel (channels not a multiple of 64): identically zero
-    scale[ch] = 0.0f; shift[ch] = 0.0f; mean_out[ch] = 0.0f; invstd[ch] = 0.0f;
+  if (moments) {
+    for (int r = 0; r < world; ++r) {
+      float* o = moments + (size_t)r * 3 * c + ch;
+      const bool own = r == rank;
+      o[0] = own ? acc.n : 0.0f;
+      o[c] = own ? acc.mean : 0.0f;
+      o[2 * (size_t)c] = own ? acc.m2 : 0.0f;
+    }
     return;
   }
-  const double n = (double)acc.n;
-  const double m = (double)acc.mean;
-  double var = n > 0.0 ? (double)acc.m2 / n : 0.0;
-  if (var < 0.0) var = 0.0;
-  const float is = (float)(1.0 / sqrt(var + (double)eps));
-  const float sc = gamma[ch] * is;
-  scale[ch] = sc;
-  shift[ch] = beta[ch] - (float)m * sc;
-  mean_out[ch] = (float)m;
-  invstd[ch] = is;
-  if (running_mean) {
-    const double unbiased = n > 1.0 ? var * n / (n - 1.0) : var;
-    running_mean[ch] = (float)((1.0 - momentum) * running_mean[ch] + momentum * m);
-    running_var[ch] = (float)((1.0 - momentum) * running_var[ch] + momentum * unbiased);
+  bn_finalize_channel(acc, ch, c_real, gamma, beta, running_mean, running_var, momentum, eps, scale,
+                      shift, mean_out, invstd);
+}
+
+// Synchronized BatchNorm, after the exchange: merge the world slots of moments [world][3][c] in
+// rank order (Chan et al., as the slab stage) and finalize with the global moments; n_out[0] = the
+// global row count (read by the backward's divisor).  One thread per channel.
+__global__ void __launch_bounds__(256)
+bn_sync_finalize_kernel(const float* __restrict__ moments, int world, int c, int c_real,
+                        const float* __restrict__ gamma, const float* __restrict__ beta,
+                        float* __restrict__ running_mean, float* __restrict__ running_var,
+                        float momentum, float eps, float* __restrict__ scale,
+                        float* __restrict__ shift, float* __restrict__ mean_out,
+                        float* __restrict__ invstd, float* __restrict__ n_out) {
+  pdl_entry();
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= c) return;
+  Moments acc = {0.0f, 0.0f, 0.0f};
+  for (int r = 0; r < world; ++r) {
+    const float* o = moments + (size_t)r * 3 * c + ch;
+    merge(acc, Moments{__ldcg(o), __ldcg(o + c), __ldcg(o + 2 * (size_t)c)});
   }
+  if (ch == 0) n_out[0] = acc.n;
+  bn_finalize_channel(acc, ch, c_real, gamma, beta, running_mean, running_var, momentum, eps, scale,
+                      shift, mean_out, invstd);
+}
+
+// out[i] = sum_r slots[r][i] (i < n) in rank order, starting from slot 0 (one rank: a copy).
+__global__ void __launch_bounds__(256)
+rank_ordered_sum_kernel(const float* __restrict__ slots, int world, int n, float* __restrict__ out) {
+  pdl_entry();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float s = __ldcg(slots + i);
+  for (int r = 1; r < world; ++r) s += __ldcg(slots + (size_t)r * n + i);
+  out[i] = s;
 }
 
 // out[st][ch] = mul_st[ch] * sum_p sum_f part[p][st][f * c + ch]   (st < nstat <= 2, f < folds):
@@ -449,13 +507,17 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
 // dz = scale*(dY - s1/n - xhat*s2/n) = scale*dY + B*z + D with per-channel
 // B = -scale*invstd*s2/n,  D = -scale*s1/n - B*mean.  frozen (BatchNorm on running statistics):
 // B = D = 0, dz = scale*dY; sums may then be null (no dgamma / dbeta wanted).
+// Synchronized BatchNorm: B and D use the global sums `gsums` and the global row count *n_global;
+// dgamma / dbeta come from this rank's `sums` (the gradient all-reduce averages them).  Otherwise
+// gsums == sums and n_global is null (n = rows).
 __global__ void __launch_bounds__(256)
 bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
                     const __nv_bfloat16* __restrict__ z, long long z_plane,
                     __nv_bfloat16* __restrict__ dz, long long dz_plane, int planes, long long rows,
                     int c, const float* __restrict__ scale, const float* __restrict__ shift,
                     const float* __restrict__ mean, const float* __restrict__ invstd,
-                    DropoutCfg drop, const float* __restrict__ sums, float* __restrict__ dgamma,
+                    DropoutCfg drop, const float* sums, const float* gsums,
+                    const float* __restrict__ n_global, float* __restrict__ dgamma,
                     float* __restrict__ dbeta, int c_real, int frozen, RowTiling tl) {
   pdl_entry();
   const int cg = threadIdx.x % tl.G, rl = threadIdx.x / tl.G, lanes = 256 / tl.G;
@@ -465,15 +527,15 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
   const bool do_drop = drop.p > 0.0f;
   const uint32_t thresh = (uint32_t)(drop.p * 65536.0f);
   const float inv_keep = do_drop ? 1.0f / (1.0f - drop.p) : 1.0f;
-  const float inv_n = 1.0f / (float)rows;
+  const float inv_n = 1.0f / (n_global ? __ldg(n_global) : (float)rows);
   float sc[8], sh[8], B[8], D[8];
   {
     float mu[8], is[8], s1[8], s2[8];
     load_vec8(scale + c0, sc);
     load_vec8(shift + c0, sh);
     if (sums) {
-      load_vec8(sums + c0, s1);
-      load_vec8(sums + c + c0, s2);
+      load_vec8(gsums + c0, s1);
+      load_vec8(gsums + c + c0, s2);
     } else {
 #pragma unroll
       for (int j = 0; j < 8; ++j) s1[j] = s2[j] = 0.0f;
@@ -489,8 +551,8 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, long long g_plane,
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         if (c0 + j >= c_real) break;   // gradient tensors hold the model's real channel count
-        if (dbeta) dbeta[c0 + j] = s1[j];
-        if (dgamma) dgamma[c0 + j] = s2[j];
+        if (dbeta) dbeta[c0 + j] = __ldg(sums + c0 + j);          // this rank's sums
+        if (dgamma) dgamma[c0 + j] = __ldg(sums + c + c0 + j);
       }
     }
 #pragma unroll
@@ -628,13 +690,35 @@ cudaError_t launch_bn_stats_finalize(const float* part, int slabs, int dilated, 
                                      float* running_mean, float* running_var, float momentum,
                                      float eps, float* scale, float* shift, float* mean,
                                      float* invstd, int c, int c_real, float* scratch,
-                                     unsigned* counter, cudaStream_t stream) {
+                                     unsigned* counter, cudaStream_t stream, float* moments,
+                                     int world, int rank) {
   if (c > kReduceMaxChannels) return cudaErrorInvalidValue;
+  if (moments && (world < 1 || rank < 0 || rank >= world)) return cudaErrorInvalidValue;
   SlabGeom g = {dilated, out_rows, tiles_per_sample};
   const dim3 grid((c + 31) / 32, pick_splits(slabs));
   const cudaError_t le = launch_pdl(bn_stats_finalize_kernel, grid, dim3(256), 0, stream, part, slabs, g, c, c_real, gamma, beta, running_mean,
                                                      running_var, momentum, eps, scale, shift, mean,
-                                                     invstd, scratch, counter);
+                                                     invstd, scratch, counter, moments, world, rank);
+  return le != cudaSuccess ? le : cudaGetLastError();
+}
+
+cudaError_t launch_bn_sync_finalize(const float* moments, int world, const float* gamma,
+                                    const float* beta, float* running_mean, float* running_var,
+                                    float momentum, float eps, float* scale, float* shift,
+                                    float* mean, float* invstd, int c, int c_real, float* n_out,
+                                    cudaStream_t stream) {
+  if (world < 1 || c < 1) return cudaErrorInvalidValue;
+  const cudaError_t le = launch_pdl(bn_sync_finalize_kernel, dim3((c + 255) / 256), dim3(256), 0,
+                                    stream, moments, world, c, c_real, gamma, beta, running_mean,
+                                    running_var, momentum, eps, scale, shift, mean, invstd, n_out);
+  return le != cudaSuccess ? le : cudaGetLastError();
+}
+
+cudaError_t launch_rank_ordered_sum(const float* slots, int world, int n, float* out,
+                                    cudaStream_t stream) {
+  if (world < 1 || n < 1) return cudaErrorInvalidValue;
+  const cudaError_t le = launch_pdl(rank_ordered_sum_kernel, dim3((n + 255) / 256), dim3(256), 0,
+                                    stream, slots, world, n, out);
   return le != cudaSuccess ? le : cudaGetLastError();
 }
 
@@ -685,14 +769,18 @@ cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* g, long long g_plane, const
                                 long long rows, int c, const float* scale, const float* shift,
                                 const float* mean, const float* invstd, DropoutCfg drop,
                                 const float* sums, float* dgamma, float* dbeta, int c_real,
-                                cudaStream_t stream, int frozen) {
+                                cudaStream_t stream, int frozen, const float* global_sums,
+                                const float* n_global) {
   if (rows <= 0) return cudaSuccess;
   if (!sums && !frozen) return cudaErrorInvalidValue;
+  if (!global_sums != !n_global) return cudaErrorInvalidValue;
+  if (!global_sums) global_sums = sums;
   dim3 grid;
   const RowTiling tl = row_tiling(rows, c, grid);
   const cudaError_t le = launch_pdl(bn_bwd_apply_kernel, grid, dim3(256), 0, stream, g, g_plane, z, z_plane, dz, dz_plane, planes, rows,
-                                                c, scale, shift, mean, invstd, drop, sums, dgamma,
-                                                dbeta, c_real, frozen, tl);
+                                                c, scale, shift, mean, invstd, drop, sums,
+                                                global_sums, n_global, dgamma, dbeta, c_real,
+                                                frozen, tl);
   return le != cudaSuccess ? le : cudaGetLastError();
 }
 

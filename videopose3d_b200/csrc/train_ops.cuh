@@ -42,7 +42,22 @@ cudaError_t launch_bn_stats_finalize(const float* part, int slabs, int dilated, 
                                      float* running_mean, float* running_var, float momentum,
                                      float eps, float* scale, float* shift, float* mean,
                                      float* invstd, int c, int c_real, float* scratch,
-                                     unsigned* counter, cudaStream_t stream);
+                                     unsigned* counter, cudaStream_t stream,
+                                     float* moments = nullptr, int world = 0, int rank = 0);
+// With `moments` (synchronized BatchNorm) the launch above stops after the slab merge: it writes
+// this rank's (n, mean, M2) into slot `rank` of moments [world][3][c], zeros into the other slots,
+// and nothing else.  After the slots have been exchanged, launch_bn_sync_finalize merges them in
+// rank order 0..world-1 and runs the same finalize (running statistics over the global n);
+// n_out[0] = the global row count.
+cudaError_t launch_bn_sync_finalize(const float* moments, int world, const float* gamma,
+                                    const float* beta, float* running_mean, float* running_var,
+                                    float momentum, float eps, float* scale, float* shift,
+                                    float* mean, float* invstd, int c, int c_real, float* n_out,
+                                    cudaStream_t stream);
+
+// out[i] = sum_r slots[r][i] for slots [world][n], in rank order (world = 1: a copy).
+cudaError_t launch_rank_ordered_sum(const float* slots, int world, int n, float* out,
+                                    cudaStream_t stream);
 
 // out_st[ch] = mul_st[ch] * sum_p sum_f part[p][st][f*c + ch], st < nstat (1 or 2), f < folds, in
 // a fixed order.  part: [n_part][nstat][ld].  mul_st may be null (= 1).
@@ -70,13 +85,16 @@ cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* g, long long g_plane, cons
 // dz = scale * (dY - sums[0]/n - xhat * sums[1]/n); also writes dgamma = sums[1], dbeta = sums[0]
 // (done by block 0).  dz: bf16 [planes][rows][c].  frozen != 0 (BatchNorm on running statistics,
 // eval-mode backward): dz = scale * dY, mean / invstd are not read, and sums may be null (then no
-// dgamma / dbeta are written).
+// dgamma / dbeta are written).  Synchronized BatchNorm: global_sums [2][c] (summed over ranks) and
+// the device scalar n_global (global row count) replace sums and rows in dz, while dgamma / dbeta
+// still come from this rank's `sums`; both null otherwise.
 cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* g, long long g_plane, const __nv_bfloat16* z,
                                 long long z_plane, __nv_bfloat16* dz, long long dz_plane, int planes,
                                 long long rows, int c, const float* scale, const float* shift,
                                 const float* mean, const float* invstd, DropoutCfg drop,
                                 const float* sums, float* dgamma, float* dbeta, int c_real,
-                                cudaStream_t stream, int frozen = 0);
+                                cudaStream_t stream, int frozen = 0,
+                                const float* global_sums = nullptr, const float* n_global = nullptr);
 
 // out[c] = sum_rows x[row][c] for fp32 x [rows][c] (shrink.bias gradient), via per-64-row partials
 // summed in a fixed order.

@@ -41,13 +41,16 @@ class _Plan:
     """A plan handle and the parameter versions (``TemporalModelBase._versions``) each kind of its
     weight packs was made from, None while never packed: ``eval`` (VP3D_PACK_CONV |
     VP3D_PACK_BN_EVAL), ``train`` (VP3D_PACK_CONV | VP3D_PACK_CONV_T) and ``expand_t``
-    (VP3D_PACK_EXPAND_T, the expand conv weight's entry only)."""
+    (VP3D_PACK_EXPAND_T, the expand conv weight's entry only).  ``bn_sync`` is (reducer, ctypes
+    exchange callback) while the plan's synchronized BatchNorm is on (vp3d_set_bn_sync): the plan
+    holds the callback as long as it may call it."""
 
-    __slots__ = ("handle", "eval", "train", "expand_t")
+    __slots__ = ("handle", "eval", "train", "expand_t", "bn_sync")
 
     def __init__(self, handle):
         self.handle = handle
         self.eval = self.train = self.expand_t = None
+        self.bn_sync = None
 
     @property
     def _as_parameter_(self):
@@ -650,6 +653,27 @@ def _backward(module, plan, ws, dy, stream, want_x, dx_shape, want_p, shapes, re
     return dx, tuple(gr if w else None for gr, w in zip(grads, want_p))
 
 
+def _configure_bn_sync(module, plan):
+    """Point `plan`'s synchronized BatchNorm at the module's reducer when it has sync_bn on, and
+    switch it off otherwise; returns that reducer or None."""
+    reducer = getattr(module, "_grad_reducer", None)
+    want = reducer if reducer is not None and reducer.sync_bn else None
+    have = plan.bn_sync[0] if plan.bn_sync is not None else None
+    if want is have:
+        return want
+    lib = _capi.load()
+    if want is None:
+        _capi.check(lib.vp3d_set_bn_sync(plan, 0, 0, None, None), "vp3d_set_bn_sync")
+        plan.bn_sync = None
+        return None
+    cb = want.bn_exchange_fn()
+    _capi.check(lib.vp3d_set_bn_sync(plan, want.world, want.rank,
+                                      _capi.ctypes.cast(cb, _capi.ctypes.c_void_p), None),
+                "vp3d_set_bn_sync")
+    plan.bn_sync = (want, cb)
+    return want
+
+
 class _TrainFunction(torch.autograd.Function):
     """Training-mode forward/backward through the C ABI (vp3d_forward_train_ex with flags 0 /
     vp3d_backward_ex).
@@ -658,7 +682,9 @@ class _TrainFunction(torch.autograd.Function):
     gradients into ``.grad`` exactly as it does for the reference's nn modules.  dL/dx is computed
     when x requires grad (the expand conv's data gradient); parameter gradients are skipped when no
     learnable tensor requires grad.  With a data-parallel reducer of more than one rank attached,
-    the backward's stage callback all-reduces the gradients while it runs."""
+    the backward's stage callback all-reduces the gradients while it runs; with one that has
+    sync_bn on (any number of ranks), forward and backward exchange every BatchNorm's statistics
+    and sums with the other ranks."""
 
     @staticmethod
     def forward(ctx, module, x, *params):
@@ -672,8 +698,11 @@ class _TrainFunction(torch.autograd.Function):
             plan = module._use_plan(device, module._train_precision)
             stream = torch.cuda.current_stream(device).cuda_stream
             module._sync_weights(plan, stream, training=True)
+            sync = _configure_bn_sync(module, plan)
             mom = (_capi.ctypes.c_float * len(momenta))(*[float(m) for m in momenta])
             y, ws = _train_forward(module, plan, x, stream, mom, p_drop, seed)
+        if sync is not None:
+            sync.raise_errors()
         # nn.BatchNorm1d bookkeeping that lives outside the kernels
         with torch.no_grad():
             module.expand_bn.num_batches_tracked += 1
@@ -688,6 +717,7 @@ class _TrainFunction(torch.autograd.Function):
         ctx.shapes = [tuple(p.shape) for p in params]
         ctx.x_shape = tuple(x.shape)
         ctx.device = device
+        ctx.bn_sync = sync     # the C backward keeps this forward's setting
         return y
 
     @staticmethod
@@ -698,6 +728,11 @@ class _TrainFunction(torch.autograd.Function):
                                "back-propagated (one forward per backward, as in run.py)")
         dy = dy.contiguous().float()
         want_x = ctx.needs_input_grad[1]
+        sync = ctx.bn_sync
+        if sync is not None and sync.step_scale != 1.0:
+            # the ragged-shard weight (set_step_rows) on dY: the BatchNorm backward sums mix every
+            # rank's dY, so scaling this rank's gradients afterwards would miss its share in theirs
+            dy = dy * sync.step_scale
         reducer = getattr(module, "_grad_reducer", None)
         if reducer is not None and reducer.world <= 1:
             reducer = None
@@ -707,6 +742,8 @@ class _TrainFunction(torch.autograd.Function):
                 module._sync_expand_t(ctx.plan, stream)
             dx, grads = _backward(module, ctx.plan, ctx.ws, dy, stream, want_x,
                                   ctx.x_shape, ctx.needs_input_grad[2:], ctx.shapes, reducer)
+        if sync is not None:
+            sync.raise_errors()
         ctx.ws = None
         return (None, dx) + grads
 
