@@ -199,3 +199,16 @@ def test_legacy_training_entries_match_the_ex_entries(cuda_device):
             assert torch.equal(a, b)
         assert (s0, f0, b0) == (s1, f1, b1)
         assert s0 == (list(range(len(ARC) + 1)) if staged else [])
+
+
+def test_training_above_the_channel_limit_fails_on_every_forward(cuda_device):
+    """Training supports at most 8192 (padded) channels.  A plan above the limit gets no training
+    state at all, so every training forward raises the same error instead of the second one running
+    on half-built state."""
+    m = vp.TemporalModel(17, 2, 17, filter_widths=[3, 3], dropout=0.0, channels=8193)   # 8256 padded
+    m = m.to(cuda_device).set_train_precision("bf16").train()
+    x = orc.make_input(2, 9, 17, 2, seed=3).to(cuda_device)
+    for _ in range(2):
+        with pytest.raises(NotImplementedError, match="at most 8192 channels"):
+            m(x)
+    torch.cuda.synchronize()

@@ -12,6 +12,7 @@
 
 #include "internal.cuh"
 #include "pack.cuh"
+#include "train_ops.cuh"
 
 using namespace vp3d;
 
@@ -280,18 +281,69 @@ int plan_alloc(vp3d_plan* p, void** out, size_t bytes) {
   return VP3D_OK;
 }
 
-}  // namespace vp3d
+// The pack table of a plan whose shape fields are set (internal.cuh, PackedConv).
+static void plan_packs(vp3d_plan* p) {
+  auto add = [p](int src, int c_out, int c_in, int taps, bool transposed, bool merged, int n_pad,
+                 int k_pad) {
+    PackedConv& k = p->packs[p->n_packs++];
+    k.src = src; k.c_out = c_out; k.c_in = c_in; k.taps = taps;
+    k.transposed = transposed; k.merged = merged;
+    k.stored_taps = merged ? 1 : taps; k.n_pad = n_pad; k.k_pad = k_pad;
+    return &k;
+  };
+  const int C = p->C, cr = p->c_real, w0 = p->cfg.filter_widths[0];
+  auto layer_taps = [p](int l) { return l % 2 == 0 ? p->taps[l / 2 + 1] : 1; };
+  p->expand_dil = add(kSrcExpand, cr, p->c_in_raw, w0, false, false, C, p->c_in_pad);
+  p->expand_flat = add(kSrcExpand, cr, p->c_in_raw, w0, false, true, C, p->k0_pad);
+  for (int l = 0; l < 2 * p->nb; ++l) p->conv[l] = add(l, cr, cr, layer_taps(l), false, false, C, C);
+  p->shrink = add(kSrcShrink, p->c_out_raw, cr, 1, false, false, p->c_out_pad, C);
+  for (int l = 0; l < 2 * p->nb; ++l) p->conv_t[l] = add(l, cr, cr, layer_taps(l), true, false, C, C);
+  // K of the shrink data gradient (dY's columns) padded to 128: also the row pitch of the padded dY
+  // in the training workspace
+  p->shrink_t = add(kSrcShrink, p->c_out_raw, cr, 1, true, false, C, round_up(p->c_out_raw, 128));
+  // the input gradient in the plan's own layout: tap-merged rows (tap*c_in + ci) for the strided model
+  p->expand_t = p->cfg.variant == VP3D_VARIANT_STRIDED
+                    ? add(kSrcExpand, cr, p->c_in_raw, w0, true, true, p->k0_pad, C)
+                    : add(kSrcExpand, cr, p->c_in_raw, w0, true, false, p->c_in_pad, C);
+}
 
-static int alloc_packed(vp3d_plan* p, PackedConv& pc, int taps, int k_per_tap, int n_pad,
-                        int merged) {
-  pc.taps = taps;
-  pc.k_per_tap = k_per_tap;
-  pc.n_pad = n_pad;
-  pc.merged = merged;
-  const size_t elems = (size_t)p->planes * taps * n_pad * k_per_tap;
-  VP3D_TRY(plan_alloc(p, reinterpret_cast<void**>(&pc.w), elems * 2));
+// the fp32 weight pack k is made from, an error if w lacks it
+static int pack_source(const PackedConv& k, const vp3d_weights* w, const float** src) {
+  *src = conv_weight(w, k.src);
+  if (!*src && k.src >= 0) return fail(VP3D_ERR_INVALID, "set_weights: missing layers_conv.%d", k.src);
+  if (!*src)
+    return fail(VP3D_ERR_INVALID, "set_weights: missing %s",
+                k.src == kSrcExpand ? "expand_conv.weight" : "shrink.weight");
   return VP3D_OK;
 }
+
+int pack_weight(const vp3d_plan* p, const PackedConv& k, const vp3d_weights* w, cudaStream_t stream,
+                const PackedConv* fwd) {
+  const float* src = nullptr;
+  VP3D_TRY(pack_source(k, w, &src));
+  if (k.transposed)
+    CUDA_TRY(launch_pack_conv_weight_t(src, k.w, p->planes, k.c_out, k.c_in, k.taps, k.n_pad, k.k_pad,
+                                       stream, fwd ? fwd->w : nullptr, fwd ? fwd->n_pad : 0,
+                                       fwd ? fwd->k_pad : 0, k.merged));
+  else
+    CUDA_TRY(launch_pack_conv_weight(src, k.w, p->planes, k.c_out, k.c_in, k.taps, k.n_pad, k.k_pad,
+                                     k.merged, stream, p->f16));
+  return VP3D_OK;
+}
+
+int pack_expand_forward(const vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream) {
+  VP3D_TRY(pack_weight(p, *p->expand_dil, w, stream));
+  return pack_weight(p, *p->expand_flat, w, stream);
+}
+
+void use_pack(vp3d_conv_desc* d, const PackedConv& k) {
+  d->w = k.w;
+  d->taps = k.stored_taps;
+  d->k_per_tap = k.k_pad;
+  d->n_pad = k.n_pad;
+}
+
+}  // namespace vp3d
 
 extern "C" __attribute__((visibility("default"))) int vp3d_version(void) { return VP3D_VERSION; }
 extern "C" __attribute__((visibility("default"))) int vp3d_set_pdl(int on) {
@@ -366,28 +418,26 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
     next_dilation *= w;
   }
 
+  plan_packs(p);
+
   int st = VP3D_OK;
   do {
-    if ((st = alloc_packed(p, p->expand_dil, cfg->filter_widths[0], p->c_in_pad, p->C, 0))) break;
-    if ((st = alloc_packed(p, p->expand_flat, 1, p->k0_pad, p->C, 1))) break;
-    for (int i = 0; i < p->nb && !st; ++i) {
-      st = alloc_packed(p, p->conv[2 * i], p->taps[i + 1], p->C, p->C, 0);
-      if (!st) st = alloc_packed(p, p->conv[2 * i + 1], 1, p->C, p->C, 0);
-    }
+    for (int i = 0; i < p->n_packs && !st; ++i)
+      if (!p->packs[i].transposed)
+        st = plan_alloc(p, reinterpret_cast<void**>(&p->packs[i].w), pack_bytes(p, p->packs[i]));
     if (st) break;
-    if ((st = alloc_packed(p, p->shrink, 1, p->C, p->c_out_pad, 0))) break;
     // affine vectors: expand + 2*nb layers (C each) + shrink (c_out_pad)
     float* aff = nullptr;
     const size_t n_aff = (size_t)(2 * p->nb + 1) * 2 * p->C + 2 * p->c_out_pad;
     if ((st = plan_alloc(p, reinterpret_cast<void**>(&aff), n_aff * sizeof(float)))) break;
-    p->expand_dil.scale = p->expand_flat.scale = aff;
-    p->expand_dil.shift = p->expand_flat.shift = aff + p->C;
+    p->expand_dil->scale = p->expand_flat->scale = aff;
+    p->expand_dil->shift = p->expand_flat->shift = aff + p->C;
     for (int l = 0; l < 2 * p->nb; ++l) {
-      p->conv[l].scale = aff + (size_t)(l + 1) * 2 * p->C;
-      p->conv[l].shift = p->conv[l].scale + p->C;
+      p->conv[l]->scale = aff + (size_t)(l + 1) * 2 * p->C;
+      p->conv[l]->shift = p->conv[l]->scale + p->C;
     }
-    p->shrink.scale = aff + (size_t)(2 * p->nb + 1) * 2 * p->C;
-    p->shrink.shift = p->shrink.scale + p->c_out_pad;
+    p->shrink->scale = aff + (size_t)(2 * p->nb + 1) * 2 * p->C;
+    p->shrink->shift = p->shrink->scale + p->c_out_pad;
   } while (0);
   if (st) {
     vp3d_plan_destroy(p);
@@ -439,30 +489,14 @@ extern "C" __attribute__((visibility("default"))) int vp3d_total_causal_shift(co
 extern "C" __attribute__((visibility("default"))) int vp3d_set_weights(vp3d_plan* p, const vp3d_weights* w, int what, void* stream_) {
   if (!p || !w) return fail(VP3D_ERR_INVALID, "set_weights: null argument");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int w0 = p->cfg.filter_widths[0];
   if (what & VP3D_PACK_CONV) {
-    if (!w->expand_conv_weight || !w->shrink_weight)
-      return fail(VP3D_ERR_INVALID, "set_weights: missing conv weights");
-    CUDA_TRY(launch_pack_conv_weight(w->expand_conv_weight, p->expand_dil.w, p->planes, p->c_real,
-                                     p->c_in_raw, w0, p->C, p->c_in_pad, 0, stream, p->f16));
-    CUDA_TRY(launch_pack_conv_weight(w->expand_conv_weight, p->expand_flat.w, p->planes, p->c_real,
-                                     p->c_in_raw, w0, p->C, p->k0_pad, 1, stream, p->f16));
-    // with VP3D_PACK_CONV_T the transposed-pack kernels below also write these forward packs
-    const bool fused = (what & VP3D_PACK_CONV_T) != 0;
-    for (int i = 0; i < p->nb; ++i) {
-      if (!w->layers_conv_weight[2 * i] || !w->layers_conv_weight[2 * i + 1])
-        return fail(VP3D_ERR_INVALID, "set_weights: missing layers_conv.%d", 2 * i);
-      if (fused) continue;
-      CUDA_TRY(launch_pack_conv_weight(w->layers_conv_weight[2 * i], p->conv[2 * i].w, p->planes,
-                                       p->c_real, p->c_real, p->taps[i + 1], p->C, p->C, 0, stream,
-                                       p->f16));
-      CUDA_TRY(launch_pack_conv_weight(w->layers_conv_weight[2 * i + 1], p->conv[2 * i + 1].w,
-                                       p->planes, p->c_real, p->c_real, 1, p->C, p->C, 0, stream,
-                                       p->f16));
-    }
-    if (!fused)
-      CUDA_TRY(launch_pack_conv_weight(w->shrink_weight, p->shrink.w, p->planes, p->c_out_raw,
-                                       p->c_real, 1, p->c_out_pad, p->C, 0, stream, p->f16));
+    const float* src = nullptr;
+    for (int i = 0; i < p->n_packs; ++i) VP3D_TRY(pack_source(p->packs[i], w, &src));
+    VP3D_TRY(pack_expand_forward(p, w, stream));
+    // with VP3D_PACK_CONV_T the transposed-pack kernels below also write the other forward packs
+    for (int i = 0; i < p->n_packs && !(what & VP3D_PACK_CONV_T); ++i)
+      if (!p->packs[i].transposed && p->packs[i].src != kSrcExpand)
+        VP3D_TRY(pack_weight(p, p->packs[i], w, stream));
     p->conv_packed = true;
   }
   if (what & VP3D_PACK_BN_EVAL) {
@@ -471,15 +505,15 @@ extern "C" __attribute__((visibility("default"))) int vp3d_set_weights(vp3d_plan
       if (!w->expand_bn[k]) return fail(VP3D_ERR_INVALID, "set_weights: missing expand_bn");
     if (!w->shrink_bias) return fail(VP3D_ERR_INVALID, "set_weights: missing shrink.bias");
     CUDA_TRY(launch_bn_fold(w->expand_bn[0], w->expand_bn[1], w->expand_bn[2], w->expand_bn[3], eps,
-                            p->expand_dil.scale, p->expand_dil.shift, p->c_real, p->C, stream));
+                            p->expand_dil->scale, p->expand_dil->shift, p->c_real, p->C, stream));
     for (int l = 0; l < 2 * p->nb; ++l) {
       for (int k = 0; k < 4; ++k)
         if (!w->layers_bn[l][k]) return fail(VP3D_ERR_INVALID, "set_weights: missing layers_bn.%d", l);
       CUDA_TRY(launch_bn_fold(w->layers_bn[l][0], w->layers_bn[l][1], w->layers_bn[l][2],
-                              w->layers_bn[l][3], eps, p->conv[l].scale, p->conv[l].shift,
+                              w->layers_bn[l][3], eps, p->conv[l]->scale, p->conv[l]->shift,
                               p->c_real, p->C, stream));
     }
-    CUDA_TRY(launch_bias_affine(w->shrink_bias, p->shrink.scale, p->shrink.shift, p->c_out_raw,
+    CUDA_TRY(launch_bias_affine(w->shrink_bias, p->shrink->scale, p->shrink->shift, p->c_out_raw,
                                 p->c_out_pad, stream));
     p->bn_packed = true;
   }
@@ -688,17 +722,17 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
                                (long long)wl.a0_plane, stream, &perm, p->f16)));
     common(d, x3[0]);
     d.a = a0; d.samples = 1; d.a_rows = N * L[0]; d.a_ld = p->k0_pad;
-    d.w = p->expand_flat.w; d.taps = 1; d.k_per_tap = p->k0_pad; d.n_pad = C;
+    use_pack(&d, *p->expand_flat);
     d.per_sample_tiles = 0; d.out_rows = N * L[0];
   } else {
     VP3D_LAUNCH(CUDA_TRY(launch_pack_input(x, a0, p->planes, N, T, p->c_in_raw, T, 1, 1, p->c_in_pad,
                                (long long)wl.a0_plane, stream, nullptr, p->f16)));
     common(d, x3[0]);
     d.a = a0; d.samples = N; d.a_rows = T; d.a_ld = p->c_in_pad;
-    d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+    use_pack(&d, *p->expand_dil);
     d.per_sample_tiles = 1; d.tap_row_step = 1; d.out_rows = L[0];
   }
-  d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
+  d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
   d.out = xb[0]; d.out_plane_stride = (long long)wl.x_plane; d.out_ld = C;
   lo_rows(0, d);
   VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
@@ -707,15 +741,15 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   int cur = 0;
   size_t cur_plane = wl.x_plane;
   for (int i = 1; i <= p->nb; ++i) {
-    const PackedConv& c0 = p->conv[2 * (i - 1)];
-    const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
+    const PackedConv& c0 = *p->conv[2 * (i - 1)];
+    const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
     const int Lin = L[i - 1], Lout = L[i];
     const size_t h_plane = (size_t)N * Lout * C;
     // first conv of the block: dilated / strided k-tap conv + BN + ReLU
     common(d, x3[i]);
     d.out_planes = x3[i] ? 2 : 1;  // H only needs a lo plane when its consumer is split-bf16
     d.a = xb[cur];
-    d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, c0);
     d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
     d.out = hb; d.out_plane_stride = (long long)h_plane; d.out_ld = C;
     if (strided) {
@@ -736,7 +770,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
     common(d, x3[i]);
     d.a_planes = x3[i] ? 2 : 1;
     d.a = hb; d.samples = 1; d.a_rows = N * Lout; d.a_ld = C;
-    d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, c1);
     d.per_sample_tiles = 0; d.out_rows = N * Lout;
     d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
     d.res = xb[cur]; d.res_plane_stride = (long long)cur_plane; d.res_ld = C;
@@ -759,9 +793,9 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   // ---- shrink (model.py:137 / :196) writing (N, T_out, J_out, 3) directly (fuses :74-75)
   common(d, x3[p->nb + 1]);
   d.a = xb[cur]; d.samples = 1; d.a_rows = N * L[p->nb]; d.a_ld = C;
-  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad;
+  use_pack(&d, *p->shrink);
   d.per_sample_tiles = 0; d.out_rows = N * L[p->nb];
-  d.scale = p->shrink.scale; d.shift = p->shrink.shift; d.relu = 0;
+  d.scale = p->shrink->scale; d.shift = p->shrink->shift; d.relu = 0;
   d.out = nullptr; d.out_f32 = y; d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
   VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
   p->last_launches = launches;

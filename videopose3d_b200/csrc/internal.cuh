@@ -43,15 +43,29 @@ int num_sms();
 int run_conv(const vp3d_conv_desc* d, cudaStream_t stream);
 
 
+// One 16-bit pack of a Conv1d weight (c_out, c_in, taps) (model.py:102,113-118), stored as
+// [planes][stored_taps][n_pad][k_pad], zero padded:
+//   forward:    [tap][co][ci]; merged: one slab [co][tap*c_in + ci] (expand conv as a plain GEMM)
+//   transposed: [tap][ci][co] for the data-gradient GEMMs; merged: one slab [tap*c_in + ci][co]
+// Every pack of a plan is one entry of its pack table (vp3d_plan::packs), whose geometry
+// vp3d_plan_create fixes once; allocation, packing, the fused optimizer and the GEMM descriptors
+// all read it from there.
+enum { kSrcExpand = -1, kSrcShrink = -2 };
 struct PackedConv {
-  __nv_bfloat16* w = nullptr;
-  int taps = 0;       // taps as stored (1 when merged)
-  int k_per_tap = 0;  // padded
-  int n_pad = 0;
-  int merged = 0;
-  float* scale = nullptr;  // eval affine [n_pad]
+  int src = 0;  // vp3d_weights tensor: kSrcExpand, kSrcShrink or l for layers_conv[l]
+  int c_out = 0, c_in = 0, taps = 0;
+  bool transposed = false, merged = false;
+  int stored_taps = 0, n_pad = 0, k_pad = 0;
+  __nv_bfloat16* w = nullptr;  // transposed packs: allocated with the training state
+  float* scale = nullptr;      // forward packs: eval affine of the conv's output [n_pad]
   float* shift = nullptr;
 };
+constexpr int kMaxPacks = 2 * VP3D_MAX_LAYERS + 5;
+
+inline const float* conv_weight(const vp3d_weights* w, int src) {
+  return src == kSrcExpand ? w->expand_conv_weight
+         : src == kSrcShrink ? w->shrink_weight : w->layers_conv_weight[src];
+}
 
 // One coordinate of the test-time flip average (run.py:677-680): p0 from the plain copy, p1 from the
 // mirrored copy (its joints already swapped back), axis 0 negated back.  Rounded as torch rounds
@@ -78,10 +92,8 @@ struct StreamHost {
 // step_ops.cu: Adam / AMSGrad update of conv weights that also refreshes their bf16 packs
 struct AdamPackItem {
   vp3d_adam_tensor t;
-  __nv_bfloat16* fwd;   // forward pack [planes][taps][fwd_n_pad][fwd_k_pad] or null
-  __nv_bfloat16* tr;    // transposed pack [planes][taps][tr_n_pad][tr_k_pad] or null
-  int c_out, c_in, taps;
-  int fwd_n_pad, fwd_k_pad, tr_n_pad, tr_k_pad;
+  const PackedConv* fwd;  // the conv's forward pack
+  const PackedConv* tr;   // and its transposed pack (neither merged)
 };
 int launch_adam_pack(const AdamPackItem* items, int n, int planes, int64_t step, double lr,
                      double beta1, double beta2, double eps, double weight_decay,
@@ -102,8 +114,15 @@ struct vp3d_plan {
   int shift_str[VP3D_MAX_WIDTHS];  // causal shift in strided units (Optimized1f, model.py:176)
   int dilation[VP3D_MAX_WIDTHS];
   int taps[VP3D_MAX_WIDTHS];       // taps of block i's first conv (dense: 2*pad+1)
-  vp3d::PackedConv expand_dil, expand_flat, shrink;
-  vp3d::PackedConv conv[VP3D_MAX_LAYERS];
+  // the pack table: forward packs (expand dilated and tap-merged, layers_conv, shrink), then the
+  // transposed ones of training (layers_conv, shrink, expand in the variant's layout)
+  vp3d::PackedConv packs[vp3d::kMaxPacks];
+  int n_packs = 0;
+  // views into it
+  vp3d::PackedConv *expand_dil = nullptr, *expand_flat = nullptr, *shrink = nullptr;
+  vp3d::PackedConv* conv[VP3D_MAX_LAYERS] = {};
+  vp3d::PackedConv *expand_t = nullptr, *shrink_t = nullptr;
+  vp3d::PackedConv* conv_t[VP3D_MAX_LAYERS] = {};
   std::vector<void*> allocs;
   bool conv_packed = false, bn_packed = false;
   // host-API staging (owned)
@@ -140,6 +159,17 @@ bool use_strided(const vp3d_plan* p, int T);
 // rows per sample after each stage: L[0] = rows out of expand, L[i] = rows out of block i
 int layer_rows(const vp3d_plan* p, int T, bool strided, int* L);
 int strided_trim(const vp3d_plan* p, int* L);
+inline size_t pack_bytes(const vp3d_plan* p, const PackedConv& k) {
+  return (size_t)p->planes * k.stored_taps * k.n_pad * k.k_pad * sizeof(__nv_bfloat16);
+}
+// packs k from its fp32 weight in w; a transposed pack given `fwd` writes that forward pack of the
+// same conv in the same pass
+int pack_weight(const vp3d_plan* p, const PackedConv& k, const vp3d_weights* w, cudaStream_t stream,
+                const PackedConv* fwd = nullptr);
+// the forward packs of the expand conv (dilated and tap-merged) from w->expand_conv_weight
+int pack_expand_forward(const vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream);
+// GEMM weight operand of a conv descriptor: pointer, taps, K per tap and N as stored in k
+void use_pack(vp3d_conv_desc* d, const PackedConv& k);
 void train_state_destroy(TrainState* t);
 int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream,
                           bool also_forward);

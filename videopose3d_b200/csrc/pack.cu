@@ -1,24 +1,10 @@
 #include "pack.cuh"
 
-#include <cuda_fp16.h>
-
 #include <string.h>
 
 #include <stdint.h>
 
 namespace vp3d {
-
-__device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(v);
-  lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-// 16-bit storage of the fp16 eval mode: IEEE half bits in a bf16-typed slot (single plane),
-// saturating at +-65504 like the GEMM epilogue does.
-__device__ __forceinline__ __nv_bfloat16 f16_bits(float v) {
-  v = fminf(fmaxf(v, -65504.0f), 65504.0f);
-  const unsigned short h = __half_as_ushort(__float2half_rn(v));
-  return __ushort_as_bfloat16(h);
-}
 
 // Rows are walked in SOURCE order (sample, then frame group) so that the fp32 read is one
 // sequential stream; the scattered side (tap-major row order) is the 16-bit output, which stays in
@@ -47,16 +33,9 @@ __device__ __forceinline__ void pack_load_pair(const float* src, int k, int k_va
 
 __device__ __forceinline__ void pack_store_pair(__nv_bfloat16* dst, long long plane_stride, int planes,
                                                 int f16, float v0, float v1) {
-  __nv_bfloat162 hi, lo;
-  if (f16) {
-    hi.x = f16_bits(v0);
-    hi.y = f16_bits(v1);
-  } else {
-    split_bf16(v0, hi.x, lo.x);
-    split_bf16(v1, hi.y, lo.y);
-  }
-  *reinterpret_cast<__nv_bfloat162*>(dst) = hi;
-  if (planes == 2) *reinterpret_cast<__nv_bfloat162*>(dst + plane_stride) = lo;
+  const Bits16 b0 = to_bits16(v0, f16), b1 = to_bits16(v1, f16);
+  *reinterpret_cast<__nv_bfloat162*>(dst) = __halves2bfloat162(b0.hi, b1.hi);
+  if (planes == 2) *reinterpret_cast<__nv_bfloat162*>(dst + plane_stride) = __halves2bfloat162(b0.lo, b1.lo);
 }
 
 template <bool VEC2>
@@ -165,20 +144,12 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, __nv_bfloat
         const int tap = k / c_in, ci = k - tap * c_in;
         v = __ldg(w + ((long long)co * c_in + ci) * taps + tap);
       }
-      __nv_bfloat16 hi, lo;
-      if (f16) { hi = f16_bits(v); lo = hi; } else split_bf16(v, hi, lo);
-      out[i] = hi;
-      if (planes == 2) out[plane_elems + i] = lo;
+      store_bits16(out, i, plane_elems, planes, v, f16);
     } else {
       const bool in = co < c_out && k < c_in;
       const float* src = w + ((long long)co * c_in + k) * taps;
-      for (int tap = 0; tap < taps; ++tap) {
-        const float v = in ? __ldg(src + tap) : 0.0f;
-        __nv_bfloat16 hi, lo;
-        if (f16) { hi = f16_bits(v); lo = hi; } else split_bf16(v, hi, lo);
-        out[tap * slab + i] = hi;
-        if (planes == 2) out[plane_elems + tap * slab + i] = lo;
-      }
+      for (int tap = 0; tap < taps; ++tap)
+        store_bits16(out, tap * slab + i, plane_elems, planes, in ? __ldg(src + tap) : 0.0f, f16);
     }
   }
 }

@@ -1,11 +1,38 @@
 // Bandwidth-bound helper kernels around the conv GEMMs: fp32 -> bf16 (hi/lo plane) packing of the
 // network input and of the Conv1d weights, and folding of BatchNorm1d eval statistics into a
-// per-channel affine.  Declarations only; definitions in pack.cu.
+// per-channel affine.  Kernel definitions in pack.cu; the 16-bit rounding every pack shares is here.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 namespace vp3d {
+
+// The one rounding of an fp32 value into the 16-bit operand slots every pack writes (input, forward
+// and transposed weight packs, the fused optimizer, the streaming rings): bf16 hi (round to nearest)
+// and the bf16 residual lo of the split (bf16x3), or with f16 IEEE half bits in a bf16-typed slot,
+// saturated at +-65504 like the GEMM epilogue (single plane: lo is not stored).
+struct Bits16 {
+  __nv_bfloat16 hi, lo;
+};
+__device__ __forceinline__ Bits16 to_bits16(float v, int f16 = 0) {
+  Bits16 b;
+  if (f16) {
+    b.hi = __ushort_as_bfloat16(__half_as_ushort(__float2half_rn(fminf(fmaxf(v, -65504.0f), 65504.0f))));
+    b.lo = b.hi;
+  } else {
+    b.hi = __float2bfloat16_rn(v);
+    b.lo = __float2bfloat16_rn(v - __bfloat162float(b.hi));
+  }
+  return b;
+}
+// element o of a [planes][...] pack: hi into plane 0, lo into plane 1 when there are two
+__device__ __forceinline__ void store_bits16(__nv_bfloat16* pack, long long o, long long plane_elems,
+                                             int planes, float v, int f16 = 0) {
+  const Bits16 b = to_bits16(v, f16);
+  pack[o] = b.hi;
+  if (planes == 2) pack[plane_elems + o] = b.lo;
+}
 
 // x: fp32 (N, T, c_raw) contiguous (model.py:68 view of (N,T,J,F)).
 // out: bf16 [planes][N][rows][k_pad]; row r of sample n gathers `group` consecutive frames starting

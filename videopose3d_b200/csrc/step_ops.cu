@@ -145,13 +145,9 @@ adam_pack_kernel(const __grid_constant__ PackBatch batch, const AdamHyper h) {
         q.t.exp_avg[k] = mv[u];
         q.t.exp_avg_sq[k] = vv[u];
         if (amsgrad) q.t.max_exp_avg_sq[k] = xv[u];
-        if (q.fwd) {
-          const long long o = ((long long)tap * q.fwd_n_pad + co) * q.fwd_k_pad + ci;
-          const __nv_bfloat16 hi = __float2bfloat16_rn(pv[u]);
-          q.fwd[o] = hi;
-          if (batch.planes == 2)
-            q.fwd[fwd_plane + o] = __float2bfloat16_rn(pv[u] - __bfloat162float(hi));
-        }
+        if (q.fwd)
+          store_bits16(q.fwd, ((long long)tap * q.fwd_n_pad + co) * q.fwd_k_pad + ci, fwd_plane,
+                       batch.planes, pv[u]);
       }
       sm[j][tx] = pv[u];
     }
@@ -160,13 +156,9 @@ adam_pack_kernel(const __grid_constant__ PackBatch batch, const AdamHyper h) {
 #pragma unroll
       for (int j = ty; j < 32; j += 8) {
         const int ci = ci0 + j, co = co0 + tx;
-        if (ci < q.c_in && co < q.c_out) {
-          const float v = sm[tx][j];
-          const long long o = ((long long)tap * q.tr_n_pad + ci) * q.tr_k_pad + co;
-          const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-          q.tr[o] = hi;
-          if (batch.planes == 2) q.tr[tr_plane + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-        }
+        if (ci < q.c_in && co < q.c_out)
+          store_bits16(q.tr, ((long long)tap * q.tr_n_pad + ci) * q.tr_k_pad + co, tr_plane,
+                       batch.planes, sm[tx][j]);
       }
     }
     __syncthreads();
@@ -341,19 +333,20 @@ int launch_adam_pack(const AdamPackItem* items, int n, int planes, int64_t step,
   int blocks = 0;
   for (int i = 0; i < n; ++i) {
     const AdamPackItem& it = items[i];
+    const PackedConv &fwd = *it.fwd, &tr = *it.tr;
     if (!it.t.param || !it.t.grad || !it.t.exp_avg || !it.t.exp_avg_sq)
       return fail(VP3D_ERR_INVALID, "adam_pack: tensor %d has a null pointer", i);
-    if (it.t.numel != (int64_t)it.c_out * it.c_in * it.taps)
+    if (it.t.numel != (int64_t)tr.c_out * tr.c_in * tr.taps)
       return fail(VP3D_ERR_INVALID, "adam_pack: tensor %d has %lld elements, expected %d x %d x %d", i,
-                  (long long)it.t.numel, it.c_out, it.c_in, it.taps);
+                  (long long)it.t.numel, tr.c_out, tr.c_in, tr.taps);
     PackTensor& q = b.t[b.n++];
-    q.t = it.t; q.fwd = it.fwd; q.tr = it.tr;
-    q.c_out = it.c_out; q.c_in = it.c_in; q.taps = it.taps;
-    q.fwd_n_pad = it.fwd_n_pad; q.fwd_k_pad = it.fwd_k_pad;
-    q.tr_n_pad = it.tr_n_pad; q.tr_k_pad = it.tr_k_pad;
+    q.t = it.t; q.fwd = fwd.w; q.tr = tr.w;
+    q.c_out = tr.c_out; q.c_in = tr.c_in; q.taps = tr.taps;
+    q.fwd_n_pad = fwd.n_pad; q.fwd_k_pad = fwd.k_pad;
+    q.tr_n_pad = tr.n_pad; q.tr_k_pad = tr.k_pad;
     q.first_block = blocks;
-    q.tiles_ci = (it.c_in + 31) / 32;
-    blocks += ((it.c_out + 31) / 32) * q.tiles_ci;
+    q.tiles_ci = (tr.c_in + 31) / 32;
+    blocks += ((tr.c_out + 31) / 32) * q.tiles_ci;
   }
   adam_pack_kernel<<<blocks, 256, 0, stream>>>(b, h);
   CUDA_TRY(cudaGetLastError());

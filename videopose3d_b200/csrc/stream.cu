@@ -38,8 +38,6 @@
 // active, length) is double-buffered by push parity: the input kernel reads buffer `parity` and
 // writes buffer `parity ^ 1`, so the pack, which depends on the bookkeeping of its slot, reads only
 // values no block of the same launch writes, whatever order the blocks run in.
-#include <cuda_fp16.h>
-
 #include "internal.cuh"
 #include "launch.cuh"
 
@@ -109,12 +107,6 @@ inline int pos_mod(long long a, int m) { return (int)(((a % m) + m) % m); }
 __device__ __forceinline__ int pos_mod_dev(int a, int m) { return ((a % m) + m) % m; }
 // the other copy of a ring position in [0, 2R)
 __device__ __forceinline__ int mirror_pos(int a, int R) { return a < R ? a + R : a - R; }
-
-__device__ __forceinline__ __nv_bfloat16 to_f16_bits(float v) {
-  // the input pack's fp16 format (pack.cu): saturate, round to nearest
-  v = fminf(fmaxf(v, -65504.0f), 65504.0f);
-  return __ushort_as_bfloat16(__half_as_ushort(__float2half_rn(v)));
-}
 
 struct StepArgs {
   StreamRing ring[kMaxRings];
@@ -229,16 +221,9 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
       float v1 = c0 + 1 < a.c_raw ? __ldg(src + i1) : 0.0f;
       if (n0) v0 = -v0;
       if (n1) v1 = -v1;
-      __nv_bfloat162 hi, lo;
-      if (a.f16) {
-        hi.x = to_f16_bits(v0);
-        hi.y = to_f16_bits(v1);
-      } else {
-        hi.x = __float2bfloat16_rn(v0);
-        hi.y = __float2bfloat16_rn(v1);
-        lo.x = __float2bfloat16_rn(v0 - __bfloat162float(hi.x));
-        lo.y = __float2bfloat16_rn(v1 - __bfloat162float(hi.y));
-      }
+      const Bits16 b0 = to_bits16(v0, a.f16), b1 = to_bits16(v1, a.f16);
+      const __nv_bfloat162 hi = __halves2bfloat162(b0.hi, b1.hi);
+      const __nv_bfloat162 lo = __halves2bfloat162(b0.lo, b1.lo);
       *reinterpret_cast<__nv_bfloat162*>(r0.base + d0) = hi;
       *reinterpret_cast<__nv_bfloat162*>(r0.base + d1) = hi;
       if (a.planes == 2) {
@@ -440,7 +425,6 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   auto new_rows = [&](int l) {
     return ring[l].base + (long long)(ring[l].w0 + ring[l].H) * P * ring[l].ld;
   };
-  const int* fw = p->cfg.filter_widths;
 
   vp3d_conv_desc d;
   auto common = [&](vp3d_conv_desc& q) {
@@ -472,25 +456,25 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i), every tap on the same row
     common(d);
     d.a = new_rows(0); d.a_plane_stride = ring[0].plane; d.a_rows = P; d.a_ld = p->c_in_pad;
-    d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+    use_pack(&d, *p->expand_dil);
     d.tap_row_step = 0; d.out_rows = P;
-    d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
+    d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
     set_out(d, 0, true);
     VP3D_TRY(run_conv(&d, stream));
     ++launches;
     for (int i = 1; i < p->nb; ++i) {
-      const PackedConv& c0 = p->conv[2 * (i - 1)];
-      const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
+      const PackedConv& c0 = *p->conv[2 * (i - 1)];
+      const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
       common(d);
       d.a = vbuf(i); d.a_plane_stride = v_plane; d.a_rows = P; d.a_ld = C;
-      d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
+      use_pack(&d, c0);
       d.tap_row_step = 0; d.out_rows = P;
       d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
       d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
       VP3D_TRY(run_conv(&d, stream));
       common(d);
       d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = P; d.a_ld = C;
-      d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = P;
+      use_pack(&d, c1); d.out_rows = P;
       d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
       d.res = vbuf(i); d.res_plane_stride = v_plane; d.res_ld = C; d.res_row_step = 1;
       d.res_row_off = 0;
@@ -527,25 +511,25 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   common(d);
   d.a = window(0); d.a_plane_stride = ring[0].plane; d.a_rows = (ring[0].H + k) * P;
   d.a_ld = p->c_in_pad;
-  d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+  use_pack(&d, *p->expand_dil);
   d.tap_row_step = P; d.out_rows = k * P;
-  d.scale = p->expand_dil.scale; d.shift = p->expand_dil.shift; d.relu = 1;
+  d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
   set_out(d, 0, false);
   VP3D_TRY(run_conv(&d, stream));
   ++launches;
   for (int i = 1; i <= p->nb; ++i) {
-    const PackedConv& c0 = p->conv[2 * (i - 1)];
-    const PackedConv& c1 = p->conv[2 * (i - 1) + 1];
+    const PackedConv& c0 = *p->conv[2 * (i - 1)];
+    const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
     common(d);
     d.a = window(i); d.a_plane_stride = ring[i].plane; d.a_rows = (ring[i].H + k) * P; d.a_ld = C;
-    d.w = c0.w; d.taps = c0.taps; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, c0);
     d.tap_row_step = p->dilation[i] * P; d.out_rows = k * P;
     d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
     d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
     VP3D_TRY(run_conv(&d, stream));
     common(d);
     d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
-    d.w = c1.w; d.taps = 1; d.k_per_tap = C; d.n_pad = C; d.out_rows = k * P;
+    use_pack(&d, c1); d.out_rows = k * P;
     d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
     // residual: the centre tap (causal: the newest) of the block input window, model.py:130-132
     d.res = window(i); d.res_plane_stride = ring[i].plane; d.res_ld = C; d.res_row_step = 1;
@@ -560,8 +544,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
   common(d);
   d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
-  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad; d.out_rows = k * P;
-  d.scale = p->shrink.scale; d.shift = p->shrink.shift; d.relu = 0;
+  use_pack(&d, *p->shrink); d.out_rows = k * P;
+  d.scale = p->shrink->scale; d.shift = p->shrink->shift; d.relu = 0;
   d.out_f32 = direct ? y + (long long)f_off * p->c_out_raw : ybuf;
   d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
   VP3D_TRY(run_conv(&d, stream));

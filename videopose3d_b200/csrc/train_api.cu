@@ -31,14 +31,11 @@
 
 namespace vp3d {
 
+// Everything a training plan adds, built whole by ensure_train_state; it owns every buffer in
+// `allocs`, among them the plan's transposed packs (vp3d_plan::conv_t, shrink_t, expand_t).
 struct TrainState {
-  __nv_bfloat16* conv_t[VP3D_MAX_LAYERS] = {};  // [planes][taps][C][C], out[tap][ci][co]
-  __nv_bfloat16* shrink_t = nullptr;            // [planes][1][C][c_out_pad128]
-  bool packed_t = false;
-  // transposed expand pack for the input gradient (VP3D_PACK_EXPAND_T): dilated [planes][w0][c_in_pad][C],
-  // strided tap-merged [planes][1][k0_pad][C] (row tap*c_in + ci)
-  __nv_bfloat16* expand_t = nullptr;
-  bool packed_expand_t = false;
+  bool packed_t = false;         // transposed layer and shrink packs are current
+  bool packed_expand_t = false;  // transposed expand pack (VP3D_PACK_EXPAND_T) is current
   float* vec = nullptr;       // per BN layer l: scale, shift, mean, invstd, stats[2C], sums[2C]
   size_t vec_floats = 0;
   float* shrink_affine = nullptr;  // scale / shift of the shrink bias [2 * c_out_pad]
@@ -69,47 +66,58 @@ struct TrainState {
 void train_state_destroy(TrainState* t) {
   if (!t) return;
   for (void* q : t->allocs) cudaFree(q);
-  if (t->sync_slots) cudaFree(t->sync_slots);
   delete t;
 }
 
 namespace {
 
-int t_alloc(TrainState* t, void** out, size_t bytes) {
+template <typename T>
+int t_alloc(TrainState* t, T** out, size_t bytes) {
   void* q = nullptr;
   CUDA_TRY(cudaMalloc(&q, bytes));
   t->allocs.push_back(q);
-  *out = q;
+  *out = static_cast<T*>(q);
   return VP3D_OK;
 }
 
-int c_out_pad128(const vp3d_plan* p) { return round_up(p->c_out_raw, 128); }
+void t_free(TrainState* t, void* q) {
+  for (size_t i = 0; i < t->allocs.size(); ++i)
+    if (t->allocs[i] == q) {
+      t->allocs.erase(t->allocs.begin() + i);
+      break;
+    }
+  cudaFree(q);
+}
 
+// every buffer of the training state, the transposed packs into tr[] (indexed like p->packs)
+int train_state_alloc(const vp3d_plan* p, TrainState* t, __nv_bfloat16** tr) {
+  for (int i = 0; i < p->n_packs; ++i)
+    if (p->packs[i].transposed) VP3D_TRY(t_alloc(t, &tr[i], pack_bytes(p, p->packs[i])));
+  t->vec_floats = (size_t)(2 * p->nb + 1) * 8 * p->C;
+  VP3D_TRY(t_alloc(t, &t->vec, t->vec_floats * sizeof(float)));
+  VP3D_TRY(t_alloc(t, &t->shrink_affine, 2 * p->c_out_pad * sizeof(float)));
+  VP3D_TRY(t_alloc(t, &t->red_scratch, kReduceScratchFloats * sizeof(float)));
+  VP3D_TRY(t_alloc(t, &t->red_counter, kReduceCounters * sizeof(unsigned)));
+  CUDA_TRY(cudaMemset(t->red_counter, 0, kReduceCounters * sizeof(unsigned)));
+  return VP3D_OK;
+}
+
+// Attaches the training state to the plan once every buffer of it exists; on a failure nothing is
+// attached, so the next call fails the same way.
 int ensure_train_state(vp3d_plan* p) {
   if (p->train) return VP3D_OK;
-  TrainState* t = new TrainState();
-  p->train = t;
-  const size_t cc = (size_t)p->C * p->C;
-  for (int i = 0; i < p->nb; ++i) {
-    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->conv_t[2 * i]),
-                     (size_t)p->planes * p->taps[i + 1] * cc * 2));
-    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->conv_t[2 * i + 1]), (size_t)p->planes * cc * 2));
-  }
-  VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->shrink_t),
-                   (size_t)p->planes * p->C * c_out_pad128(p) * 2));
-  {
-    const size_t rows_dil = (size_t)p->cfg.filter_widths[0] * p->c_in_pad;
-    const size_t rows = rows_dil > (size_t)p->k0_pad ? rows_dil : (size_t)p->k0_pad;
-    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->expand_t), (size_t)p->planes * rows * p->C * 2));
-  }
-  t->vec_floats = (size_t)(2 * p->nb + 1) * 8 * p->C;
-  VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->vec), t->vec_floats * sizeof(float)));
-  VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->shrink_affine), 2 * p->c_out_pad * sizeof(float)));
   if (p->C > kReduceMaxChannels)
     return fail(VP3D_ERR_UNSUPPORTED, "training supports at most %d channels", kReduceMaxChannels);
-  VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->red_scratch), kReduceScratchFloats * sizeof(float)));
-  VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->red_counter), kReduceCounters * sizeof(unsigned)));
-  CUDA_TRY(cudaMemset(t->red_counter, 0, kReduceCounters * sizeof(unsigned)));
+  TrainState* t = new TrainState();
+  __nv_bfloat16* tr[kMaxPacks] = {};
+  const int st = train_state_alloc(p, t, tr);
+  if (st) {
+    train_state_destroy(t);
+    return st;
+  }
+  for (int i = 0; i < p->n_packs; ++i)
+    if (p->packs[i].transposed) p->packs[i].w = tr[i];
+  p->train = t;
   return VP3D_OK;
 }
 
@@ -172,7 +180,7 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
   w.g0 = take(big);
   w.g1 = take(big);
   w.dz = take(big);
-  w.dyp = take(pl * w.rows[p->nb] * c_out_pad128(p) * 2);
+  w.dyp = take(pl * w.rows[p->nb] * p->shrink_t->k_pad * 2);   // dY in K layout of shrink_t
   // wgrad partials: up to 8 splits x taps x C x max(C, k0_pad) fp32
   int max_taps = 1;
   for (int i = 1; i <= p->nb; ++i) max_taps = p->taps[i] > max_taps ? p->taps[i] : max_taps;
@@ -279,39 +287,29 @@ DropoutCfg drop_cfg(const TrainState* t, int layer) {
 
 }  // namespace
 
+// the forward pack a transposed layer / shrink pack is written with
+static const PackedConv* forward_of(const vp3d_plan* p, const PackedConv& k) {
+  return k.src == kSrcShrink ? p->shrink : p->conv[k.src];
+}
+
 // also_forward: the same kernels write the forward packs of the block convs and of shrink (one read
 // of the fp32 weights per optimizer step instead of two).
 int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream,
                           bool also_forward) {
   VP3D_TRY(ensure_train_state(p));
-  TrainState* t = p->train;
-  for (int i = 0; i < p->nb; ++i) {
-    CUDA_TRY(launch_pack_conv_weight_t(w->layers_conv_weight[2 * i], t->conv_t[2 * i], p->planes,
-                                       p->c_real, p->c_real, p->taps[i + 1], p->C, p->C, stream,
-                                       also_forward ? p->conv[2 * i].w : nullptr, p->C, p->C));
-    CUDA_TRY(launch_pack_conv_weight_t(w->layers_conv_weight[2 * i + 1], t->conv_t[2 * i + 1],
-                                       p->planes, p->c_real, p->c_real, 1, p->C, p->C, stream,
-                                       also_forward ? p->conv[2 * i + 1].w : nullptr, p->C, p->C));
+  for (int i = 0; i < p->n_packs; ++i) {
+    const PackedConv& k = p->packs[i];
+    if (k.transposed && k.src != kSrcExpand)
+      VP3D_TRY(pack_weight(p, k, w, stream, also_forward ? forward_of(p, k) : nullptr));
   }
-  CUDA_TRY(launch_pack_conv_weight_t(w->shrink_weight, t->shrink_t, p->planes, p->c_out_raw,
-                                     p->c_real, 1, p->C, c_out_pad128(p), stream,
-                                     also_forward ? p->shrink.w : nullptr, p->c_out_pad, p->C));
-  t->packed_t = true;
+  p->train->packed_t = true;
   return VP3D_OK;
 }
 
 int train_pack_expand_t(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream) {
-  if (!w->expand_conv_weight) return fail(VP3D_ERR_INVALID, "set_weights: missing expand_conv.weight");
   VP3D_TRY(ensure_train_state(p));
-  TrainState* t = p->train;
-  const int w0 = p->cfg.filter_widths[0];
-  if (p->cfg.variant == VP3D_VARIANT_STRIDED)
-    CUDA_TRY(launch_pack_conv_weight_t(w->expand_conv_weight, t->expand_t, p->planes, p->c_real,
-                                       p->c_in_raw, w0, p->k0_pad, p->C, stream, nullptr, 0, 0, 1));
-  else
-    CUDA_TRY(launch_pack_conv_weight_t(w->expand_conv_weight, t->expand_t, p->planes, p->c_real,
-                                       p->c_in_raw, w0, p->c_in_pad, p->C, stream));
-  t->packed_expand_t = true;
+  VP3D_TRY(pack_weight(p, *p->expand_t, w, stream));
+  p->train->packed_expand_t = true;
   return VP3D_OK;
 }
 
@@ -342,15 +340,13 @@ VP3D_API int vp3d_set_bn_sync(vp3d_plan* p, int world, int rank, vp3d_bn_exchang
     t->sync = TrainState::BnSync();
     return VP3D_OK;
   }
-  if (!t->sync_n)
-    VP3D_TRY(t_alloc(t, reinterpret_cast<void**>(&t->sync_n), (VP3D_MAX_LAYERS + 1) * sizeof(float)));
+  if (!t->sync_n) VP3D_TRY(t_alloc(t, &t->sync_n, (VP3D_MAX_LAYERS + 1) * sizeof(float)));
   if (world > t->sync_cap) {
     // grows only; a backward still pending across the reallocation stays valid: it zeroes its
     // slots itself and the forward's global counts live in sync_n
-    const size_t floats = (size_t)(2 * p->nb + 1) * 5 * world * p->C;
     float* q = nullptr;
-    CUDA_TRY(cudaMalloc(&q, floats * sizeof(float)));
-    if (t->sync_slots) cudaFree(t->sync_slots);
+    VP3D_TRY(t_alloc(t, &q, (size_t)(2 * p->nb + 1) * 5 * world * p->C * sizeof(float)));
+    if (t->sync_slots) t_free(t, t->sync_slots);
     t->sync_slots = q;
     t->sync_cap = world;
   }
@@ -484,13 +480,13 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
     CUDA_TRY(launch_pack_input(x, bf(wl.a0), pl, N, T, p->c_in_raw, L[0], fw[0], fw[0], p->k0_pad,
                                wl.rows[0] * p->k0_pad, stream));
     d.a = bf(wl.a0); d.a_rows = (int)wl.rows[0]; d.a_ld = p->k0_pad;
-    d.w = p->expand_flat.w; d.taps = 1; d.k_per_tap = p->k0_pad; d.n_pad = C;
+    use_pack(&d, *p->expand_flat);
     d.out_rows = (int)wl.rows[0];
   } else {
     CUDA_TRY(launch_pack_input(x, bf(wl.a0), pl, N, T, p->c_in_raw, T, 1, 1, p->c_in_pad,
                                (long long)N * T * p->c_in_pad, stream));
     d.a = bf(wl.a0); d.samples = N; d.a_rows = T; d.a_ld = p->c_in_pad;
-    d.w = p->expand_dil.w; d.taps = fw[0]; d.k_per_tap = p->c_in_pad; d.n_pad = C;
+    use_pack(&d, *p->expand_dil);
     d.per_sample_tiles = 1; d.tap_row_step = 1; d.out_rows = L[0];
   }
   ++launches;
@@ -506,7 +502,7 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
     const long long rows = wl.rows[i];
     const int l1 = 2 * i - 1, l2 = 2 * i;
     common(d);
-    d.w = p->conv[2 * (i - 1)].w; d.taps = p->taps[i]; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, *p->conv[2 * (i - 1)]);
     if (strided) {
       d.a = bf(wl.x[i - 1]); d.a_rows = (int)rows; d.a_ld = fw[i] * C;
       d.tap_col_step = C; d.out_rows = (int)rows;
@@ -523,7 +519,7 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
 
     common(d);
     d.a = bf(wl.h[i]); d.a_rows = (int)rows; d.a_ld = C;
-    d.w = p->conv[2 * (i - 1) + 1].w; d.taps = 1; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, *p->conv[2 * (i - 1) + 1]);
     d.out_rows = (int)rows;
     d.out = bf(wl.z[l2]); d.out_plane_stride = rows * C; d.out_ld = C;
     d.stats = frozen ? nullptr : slab_part;
@@ -539,7 +535,7 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
   // ---- shrink (model.py:196)
   common(d);
   d.a = bf(wl.x[p->nb]); d.a_rows = (int)wl.rows[p->nb]; d.a_ld = C;
-  d.w = p->shrink.w; d.taps = 1; d.k_per_tap = C; d.n_pad = p->c_out_pad;
+  use_pack(&d, *p->shrink);
   d.out_rows = (int)wl.rows[p->nb];
   d.scale = t->shrink_affine; d.shift = t->shrink_affine + p->c_out_pad;
   d.out_f32 = y; d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
@@ -605,7 +601,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
         return fail(VP3D_ERR_INVALID, "backward: missing gradient buffer for layer %d", l);
   }
   int launches = 0;
-  const int co128 = c_out_pad128(p);
+  const int dy_ld = p->shrink_t->k_pad;   // padded dY, the K operand of the shrink data gradient
   const long long rows_top = wl.rows[p->nb];
   // the forward's synchronized-BatchNorm setting (never set after a frozen-BatchNorm forward)
   const TrainState::BnSync sync = t->fwd_sync;
@@ -687,14 +683,14 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
 
   // ---- shrink backward: y = X_nb * Wsh^T + b
   CUDA_TRY(launch_pack_input(dy, bf(wl.dyp), pl, 1, (int)rows_top, p->c_out_raw, (int)rows_top, 1, 1,
-                             co128, rows_top * co128, stream));
+                             dy_ld, rows_top * dy_ld, stream));
   ++launches;
   if (want_w) {
     CUDA_TRY(launch_col_sum_f32(dy, rows_top, p->c_out_raw, slab_part, wl.slab_floats, g->shrink_bias,
                                 t->red_scratch, t->red_counter, stream));
     launches += 2;
     WgradCall c;
-    c.dz = bf(wl.dyp); c.dz_ld = co128; c.x = bf(wl.x[p->nb]); c.x_ld = C; c.rows = rows_top;
+    c.dz = bf(wl.dyp); c.dz_ld = dy_ld; c.x = bf(wl.x[p->nb]); c.x_ld = C; c.rows = rows_top;
     c.c_out = p->c_out_raw; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->shrink_weight;
     VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
     launches += 2;
@@ -702,8 +698,8 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
   __nv_bfloat16* gb[2] = {bf(wl.g0), bf(wl.g1)};
   int cur = 0;
   common(d);
-  d.a = bf(wl.dyp); d.a_rows = (int)rows_top; d.a_ld = co128;
-  d.w = t->shrink_t; d.taps = 1; d.k_per_tap = co128; d.n_pad = C;
+  d.a = bf(wl.dyp); d.a_rows = (int)rows_top; d.a_ld = dy_ld;
+  use_pack(&d, *p->shrink_t);
   d.out_rows = (int)rows_top;
   d.out = gb[cur]; d.out_plane_stride = rows_top * C; d.out_ld = C;
   fuse_bnb(d, 2 * p->nb);  // G_nb feeds the BN backward of the top block's second conv (or expand)
@@ -728,7 +724,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
     }
     common(d);
     d.a = bf(wl.dz); d.a_rows = (int)rows; d.a_ld = C;
-    d.w = t->conv_t[c2]; d.taps = 1; d.k_per_tap = C; d.n_pad = C;
+    use_pack(&d, *p->conv_t[c2]);
     d.out_rows = (int)rows;
     d.out = gb[cur ^ 1]; d.out_plane_stride = rows * C; d.out_ld = C;
     fuse_bnb(d, l1);
@@ -752,13 +748,14 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       launches += 2;
     }
     common(d);
-    d.w = t->conv_t[c1]; d.k_per_tap = C;
+    use_pack(&d, *p->conv_t[c1]);
     d.res = gb[cur]; d.res_planes = pl; d.res_plane_stride = rows * C; d.res_ld = C;
     d.out = gb[cur ^ 1];
     if (strided) {
-      // G_{i-1}[rows, w*C] = dZ1 * W1^T  (+ G_i in the columns of the residual tap)
+      // G_{i-1}[rows, w*C] = dZ1 * W1^T  (+ G_i in the columns of the residual tap): the pack's
+      // taps slabs [ci][co] read as one [taps*ci][co] slab
       d.a = bf(wl.dz); d.a_rows = (int)rows; d.a_ld = C;
-      d.taps = 1; d.n_pad = p->taps[i] * C;
+      d.n_pad = d.taps * d.n_pad; d.taps = 1;
       d.out_rows = (int)rows;
       d.out_plane_stride = rows * fw[i] * C; d.out_ld = fw[i] * C;
       d.res_rows_per_sample = 0; d.res_row_step = 1; d.res_row_off = 0;
@@ -767,7 +764,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       // transposed convolution: G_{i-1}[n, t] = sum_k dZ1[n, t - k*d] * W1_k^T  (+ G_i[n, t - off]);
       // rows outside [0, L_i) are zero-filled by the A / residual tensor maps
       d.a = bf(wl.dz); d.samples = N; d.a_rows = L[i]; d.a_ld = C;
-      d.taps = p->taps[i]; d.n_pad = C; d.per_sample_tiles = 1;
+      d.per_sample_tiles = 1;
       d.tap_row_step = -p->dilation[i];
       d.out_rows = L[i - 1];
       d.out_plane_stride = wl.rows[i - 1] * C; d.out_ld = C;
@@ -802,12 +799,12 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
     // dX = dZ0 * W0^T through the conv GEMM, fp32 epilogue straight into x's (N, T, J*F) layout
     const int cin = p->c_in_raw, T = t->T;
     common(d);
-    d.a = bf(wl.dz); d.a_ld = C; d.w = t->expand_t; d.k_per_tap = C;
+    d.a = bf(wl.dz); d.a_ld = C;
+    use_pack(&d, *p->expand_t);   // tap-merged (strided) or per tap (dilated)
     d.out_f32 = dx;
     if (strided) {
       // G_x[rows0, w0*cin] = dZ0 * W0^T with the tap-merged pack: column tap*cin + ci of row
       // (n, r) is x[n, r*w0 + tap, ci], i.e. x's own memory order when T = w0 * L0
-      d.taps = 1; d.n_pad = p->k0_pad;
       d.a_rows = (int)wl.rows[0]; d.out_rows = (int)wl.rows[0];
       d.out_f32_ld = fw[0] * cin; d.n_valid = fw[0] * cin;
       const size_t used = (size_t)fw[0] * L[0] * cin;   // floats per sample the output depends on
@@ -828,7 +825,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
       // transposed convolution: dX[n, t] = sum_k dZ0[n, t - k] * W0_k^T; rows outside [0, L0) are
       // zero-filled by the A tensor map, so every one of the T rows is written
       d.samples = N; d.a_rows = L[0]; d.per_sample_tiles = 1;
-      d.taps = fw[0]; d.tap_row_step = -1; d.n_pad = p->c_in_pad;
+      d.tap_row_step = -1;
       d.out_rows = T; d.out_f32_ld = cin; d.n_valid = cin;
       VP3D_TRY(run_conv(&d, stream));
       ++launches;
@@ -861,26 +858,13 @@ VP3D_API int vp3d_adam_step_packed(vp3d_plan* p, const vp3d_weights* w,
   bool expand_seen = false;
   for (int i = 0; i < n_tensors; ++i) {
     const vp3d_adam_tensor& a = tensors[i];
-    AdamPackItem it;
-    memset(&it, 0, sizeof(it));
-    it.t = a;
-    bool is_conv = false;
-    for (int l = 0; l < 2 * p->nb && !is_conv; ++l) {
-      if (a.param != w->layers_conv_weight[l] || !a.param) continue;
-      const int taps = (l % 2 == 0) ? p->taps[l / 2 + 1] : 1;
-      it.fwd = p->conv[l].w; it.tr = t->conv_t[l];
-      it.c_out = p->c_real; it.c_in = p->c_real; it.taps = taps;
-      it.fwd_n_pad = p->C; it.fwd_k_pad = p->C; it.tr_n_pad = p->C; it.tr_k_pad = p->C;
-      is_conv = true;
+    // a layer or shrink weight: the fused update writes its forward and transposed packs
+    const PackedConv* tr = nullptr;
+    for (int j = 0; j < p->n_packs && a.param && !tr; ++j) {
+      const PackedConv& k = p->packs[j];
+      if (k.transposed && k.src != kSrcExpand && conv_weight(w, k.src) == a.param) tr = &k;
     }
-    if (!is_conv && a.param && a.param == w->shrink_weight) {
-      it.fwd = p->shrink.w; it.tr = t->shrink_t;
-      it.c_out = p->c_out_raw; it.c_in = p->c_real; it.taps = 1;
-      it.fwd_n_pad = p->c_out_pad; it.fwd_k_pad = p->C;
-      it.tr_n_pad = p->C; it.tr_k_pad = c_out_pad128(p);
-      is_conv = true;
-    }
-    if (is_conv) packed.push_back(it);
+    if (tr) packed.push_back({a, forward_of(p, *tr), tr});
     else plain.push_back(a);
     if (a.param && a.param == w->expand_conv_weight) expand_seen = true;
   }
@@ -888,13 +872,8 @@ VP3D_API int vp3d_adam_step_packed(vp3d_plan* p, const vp3d_weights* w,
                           weight_decay, stream_));
   VP3D_TRY(launch_adam_pack(packed.data(), (int)packed.size(), p->planes, step, lr, beta1, beta2, eps,
                             weight_decay, stream));
-  if (expand_seen) {  // 104 k elements: the two expand packs (dilated / tap-merged) the usual way
-    const int w0 = p->cfg.filter_widths[0];
-    CUDA_TRY(launch_pack_conv_weight(w->expand_conv_weight, p->expand_dil.w, p->planes, p->c_real,
-                                     p->c_in_raw, w0, p->C, p->c_in_pad, 0, stream));
-    CUDA_TRY(launch_pack_conv_weight(w->expand_conv_weight, p->expand_flat.w, p->planes, p->c_real,
-                                     p->c_in_raw, w0, p->C, p->k0_pad, 1, stream));
-  }
+  // 104 k elements: the two expand packs (dilated / tap-merged) the usual way
+  if (expand_seen) VP3D_TRY(pack_expand_forward(p, w, stream));
   p->last_launches = (plain.empty() ? 0 : 1) + (packed.empty() ? 0 : 1) + (expand_seen ? 2 : 0);
   return VP3D_OK;
 }

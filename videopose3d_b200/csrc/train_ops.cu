@@ -1,6 +1,7 @@
 #include "train_ops.cuh"
 
 #include "launch.cuh"
+#include "pack.cuh"
 
 namespace vp3d {
 
@@ -632,12 +633,8 @@ pack_conv_weight_t_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict
       const float v = (co < c_out && ci < c_in)
                           ? __ldg(w + ((long long)co * c_in + ci) * taps + tap) : 0.0f;
       sm[j][tx] = v;
-      if (fwd && co < fwd_n_pad && ci < fwd_k_pad) {
-        const long long o = ((long long)tap * fwd_n_pad + co) * fwd_k_pad + ci;
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        fwd[o] = hi;
-        if (planes == 2) fwd[fwd_plane + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-      }
+      if (fwd && co < fwd_n_pad && ci < fwd_k_pad)
+        store_bits16(fwd, ((long long)tap * fwd_n_pad + co) * fwd_k_pad + ci, fwd_plane, planes, v);
     }
     __syncthreads();
 #pragma unroll
@@ -645,13 +642,9 @@ pack_conv_weight_t_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict
       const int ci = ci0 + j, co = co0 + tx;
       const int row = merged ? tap * c_in + ci : ci;
       const bool own = !merged || ci < c_in || tap == taps - 1;
-      if (own && row < n_pad && co < k_pad) {
-        const float v = sm[tx][j];
-        const long long o = ((long long)(merged ? 0 : tap) * n_pad + row) * k_pad + co;
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        out[o] = hi;
-        if (planes == 2) out[plane_elems + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-      }
+      if (own && row < n_pad && co < k_pad)
+        store_bits16(out, ((long long)(merged ? 0 : tap) * n_pad + row) * k_pad + co, plane_elems,
+                     planes, sm[tx][j]);
     }
     __syncthreads();
   }
