@@ -211,36 +211,14 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
   return w;
 }
 
-// dW = dZ^T X for one conv layer.  dz: [planes][samples][rows][dz_ld]; x: [planes][samples][x_rows][x_ld]
-// (flat layers: samples = 1).
-struct WgradCall {
-  const __nv_bfloat16* dz = nullptr;
-  int dz_ld = 0;
-  const __nv_bfloat16* x = nullptr;
-  int x_ld = 0;
-  long long rows = 0;     // dZ rows (per sample when per_sample)
-  int per_sample = 0;
-  int samples = 1;
-  long long x_rows = 0;   // X rows per sample (per_sample only)
-  int taps = 1;
-  int tap_col_step = 0;
-  int tap_row_step = 0;
-  int c_out = 0;
-  int c_in_cols = 0;      // columns of X spanned by one tap (merged: taps*c_in)
-  int c_in = 0;
-  int taps_out = 1;
-  int merged = 0;
-  float* grad = nullptr;
-};
-
-// planes: 1 (bf16) or 2 (hi + lo, three products per pair of planes).  The tile width and the
-// split count follow from the shape alone; vp3d_wgrad_gemm reaches the same code.
-int run_wgrad(int planes, const WgradCall& c, float* partial, size_t partial_bytes,
-              cudaStream_t stream) {
+// dW = dZ^T X for one conv layer (the descriptor of vp3d_wgrad_gemm).  The tile width and the
+// split count follow from the shape alone.
+int run_wgrad(const vp3d_wgrad_desc& c, cudaStream_t stream) {
+  const int planes = c.planes;
   const int block_n = pick_block_n(round_up(c.c_in_cols, 64));
   WgradArgs a;
   memset(&a, 0, sizeof(a));
-  a.per_sample = c.per_sample;
+  a.per_sample = c.per_sample ? 1 : 0;
   a.samples = c.per_sample ? c.samples : 1;
   a.rows = (int)c.rows;
   a.kchunks = (int)((c.rows + 63) / 64);
@@ -259,11 +237,11 @@ int run_wgrad(int planes, const WgradCall& c, float* partial, size_t partial_byt
   if (splits > 16) splits = 16;
   if (splits > total_kb) splits = (int)total_kb;
   if (splits < 1) splits = 1;
-  while ((size_t)splits * c.taps * a.m_pad * a.n_pad * 4 > partial_bytes && splits > 1) --splits;
-  if ((size_t)splits * c.taps * a.m_pad * a.n_pad * 4 > partial_bytes)
+  while ((size_t)splits * c.taps * a.m_pad * a.n_pad * 4 > c.partial_bytes && splits > 1) --splits;
+  if ((size_t)splits * c.taps * a.m_pad * a.n_pad * 4 > c.partial_bytes)
     return fail(VP3D_ERR_WORKSPACE, "wgrad partial buffer too small");
   a.splits = splits;
-  a.partial = partial;
+  a.partial = c.partial;
   CUtensorMap mdz, mx;
   const uint64_t x_rows = c.per_sample ? (uint64_t)c.x_rows : (uint64_t)c.rows;
   VP3D_TRY(make_map_4d(&mdz, c.dz, c.dz_ld, c.rows, c.dz_ld, a.samples, (uint64_t)c.rows * c.dz_ld,
@@ -271,17 +249,152 @@ int run_wgrad(int planes, const WgradCall& c, float* partial, size_t partial_byt
   VP3D_TRY(make_map_4d(&mx, c.x, c.x_ld, x_rows, c.x_ld, a.samples, x_rows * c.x_ld, planes,
                        (uint64_t)a.samples * x_rows * c.x_ld, 64));
   CUDA_TRY(launch_wgrad_gemm(mdz, mx, a, block_n, num_sms(), stream));
-  CUDA_TRY(launch_wgrad_reduce(partial, c.grad, splits, c.taps, a.m_pad, a.n_pad, c.c_out, c.c_in,
-                               c.taps_out, c.merged, stream));
+  CUDA_TRY(launch_wgrad_reduce(c.partial, c.grad, splits, c.taps, a.m_pad, a.n_pad, c.c_out, c.c_in,
+                               c.taps_out, c.merged ? 1 : 0, stream));
   return VP3D_OK;
 }
 
-DropoutCfg drop_cfg(const TrainState* t, int layer) {
+DropoutCfg dropout_cfg(float p, unsigned long long seed, int layer) {
   DropoutCfg d;
-  d.p = t->dropout_p;
-  d.seed_lo = (uint32_t)(t->seed & 0xFFFFFFFFu);
-  d.seed_hi = (uint32_t)(t->seed >> 32);
+  d.p = p;
+  d.seed_lo = (uint32_t)(seed & 0xFFFFFFFFu);
+  d.seed_hi = (uint32_t)(seed >> 32);
   d.layer = (uint32_t)layer;
+  return d;
+}
+
+// a conv GEMM descriptor in the plan's precision and planes, every other field cleared
+vp3d_conv_desc conv_desc(const vp3d_plan* p) {
+  vp3d_conv_desc d;
+  memset(&d, 0, sizeof(d));
+  d.a_planes = d.out_planes = p->planes;
+  d.precision = p->cfg.precision;
+  d.samples = 1;
+  return d;
+}
+
+// elements of one plane of a GEMM's A operand, the conv's input
+long long in_plane(const vp3d_conv_desc& d) { return (long long)d.samples * d.a_rows * d.a_ld; }
+
+// 32-row slabs of the per-channel partials a GEMM epilogue writes (statistics or fused BatchNorm
+// backward): four per 128-row tile, the tiles per sample (per-sample tiling) or over all rows
+int stat_slabs(const vp3d_conv_desc& d) {
+  return (d.per_sample_tiles ? d.samples : 1) * ((d.out_rows + 127) / 128) * 4;
+}
+
+// columns of the input one tap of conv k spans: all taps' when they are merged into one GEMM
+int in_cols(const PackedConv& k) { return k.merged ? k.taps * k.c_in : k.c_in; }
+
+// One conv of the training step.  `fwd` is its forward GEMM: the A view of its input (samples,
+// rows, ld, per-sample tiles, tap step), the output rows and the forward pack, writing Z.  The
+// backward derives its weight and data gradients from it (wgrad_desc, dgrad_desc), so that they
+// read and write the views the forward used.
+struct TrainConv {
+  vp3d_conv_desc fwd;        // shrink: no output set (the forward adds its fp32 epilogue)
+  const PackedConv* pack;    // forward pack: the gradient's c_out, c_in, taps, merged
+  const PackedConv* t;       // transposed pack of the data gradient
+  __nv_bfloat16 *in, *z, *act;   // input (= fwd.a), Z (= fwd.out), the BatchNorm's output
+  RowMap res;                // block second conv: the block input rows its skip connection adds
+                             // (res.off: the frame of the input row, or the row offset, it takes)
+};
+
+// The convs of the training step indexed by BatchNorm layer (0 expand, 2i-1 / 2i block i's first
+// and second conv) and shrink at 2B + 1.  Besides train_layout the only code that tells the two
+// layouts apart: strided (flat rows; the expand conv's taps merged into one GEMM over w0 frames per
+// input row, a first conv's taps column blocks of a w*C-wide view of the rows) and dilated
+// (per-sample tiles, the taps rows `dilation` apart).
+void train_convs(const vp3d_plan* p, const TrainLayout& wl, uint8_t* base, int N, int T,
+                 const int* L, TrainConv* cv) {
+  const bool strided = p->cfg.variant == VP3D_VARIANT_STRIDED;
+  const int C = p->C, nb = p->nb;
+  const int* fw = p->cfg.filter_widths;
+  auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
+  auto conv = [&](int l, const PackedConv* k, const PackedConv* kt, size_t in, long long a_rows,
+                  int a_ld, long long out_rows) -> vp3d_conv_desc& {
+    TrainConv& c = cv[l];
+    c.pack = k; c.t = kt; c.in = bf(in); c.z = c.act = nullptr; c.res = RowMap{0, 0, 1, 0};
+    vp3d_conv_desc& d = c.fwd = conv_desc(p);
+    use_pack(&d, *k);
+    d.a = c.in; d.a_rows = (int)a_rows; d.a_ld = a_ld; d.out_rows = (int)out_rows;
+    return d;
+  };
+  auto per_sample = [&](vp3d_conv_desc& d, int step) {
+    d.samples = N; d.per_sample_tiles = 1; d.tap_row_step = step;
+  };
+  if (strided) {
+    conv(0, p->expand_flat, p->expand_t, wl.a0, wl.rows[0], p->k0_pad, wl.rows[0]);
+  } else {
+    per_sample(conv(0, p->expand_dil, p->expand_t, wl.a0, T, p->c_in_pad, L[0]), 1);
+  }
+  for (int i = 1; i <= nb; ++i) {
+    const int l1 = 2 * i - 1, l2 = 2 * i;
+    if (strided) {
+      conv(l1, p->conv[l1 - 1], p->conv_t[l1 - 1], wl.x[i - 1], wl.rows[i], fw[i] * C, wl.rows[i])
+          .tap_col_step = C;
+    } else {
+      per_sample(conv(l1, p->conv[l1 - 1], p->conv_t[l1 - 1], wl.x[i - 1], L[i - 1], C, L[i]),
+                 p->dilation[i]);
+    }
+    conv(l2, p->conv[l2 - 1], p->conv_t[l2 - 1], wl.h[i], wl.rows[i], C, wl.rows[i]);
+    cv[l2].res = strided ? RowMap{0, 0, fw[i], fw[i] / 2 + p->shift_str[i]}
+                         : RowMap{L[i], L[i - 1], 1, p->pad[i] + p->shift_dil[i]};
+  }
+  conv(2 * nb + 1, p->shrink, p->shrink_t, wl.x[nb], wl.rows[nb], C, wl.rows[nb]);
+  for (int l = 0; l <= 2 * nb; ++l) {
+    const int i = (l + 1) / 2;   // the block whose rows layer l has (0: expand)
+    TrainConv& c = cv[l];
+    c.z = bf(wl.z[l]);
+    c.act = bf(l % 2 ? wl.h[i] : wl.x[i]);
+    c.fwd.out = c.z; c.fwd.out_plane_stride = wl.rows[i] * C; c.fwd.out_ld = C;
+  }
+}
+
+// The weight gradient of conv c from its forward GEMM: dZ (rows as the forward's output, pitch the
+// transposed pack's K) against the forward's A view with the forward's taps.
+vp3d_wgrad_desc wgrad_desc(const TrainConv& c, const __nv_bfloat16* dz, float* grad, float* partial,
+                           size_t partial_bytes) {
+  const vp3d_conv_desc& f = c.fwd;
+  vp3d_wgrad_desc w;
+  memset(&w, 0, sizeof(w));
+  w.dz = dz; w.dz_ld = c.t->k_pad;
+  w.x = f.a; w.x_ld = f.a_ld; w.x_rows = f.a_rows;
+  w.planes = f.a_planes;
+  w.rows = f.out_rows; w.per_sample = f.per_sample_tiles; w.samples = f.samples;
+  w.taps = f.taps; w.tap_row_step = f.tap_row_step; w.tap_col_step = f.tap_col_step;
+  w.c_out = c.pack->c_out; w.c_in = c.pack->c_in; w.taps_out = c.pack->taps;
+  w.merged = c.pack->merged; w.c_in_cols = in_cols(*c.pack);
+  w.grad = grad; w.partial = partial; w.partial_bytes = partial_bytes;
+  return w;
+}
+
+// The data gradient of conv c from its forward GEMM: dZ, read in the view the forward wrote Z in
+// (pitch the transposed pack's K: C, or the padded dY of shrink), times the transposed pack, into
+// `out` in the view the forward read its input from.  With `res`: plus the skip gradient (dZ's
+// shape) at the input rows the forward's skip connection took, res_off as in TrainConv::res.
+vp3d_conv_desc dgrad_desc(const vp3d_plan* p, const TrainConv& c, const __nv_bfloat16* dz,
+                          __nv_bfloat16* out, const __nv_bfloat16* res = nullptr, int res_off = 0) {
+  const vp3d_conv_desc& f = c.fwd;
+  vp3d_conv_desc d = conv_desc(p);
+  use_pack(&d, *c.t);
+  d.a = dz; d.a_rows = f.out_rows; d.a_ld = c.t->k_pad;
+  d.out = out; d.out_rows = f.a_rows; d.out_plane_stride = in_plane(f); d.out_ld = f.a_ld;
+  if (f.per_sample_tiles) {
+    // row taps: the transposed convolution G[n, t] = sum_k dZ[n, t - k*step] * W_k^T; rows outside
+    // the sample are zero-filled by the A / residual tensor maps
+    d.samples = f.samples; d.per_sample_tiles = 1; d.tap_row_step = -f.tap_row_step;
+  } else {
+    // column or merged taps: one flat GEMM, the pack's tap slabs [ci][co] read as one [taps*ci][co]
+    d.n_pad *= d.taps; d.taps = 1;
+  }
+  if (res) {
+    d.res = res; d.res_planes = f.out_planes; d.res_plane_stride = f.out_plane_stride;
+    d.res_ld = f.out_ld; d.res_row_step = 1;
+    if (f.per_sample_tiles) {   // G_in[n, t] += res[n, t - off]
+      d.res_rows_per_sample = f.out_rows; d.res_row_off = -res_off; d.res_check_rows = 1;
+    } else {                    // frame `off` of each input row
+      d.res_col_begin = res_off * f.out_ld; d.res_cols = f.out_ld;
+    }
+  }
   return d;
 }
 
@@ -408,14 +521,16 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
   if (!ws || ws_bytes < wl.total)
     return fail(VP3D_ERR_WORKSPACE, "train workspace too small: %zu < %zu", ws_bytes, wl.total);
   uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
-  auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
   const int C = p->C, pl = p->planes;
   t->N = N; t->T = T; t->dropout_p = dropout_p; t->seed = seed; t->frozen_bn = frozen;
   t->have_forward = false;
   // frozen BatchNorm has no batch statistics: nothing to exchange, in this forward or its backward
   t->fwd_sync = frozen ? TrainState::BnSync() : t->sync;
   const TrainState::BnSync sync = t->fwd_sync;
+  const bool synced = sync.world > 0;
   for (int i = 0; i <= p->nb; ++i) t->L[i] = L[i];
+  TrainConv cv[VP3D_MAX_LAYERS + 2];
+  train_convs(p, wl, base, N, T, L, cv);
   int launches = 0;
 
   float* slab_part = reinterpret_cast<float*>(base + wl.slab);
@@ -423,120 +538,62 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
                               p->c_out_raw, p->c_out_pad, stream));
   ++launches;
 
-  vp3d_conv_desc d;
-  auto common = [&](vp3d_conv_desc& q) {
-    memset(&q, 0, sizeof(q));
-    q.a_planes = pl;
-    q.precision = p->cfg.precision;
-    q.out_planes = pl;
-    q.samples = 1;
-    q.per_sample_tiles = 0;
-  };
-  int stats_per_sample_rows = 0;  // rows per sample of the last stats-producing GEMM if it ran on
-                                  // per-sample tiles (dilated layout), else 0
-  auto bn = [&](int layer, const float* const* bnp, long long rows, const __nv_bfloat16* z,
-                __nv_bfloat16* out, const __nv_bfloat16* res, long long res_plane, RowMap map) -> int {
+  // BatchNorm (+ ReLU, dropout, skip connection) of `layer` over the Z that GEMM d wrote, whose
+  // epilogue left the per-slab statistics partials in slab_part with its own row tiling
+  auto bn = [&](int layer, const vp3d_conv_desc& d, const float* const* bnp, __nv_bfloat16* out,
+                const __nv_bfloat16* res, long long res_plane, RowMap map) -> int {
     const LayerVec v = layer_vec(p, layer);
-    // the GEMM that produced z left per-slab sums in slab_part; its row tiling: flat over all rows
-    // (strided model and every 1x1 conv) or per-sample tiles (dilated model's k-tap convs)
-    const int per_sample_rows = stats_per_sample_rows;
-    const int tps = per_sample_rows ? (per_sample_rows + 127) / 128 : 0;
-    const int slabs = per_sample_rows ? N * tps * 4 : (int)((rows + 127) / 128) * 4;
+    const long long rows = (long long)d.samples * d.out_rows;
     if (frozen) {  // the eval fold of the running statistics, plus the mean / invstd backward reads
       CUDA_TRY(launch_bn_fold(bnp[0], bnp[1], bnp[2], bnp[3], 1e-5f, v.scale, v.shift, p->c_real, C,
                               stream, v.mean, v.invstd));
-    } else if (sync.world > 0) {
-      // this rank's moments into its slot, the exchange fills the others, then the rank-ordered
-      // merge and the finalize over the global batch
-      float* slots = sync_fwd_slots(p, layer);
-      CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
-                                        per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
-                                        bnp[1], nullptr, nullptr, 0.0f, 1e-5f, v.scale, v.shift,
-                                        v.mean, v.invstd, C, p->c_real, t->red_scratch,
-                                        t->red_counter, stream, slots, sync.world, sync.rank));
-      sync.exchange(layer, VP3D_BN_SYNC_FORWARD, slots, 3 * C, sync.user);
-      CUDA_TRY(launch_bn_sync_finalize(slots, sync.world, bnp[0], bnp[1], const_cast<float*>(bnp[2]),
-                                       const_cast<float*>(bnp[3]), bn_momentum[layer], 1e-5f,
-                                       v.scale, v.shift, v.mean, v.invstd, C, p->c_real,
-                                       t->sync_n + layer, stream));
-      ++launches;
     } else {
-      CUDA_TRY(launch_bn_stats_finalize(slab_part, slabs, per_sample_rows ? 1 : 0,
-                                        per_sample_rows ? per_sample_rows : (int)rows, tps, bnp[0],
-                                        bnp[1], const_cast<float*>(bnp[2]), const_cast<float*>(bnp[3]),
-                                        bn_momentum[layer], 1e-5f, v.scale, v.shift, v.mean, v.invstd,
-                                        C, p->c_real, t->red_scratch, t->red_counter, stream));
+      // synchronized: this rank's moments into its slot, the exchange fills the others, then the
+      // rank-ordered merge and the finalize over the global batch update the running statistics
+      float* slots = synced ? sync_fwd_slots(p, layer) : nullptr;
+      CUDA_TRY(launch_bn_stats_finalize(
+          slab_part, stat_slabs(d), d.per_sample_tiles, d.out_rows,
+          d.per_sample_tiles ? (d.out_rows + 127) / 128 : 0, bnp[0], bnp[1],
+          synced ? nullptr : const_cast<float*>(bnp[2]), synced ? nullptr : const_cast<float*>(bnp[3]),
+          synced ? 0.0f : bn_momentum[layer], 1e-5f, v.scale, v.shift, v.mean, v.invstd, C,
+          p->c_real, t->red_scratch, t->red_counter, stream, slots, sync.world, sync.rank));
+      if (synced) {
+        sync.exchange(layer, VP3D_BN_SYNC_FORWARD, slots, 3 * C, sync.user);
+        CUDA_TRY(launch_bn_sync_finalize(slots, sync.world, bnp[0], bnp[1], const_cast<float*>(bnp[2]),
+                                         const_cast<float*>(bnp[3]), bn_momentum[layer], 1e-5f,
+                                         v.scale, v.shift, v.mean, v.invstd, C, p->c_real,
+                                         t->sync_n + layer, stream));
+        ++launches;
+      }
     }
-    CUDA_TRY(launch_bn_apply(z, rows * C, out, rows * C, pl, rows, C, v.scale, v.shift,
-                             drop_cfg(t, layer), res, res_plane, map, stream));
+    CUDA_TRY(launch_bn_apply(static_cast<const __nv_bfloat16*>(d.out), rows * C, out, rows * C, pl,
+                             rows, C, v.scale, v.shift, dropout_cfg(dropout_p, seed, layer), res,
+                             res_plane, map, stream));
     launches += 2;
     return VP3D_OK;
   };
-  const RowMap no_map = {0, 0, 1, 0};
 
-  // ---- expand (model.py:188 strided / :127 dilated)
-  common(d);
-  if (strided) {
-    CUDA_TRY(launch_pack_input(x, bf(wl.a0), pl, N, T, p->c_in_raw, L[0], fw[0], fw[0], p->k0_pad,
-                               wl.rows[0] * p->k0_pad, stream));
-    d.a = bf(wl.a0); d.a_rows = (int)wl.rows[0]; d.a_ld = p->k0_pad;
-    use_pack(&d, *p->expand_flat);
-    d.out_rows = (int)wl.rows[0];
-  } else {
-    CUDA_TRY(launch_pack_input(x, bf(wl.a0), pl, N, T, p->c_in_raw, T, 1, 1, p->c_in_pad,
-                               (long long)N * T * p->c_in_pad, stream));
-    d.a = bf(wl.a0); d.samples = N; d.a_rows = T; d.a_ld = p->c_in_pad;
-    use_pack(&d, *p->expand_dil);
-    d.per_sample_tiles = 1; d.tap_row_step = 1; d.out_rows = L[0];
-  }
+  // the input rows the expand GEMM reads, w0 frames per row when its taps are merged (model.py:188
+  // strided / :127 dilated)
+  const vp3d_conv_desc& e = cv[0].fwd;
+  const int group = cv[0].pack->merged ? cv[0].pack->taps : 1;
+  CUDA_TRY(launch_pack_input(x, cv[0].in, pl, N, T, p->c_in_raw, e.samples * e.a_rows / N, group,
+                             group, e.a_ld, in_plane(e), stream));
   ++launches;
-  d.out = bf(wl.z[0]); d.out_plane_stride = wl.rows[0] * C; d.out_ld = C;
-  d.stats = frozen ? nullptr : slab_part;
-  stats_per_sample_rows = d.per_sample_tiles ? d.out_rows : 0;
-  VP3D_TRY(run_conv(&d, stream));
-  ++launches;
-  VP3D_TRY(bn(0, w->expand_bn, wl.rows[0], bf(wl.z[0]), bf(wl.x[0]), nullptr, 0, no_map));
-
-  // ---- residual blocks (model.py:190-194)
-  for (int i = 1; i <= p->nb; ++i) {
-    const long long rows = wl.rows[i];
-    const int l1 = 2 * i - 1, l2 = 2 * i;
-    common(d);
-    use_pack(&d, *p->conv[2 * (i - 1)]);
-    if (strided) {
-      d.a = bf(wl.x[i - 1]); d.a_rows = (int)rows; d.a_ld = fw[i] * C;
-      d.tap_col_step = C; d.out_rows = (int)rows;
-    } else {
-      d.a = bf(wl.x[i - 1]); d.samples = N; d.a_rows = L[i - 1]; d.a_ld = C;
-      d.per_sample_tiles = 1; d.tap_row_step = p->dilation[i]; d.out_rows = L[i];
-    }
-    d.out = bf(wl.z[l1]); d.out_plane_stride = rows * C; d.out_ld = C;
+  // expand, then the residual blocks (model.py:190-194)
+  for (int l = 0; l <= 2 * p->nb; ++l) {
+    vp3d_conv_desc d = cv[l].fwd;
     d.stats = frozen ? nullptr : slab_part;
-    stats_per_sample_rows = d.per_sample_tiles ? d.out_rows : 0;
     VP3D_TRY(run_conv(&d, stream));
     ++launches;
-    VP3D_TRY(bn(l1, w->layers_bn[2 * (i - 1)], rows, bf(wl.z[l1]), bf(wl.h[i]), nullptr, 0, no_map));
-
-    common(d);
-    d.a = bf(wl.h[i]); d.a_rows = (int)rows; d.a_ld = C;
-    use_pack(&d, *p->conv[2 * (i - 1) + 1]);
-    d.out_rows = (int)rows;
-    d.out = bf(wl.z[l2]); d.out_plane_stride = rows * C; d.out_ld = C;
-    d.stats = frozen ? nullptr : slab_part;
-    stats_per_sample_rows = 0;
-    VP3D_TRY(run_conv(&d, stream));
-    ++launches;
-    const RowMap rm = strided ? RowMap{0, 0, fw[i], fw[i] / 2 + p->shift_str[i]}
-                              : RowMap{L[i], L[i - 1], 1, p->pad[i] + p->shift_dil[i]};
-    VP3D_TRY(bn(l2, w->layers_bn[2 * (i - 1) + 1], rows, bf(wl.z[l2]), bf(wl.x[i]), bf(wl.x[i - 1]),
-                wl.rows[i - 1] * C, rm));
+    // a block's second conv adds the block's input back (the skip connection)
+    const TrainConv* skip = l > 0 && l % 2 == 0 ? &cv[l - 1] : nullptr;
+    VP3D_TRY(bn(l, d, l ? w->layers_bn[l - 1] : w->expand_bn, cv[l].act, skip ? skip->in : nullptr,
+                skip ? in_plane(skip->fwd) : 0, cv[l].res));
   }
 
   // ---- shrink (model.py:196)
-  common(d);
-  d.a = bf(wl.x[p->nb]); d.a_rows = (int)wl.rows[p->nb]; d.a_ld = C;
-  use_pack(&d, *p->shrink);
-  d.out_rows = (int)wl.rows[p->nb];
+  vp3d_conv_desc d = cv[2 * p->nb + 1].fwd;
   d.scale = t->shrink_affine; d.shift = t->shrink_affine + p->c_out_pad;
   d.out_f32 = y; d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
   VP3D_TRY(run_conv(&d, stream));
@@ -582,10 +639,8 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
   const bool frozen = t->frozen_bn;
   const bool need_sums = want_w || !frozen;   // BatchNorm-backward reductions
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int N = t->N, C = p->C, Cr = p->c_real, pl = p->planes;   // padded / real channels
+  const int N = t->N, C = p->C, pl = p->planes;
   const int* L = t->L;
-  const int* fw = p->cfg.filter_widths;
-  const bool strided = p->cfg.variant == VP3D_VARIANT_STRIDED;
   const TrainLayout wl = train_layout(p, N, t->T, L);
   if (!ws || ws_bytes < wl.total) return fail(VP3D_ERR_WORKSPACE, "backward: workspace too small");
   uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
@@ -614,16 +669,10 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
                              (size_t)(2 * p->nb + 1) * 2 * t->sync_cap * C * sizeof(float), stream));
     ++launches;
   }
+  TrainConv cv[VP3D_MAX_LAYERS + 2];
+  train_convs(p, wl, base, N, t->T, L, cv);
+  const int top = 2 * p->nb;   // the BatchNorm under shrink
 
-  vp3d_conv_desc d;
-  auto common = [&](vp3d_conv_desc& q) {
-    memset(&q, 0, sizeof(q));
-    q.a_planes = pl;
-    q.precision = p->cfg.precision;
-    q.out_planes = pl;
-    q.samples = 1;
-    q.per_sample_tiles = 0;
-  };
   // In single-plane bf16 mode the per-channel reductions of the BatchNorm backward are fused into
   // the epilogue of the GEMM that produces the incoming gradient (fuse_bnb); otherwise a separate
   // pass over (G, Z) computes them.
@@ -633,19 +682,20 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
   auto fuse_bnb = [&](vp3d_conv_desc& q, int layer) {
     if (!fuse || !need_sums) return;
     const LayerVec v = layer_vec(p, layer);
-    q.bnb_z = bf(wl.z[layer]);
+    q.bnb_z = cv[layer].z;
     q.bnb_scale = v.scale; q.bnb_shift = v.shift; q.bnb_mean = v.mean; q.bnb_invstd = v.invstd;
     q.bnb_sums = slab_part; q.bnb_c = C; q.bnb_p = t->dropout_p; q.bnb_seed = t->seed;
     q.bnb_layer = layer;
-    const int tiles = (q.out_rows + 127) / 128;
-    bnb_slabs = (q.per_sample_tiles ? q.samples * tiles : tiles) * 4;
+    bnb_slabs = stat_slabs(q);
     bnb_ld = q.n_pad;
   };
   // BN + ReLU + dropout backward of `layer`: (gin, z) -> dz (+ dgamma, dbeta)
-  auto bn_bwd = [&](int layer, long long rows, const __nv_bfloat16* gin, const __nv_bfloat16* z,
-                    float* dgamma, float* dbeta) -> int {
+  auto bn_bwd = [&](int layer, const __nv_bfloat16* gin) -> int {
     const LayerVec v = layer_vec(p, layer);
-    const DropoutCfg dc = drop_cfg(t, layer);
+    const DropoutCfg dc = dropout_cfg(t->dropout_p, t->seed, layer);
+    const long long rows = (long long)cv[layer].fwd.samples * cv[layer].fwd.out_rows;
+    const __nv_bfloat16* z = cv[layer].z;
+    float* const* dbn = !want_w ? nullptr : layer ? g->layers_bn[layer - 1] : g->expand_bn;
     // synchronized BatchNorm: this rank's sums go to its exchange slot, v.sums receives the
     // rank-ordered global sums
     float* slots = synced ? sync_bwd_slots(p, layer) : nullptr;
@@ -674,14 +724,21 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
     }
     CUDA_TRY(launch_bn_bwd_apply(gin, rows * C, z, rows * C, bf(wl.dz), rows * C, pl, rows, C,
                                  v.scale, v.shift, v.mean, v.invstd, dc,
-                                 need_sums ? local : nullptr, want_w ? dgamma : nullptr,
-                                 want_w ? dbeta : nullptr, p->c_real, stream, frozen ? 1 : 0,
+                                 need_sums ? local : nullptr, dbn ? dbn[0] : nullptr,
+                                 dbn ? dbn[1] : nullptr, p->c_real, stream, frozen ? 1 : 0,
                                  synced ? v.sums : nullptr, synced ? t->sync_n + layer : nullptr));
     ++launches;
     return VP3D_OK;
   };
 
+  auto wgrad = [&](const TrainConv& c, const __nv_bfloat16* dz, float* grad) -> int {
+    VP3D_TRY(run_wgrad(wgrad_desc(c, dz, grad, partial, wl.partial_bytes), stream));
+    launches += 2;
+    return VP3D_OK;
+  };
+
   // ---- shrink backward: y = X_nb * Wsh^T + b
+  const TrainConv& sh = cv[top + 1];
   CUDA_TRY(launch_pack_input(dy, bf(wl.dyp), pl, 1, (int)rows_top, p->c_out_raw, (int)rows_top, 1, 1,
                              dy_ld, rows_top * dy_ld, stream));
   ++launches;
@@ -689,146 +746,58 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
     CUDA_TRY(launch_col_sum_f32(dy, rows_top, p->c_out_raw, slab_part, wl.slab_floats, g->shrink_bias,
                                 t->red_scratch, t->red_counter, stream));
     launches += 2;
-    WgradCall c;
-    c.dz = bf(wl.dyp); c.dz_ld = dy_ld; c.x = bf(wl.x[p->nb]); c.x_ld = C; c.rows = rows_top;
-    c.c_out = p->c_out_raw; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->shrink_weight;
-    VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
-    launches += 2;
+    VP3D_TRY(wgrad(sh, bf(wl.dyp), g->shrink_weight));
   }
   __nv_bfloat16* gb[2] = {bf(wl.g0), bf(wl.g1)};
   int cur = 0;
-  common(d);
-  d.a = bf(wl.dyp); d.a_rows = (int)rows_top; d.a_ld = dy_ld;
-  use_pack(&d, *p->shrink_t);
-  d.out_rows = (int)rows_top;
-  d.out = gb[cur]; d.out_plane_stride = rows_top * C; d.out_ld = C;
-  fuse_bnb(d, 2 * p->nb);  // G_nb feeds the BN backward of the top block's second conv (or expand)
+  vp3d_conv_desc d = dgrad_desc(p, sh, bf(wl.dyp), gb[cur]);
+  fuse_bnb(d, top);  // G_nb feeds the BN backward of the top block's second conv (or expand)
   VP3D_TRY(run_conv(&d, stream));
   ++launches;
   if (stage_done) stage_done(0, user);  // shrink.weight / shrink.bias gradients are enqueued
 
-  // ---- residual blocks, top-down
-  for (int i = p->nb; i >= 1; --i) {
-    const long long rows = wl.rows[i];
-    const int l1 = 2 * i - 1, l2 = 2 * i;
-    const int c1 = 2 * (i - 1), c2 = c1 + 1;
-    // second conv (1x1): X_i = res + act(bn(conv2(H_i)))
-    VP3D_TRY(bn_bwd(l2, rows, gb[cur], bf(wl.z[l2]), want_w ? g->layers_bn[c2][0] : nullptr,
-                    want_w ? g->layers_bn[c2][1] : nullptr));
-    if (want_w) {
-      WgradCall c;
-      c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.h[i]); c.x_ld = C; c.rows = rows;
-      c.c_out = Cr; c.c_in_cols = Cr; c.c_in = Cr; c.grad = g->layers_conv_weight[c2];
-      VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
-      launches += 2;
-    }
-    common(d);
-    d.a = bf(wl.dz); d.a_rows = (int)rows; d.a_ld = C;
-    use_pack(&d, *p->conv_t[c2]);
-    d.out_rows = (int)rows;
-    d.out = gb[cur ^ 1]; d.out_plane_stride = rows * C; d.out_ld = C;
-    fuse_bnb(d, l1);
-    VP3D_TRY(run_conv(&d, stream));
-    ++launches;
-    // first conv (w taps, stride w): H_i = act(bn(conv1(X_{i-1})))
-    VP3D_TRY(bn_bwd(l1, rows, gb[cur ^ 1], bf(wl.z[l1]), want_w ? g->layers_bn[c1][0] : nullptr,
-                    want_w ? g->layers_bn[c1][1] : nullptr));
-    if (want_w) {
-      WgradCall c;
-      c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.x[i - 1]); c.taps = p->taps[i];
-      c.c_out = Cr; c.c_in_cols = Cr; c.c_in = Cr; c.taps_out = p->taps[i];
-      c.grad = g->layers_conv_weight[c1];
-      if (strided) {
-        c.x_ld = fw[i] * C; c.rows = rows; c.tap_col_step = C;
-      } else {
-        c.x_ld = C; c.per_sample = 1; c.samples = N; c.rows = L[i]; c.x_rows = L[i - 1];
-        c.tap_row_step = p->dilation[i];
-      }
-      VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
-      launches += 2;
-    }
-    common(d);
-    use_pack(&d, *p->conv_t[c1]);
-    d.res = gb[cur]; d.res_planes = pl; d.res_plane_stride = rows * C; d.res_ld = C;
-    d.out = gb[cur ^ 1];
-    if (strided) {
-      // G_{i-1}[rows, w*C] = dZ1 * W1^T  (+ G_i in the columns of the residual tap): the pack's
-      // taps slabs [ci][co] read as one [taps*ci][co] slab
-      d.a = bf(wl.dz); d.a_rows = (int)rows; d.a_ld = C;
-      d.n_pad = d.taps * d.n_pad; d.taps = 1;
-      d.out_rows = (int)rows;
-      d.out_plane_stride = rows * fw[i] * C; d.out_ld = fw[i] * C;
-      d.res_rows_per_sample = 0; d.res_row_step = 1; d.res_row_off = 0;
-      d.res_col_begin = (fw[i] / 2 + p->shift_str[i]) * C; d.res_cols = C;
-    } else {
-      // transposed convolution: G_{i-1}[n, t] = sum_k dZ1[n, t - k*d] * W1_k^T  (+ G_i[n, t - off]);
-      // rows outside [0, L_i) are zero-filled by the A / residual tensor maps
-      d.a = bf(wl.dz); d.samples = N; d.a_rows = L[i]; d.a_ld = C;
-      d.per_sample_tiles = 1;
-      d.tap_row_step = -p->dilation[i];
-      d.out_rows = L[i - 1];
-      d.out_plane_stride = wl.rows[i - 1] * C; d.out_ld = C;
-      d.res_rows_per_sample = L[i]; d.res_row_step = 1;
-      d.res_row_off = -(p->pad[i] + p->shift_dil[i]); d.res_check_rows = 1;
-    }
-    fuse_bnb(d, 2 * (i - 1));  // G_{i-1}: BN backward of block i-1's second conv (expand for i = 1)
-    VP3D_TRY(run_conv(&d, stream));
-    ++launches;
-    cur ^= 1;
-    if (stage_done) stage_done(p->nb - i + 1, user);  // all four parameter groups of block i
-  }
-
-  // ---- expand backward (the data gradient only on request: run.py's 2-D input needs none,
-  // run.py:402-412; a differentiable front end or test-time refinement of x does)
-  VP3D_TRY(bn_bwd(0, wl.rows[0], gb[cur], bf(wl.z[0]), want_w ? g->expand_bn[0] : nullptr,
-                  want_w ? g->expand_bn[1] : nullptr));
-  if (want_w) {
-    WgradCall c;
-    c.dz = bf(wl.dz); c.dz_ld = C; c.x = bf(wl.a0); c.c_out = Cr; c.c_in = p->c_in_raw;
-    c.taps_out = fw[0]; c.grad = g->expand_conv_weight;
-    if (strided) {
-      c.x_ld = p->k0_pad; c.rows = wl.rows[0]; c.c_in_cols = fw[0] * p->c_in_raw; c.merged = 1;
-    } else {
-      c.x_ld = p->c_in_pad; c.per_sample = 1; c.samples = N; c.rows = L[0]; c.x_rows = t->T;
-      c.taps = fw[0]; c.tap_row_step = 1; c.c_in_cols = p->c_in_raw;
-    }
-    VP3D_TRY(run_wgrad(pl, c, partial, wl.partial_bytes, stream));
-    launches += 2;
-  }
-  if (dx) {
-    // dX = dZ0 * W0^T through the conv GEMM, fp32 epilogue straight into x's (N, T, J*F) layout
-    const int cin = p->c_in_raw, T = t->T;
-    common(d);
-    d.a = bf(wl.dz); d.a_ld = C;
-    use_pack(&d, *p->expand_t);   // tap-merged (strided) or per tap (dilated)
-    d.out_f32 = dx;
-    if (strided) {
-      // G_x[rows0, w0*cin] = dZ0 * W0^T with the tap-merged pack: column tap*cin + ci of row
-      // (n, r) is x[n, r*w0 + tap, ci], i.e. x's own memory order when T = w0 * L0
-      d.a_rows = (int)wl.rows[0]; d.out_rows = (int)wl.rows[0];
-      d.out_f32_ld = fw[0] * cin; d.n_valid = fw[0] * cin;
-      const size_t used = (size_t)fw[0] * L[0] * cin;   // floats per sample the output depends on
-      const bool tail = T != fw[0] * L[0];
+  // ---- the BatchNorm layers top-down, each with its conv's weight and data gradient.  Block i's
+  // output gradient G_i stays in gb[cur] while its second conv's data gradient goes to gb[cur ^ 1];
+  // its first conv's data gradient G_{i-1} overwrites that, plus G_i through the skip connection.
+  for (int l = top; l >= 0; --l) {
+    const TrainConv& c = cv[l];
+    VP3D_TRY(bn_bwd(l, gb[l % 2 ? cur ^ 1 : cur]));
+    if (want_w)
+      VP3D_TRY(wgrad(c, bf(wl.dz), l ? g->layers_conv_weight[l - 1] : g->expand_conv_weight));
+    if (l > 0) {
+      d = l % 2 ? dgrad_desc(p, c, bf(wl.dz), gb[cur ^ 1], gb[cur], cv[l + 1].res.off)
+                : dgrad_desc(p, c, bf(wl.dz), gb[cur ^ 1]);
+      fuse_bnb(d, l - 1);  // BN backward of the layer below: block i-1's second conv, or expand
+      VP3D_TRY(run_conv(&d, stream));
+      ++launches;
+    } else if (dx) {
+      // the expand conv's data gradient only on request (run.py's 2-D input needs none,
+      // run.py:402-412; a differentiable front end or test-time refinement of x does): fp32
+      // epilogue straight into x's (N, T, J*F) layout.  The strided model's tap-merged row (n, r)
+      // holds x[n, r*w0 + tap, ci] at column tap*cin + ci, x's own memory order when T = w0 * L0;
+      // the dilated model's transposed convolution writes every one of the T rows.
+      d = dgrad_desc(p, c, bf(wl.dz), nullptr);
+      d.out_f32 = dx; d.out_f32_ld = d.n_valid = in_cols(*c.pack);
+      const int cin = p->c_in_raw, T = t->T, w0 = p->cfg.filter_widths[0];
       // trailing frames no output depends on: the GEMM writes a staging buffer, one strided copy
       // moves each sample's rows into place and one strided memset zeroes the tails
+      const bool tail = p->cfg.variant == VP3D_VARIANT_STRIDED && T != w0 * L[0];
       if (tail) d.out_f32 = reinterpret_cast<float*>(base + wl.dx_stage);
       VP3D_TRY(run_conv(&d, stream));
       ++launches;
       if (tail) {
+        const size_t used = (size_t)w0 * L[0] * cin;   // floats per sample the output depends on
         const size_t pitch = (size_t)T * cin * sizeof(float);
         CUDA_TRY(cudaMemcpy2DAsync(dx, pitch, d.out_f32, used * sizeof(float), used * sizeof(float),
                                    N, cudaMemcpyDeviceToDevice, stream));
         CUDA_TRY(cudaMemset2DAsync(dx + used, pitch, 0, pitch - used * sizeof(float), N, stream));
         launches += 2;
       }
-    } else {
-      // transposed convolution: dX[n, t] = sum_k dZ0[n, t - k] * W0_k^T; rows outside [0, L0) are
-      // zero-filled by the A tensor map, so every one of the T rows is written
-      d.samples = N; d.a_rows = L[0]; d.per_sample_tiles = 1;
-      d.tap_row_step = -1;
-      d.out_rows = T; d.out_f32_ld = cin; d.n_valid = cin;
-      VP3D_TRY(run_conv(&d, stream));
-      ++launches;
+    }
+    if (l % 2) {
+      cur ^= 1;
+      const int i = (l + 1) / 2;
+      if (stage_done) stage_done(p->nb - i + 1, user);  // all four parameter groups of block i
     }
   }
   if (stage_done) stage_done(p->nb + 1, user);  // expand_conv / expand_bn
@@ -892,14 +861,7 @@ VP3D_API int vp3d_wgrad_gemm(const vp3d_wgrad_desc* d, void* stream) {
     return fail(VP3D_ERR_INVALID, "wgrad_gemm: taps / columns inconsistent with merged = %d", d->merged);
   if (d->dz_ld < round_up(d->c_out, 64) || d->dz_ld % 64 || d->x_ld % 64)
     return fail(VP3D_ERR_INVALID, "wgrad_gemm: row pitches must be multiples of 64 covering the channels");
-  WgradCall c;
-  c.dz = static_cast<const __nv_bfloat16*>(d->dz); c.dz_ld = d->dz_ld;
-  c.x = static_cast<const __nv_bfloat16*>(d->x); c.x_ld = d->x_ld;
-  c.rows = d->rows; c.per_sample = d->per_sample ? 1 : 0; c.samples = d->samples;
-  c.x_rows = d->x_rows; c.taps = d->taps; c.tap_col_step = d->tap_col_step;
-  c.tap_row_step = d->tap_row_step; c.c_out = d->c_out; c.c_in_cols = d->c_in_cols; c.c_in = d->c_in;
-  c.taps_out = d->taps_out; c.merged = d->merged ? 1 : 0; c.grad = d->grad;
-  return run_wgrad(d->planes, c, d->partial, d->partial_bytes, static_cast<cudaStream_t>(stream));
+  return run_wgrad(*d, static_cast<cudaStream_t>(stream));
 }
 
 namespace {
@@ -917,15 +879,6 @@ int check_rows_c(const char* what, long long rows, int c, int planes) {
   if (rows < 1 || c < 64 || c % 64) return fail(VP3D_ERR_INVALID, "%s: rows >= 1 and channels a multiple of 64", what);
   if (planes != 1 && planes != 2) return fail(VP3D_ERR_INVALID, "%s: planes must be 1 or 2", what);
   return VP3D_OK;
-}
-
-DropoutCfg flat_drop(float p, unsigned long long seed, int layer) {
-  DropoutCfg d;
-  d.p = p;
-  d.seed_lo = (uint32_t)(seed & 0xFFFFFFFFu);
-  d.seed_hi = (uint32_t)(seed >> 32);
-  d.layer = (uint32_t)layer;
-  return d;
 }
 }  // namespace
 
@@ -975,7 +928,7 @@ VP3D_API int vp3d_bn_apply(const void* z, long long z_plane, void* x, long long 
   const RowMap map = {res_div, res_rows_per_sample, res_step, res_off};
   CUDA_TRY(launch_bn_apply(static_cast<const __nv_bfloat16*>(z), z_plane,
                            static_cast<__nv_bfloat16*>(x), x_plane, planes, rows, c, scale, shift,
-                           flat_drop(dropout_p, seed, layer), static_cast<const __nv_bfloat16*>(res),
+                           dropout_cfg(dropout_p, seed, layer), static_cast<const __nv_bfloat16*>(res),
                            res_plane, map, static_cast<cudaStream_t>(stream)));
   return VP3D_OK;
 }
@@ -995,7 +948,7 @@ VP3D_API int vp3d_bn_bwd_reduce(const void* g, long long g_plane, const void* z,
   VP3D_TRY(check_reduce_scratch("bn_bwd_reduce", c, 2, scratch_floats, counters));
   const cudaError_t e = launch_bn_bwd_reduce(
       static_cast<const __nv_bfloat16*>(g), g_plane, static_cast<const __nv_bfloat16*>(z), z_plane,
-      planes, rows, c, scale, shift, mean, invstd, flat_drop(dropout_p, seed, layer), partials,
+      planes, rows, c, scale, shift, mean, invstd, dropout_cfg(dropout_p, seed, layer), partials,
       partial_floats, sums, scratch, counter, static_cast<cudaStream_t>(stream));
   // the one argument error of the launch: per-block partials larger than `partials` (nothing ran)
   if (e == cudaErrorInvalidValue)
@@ -1019,7 +972,7 @@ VP3D_API int vp3d_bn_bwd_apply(const void* g, long long g_plane, const void* z, 
   CUDA_TRY(launch_bn_bwd_apply(static_cast<const __nv_bfloat16*>(g), g_plane,
                                static_cast<const __nv_bfloat16*>(z), z_plane,
                                static_cast<__nv_bfloat16*>(dz), dz_plane, planes, rows, c, scale,
-                               shift, mean, invstd, flat_drop(dropout_p, seed, layer), sums, dgamma,
+                               shift, mean, invstd, dropout_cfg(dropout_p, seed, layer), sums, dgamma,
                                dbeta, c_real, static_cast<cudaStream_t>(stream), frozen ? 1 : 0));
   return VP3D_OK;
 }
