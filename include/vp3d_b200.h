@@ -541,6 +541,39 @@ int vp3d_pose_errors(const float* pred, int32_t copies, const int32_t* mirror_sr
                      int64_t frames, int32_t joints, int32_t which, float* averaged, double* means,
                      void* scratch, size_t scratch_bytes, void* stream);
 
+/* ---- differentiable pose losses (common/loss.py:11-17, :27-89) ------------------------------
+ * Any weighted subset of four terms and the gradient of their weighted sum with respect to `pred`,
+ * in one cooperative launch.  pred, target: [seqs][frames_per_seq][joints][3] fp32, device; a pose
+ * is one (seq, frame) slice.  Term k (flag bit 1 << k) is evaluated when term_weights[k] != 0:
+ *   [0] VP3D_POSE_LOSS_MPJPE     mean ||p - t||                                  loss.py:11-17
+ *   [1] VP3D_POSE_LOSS_N_MPJPE   mean ||s p - t||, s = mean <t, p> / mean <p, p> per pose
+ *                                (ds/dp included in the gradient)                loss.py:68-78
+ *   [2] VP3D_POSE_LOSS_P_MPJPE   mean distance after per-pose similarity Procrustes (centre,
+ *                                normalise, rotation, scale, translation; the gradient flows through
+ *                                all of them)                                    loss.py:27-66
+ *   [3] VP3D_POSE_LOSS_VELOCITY  mean ||diff(p) - diff(t)||, first differences along the frame axis
+ *                                within each sequence; NaN for frames_per_seq == 1 (np.mean of
+ *                                nothing)                                        loss.py:80-89
+ * term_weights: 4 host doubles.  terms_out[k] (device, 4 floats) receives term k, 0 when it is not
+ * evaluated; loss_out (device float) receives sum_k term_weights[k] * terms_out[k] over the
+ * evaluated terms.  dpred (shape of pred, or NULL: no backward) receives d loss / d pred.
+ * Rotations: the top eigenpair of Horn's 4x4 matrix (fp64 Jacobi); a pose whose two largest
+ * eigenvalues satisfy lambda_0 - lambda_1 <= 1e-12 max(|lambda_0|, 1) has no differentiable rotation
+ * and gets the gradient with its rotation held fixed; degenerate_out (device int32, or NULL)
+ * receives the number of such poses.  All-zero predictions give NaN, as the reference does.
+ * fp64 inside, one rounding to fp32 per output; sums in a fixed order: the same input gives the same
+ * bits.  joints <= 32; seqs == 0 is a no-op.  `scratch`: device memory of
+ * vp3d_pose_loss_scratch_bytes(frames_per_seq, seqs) bytes. */
+#define VP3D_POSE_LOSS_MPJPE 1
+#define VP3D_POSE_LOSS_N_MPJPE 2
+#define VP3D_POSE_LOSS_P_MPJPE 4
+#define VP3D_POSE_LOSS_VELOCITY 8
+size_t vp3d_pose_loss_scratch_bytes(int32_t frames_per_seq, int64_t seqs);
+int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frames_per_seq, int64_t seqs,
+                           int32_t joints, const double* term_weights, float* terms_out, float* loss_out,
+                           float* dpred, int32_t* degenerate_out, void* scratch, size_t scratch_bytes,
+                           void* stream);
+
 /* ---- streaming inference (common/model.py:63-77, 126-138 applied incrementally) ---------------
  * A session of S stream slots pushes k <= K new frames per slot at a time and gets back the output
  * frames they complete.  Per slot the concatenated outputs equal vp3d_forward_eval on the sequence

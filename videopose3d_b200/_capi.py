@@ -25,6 +25,7 @@ VP3D_TRAIN_FROZEN_BN = 1
 VP3D_BN_SYNC_FORWARD, VP3D_BN_SYNC_BACKWARD = 0, 1
 VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
+VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_LOSS_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
 
 _LIB_NAME = "libvp3d_b200.so"
@@ -273,6 +274,11 @@ SIGNATURES = {
                                         ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32,
                                         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "vp3d_pose_loss_scratch_bytes": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "vp3d_pose_loss_fwd_bwd": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                                              ctypes.c_int64, ctypes.c_int32,
+                                              ctypes.POINTER(ctypes.c_double)] + [ctypes.c_void_p] * 5
+                               + [ctypes.c_size_t, ctypes.c_void_p]),
     "vp3d_stream_lookahead": (ctypes.c_int, [ctypes.c_void_p]),
     "vp3d_stream_state_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]),
     "vp3d_stream_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,

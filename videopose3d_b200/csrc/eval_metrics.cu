@@ -6,7 +6,7 @@
 //   MPJVE= mean ||diff(avg) - diff(target)|| along the flattened frame axis, loss.py:80-89
 // One warp per frame, one lane per joint (J <= 32).  Inputs are fp32; the flip average is formed in
 // fp32 with the rounding of the torch expression (and optionally stored); everything after it is
-// fp64.  Procrustes uses Horn's closed form: the largest eigenpair of the 4x4 symmetric matrix built
+// fp64.  Procrustes uses Horn's closed form (procrustes.cuh): the largest eigenpair of the 4x4 symmetric matrix built
 // from H = X0^T Y0 (cyclic Jacobi in fp64) gives the optimal trace s1 + s2 + sign(det H) s3 of the
 // reference's SVD as the eigenvalue and the rotation as a unit quaternion.  Reductions: per-lane
 // running sums in a fixed frame order, warp sums, warps in order, a grid-wide barrier, then blocks
@@ -14,6 +14,7 @@
 #include <cooperative_groups.h>
 
 #include "internal.cuh"
+#include "procrustes.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -24,7 +25,6 @@ constexpr int kWarps = 8;
 constexpr int kThreads = 32 * kWarps;
 constexpr int kMaxJoints = 32;
 constexpr int kMaxBlocks = 1024;
-constexpr int kJacobiSweeps = 12;
 
 struct EvalArgs {
   const float* pred;      // [copies][frames][J][3]
@@ -55,70 +55,6 @@ __device__ __forceinline__ void load_avg(const EvalArgs& a, long long f, int j, 
   out[0] = flip_average(p0[0], p1[0], 0);
   out[1] = flip_average(p0[1], p1[1], 1);
   out[2] = flip_average(p0[2], p1[2], 2);
-}
-
-// One Jacobi rotation zeroing A[p][q] of the symmetric 4x4 A, accumulated into the columns of V.
-template <int p, int q>
-__device__ __forceinline__ void jacobi_rotate(double (&A)[4][4], double (&V)[4][4]) {
-  const double apq = A[p][q];
-  if (apq == 0.0) return;
-  const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
-  const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-  const double c = rsqrt(t * t + 1.0), s = t * c;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {  // A <- A J (columns p, q)
-    const double akp = A[k][p], akq = A[k][q];
-    A[k][p] = c * akp - s * akq;
-    A[k][q] = s * akp + c * akq;
-  }
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {  // A <- J^T A (rows p, q)
-    const double apk = A[p][k], aqk = A[q][k];
-    A[p][k] = c * apk - s * aqk;
-    A[q][k] = s * apk + c * aqk;
-  }
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const double vkp = V[k][p], vkq = V[k][q];
-    V[k][p] = c * vkp - s * vkq;
-    V[k][q] = s * vkp + c * vkq;
-  }
-}
-
-// Rotation (row-major, applied as Q y to column vectors) and optimal trace for the normalised,
-// centred H = X0^T Y0.  The reference aligns `predicted @ R`, i.e. R = Q^T.
-__device__ void procrustes(const double (&H)[3][3], double (&Q)[3][3], double* trace) {
-  // S = H^T: S_ab = sum_j y_a x_b (Horn 1987, eq. for N)
-  const double Sxx = H[0][0], Sxy = H[1][0], Sxz = H[2][0];
-  const double Syx = H[0][1], Syy = H[1][1], Syz = H[2][1];
-  const double Szx = H[0][2], Szy = H[1][2], Szz = H[2][2];
-  double A[4][4] = {{Sxx + Syy + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx},
-                    {Syz - Szy, Sxx - Syy - Szz, Sxy + Syx, Szx + Sxz},
-                    {Szx - Sxz, Sxy + Syx, -Sxx + Syy - Szz, Syz + Szy},
-                    {Sxy - Syx, Szx + Sxz, Syz + Szy, -Sxx - Syy + Szz}};
-  double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
-  for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
-    const double off = A[0][1] * A[0][1] + A[0][2] * A[0][2] + A[0][3] * A[0][3] +
-                       A[1][2] * A[1][2] + A[1][3] * A[1][3] + A[2][3] * A[2][3];
-    if (off < 1e-36) break;  // |entries| <= ~3 after normalisation: converged to fp64 round-off
-    jacobi_rotate<0, 1>(A, V); jacobi_rotate<0, 2>(A, V); jacobi_rotate<0, 3>(A, V);
-    jacobi_rotate<1, 2>(A, V); jacobi_rotate<1, 3>(A, V); jacobi_rotate<2, 3>(A, V);
-  }
-  int k = 0;
-  double lam = A[0][0];
-  if (A[1][1] > lam) { lam = A[1][1]; k = 1; }
-  if (A[2][2] > lam) { lam = A[2][2]; k = 2; }
-  if (A[3][3] > lam) { lam = A[3][3]; k = 3; }
-  double w = V[0][0], x = V[1][0], y = V[2][0], z = V[3][0];
-  if (k == 1) { w = V[0][1]; x = V[1][1]; y = V[2][1]; z = V[3][1]; }
-  if (k == 2) { w = V[0][2]; x = V[1][2]; y = V[2][2]; z = V[3][2]; }
-  if (k == 3) { w = V[0][3]; x = V[1][3]; y = V[2][3]; z = V[3][3]; }
-  const double n = rsqrt(w * w + x * x + y * y + z * z);
-  w *= n; x *= n; y *= n; z *= n;
-  Q[0][0] = w * w + x * x - y * y - z * z; Q[0][1] = 2.0 * (x * y - w * z); Q[0][2] = 2.0 * (x * z + w * y);
-  Q[1][0] = 2.0 * (x * y + w * z); Q[1][1] = w * w - x * x + y * y - z * z; Q[1][2] = 2.0 * (y * z - w * x);
-  Q[2][0] = 2.0 * (x * z - w * y); Q[2][1] = 2.0 * (y * z + w * x); Q[2][2] = w * w - x * x - y * y + z * z;
-  *trace = lam;
 }
 
 __global__ void __launch_bounds__(kThreads) pose_errors_kernel(const EvalArgs a) {

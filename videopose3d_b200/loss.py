@@ -10,14 +10,18 @@ both model outputs, in one launch (`vp3d_projected_mpjpe_fwd_bwd`).  `semi_super
 whole loss head of the semi-supervised step -- 3-D loss, depth-weighted trajectory loss,
 re-projection loss and the bone-length penalty (run.py:350-390) with the gradients for both model
 outputs -- in one cooperative launch (`vp3d_semi_loss_fwd_bwd`, csrc/semi_loss.cu);
-`bone_length_penalty` is that kernel with only the penalty enabled.  CUDA float32 only, no fallback.
+`bone_length_penalty` is that kernel with only the penalty enabled.  `pose_loss` is any weighted
+combination of mpjpe, `n_mpjpe`, `p_mpjpe` and `mean_velocity_error` (loss.py:27-89, NumPy or
+gradient-free in the reference) with the gradient of the sum, in one cooperative launch
+(`vp3d_pose_loss_fwd_bwd`, csrc/pose_loss.cu); the three named functions are that kernel with one
+term enabled.  CUDA float32 only, no fallback.
 """
 import torch
 
 from . import _capi
 
 __all__ = ["mpjpe", "weighted_mpjpe", "projected_mpjpe", "bone_length_penalty",
-           "semi_supervised_loss"]
+           "semi_supervised_loss", "n_mpjpe", "p_mpjpe", "mean_velocity_error", "pose_loss"]
 
 
 class _Mpjpe(torch.autograd.Function):
@@ -196,3 +200,98 @@ def bone_length_penalty(predicted_3d_pos_cat, split_idx, parents):
     pen, _ = _SemiLoss.apply(predicted_3d_pos_cat, traj, None, None, None, parents, int(split_idx),
                              False, _capi.VP3D_SEMI_BONE, 3)
     return pen
+
+
+class _PoseLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, predicted, target, weights):
+        for t, what in ((predicted, "predicted"), (target, "target")):
+            if not (t.is_cuda and t.dtype == torch.float32):
+                raise RuntimeError(f"videopose3d_b200.loss: {what} must be a CUDA float32 tensor "
+                                   f"(got {t.device}, {t.dtype}); there is no fallback path")
+        assert predicted.shape == target.shape, (tuple(predicted.shape), tuple(target.shape))
+        if predicted.dim() < 2 or predicted.shape[-1] != 3:
+            raise ValueError(f"videopose3d_b200.loss: expected (..., frames, joints, 3) poses, got "
+                             f"{tuple(predicted.shape)}")
+        lib = _capi.load()
+        dev = predicted.device
+        pred, tgt = predicted.contiguous(), target.contiguous()
+        joints = pred.shape[-2]
+        frames = pred.shape[-3] if pred.dim() >= 3 else 1
+        seqs = pred.numel() // (3 * joints * frames) if joints * frames else 0
+        out = torch.empty(6, dtype=torch.float32, device=dev)      # loss, 4 terms, degenerate count
+        need_grad = ctx.needs_input_grad[0]
+        dpred = torch.empty_like(pred) if need_grad else None
+        w = (_capi.ctypes.c_double * 4)(*weights)
+        scratch = torch.empty(max(1, lib.vp3d_pose_loss_scratch_bytes(max(frames, 1), seqs)),
+                              dtype=torch.uint8, device=dev)
+        if seqs == 0 or joints == 0:
+            out.fill_(float("nan"))            # torch.mean / np.mean of nothing
+            out[5] = 0
+            if need_grad:
+                dpred.zero_()
+        else:
+            degenerate = out[5:].view(torch.int32)
+            with torch.cuda.device(dev):
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                _capi.check(lib.vp3d_pose_loss_fwd_bwd(
+                    pred.data_ptr(), tgt.data_ptr(), frames, seqs, joints, w, out[1:5].data_ptr(),
+                    out.data_ptr(), dpred.data_ptr() if need_grad else None, degenerate.data_ptr(),
+                    scratch.data_ptr(), scratch.numel(), stream), "vp3d_pose_loss_fwd_bwd")
+        # kept for the lifetime of the graph, as in _Mpjpe (retain_graph=True gets it again)
+        ctx.dpred = dpred
+        terms = out[1:5].clone()
+        n_degenerate = out[5:].view(torch.int32).clone().squeeze(0)
+        ctx.mark_non_differentiable(terms, n_degenerate)
+        return out[0].clone(), terms, n_degenerate
+
+    @staticmethod
+    def backward(ctx, grad_out, _grad_terms, _grad_degenerate):
+        dpred = ctx.dpred
+        return (dpred * grad_out if dpred is not None else None), None, None
+
+
+def _one_term(predicted, target, k):
+    weights = [0.0] * 4
+    weights[k] = 1.0
+    loss, _, _ = _PoseLoss.apply(predicted, target, tuple(weights))
+    return loss
+
+
+def n_mpjpe(predicted, target):
+    """Normalized MPJPE (loss.py:68-78): per pose (one (..., frame) slice of joints) the prediction
+    is scaled by the least-squares factor mean <t, p> / mean <p, p>, then mpjpe.  The gradient
+    includes the scale's own derivative."""
+    assert predicted.shape == target.shape
+    return _one_term(predicted, target, 1)
+
+
+def p_mpjpe(predicted, target):
+    """Procrustes-aligned MPJPE (loss.py:27-66) with a gradient: per pose, the similarity transform
+    (rotation, scale, translation) fitted to the target, then mpjpe.  The gradient flows through the
+    alignment itself.  (frames, joints, 3) as the reference takes it, or any (..., joints, 3)."""
+    assert predicted.shape == target.shape
+    return _one_term(predicted, target, 2)
+
+
+def mean_velocity_error(predicted, target):
+    """Mean per-joint velocity error (loss.py:80-89) with a gradient: mpjpe of the first differences
+    along dim -3 -- the reference's axis 0 for (frames, joints, 3); along T within each sample for a
+    (N, T, joints, 3) batch.  NaN for a single frame, like np.mean of nothing."""
+    assert predicted.shape == target.shape
+    return _one_term(predicted, target, 3)
+
+
+def pose_loss(predicted, target, mpjpe=1.0, n_mpjpe=0.0, p_mpjpe=0.0, velocity=0.0,
+              return_degenerate=False):
+    """Weighted sum of mpjpe, n_mpjpe, p_mpjpe and mean_velocity_error (dim -3) and its gradient in
+    ONE launch.  Terms with weight 0 are not evaluated.  Returns (loss, terms) with terms a detached
+    (4,) tensor [mpjpe, n_mpjpe, p_mpjpe, velocity] (0 for a term not evaluated); with
+    `return_degenerate`, also the 0-d int32 count of poses whose Procrustes rotation is not
+    differentiable (the two largest eigenvalues of Horn's matrix closer than 1e-12 relative: their
+    gradient holds the rotation fixed)."""
+    weights = tuple(float(w) for w in (mpjpe, n_mpjpe, p_mpjpe, velocity))
+    if not any(weights):
+        raise ValueError("pose_loss: every term weight is 0")
+    loss, terms, n_degenerate = _PoseLoss.apply(predicted, target, weights)
+    return (loss, terms, n_degenerate) if return_degenerate else (loss, terms)
