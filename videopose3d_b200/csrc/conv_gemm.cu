@@ -162,13 +162,16 @@ __device__ __forceinline__ void tl_stamp(const ConvGemmArgs& p, int ev) {
 
 // TRAIN compiles in the training-only epilogue paths (BatchNorm batch statistics of the stored
 // value, fused BatchNorm-backward reductions); eval launches use the leaner TRAIN = false build.
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN>
+// F16 (LEAN only): the operand / storage format at compile time (fp16, else bf16), so that each
+// k-block is one branch-free group of wgmma; the other instances read it from p.f16.
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ CUtensorMap tmap_out,
                  const __grid_constant__ CUtensorMap tmap_res,
                  const __grid_constant__ CUtensorMap tmap_z, const ConvGemmArgs p) {
+  static_assert(LEAN || !F16, "only the lean instances fix the operand format at compile time");
   using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBlocksPerTile = BLOCK_N / 64;
@@ -342,7 +345,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const uint32_t bar_wg = 2u + (uint32_t)wg;               // named barrier: this warpgroup
     const uint32_t bar_slab = 4u + (uint32_t)(wg * 2 + (wq >> 1));   // the two warps of a slab
     float* s_pair = s_pairs + (wg * 2 + (wq >> 1)) * 128;
-    const bool f16 = p.f16 != 0;  // IEEE fp16 operands / storage instead of bf16 (eval fp16 mode)
+    // IEEE fp16 operands / storage instead of bf16 (eval fp16 mode)
+    const bool f16 = LEAN ? F16 : p.f16 != 0;
     const bool do_relu = LEAN || (p.flags & kEpiRelu);
     const bool do_res = LEAN ? RES : (p.flags & kEpiResidual) != 0;
     const bool do_stats = TRAIN && (p.flags & kEpiStats);
@@ -374,7 +378,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const uint64_t db = make_gmma_desc_sw128(smem_b + stage * Cfg::kBBytes, 16, 1024);
         wgmma_fence_operands(acc);
         wgmma_fence();
-        if (f16) wgmma_kblock<BLOCK_N, true>(acc, da, db, it == 0);
+        if constexpr (LEAN) wgmma_kblock<BLOCK_N, F16>(acc, da, db, it == 0);
+        else if (f16) wgmma_kblock<BLOCK_N, true>(acc, da, db, it == 0);
         else wgmma_kblock<BLOCK_N, false>(acc, da, db, it == 0);
         wgmma_commit();
         wgmma_fence_operands(acc);
@@ -623,13 +628,13 @@ static bool pdl_enabled() {
 void conv_gemm_set_pdl(int on) { g_pdl = on ? 1 : 0; }
 bool conv_gemm_pdl_enabled() { return pdl_enabled(); }
 
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false>
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false, bool F16 = false>
 static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                                const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                                const CUtensorMap& tmap_z, const ConvGemmArgs& args, int num_sms,
                                cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN>;
-  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN>;
+  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16>;
   // the dynamic shared memory opt-in is a per-device attribute
   static bool attr_set[kMaxDevices] = {};
   int dev = 0;
@@ -688,7 +693,8 @@ static cudaError_t launch_train(const CUtensorMap& a, const CUtensorMap& w, cons
     return launch_impl<BLOCK_N, RES, OUT2, true>(a, w, o, r, z, args, num_sms, stream);
   if constexpr (!OUT2) {
     if (lean_ok(args, RES))
-      return launch_impl<BLOCK_N, RES, false, false, true>(a, w, o, r, z, args, num_sms, stream);
+      return args.f16 ? launch_impl<BLOCK_N, RES, false, false, true, true>(a, w, o, r, z, args, num_sms, stream)
+                      : launch_impl<BLOCK_N, RES, false, false, true, false>(a, w, o, r, z, args, num_sms, stream);
   }
   return launch_impl<BLOCK_N, RES, OUT2, false>(a, w, o, r, z, args, num_sms, stream);
 }
