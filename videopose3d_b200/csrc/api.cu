@@ -616,6 +616,116 @@ extern "C" __attribute__((visibility("default"))) size_t vp3d_workspace_bytes(co
   return ws_layout(p, N, T, strided, L).total;
 }
 
+// measurement hook: record an event pair around launch number p->prof_launch
+static int prof_event(vp3d_plan* p, int launch, bool begin, cudaStream_t stream) {
+  if (p->prof_launch < 0 || launch != p->prof_launch) return VP3D_OK;
+  const size_t idx = p->prof_used + (begin ? 0 : 1);
+  while (p->prof_events.size() <= idx) {
+    cudaEvent_t e;
+    CUDA_TRY(cudaEventCreate(&e));
+    p->prof_events.push_back(e);
+  }
+  CUDA_TRY(cudaEventRecord(p->prof_events[idx], stream));
+  if (!begin) p->prof_used += 2;
+  return VP3D_OK;
+}
+
+// expand (model.py:127 / :188), the residual blocks (:129-135 / :190-194), shrink (:137 / :196)
+// writing (N, T_out, J_out, 3) directly (fuses :74-75)
+int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream, int* launches) {
+  const int C = p->C;
+  // conv k + BN + ReLU of stage i in the chain's tiling
+  auto conv = [&](int i, const PackedConv& k, const __nv_bfloat16* a, long long a_plane, int a_rows,
+                  int a_ld) {
+    vp3d_conv_desc d = conv_desc(p, c.precision[i]);
+    d.a = a; d.a_plane_stride = a_plane; d.samples = c.samples; d.a_rows = a_rows; d.a_ld = a_ld;
+    use_pack(&d, k);
+    d.per_sample_tiles = c.per_sample_tiles; d.out_rows = c.st[i].out_rows;
+    d.scale = k.scale; d.shift = k.shift; d.relu = 1;
+    d.out_ld = C;
+    return d;
+  };
+  auto launch = [&](const vp3d_conv_desc& d) -> int {
+    if (c.profile) VP3D_TRY(prof_event(p, *launches, true, stream));
+    VP3D_TRY(run_conv(&d, stream));
+    if (c.profile) VP3D_TRY(prof_event(p, *launches, false, stream));
+    ++*launches;
+    return VP3D_OK;
+  };
+  for (int i = 0; i < c.stages; ++i) {
+    const ChainStage& s = c.st[i];
+    // the planes of a stage's input lie where its producer wrote them, and must hold its rows
+    const long long in_plane = i == 0 ? c.in_plane : c.st[i - 1].out_plane;
+    const int in_ld = i == 0 ? c.expand->k_pad : C;
+    if (in_plane < (long long)c.samples * s.in_rows * in_ld)
+      return fail(VP3D_ERR_STATE, "internal: activation plane mismatch in block %d", i);
+    // the k-tap conv: the expand conv writes X_0, a block's first conv H
+    vp3d_conv_desc d = conv(i, i == 0 ? *c.expand : *p->conv[2 * (i - 1)], s.in, in_plane,
+                            s.in_rows, in_ld);
+    d.tap_row_step = s.tap_row_step;
+    if (i > 0) {
+      // H only needs a lo plane when its consumer is split-bf16
+      const int h_planes = c.precision[i] == VP3D_PRECISION_BF16X3 ? 2 : 1;
+      d.out_planes = h_planes; d.out = c.h; d.out_plane_stride = s.h_plane;
+      VP3D_TRY(launch(d));
+      // second conv: 1x1 + the block input's centre (causal: newest) tap as residual; with
+      // per-sample tiles the residual rows of a tile are then one TMA box of the block input
+      d = conv(i, *p->conv[2 * (i - 1) + 1], c.h, s.h_plane, s.out_rows, C);
+      d.a_planes = h_planes;
+      d.res = s.in; d.res_plane_stride = in_plane; d.res_ld = C; d.res_row_step = 1;
+      d.res_row_off = s.res_row_off;
+      d.res_rows_per_sample = c.per_sample_tiles ? s.in_rows : 0;
+    }
+    d.out = s.out; d.out_plane_stride = s.out_plane;
+    d.lo_row_begin = s.lo_row_begin; d.lo_row_end = s.lo_row_end;
+    VP3D_TRY(launch(d));
+  }
+  if (!c.y) return VP3D_OK;
+  // shrink: one flat GEMM over all rows of the last stage, the bias as its affine, fp32 out
+  const ChainStage& s = c.st[c.stages - 1];
+  vp3d_conv_desc d = conv_desc(p, c.precision[p->nb + 1]);
+  d.a = s.out; d.a_plane_stride = s.out_plane; d.a_ld = C;
+  d.a_rows = d.out_rows = (c.per_sample_tiles ? c.samples : 1) * s.out_rows;
+  use_pack(&d, *p->shrink);
+  d.scale = p->shrink->scale; d.shift = p->shrink->shift;
+  d.out_f32 = c.y; d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
+  return launch(d);
+}
+
+// The two offline geometries, over the N * L[i] rows of stage i.
+//
+// Strided schedule: every activation is kept in tap-major row order (pack.cuh), so the w taps of
+// block i are w contiguous row regions of R = N * L[i] rows: tap k of output row j is row k * R + j
+// of the block input, and the residual of the block is its centre (or, causal, last) region.
+static void strided_chain(const vp3d_plan* p, int N, const int* L, InferChain* c) {
+  c->samples = 1;
+  c->per_sample_tiles = 0;
+  c->expand = p->expand_flat;
+  for (int i = 0; i <= p->nb; ++i) {
+    ChainStage& s = c->st[i];
+    const int R = N * L[i];
+    s.in_rows = i == 0 ? R : N * L[i - 1];
+    s.out_rows = R;
+    s.tap_row_step = i == 0 ? 0 : R;
+    s.res_row_off = (p->cfg.filter_widths[i] / 2 + p->shift_str[i]) * R;
+  }
+}
+
+// Dilated schedule: every GEMM but shrink tiles per sample, the 1x1 convs too; taps are rows
+// `dilation` apart and the residual starts pad + shift rows into the sample.
+static void dilated_chain(const vp3d_plan* p, int N, int T, const int* L, InferChain* c) {
+  c->samples = N;
+  c->per_sample_tiles = 1;
+  c->expand = p->expand_dil;
+  for (int i = 0; i <= p->nb; ++i) {
+    ChainStage& s = c->st[i];
+    s.in_rows = i == 0 ? T : L[i - 1];
+    s.out_rows = L[i];
+    s.tap_row_step = p->dilation[i];
+    s.res_row_off = p->pad[i] + p->shift_dil[i];
+  }
+}
+
 extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
                                  size_t ws_bytes, void* stream_) {
   if (!p || !x || !y) return fail(VP3D_ERR_INVALID, "forward_eval: null argument");
@@ -632,34 +742,25 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   const WsLayout wl = ws_layout(p, N, T, strided, L);
   if (!ws || ws_bytes < wl.total) return fail(VP3D_ERR_WORKSPACE, "workspace too small: %zu < %zu",
                                               ws_bytes, wl.total);
-  uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
-  __nv_bfloat16* a0 = reinterpret_cast<__nv_bfloat16*>(base + wl.a0);
-  __nv_bfloat16* xb[2] = {reinterpret_cast<__nv_bfloat16*>(base + wl.x0),
-                          reinterpret_cast<__nv_bfloat16*>(base + wl.x1)};
-  __nv_bfloat16* hb = reinterpret_cast<__nv_bfloat16*>(base + wl.h);
+  uint8_t* base = ws_base(ws);
   const int* fw = p->cfg.filter_widths;
   const int C = p->C;
-  int launches = 0;
-  // measurement hook: record an event pair around launch number p->prof_launch
-  auto prof_event = [&](bool begin) -> int {
-    if (p->prof_launch < 0 || launches != p->prof_launch) return VP3D_OK;
-    const size_t idx = p->prof_used + (begin ? 0 : 1);
-    while (p->prof_events.size() <= idx) {
-      cudaEvent_t e;
-      CUDA_TRY(cudaEventCreate(&e));
-      p->prof_events.push_back(e);
-    }
-    CUDA_TRY(cudaEventRecord(p->prof_events[idx], stream));
-    if (!begin) p->prof_used += 2;
-    return VP3D_OK;
-  };
-#define VP3D_LAUNCH(call)          \
-  do {                             \
-    VP3D_TRY(prof_event(true));    \
-    call;                          \
-    VP3D_TRY(prof_event(false));   \
-    ++launches;                    \
-  } while (0)
+  auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
+  // the chain's buffers: X_i alternates between the workspace's two X buffers, its planes and H's
+  // packed to the rows of stage i
+  InferChain c;
+  memset(&c, 0, sizeof(c));
+  c.stages = p->nb + 1;
+  c.in_plane = (long long)wl.a0_plane;
+  c.h = bf(wl.h);
+  c.y = y;
+  c.profile = true;
+  for (int i = 0; i <= p->nb; ++i) {
+    ChainStage& s = c.st[i];
+    s.in = i == 0 ? bf(wl.a0) : c.st[i - 1].out;
+    s.out = bf(i % 2 ? wl.x1 : wl.x0);
+    s.out_plane = s.h_plane = (long long)N * L[i] * C;
+  }
 
   // Per-layer operand precision.  index 0 = expand, 1..nb = residual blocks, nb+1 = shrink.
   //   bf16   : every GEMM single-plane bf16.
@@ -668,7 +769,6 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   //            split-bf16 (they carry most of the bf16 error, tools/precision_study.py),
   //            residual blocks run plain bf16 on the hi plane unless they hold < 0.5% of the
   //            forward FLOPs (negligible even at the narrow-tile rate of such layers).
-  bool x3[VP3D_MAX_WIDTHS + 1];
   {
     double fl[VP3D_MAX_WIDTHS + 1], total = 0.0;
     fl[0] = (double)N * L[0] * p->c_in_raw * fw[0] * C;
@@ -676,128 +776,44 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
     fl[p->nb + 1] = (double)N * L[p->nb] * C * p->c_out_raw;
     for (int i = 0; i <= p->nb + 1; ++i) total += fl[i];
     for (int i = 0; i <= p->nb + 1; ++i) {
-      if (p->cfg.precision == VP3D_PRECISION_BF16 || p->f16) x3[i] = false;
-      else if (p->cfg.precision == VP3D_PRECISION_BF16X3) x3[i] = true;
-      else x3[i] = (i == 0 || i == p->nb + 1) ? true : (fl[i] < 0.005 * total);
+      const bool x3 = i == 0 || i == p->nb + 1 || fl[i] < 0.005 * total;
+      c.precision[i] = p->cfg.precision != VP3D_PRECISION_MIXED ? p->cfg.precision
+                       : x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16;
     }
   }
 
-  vp3d_conv_desc d;
-  auto common = [&](vp3d_conv_desc& q, bool layer_x3) {
-    memset(&q, 0, sizeof(q));
-    q.a_planes = p->planes;
-    q.precision = p->f16 ? VP3D_PRECISION_FP16
-                         : (layer_x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16);
-    q.out_planes = p->planes;
-    q.res_planes = p->planes;
-  };
-
-  // ---- input packing + expand conv (model.py:127 / :188)
-  // Strided schedule: every activation is kept in tap-major row order (pack.cuh), so the w taps
-  // of block i are w contiguous row regions of R[i] = N * L[i] rows: tap k of output row j is row
-  // k * R[i] + j of the block input, and the residual of the block is its centre (or, causal, last)
-  // region.  Only that region of X needs the lo plane in `mixed` mode.
-  long long R[VP3D_MAX_WIDTHS];
-  for (int i = 0; i <= p->nb; ++i) R[i] = (long long)N * L[i];
-  auto lo_rows = [&](int i, vp3d_conv_desc& q) {  // q produces X_i
-    q.lo_row_begin = 0;
-    q.lo_row_end = 0;  // every row
-    if (!strided || p->planes != 2 || i >= p->nb || x3[i + 1]) return;
-    const long long c = fw[i + 1] / 2 + p->shift_str[i + 1];
-    q.lo_row_begin = (int)(c * R[i + 1]);
-    q.lo_row_end = (int)((c + 1) * R[i + 1]);
-  };
+  // ---- input packing (model.py:127 / :188), then the chain
+  int launches = 0;
+  if (strided && (long long)N * L[0] > 0x7fffffffll)
+    return fail(VP3D_ERR_UNSUPPORTED, "forward_eval: too many rows (%lld)", (long long)N * L[0]);
+  VP3D_TRY(prof_event(p, launches, true, stream));
   if (strided) {
-    if ((long long)N * L[0] > 0x7fffffffll)
-      return fail(VP3D_ERR_UNSUPPORTED, "forward_eval: too many rows (%lld)", (long long)N * L[0]);
     PackPerm perm;
     memset(&perm, 0, sizeof(perm));
     perm.levels = p->nb;
     perm.last_rows = L[p->nb];
     for (int i = 1; i <= p->nb; ++i) {
-      perm.region[i - 1] = (unsigned)R[i];
+      perm.region[i - 1] = (unsigned)((long long)N * L[i]);
       perm.width[i - 1] = fw[i];
     }
-    VP3D_LAUNCH(CUDA_TRY(launch_pack_input(x, a0, p->planes, N, T, p->c_in_raw, L[0], fw[0], fw[0], p->k0_pad,
-                               (long long)wl.a0_plane, stream, &perm, p->f16)));
-    common(d, x3[0]);
-    d.a = a0; d.samples = 1; d.a_rows = N * L[0]; d.a_ld = p->k0_pad;
-    use_pack(&d, *p->expand_flat);
-    d.per_sample_tiles = 0; d.out_rows = N * L[0];
+    CUDA_TRY(launch_pack_input(x, bf(wl.a0), p->planes, N, T, p->c_in_raw, L[0], fw[0], fw[0], p->k0_pad,
+                               (long long)wl.a0_plane, stream, &perm, p->f16));
+    strided_chain(p, N, L, &c);
+    // Only the residual region of X_i needs the lo plane when block i + 1 runs plain bf16 (`mixed`)
+    for (int i = 0; i < p->nb; ++i) {
+      if (p->planes != 2 || c.precision[i + 1] == VP3D_PRECISION_BF16X3) continue;
+      const long long r = fw[i + 1] / 2 + p->shift_str[i + 1], R = (long long)N * L[i + 1];
+      c.st[i].lo_row_begin = (int)(r * R);
+      c.st[i].lo_row_end = (int)((r + 1) * R);
+    }
   } else {
-    VP3D_LAUNCH(CUDA_TRY(launch_pack_input(x, a0, p->planes, N, T, p->c_in_raw, T, 1, 1, p->c_in_pad,
-                               (long long)wl.a0_plane, stream, nullptr, p->f16)));
-    common(d, x3[0]);
-    d.a = a0; d.samples = N; d.a_rows = T; d.a_ld = p->c_in_pad;
-    use_pack(&d, *p->expand_dil);
-    d.per_sample_tiles = 1; d.tap_row_step = 1; d.out_rows = L[0];
+    CUDA_TRY(launch_pack_input(x, bf(wl.a0), p->planes, N, T, p->c_in_raw, T, 1, 1, p->c_in_pad,
+                               (long long)wl.a0_plane, stream, nullptr, p->f16));
+    dilated_chain(p, N, T, L, &c);
   }
-  d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
-  d.out = xb[0]; d.out_plane_stride = (long long)wl.x_plane; d.out_ld = C;
-  lo_rows(0, d);
-  VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
-
-  // ---- residual blocks (model.py:129-135 / :190-194)
-  int cur = 0;
-  size_t cur_plane = wl.x_plane;
-  for (int i = 1; i <= p->nb; ++i) {
-    const PackedConv& c0 = *p->conv[2 * (i - 1)];
-    const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
-    const int Lin = L[i - 1], Lout = L[i];
-    const size_t h_plane = (size_t)N * Lout * C;
-    // first conv of the block: dilated / strided k-tap conv + BN + ReLU
-    common(d, x3[i]);
-    d.out_planes = x3[i] ? 2 : 1;  // H only needs a lo plane when its consumer is split-bf16
-    d.a = xb[cur];
-    use_pack(&d, c0);
-    d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
-    d.out = hb; d.out_plane_stride = (long long)h_plane; d.out_ld = C;
-    if (strided) {
-      d.tap_col_step = 0; d.tap_row_step = (int)R[i];  // tap k = row region k of the block input
-      d.samples = 1; d.a_rows = N * Lin; d.a_ld = C;
-      d.per_sample_tiles = 0; d.out_rows = N * Lout;
-    } else {
-      d.samples = N; d.a_rows = Lin; d.a_ld = C;
-      d.per_sample_tiles = 1; d.tap_row_step = p->dilation[i]; d.tap_col_step = 0;
-      d.out_rows = Lout;
-    }
-    // plane stride of A is implied by (samples, a_rows, a_ld) == cur_plane by construction
-    if ((size_t)d.samples * d.a_rows * d.a_ld != cur_plane)
-      return fail(VP3D_ERR_STATE, "internal: activation plane mismatch in block %d", i);
-    VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
-
-    // second conv: 1x1 + BN + ReLU + sliced residual
-    common(d, x3[i]);
-    d.a_planes = x3[i] ? 2 : 1;
-    d.a = hb; d.samples = 1; d.a_rows = N * Lout; d.a_ld = C;
-    use_pack(&d, c1);
-    d.per_sample_tiles = 0; d.out_rows = N * Lout;
-    d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
-    d.res = xb[cur]; d.res_plane_stride = (long long)cur_plane; d.res_ld = C;
-    if (strided) {
-      d.res_rows_per_sample = 0; d.res_row_step = 1;
-      d.res_row_off = (int)((fw[i] / 2 + p->shift_str[i]) * R[i]); d.res_sample_div = 0;
-    } else {
-      // per-sample tiles: the residual rows of a tile are then one TMA box of the block input
-      d.samples = N; d.a_rows = Lout; d.per_sample_tiles = 1; d.out_rows = Lout;
-      d.res_rows_per_sample = Lin; d.res_row_step = 1;
-      d.res_row_off = p->pad[i] + p->shift_dil[i]; d.res_sample_div = 0;
-    }
-    d.out = xb[cur ^ 1]; d.out_plane_stride = (long long)h_plane; d.out_ld = C;
-    lo_rows(i, d);
-    VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
-    cur ^= 1;
-    cur_plane = h_plane;
-  }
-
-  // ---- shrink (model.py:137 / :196) writing (N, T_out, J_out, 3) directly (fuses :74-75)
-  common(d, x3[p->nb + 1]);
-  d.a = xb[cur]; d.samples = 1; d.a_rows = N * L[p->nb]; d.a_ld = C;
-  use_pack(&d, *p->shrink);
-  d.per_sample_tiles = 0; d.out_rows = N * L[p->nb];
-  d.scale = p->shrink->scale; d.shift = p->shrink->shift; d.relu = 0;
-  d.out = nullptr; d.out_f32 = y; d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
-  VP3D_LAUNCH(VP3D_TRY(run_conv(&d, stream)));
+  VP3D_TRY(prof_event(p, launches, false, stream));
+  ++launches;
+  VP3D_TRY(run_infer_chain(p, c, stream, &launches));
   p->last_launches = launches;
   return VP3D_OK;
 }

@@ -39,6 +39,10 @@ int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, 
 int pick_block_n(int n_pad);
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// the 1 KiB-aligned base of a caller's workspace or state buffer (their sizes include the slack)
+inline uint8_t* ws_base(void* ws) {
+  return reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
+}
 int num_sms();
 int run_conv(const vp3d_conv_desc* d, cudaStream_t stream);
 
@@ -170,6 +174,46 @@ int pack_weight(const vp3d_plan* p, const PackedConv& k, const vp3d_weights* w, 
 int pack_expand_forward(const vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream);
 // GEMM weight operand of a conv descriptor: pointer, taps, K per tap and N as stored in k
 void use_pack(vp3d_conv_desc* d, const PackedConv& k);
+// a conv GEMM descriptor over one flat sample with the plan's planes and operands in `precision`,
+// every other field cleared
+inline vp3d_conv_desc conv_desc(const vp3d_plan* p, int precision) {
+  vp3d_conv_desc d;
+  memset(&d, 0, sizeof(d));
+  d.a_planes = d.out_planes = d.res_planes = p->planes;
+  d.precision = precision;
+  d.samples = 1;
+  return d;
+}
+
+// One stage of the eval-mode GEMM chain: the expand conv (stage 0) or residual block i, whose k-tap
+// conv writes H and whose 1x1 conv reads H, adds the block input as residual and writes X_i.
+struct ChainStage {
+  // input [plane][samples][in_rows][pitch], pitch the expand pack's K (stage 0) or C, planes as the
+  // stage before wrote them: A of the k-tap conv and, res_row_off rows into a sample, the residual
+  const __nv_bfloat16* in;
+  int in_rows;
+  __nv_bfloat16* out;        // X_i, [plane][rows][C]
+  long long out_plane, h_plane;   // elements between the planes of X_i, and of H in this block
+  int out_rows;              // per sample (per-sample tiles) or in all (flat)
+  int tap_row_step, res_row_off;
+  int lo_row_begin, lo_row_end;   // as in vp3d_conv_desc, of the GEMM that writes X_i
+};
+// The geometry of one run of the chain: what the offline forward (strided, dilated), the streaming
+// push and its start pass differ in.  run_infer_chain makes every GEMM descriptor from it.
+struct InferChain {
+  ChainStage st[VP3D_MAX_WIDTHS];
+  int stages;                  // stages 0 .. stages-1 run
+  int samples;                 // of every stage's input
+  long long in_plane;          // elements between the planes of stage 0's input
+  int per_sample_tiles;        // of every GEMM but shrink (else: flat rows)
+  const PackedConv* expand;    // the plan's expand_flat or expand_dil
+  __nv_bfloat16* h;
+  float* y;                    // fp32 rows shrink writes from the last stage's output; null: no shrink
+  int precision[VP3D_MAX_WIDTHS + 1];   // operands of expand, of block i, of shrink (nb + 1)
+  bool profile;                // honour vp3d_profile_launch
+};
+// runs the chain on `stream` and adds its launches to *launches
+int run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream, int* launches);
 void train_state_destroy(TrainState* t);
 int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream,
                           bool also_forward);

@@ -339,6 +339,58 @@ inline int grid_for(long long work) {
   return (int)b;
 }
 
+// rows of ring r from frame position pos on
+inline __nv_bfloat16* ring_rows(const StreamRing& r, int pos, int P) {
+  return r.base + (long long)pos * P * r.ld;
+}
+
+// The push of k frames as a flat chain over ring windows.  The window of ring i is its frame
+// positions [w0, w0 + H + k): tap j of the k * P new rows lies dilation * P rows after tap j - 1, the
+// residual (the centre tap, causal: the newest; model.py:130-132) a row offset into the same window.
+// Stage i writes the new rows of ring i + 1, the last stage the buffer shrink reads.
+void push_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const StreamRing* ring,
+                int P, int K, int k, float* y, InferChain* c) {
+  memset(c, 0, sizeof(*c));
+  c->stages = p->nb + 1;
+  c->samples = 1;
+  c->in_plane = ring[0].plane;
+  c->expand = p->expand_dil;
+  c->h = reinterpret_cast<__nv_bfloat16*>(base + L.h);
+  c->y = y;
+  for (int i = 0; i <= p->nb + 1; ++i) c->precision[i] = p->cfg.precision;   // (never `mixed`)
+  for (int i = 0; i <= p->nb; ++i) {
+    ChainStage& s = c->st[i];
+    s.in = ring_rows(ring[i], ring[i].w0, P);
+    s.in_rows = (ring[i].H + k) * P;
+    const StreamRing* next = i < p->nb ? &ring[i + 1] : nullptr;
+    s.out = next ? ring_rows(*next, next->w0 + next->H, P)
+                 : reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
+    s.h_plane = (long long)K * P * p->C;
+    s.out_plane = next ? next->plane : s.h_plane;
+    s.out_rows = k * P;
+    s.tap_row_step = p->dilation[i] * P;
+    s.res_row_off = (p->pad[i] + p->shift_dil[i]) * P;
+  }
+}
+
+// The start pass, from the push's chain: the same GEMMs on the P rows of the new frame with every
+// tap (and the residual) on the same row, v_{i+1} the input of v_{i+2}; ring nb's vector is the last
+// it needs, so block nb and shrink do not run.
+void vpass_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const StreamRing* ring,
+                 int P, InferChain* c) {
+  const long long v_plane = (long long)P * p->C;
+  c->stages = p->nb;
+  c->y = nullptr;
+  for (int i = 0; i < p->nb; ++i) {
+    ChainStage& s = c->st[i];
+    s.in = i == 0 ? ring_rows(ring[0], ring[0].w0 + ring[0].H, P) : c->st[i - 1].out;
+    s.in_rows = s.out_rows = P;
+    s.out = reinterpret_cast<__nv_bfloat16*>(base + L.v[i + 1]);
+    s.out_plane = v_plane;
+    s.tap_row_step = s.res_row_off = 0;
+  }
+}
+
 }  // namespace
 
 // run.py:186-193 pads pad + causal_shift frames in front and pad - causal_shift behind, with
@@ -415,73 +467,20 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     ++launches;
   }
 
-  __nv_bfloat16* hbuf = reinterpret_cast<__nv_bfloat16*>(base + L.h);
-  __nv_bfloat16* xlast = reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
-  const long long act_plane = (long long)K * P * C;
   const long long v_plane = (long long)P * C;
   auto vbuf = [&](int l) { return reinterpret_cast<__nv_bfloat16*>(base + L.v[l]); };
-  // window of ring l: frame positions [w0, w0 + H + k); new frames start at w0 + H
-  auto window = [&](int l) { return ring[l].base + (long long)ring[l].w0 * P * ring[l].ld; };
-  auto new_rows = [&](int l) {
-    return ring[l].base + (long long)(ring[l].w0 + ring[l].H) * P * ring[l].ld;
-  };
-
-  vp3d_conv_desc d;
-  auto common = [&](vp3d_conv_desc& q) {
-    memset(&q, 0, sizeof(q));
-    q.a_planes = planes;
-    q.precision = p->f16 ? VP3D_PRECISION_FP16
-                         : (planes == 2 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16);
-    q.out_planes = planes;
-    q.res_planes = planes;
-    q.samples = 1;
-    q.per_sample_tiles = 0;
-  };
-  auto set_out = [&](vp3d_conv_desc& q, int layer_out, bool vpass) {
-    // layer_out = i: X_i, the output of block i (0 = expand)
-    q.out_ld = C;
-    if (vpass) {
-      q.out = vbuf(layer_out + 1);
-      q.out_plane_stride = v_plane;
-    } else if (layer_out < p->nb) {
-      q.out = new_rows(layer_out + 1);
-      q.out_plane_stride = ring[layer_out + 1].plane;
-    } else {
-      q.out = xlast;
-      q.out_plane_stride = act_plane;
-    }
-  };
+  // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
+  // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs)
+  const bool direct = !aug && !y_rows && (y_frames == 1 || S == 1);
+  float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
+  InferChain push;
+  push_chain(p, L, base, ring, P, K, k, direct ? y + (long long)f_off * p->c_out_raw : ybuf, &push);
 
   if (start && p->nb >= 1) {
-    // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i), every tap on the same row
-    common(d);
-    d.a = new_rows(0); d.a_plane_stride = ring[0].plane; d.a_rows = P; d.a_ld = p->c_in_pad;
-    use_pack(&d, *p->expand_dil);
-    d.tap_row_step = 0; d.out_rows = P;
-    d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
-    set_out(d, 0, true);
-    VP3D_TRY(run_conv(&d, stream));
-    ++launches;
-    for (int i = 1; i < p->nb; ++i) {
-      const PackedConv& c0 = *p->conv[2 * (i - 1)];
-      const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
-      common(d);
-      d.a = vbuf(i); d.a_plane_stride = v_plane; d.a_rows = P; d.a_ld = C;
-      use_pack(&d, c0);
-      d.tap_row_step = 0; d.out_rows = P;
-      d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
-      d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
-      VP3D_TRY(run_conv(&d, stream));
-      common(d);
-      d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = P; d.a_ld = C;
-      use_pack(&d, c1); d.out_rows = P;
-      d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
-      d.res = vbuf(i); d.res_plane_stride = v_plane; d.res_ld = C; d.res_row_step = 1;
-      d.res_row_off = 0;
-      set_out(d, i, true);
-      VP3D_TRY(run_conv(&d, stream));
-      launches += 2;
-    }
+    // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i)
+    InferChain v = push;
+    vpass_chain(p, L, base, ring, P, &v);
+    VP3D_TRY(run_infer_chain(p, v, stream, &launches));
   }
   if (start) {
     BcastArgs b;
@@ -490,7 +489,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     for (int l = 0; l < L.rings; ++l) {
       b.ring[l] = ring[l];
       if (l == 0) {
-        b.src[0] = new_rows(0);   // the starting slot's first frame, just packed
+        // the starting slot's first frame, just packed
+        b.src[0] = ring_rows(ring[0], ring[0].w0 + ring[0].H, P);
         b.src_plane[0] = ring[0].plane;
       } else {
         b.src[l] = vbuf(l);
@@ -508,48 +508,7 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   }
 
   // ---- the push: expand (model.py:127), residual blocks (:129-135), shrink (:137)
-  common(d);
-  d.a = window(0); d.a_plane_stride = ring[0].plane; d.a_rows = (ring[0].H + k) * P;
-  d.a_ld = p->c_in_pad;
-  use_pack(&d, *p->expand_dil);
-  d.tap_row_step = P; d.out_rows = k * P;
-  d.scale = p->expand_dil->scale; d.shift = p->expand_dil->shift; d.relu = 1;
-  set_out(d, 0, false);
-  VP3D_TRY(run_conv(&d, stream));
-  ++launches;
-  for (int i = 1; i <= p->nb; ++i) {
-    const PackedConv& c0 = *p->conv[2 * (i - 1)];
-    const PackedConv& c1 = *p->conv[2 * (i - 1) + 1];
-    common(d);
-    d.a = window(i); d.a_plane_stride = ring[i].plane; d.a_rows = (ring[i].H + k) * P; d.a_ld = C;
-    use_pack(&d, c0);
-    d.tap_row_step = p->dilation[i] * P; d.out_rows = k * P;
-    d.scale = c0.scale; d.shift = c0.shift; d.relu = 1;
-    d.out = hbuf; d.out_plane_stride = act_plane; d.out_ld = C;
-    VP3D_TRY(run_conv(&d, stream));
-    common(d);
-    d.a = hbuf; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
-    use_pack(&d, c1); d.out_rows = k * P;
-    d.scale = c1.scale; d.shift = c1.shift; d.relu = 1;
-    // residual: the centre tap (causal: the newest) of the block input window, model.py:130-132
-    d.res = window(i); d.res_plane_stride = ring[i].plane; d.res_ld = C; d.res_row_step = 1;
-    d.res_row_off = (p->pad[i] + p->shift_dil[i]) * P;
-    set_out(d, i, false);
-    VP3D_TRY(run_conv(&d, stream));
-    launches += 2;
-  }
-  // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
-  // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs)
-  const bool direct = !aug && !y_rows && (y_frames == 1 || S == 1);
-  float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
-  common(d);
-  d.a = xlast; d.a_plane_stride = act_plane; d.a_rows = k * P; d.a_ld = C;
-  use_pack(&d, *p->shrink); d.out_rows = k * P;
-  d.scale = p->shrink->scale; d.shift = p->shrink->shift; d.relu = 0;
-  d.out_f32 = direct ? y + (long long)f_off * p->c_out_raw : ybuf;
-  d.out_f32_ld = p->c_out_raw; d.n_valid = p->c_out_raw;
-  VP3D_TRY(run_conv(&d, stream));
-  ++launches;
+  VP3D_TRY(run_infer_chain(p, push, stream, &launches));
   if (!direct) {
     CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
                         dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
@@ -575,8 +534,9 @@ static int stream_supported(const vp3d_plan* p, const char* what) {
   return VP3D_OK;
 }
 
-static uint8_t* aligned_state(void* state) {
-  return reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(state), 1024));
+// every row index of a session's rings and buffers fits an int
+static bool stream_fits(const vp3d_plan* p, int S, int K, int flags) {
+  return (long long)physical_rows(S, flags) * (K + 2LL * vp3d_receptive_field(p)) <= 0x7fffffffLL;
 }
 
 }  // namespace vp3d
@@ -591,8 +551,7 @@ VP3D_EXPORT int vp3d_stream_lookahead(const vp3d_plan* p) {
 }
 
 VP3D_EXPORT size_t vp3d_stream_state_bytes_ex(const vp3d_plan* p, int S, int K, int flags) {
-  if (!p || S < 1 || K < 1 || (flags & ~VP3D_STREAM_AUGMENT) ||
-      (long long)physical_rows(S, flags) * (K + 2LL * vp3d_receptive_field(p)) > 0x7fffffffLL)
+  if (!p || S < 1 || K < 1 || (flags & ~VP3D_STREAM_AUGMENT) || !stream_fits(p, S, K, flags))
     return 0;
   return stream_layout(p, S, K, flags).total;
 }
@@ -629,24 +588,24 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
     VP3D_TRY(check_mirror_map(kps_src, j_in, what, "kps_src"));
     if (joints_src) VP3D_TRY(check_mirror_map(joints_src, j_out, what, "joints_src"));
   }
-  const size_t need = vp3d_stream_state_bytes_ex(p, S, K, flags);
-  if (need == 0) return fail(VP3D_ERR_UNSUPPORTED, "%s: %d streams x %d frames is too large", what, S, K);
-  if (state_bytes < need)
-    return fail(VP3D_ERR_WORKSPACE, "%s: state too small: %zu < %zu", what, state_bytes, need);
+  if (!stream_fits(p, S, K, flags))
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: %d streams x %d frames is too large", what, S, K);
+  const StreamLayout L = stream_layout(p, S, K, flags);
+  if (state_bytes < L.total)
+    return fail(VP3D_ERR_WORKSPACE, "%s: state too small: %zu < %zu", what, state_bytes, L.total);
   StreamHost h;
   h.S = S;
   h.K = K;
   h.flags = flags;
   h.joint_src = aug && joints_src;
   p->streams[state] = h;
-  uint8_t* base = aligned_state(state);
+  uint8_t* base = ws_base(state);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  CUDA_TRY(cudaMemsetAsync(base, 0, need - 1024, s));
+  CUDA_TRY(cudaMemsetAsync(base, 0, L.total - 1024, s));
   // every sequence open (length -1) in both bookkeeping buffers
-  CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, S, K, flags).length, 0xff, (size_t)2 * S * 8, s));
+  CUDA_TRY(cudaMemsetAsync(base + L.length, 0xff, (size_t)2 * S * 8, s));
   if (aug) {
     // the maps live in the state from here on: pushes read them on the device
-    const StreamLayout L = stream_layout(p, S, K, flags);
     CUDA_TRY(cudaMemcpyAsync(base + L.kps, kps_src, (size_t)j_in * 4, cudaMemcpyHostToDevice, s));
     if (joints_src)
       CUDA_TRY(cudaMemcpyAsync(base + L.jsrc, joints_src, (size_t)j_out * 4, cudaMemcpyHostToDevice, s));
@@ -696,7 +655,7 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
     return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
   if (!p->conv_packed || !p->bn_packed)
     return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
-  return stream_step(p, aligned_state(state), *h, x, k, start_mask, end,
+  return stream_step(p, ws_base(state), *h, x, k, start_mask, end,
                      reinterpret_cast<const long long*>(x_rows),
                      reinterpret_cast<const long long*>(y_rows), y, k, 0,
                      reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
@@ -727,7 +686,7 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
     return fail(VP3D_ERR_STATE, "stream_finish: vp3d_set_weights has not been called");
   const int la = stream_lookahead(p);
   if (la > 0 && (!y || !frame)) return fail(VP3D_ERR_INVALID, "stream_finish: null y or frame");
-  uint8_t* base = aligned_state(state);
+  uint8_t* base = ws_base(state);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int launches = 0;
   for (int off = 0; off < la; off += h->K) {

@@ -263,16 +263,6 @@ DropoutCfg dropout_cfg(float p, unsigned long long seed, int layer) {
   return d;
 }
 
-// a conv GEMM descriptor in the plan's precision and planes, every other field cleared
-vp3d_conv_desc conv_desc(const vp3d_plan* p) {
-  vp3d_conv_desc d;
-  memset(&d, 0, sizeof(d));
-  d.a_planes = d.out_planes = p->planes;
-  d.precision = p->cfg.precision;
-  d.samples = 1;
-  return d;
-}
-
 // elements of one plane of a GEMM's A operand, the conv's input
 long long in_plane(const vp3d_conv_desc& d) { return (long long)d.samples * d.a_rows * d.a_ld; }
 
@@ -313,7 +303,7 @@ void train_convs(const vp3d_plan* p, const TrainLayout& wl, uint8_t* base, int N
                   int a_ld, long long out_rows) -> vp3d_conv_desc& {
     TrainConv& c = cv[l];
     c.pack = k; c.t = kt; c.in = bf(in); c.z = c.act = nullptr; c.res = RowMap{0, 0, 1, 0};
-    vp3d_conv_desc& d = c.fwd = conv_desc(p);
+    vp3d_conv_desc& d = c.fwd = conv_desc(p, p->cfg.precision);
     use_pack(&d, *k);
     d.a = c.in; d.a_rows = (int)a_rows; d.a_ld = a_ld; d.out_rows = (int)out_rows;
     return d;
@@ -374,7 +364,7 @@ vp3d_wgrad_desc wgrad_desc(const TrainConv& c, const __nv_bfloat16* dz, float* g
 vp3d_conv_desc dgrad_desc(const vp3d_plan* p, const TrainConv& c, const __nv_bfloat16* dz,
                           __nv_bfloat16* out, const __nv_bfloat16* res = nullptr, int res_off = 0) {
   const vp3d_conv_desc& f = c.fwd;
-  vp3d_conv_desc d = conv_desc(p);
+  vp3d_conv_desc d = conv_desc(p, p->cfg.precision);
   use_pack(&d, *c.t);
   d.a = dz; d.a_rows = f.out_rows; d.a_ld = c.t->k_pad;
   d.out = out; d.out_rows = f.a_rows; d.out_plane_stride = in_plane(f); d.out_ld = f.a_ld;
@@ -520,7 +510,7 @@ VP3D_API int vp3d_forward_train_ex(vp3d_plan* p, const float* x, float* y, int N
   const TrainLayout wl = train_layout(p, N, T, L);
   if (!ws || ws_bytes < wl.total)
     return fail(VP3D_ERR_WORKSPACE, "train workspace too small: %zu < %zu", ws_bytes, wl.total);
-  uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
+  uint8_t* base = ws_base(ws);
   const int C = p->C, pl = p->planes;
   t->N = N; t->T = T; t->dropout_p = dropout_p; t->seed = seed; t->frozen_bn = frozen;
   t->have_forward = false;
@@ -643,7 +633,7 @@ static int backward_impl(vp3d_plan* p, const float* dy, const vp3d_grads* g, flo
   const int* L = t->L;
   const TrainLayout wl = train_layout(p, N, t->T, L);
   if (!ws || ws_bytes < wl.total) return fail(VP3D_ERR_WORKSPACE, "backward: workspace too small");
-  uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
+  uint8_t* base = ws_base(ws);
   auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
   float* partial = reinterpret_cast<float*>(base + wl.partial);
   float* slab_part = reinterpret_cast<float*>(base + wl.slab);
