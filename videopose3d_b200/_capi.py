@@ -269,6 +269,16 @@ SIGNATURES = {
     "vp3d_mpjpe_fwd_bwd": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_mpjpe_scratch_bytes": (ctypes.c_size_t, [ctypes.c_int64]),
+    "vp3d_mpjpe_fwd_bwd_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p,
+                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                             ctypes.c_void_p]),
+    "vp3d_projected_mpjpe_scratch_bytes": (ctypes.c_size_t, [ctypes.c_int64, ctypes.c_int32]),
+    "vp3d_projected_mpjpe_fwd_bwd_ex": (ctypes.c_int, [ctypes.c_void_p] * 4
+                                        + [ctypes.c_int64, ctypes.c_int32, ctypes.c_int32,
+                                           ctypes.c_int32] + [ctypes.c_void_p] * 4
+                                        + [ctypes.c_size_t, ctypes.c_void_p]),
     "vp3d_pose_errors_scratch_bytes": (ctypes.c_size_t, [ctypes.c_int64]),
     "vp3d_pose_errors": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32,

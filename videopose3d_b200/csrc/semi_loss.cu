@@ -262,7 +262,9 @@ extern "C" __attribute__((visibility("default"))) int vp3d_semi_loss_fwd_bwd(
     return fail(VP3D_ERR_INVALID, "semi_loss: the 3-D terms need target_3d");
   if (n_unlabeled > 0 && t_proj && (!cam || !target_2d))
     return fail(VP3D_ERR_INVALID, "semi_loss: the re-projection term needs cam and target_2d");
-  const bool bone = t_bone && n_labeled > 0 && n_unlabeled > 0 && joints > 1;
+  // one joint has no bones: the penalty is the mean over none, 0 / 0 = NaN as in the reference,
+  // and adds no gradient
+  const bool bone = t_bone && n_labeled > 0 && n_unlabeled > 0;
   if (bone && !parents) return fail(VP3D_ERR_INVALID, "semi_loss: the bone-length term needs parents");
   const long long units = (n_labeled + n_unlabeled) * frames;
   if (units > 0x7fffffffll * 64) return fail(VP3D_ERR_UNSUPPORTED, "semi_loss: too large");

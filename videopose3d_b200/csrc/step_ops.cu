@@ -6,7 +6,8 @@
 //    launches over 16.95 M parameters; this is one HBM-bound pass: 20 B read + 16 B written per
 //    element.
 //  * vp3d_mpjpe_fwd_bwd: mean per-joint position error (loss.py:11-17, run.py:413-418) and its
-//    gradient w.r.t. the prediction in one launch.
+//    gradient w.r.t. the prediction in one launch.  The loss is summed in block order (no
+//    floating-point atomics): the same input gives the same bits.
 #include "internal.cuh"
 
 namespace vp3d {
@@ -168,19 +169,62 @@ adam_pack_kernel(const __grid_constant__ PackBatch batch, const AdamHyper h) {
 // ---- MPJPE ------------------------------------------------------------------------------------
 
 constexpr int kLossThreads = 256;
+constexpr long long kLossMaxBlocks = 4096;  // grid cap of the scratch-taking entry points
 
-// One thread per joint: d = ||pred - target||_2 over the last axis (dims = 3 for poses);
-// loss += weight * w_j * d, dpred = weight * w_j * (pred - target) / d  (0 where d == 0, as
-// autograd's norm backward yields for a zero vector).  weight = 1 / joints_total folds the mean;
-// w_j = 1 without per-joint weights (mpjpe) or the caller's weight (weighted_mpjpe).
+// Sum of v over the block in a fixed tree (lanes by xor shuffle, then warps 0..7); the total is
+// valid in thread 0.
+__device__ __forceinline__ float block_total(float v, float* s_part) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();  // s_part may still be read by the previous call
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < kLossThreads / 32 ? s_part[threadIdx.x] : 0.0f;
+    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  }
+  return v;
+}
+
+// loss = weight * (sum of the block totals in block order).  One block writes its total directly.
+// Otherwise every block stores its total in part[blockIdx.x] and takes an integer ticket; the
+// block that draws the last ticket adds the partials, each thread a fixed strided subset and then
+// the fixed block tree, so the bits do not depend on which block finishes when.  *ticket must be
+// 0 at launch.
+__device__ void store_loss(float block_sum, float weight, float* loss, float* part,
+                           unsigned* ticket, float* s_part) {
+  __shared__ bool is_last;
+  if (gridDim.x == 1) {
+    if (threadIdx.x == 0) *loss = block_sum * weight;
+    return;
+  }
+  if (threadIdx.x == 0) {
+    part[blockIdx.x] = block_sum;
+    __threadfence();
+    is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  float t = 0.0f;
+  for (unsigned b = threadIdx.x; b < gridDim.x; b += kLossThreads) t += __ldcg(part + b);
+  t = block_total(t, s_part);
+  if (threadIdx.x == 0) *loss = t * weight;
+}
+
+// One thread per joint (grid-stride): d = ||pred - target||_2 over the last axis (dims = 3 for
+// poses); loss = weight * sum w_j * d, dpred = weight * w_j * (pred - target) / d  (0 where d == 0,
+// as autograd's norm backward yields for a zero vector).  weight = 1 / joints_total folds the mean
+// (NaN for no joints: torch.mean of nothing); w_j = 1 without per-joint weights (mpjpe) or the
+// caller's weight (weighted_mpjpe).
 __global__ void __launch_bounds__(kLossThreads)
 mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ target,
              const float* __restrict__ joint_w, float* __restrict__ dpred, float* __restrict__ loss,
-             long long joints_total, int dims, float weight) {
+             float* __restrict__ part, unsigned* __restrict__ ticket, long long joints_total,
+             int dims, float weight) {
   __shared__ float s_part[kLossThreads / 32];
-  const long long j = (long long)blockIdx.x * kLossThreads + threadIdx.x;
-  float d = 0.0f;
-  if (j < joints_total) {
+  float acc = 0.0f;
+  for (long long j = (long long)blockIdx.x * kLossThreads + threadIdx.x; j < joints_total;
+       j += (long long)gridDim.x * kLossThreads) {
     const float* p = pred + j * dims;
     const float* q = target + j * dims;
     float sq = 0.0f;
@@ -188,22 +232,15 @@ mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ target,
       const float e = p[k] - q[k];
       sq = fmaf(e, e, sq);
     }
-    d = sqrtf(sq);
+    const float d = sqrtf(sq);
     const float wj = joint_w != nullptr ? joint_w[j] : 1.0f;
     if (dpred != nullptr) {
       const float s = d > 0.0f ? weight * wj / d : 0.0f;
       for (int k = 0; k < dims; ++k) dpred[j * dims + k] = (p[k] - q[k]) * s;
     }
-    d *= wj;
+    acc += d * wj;
   }
-  for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = d;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float v = threadIdx.x < kLossThreads / 32 ? s_part[threadIdx.x] : 0.0f;
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss, v * weight);
-  }
+  store_loss(block_total(acc, s_part), weight, loss, part, ticket, s_part);
 }
 
 // ---- re-projection loss (semi-supervised branch) -------------------------------------------------
@@ -212,17 +249,19 @@ mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ target,
 // (camera.py:37-67: perspective divide clamped to [-1, 1], radial k1..k3 and tangential p1, p2
 // distortion, focal length, principal point; or only the linear part, :69-88), accumulate the 2-D
 // distance to the target, and write d loss / d pos per joint and d loss / d traj per frame (the
-// joint sum -- no atomics needed since the frame's joints live in one thread).
+// joint sum -- no atomics needed since the frame's joints live in one thread).  Frames are
+// grid-strided; the loss is summed as in mpjpe_kernel.
 __global__ void __launch_bounds__(kLossThreads)
 projected_mpjpe_kernel(const float* __restrict__ pos, const float* __restrict__ traj,
                        const float* __restrict__ cam, const float* __restrict__ target,
                        float* __restrict__ dpos, float* __restrict__ dtraj, float* __restrict__ loss,
+                       float* __restrict__ part, unsigned* __restrict__ ticket,
                        long long frames_total, int frames_per_sample, int joints, int linear,
                        float weight) {
   __shared__ float s_part[kLossThreads / 32];
-  const long long fr = (long long)blockIdx.x * kLossThreads + threadIdx.x;
   float acc = 0.0f;
-  if (fr < frames_total) {
+  for (long long fr = (long long)blockIdx.x * kLossThreads + threadIdx.x; fr < frames_total;
+       fr += (long long)gridDim.x * kLossThreads) {
     const float* cp = cam + (fr / frames_per_sample) * 9;
     const float fx = cp[0], fy = cp[1], cx = cp[2], cy = cp[3];
     const float k0 = cp[4], k1 = cp[5], k2 = cp[6], p0 = cp[7], p1 = cp[8];
@@ -279,14 +318,19 @@ projected_mpjpe_kernel(const float* __restrict__ pos, const float* __restrict__ 
       dtraj[fr * 3 + 2] = gtz;
     }
   }
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float v = threadIdx.x < kLossThreads / 32 ? s_part[threadIdx.x] : 0.0f;
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss, v * weight);
-  }
+  store_loss(block_total(acc, s_part), weight, loss, part, ticket, s_part);
+}
+
+// Grid of the loss kernels: one thread per item up to kLossMaxBlocks blocks with caller scratch,
+// one block without.  Scratch = the ticket + one partial per block; none for a single block.
+long long loss_blocks(long long items, bool scratch) {
+  if (!scratch) return 1;
+  const long long b = (items + kLossThreads - 1) / kLossThreads;
+  return b < 1 ? 1 : (b > kLossMaxBlocks ? kLossMaxBlocks : b);
+}
+size_t loss_scratch_bytes(long long items) {
+  const long long b = loss_blocks(items, true);
+  return b > 1 ? (size_t)(b + 1) * sizeof(float) : 0;
 }
 
 }  // namespace
@@ -387,24 +431,97 @@ VP3D_EXPORT int vp3d_adam_step(const vp3d_adam_tensor* tensors, int32_t n_tensor
   return VP3D_OK;
 }
 
+namespace vp3d {
+// Scratch layout of the loss entry points: [0] the ticket (zeroed here, before the launch),
+// [1 .. blocks] the block partials.
+static int mpjpe_launch(const char* who, const float* pred, const float* target,
+                        const float* joint_w, int64_t joints_total, int32_t dims, float* loss,
+                        float* dpred, void* scratch, size_t scratch_bytes, bool ex, void* stream) {
+  if (joints_total < 0 || dims < 1 || dims > 16)
+    return fail(VP3D_ERR_INVALID, "%s: bad sizes (joints %lld, dims %d)", who,
+                (long long)joints_total, dims);
+  if (loss == nullptr) return fail(VP3D_ERR_INVALID, "%s: null loss pointer", who);
+  if (joints_total > 0 && (pred == nullptr || target == nullptr))
+    return fail(VP3D_ERR_INVALID, "%s: null pointer", who);
+  const long long blocks = loss_blocks(joints_total, ex);
+  const size_t need = ex ? loss_scratch_bytes(joints_total) : 0;
+  if (need > 0 && (scratch == nullptr || scratch_bytes < need))
+    return fail(VP3D_ERR_WORKSPACE, "%s: scratch too small (%zu bytes, need %zu)", who,
+                scratch_bytes, need);
+  unsigned* ticket = blocks > 1 ? static_cast<unsigned*>(scratch) : nullptr;
+  float* part = blocks > 1 ? static_cast<float*>(scratch) + 1 : nullptr;
+  if (ticket) CUDA_TRY(cudaMemsetAsync(ticket, 0, sizeof(unsigned), (cudaStream_t)stream));
+  // the mean over no joints is NaN, as torch.mean of an empty tensor
+  const float weight = joints_total > 0 ? (float)(1.0 / (double)joints_total) : __builtin_nanf("");
+  mpjpe_kernel<<<(unsigned)blocks, kLossThreads, 0, (cudaStream_t)stream>>>(
+      pred, target, joint_w, dpred, loss, part, ticket, joints_total, dims, weight);
+  CUDA_TRY(cudaGetLastError());
+  return VP3D_OK;
+}
+
+static int projected_launch(const char* who, const float* pos, const float* traj, const float* cam,
+                            const float* target, int64_t samples, int32_t frames_per_sample,
+                            int32_t joints, int32_t linear, float* loss, float* dpos, float* dtraj,
+                            void* scratch, size_t scratch_bytes, bool ex, void* stream) {
+  if (samples < 0 || frames_per_sample < 1 || joints < 1)
+    return fail(VP3D_ERR_INVALID, "%s: bad sizes (samples %lld, frames %d, joints %d)", who,
+                (long long)samples, frames_per_sample, joints);
+  if (loss == nullptr) return fail(VP3D_ERR_INVALID, "%s: null loss pointer", who);
+  if ((dpos == nullptr) != (dtraj == nullptr))
+    return fail(VP3D_ERR_INVALID, "%s: dpos and dtraj go together", who);
+  if (samples > 0 && (!pos || !traj || !cam || !target))
+    return fail(VP3D_ERR_INVALID, "%s: null pointer", who);
+  const long long frames_total = samples * frames_per_sample;
+  const long long blocks = loss_blocks(frames_total, ex);
+  const size_t need = ex ? loss_scratch_bytes(frames_total) : 0;
+  if (need > 0 && (scratch == nullptr || scratch_bytes < need))
+    return fail(VP3D_ERR_WORKSPACE, "%s: scratch too small (%zu bytes, need %zu)", who,
+                scratch_bytes, need);
+  unsigned* ticket = blocks > 1 ? static_cast<unsigned*>(scratch) : nullptr;
+  float* part = blocks > 1 ? static_cast<float*>(scratch) + 1 : nullptr;
+  if (ticket) CUDA_TRY(cudaMemsetAsync(ticket, 0, sizeof(unsigned), (cudaStream_t)stream));
+  const float weight = frames_total > 0 ? (float)(1.0 / ((double)frames_total * joints))
+                                        : __builtin_nanf("");
+  projected_mpjpe_kernel<<<(unsigned)blocks, kLossThreads, 0, (cudaStream_t)stream>>>(
+      pos, traj, cam, target, dpos, dtraj, loss, part, ticket, frames_total, frames_per_sample,
+      joints, linear, weight);
+  CUDA_TRY(cudaGetLastError());
+  return VP3D_OK;
+}
+}  // namespace vp3d
+
+VP3D_EXPORT size_t vp3d_mpjpe_scratch_bytes(int64_t joints_total) {
+  return vp3d::loss_scratch_bytes(joints_total);
+}
+
+VP3D_EXPORT int vp3d_mpjpe_fwd_bwd_ex(const float* pred, const float* target, const float* joint_w,
+                                      int64_t joints_total, int32_t dims, float* loss, float* dpred,
+                                      void* scratch, size_t scratch_bytes, void* stream) {
+  return vp3d::mpjpe_launch("vp3d_mpjpe_fwd_bwd_ex", pred, target, joint_w, joints_total, dims,
+                            loss, dpred, scratch, scratch_bytes, true, stream);
+}
+
 VP3D_EXPORT int vp3d_mpjpe_fwd_bwd(const float* pred, const float* target, const float* joint_w,
                                    int64_t joints_total, int32_t dims, float* loss, float* dpred,
                                    void* stream) {
-  using namespace vp3d;
-  if (joints_total < 0 || dims < 1 || dims > 16)
-    return fail(VP3D_ERR_INVALID, "vp3d_mpjpe_fwd_bwd: bad sizes (joints %lld, dims %d)",
-                (long long)joints_total, dims);
-  if (loss == nullptr) return fail(VP3D_ERR_INVALID, "vp3d_mpjpe_fwd_bwd: null loss pointer");
-  if (joints_total > 0 && (pred == nullptr || target == nullptr))
-    return fail(VP3D_ERR_INVALID, "vp3d_mpjpe_fwd_bwd: null pointer");
-  CUDA_TRY(cudaMemsetAsync(loss, 0, sizeof(float), (cudaStream_t)stream));
-  if (joints_total == 0) return VP3D_OK;
-  const long long blocks = (joints_total + kLossThreads - 1) / kLossThreads;
-  if (blocks > 0x7fffffffll) return fail(VP3D_ERR_UNSUPPORTED, "vp3d_mpjpe_fwd_bwd: too large");
-  mpjpe_kernel<<<(unsigned)blocks, kLossThreads, 0, (cudaStream_t)stream>>>(
-      pred, target, joint_w, dpred, loss, joints_total, dims, (float)(1.0 / (double)joints_total));
-  CUDA_TRY(cudaGetLastError());
-  return VP3D_OK;
+  return vp3d::mpjpe_launch("vp3d_mpjpe_fwd_bwd", pred, target, joint_w, joints_total, dims, loss,
+                            dpred, nullptr, 0, false, stream);
+}
+
+VP3D_EXPORT size_t vp3d_projected_mpjpe_scratch_bytes(int64_t samples, int32_t frames_per_sample) {
+  if (samples < 0 || frames_per_sample < 1) return 0;
+  return vp3d::loss_scratch_bytes(samples * frames_per_sample);
+}
+
+VP3D_EXPORT int vp3d_projected_mpjpe_fwd_bwd_ex(const float* pos, const float* traj,
+                                                const float* cam, const float* target,
+                                                int64_t samples, int32_t frames_per_sample,
+                                                int32_t joints, int32_t linear, float* loss,
+                                                float* dpos, float* dtraj, void* scratch,
+                                                size_t scratch_bytes, void* stream) {
+  return vp3d::projected_launch("vp3d_projected_mpjpe_fwd_bwd_ex", pos, traj, cam, target, samples,
+                                frames_per_sample, joints, linear, loss, dpos, dtraj, scratch,
+                                scratch_bytes, true, stream);
 }
 
 VP3D_EXPORT int vp3d_projected_mpjpe_fwd_bwd(const float* pos, const float* traj, const float* cam,
@@ -412,24 +529,7 @@ VP3D_EXPORT int vp3d_projected_mpjpe_fwd_bwd(const float* pos, const float* traj
                                              int32_t frames_per_sample, int32_t joints,
                                              int32_t linear, float* loss, float* dpos, float* dtraj,
                                              void* stream) {
-  using namespace vp3d;
-  if (samples < 0 || frames_per_sample < 1 || joints < 1)
-    return fail(VP3D_ERR_INVALID, "vp3d_projected_mpjpe_fwd_bwd: bad sizes (samples %lld, frames %d, "
-                "joints %d)", (long long)samples, frames_per_sample, joints);
-  if (loss == nullptr) return fail(VP3D_ERR_INVALID, "vp3d_projected_mpjpe_fwd_bwd: null loss pointer");
-  if ((dpos == nullptr) != (dtraj == nullptr))
-    return fail(VP3D_ERR_INVALID, "vp3d_projected_mpjpe_fwd_bwd: dpos and dtraj go together");
-  if (samples > 0 && (!pos || !traj || !cam || !target))
-    return fail(VP3D_ERR_INVALID, "vp3d_projected_mpjpe_fwd_bwd: null pointer");
-  CUDA_TRY(cudaMemsetAsync(loss, 0, sizeof(float), (cudaStream_t)stream));
-  if (samples == 0) return VP3D_OK;
-  const long long frames_total = samples * frames_per_sample;
-  const long long blocks = (frames_total + kLossThreads - 1) / kLossThreads;
-  if (blocks > 0x7fffffffll)
-    return fail(VP3D_ERR_UNSUPPORTED, "vp3d_projected_mpjpe_fwd_bwd: too large");
-  projected_mpjpe_kernel<<<(unsigned)blocks, kLossThreads, 0, (cudaStream_t)stream>>>(
-      pos, traj, cam, target, dpos, dtraj, loss, frames_total, frames_per_sample, joints, linear,
-      (float)(1.0 / ((double)frames_total * joints)));
-  CUDA_TRY(cudaGetLastError());
-  return VP3D_OK;
+  return vp3d::projected_launch("vp3d_projected_mpjpe_fwd_bwd", pos, traj, cam, target, samples,
+                                frames_per_sample, joints, linear, loss, dpos, dtraj, nullptr, 0,
+                                false, stream);
 }

@@ -2,11 +2,11 @@
 
 `mpjpe` and `weighted_mpjpe` with the reference's signatures and values (common/loss.py:11-17,
 :19-25; used at run.py:359, 413, 452, 501): the loss and its gradient with respect to the
-prediction come out of ONE launch (`vp3d_mpjpe_fwd_bwd`, csrc/step_ops.cu) instead of the
+prediction come out of ONE launch (`vp3d_mpjpe_fwd_bwd_ex`, csrc/step_ops.cu) instead of the
 subtract / norm / mean kernels and their four backward kernels.  `projected_mpjpe` is the
 re-projection loss of the semi-supervised branch (run.py:374-379): camera projection of
 `predicted_pos + predicted_traj` (common/camera.py:37-88) and the 2-D mpjpe, with the gradients for
-both model outputs, in one launch (`vp3d_projected_mpjpe_fwd_bwd`).  `semi_supervised_loss` is the
+both model outputs, in one launch (`vp3d_projected_mpjpe_fwd_bwd_ex`).  `semi_supervised_loss` is the
 whole loss head of the semi-supervised step -- 3-D loss, depth-weighted trajectory loss,
 re-projection loss and the bone-length penalty (run.py:350-390) with the gradients for both model
 outputs -- in one cooperative launch (`vp3d_semi_loss_fwd_bwd`, csrc/semi_loss.cu);
@@ -22,6 +22,19 @@ from . import _capi
 
 __all__ = ["mpjpe", "weighted_mpjpe", "projected_mpjpe", "bone_length_penalty",
            "semi_supervised_loss", "n_mpjpe", "p_mpjpe", "mean_velocity_error", "pose_loss"]
+
+
+def _scratch(nbytes, dev):
+    """Device scratch of the block-ordered loss sums (None when one block does the whole sum)."""
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _numel(t):
+    return t.numel() if t is not None else 0
 
 
 class _Mpjpe(torch.autograd.Function):
@@ -42,13 +55,15 @@ class _Mpjpe(torch.autograd.Function):
         loss = torch.empty((), dtype=torch.float32, device=pred.device)
         need_grad = ctx.needs_input_grad[0]
         dpred = torch.empty_like(pred) if need_grad else None
+        scratch = _scratch(lib.vp3d_mpjpe_scratch_bytes(joints), pred.device)
         with torch.cuda.device(pred.device):
             stream = torch.cuda.current_stream(pred.device).cuda_stream
-            _capi.check(lib.vp3d_mpjpe_fwd_bwd(pred.data_ptr(), tgt.data_ptr(),
-                                               w.data_ptr() if w is not None else None, joints, dims,
-                                               loss.data_ptr(),
-                                               dpred.data_ptr() if need_grad else None, stream),
-                        "vp3d_mpjpe_fwd_bwd")
+            _capi.check(lib.vp3d_mpjpe_fwd_bwd_ex(pred.data_ptr(), tgt.data_ptr(),
+                                                  w.data_ptr() if w is not None else None, joints,
+                                                  dims, loss.data_ptr(),
+                                                  dpred.data_ptr() if need_grad else None,
+                                                  _ptr(scratch), _numel(scratch), stream),
+                        "vp3d_mpjpe_fwd_bwd_ex")
         # kept for the lifetime of the graph: a second backward (retain_graph=True, or the loss
         # feeding two backward passes) gets the same gradient again, as with the torch expression
         ctx.dpred = dpred
@@ -92,13 +107,14 @@ class _ProjectedMpjpe(torch.autograd.Function):
         need_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         dpos = torch.empty_like(pos_c) if need_grad else None
         dtraj = torch.empty_like(traj_c) if need_grad else None
+        scratch = _scratch(lib.vp3d_projected_mpjpe_scratch_bytes(n, frames), pos.device)
         with torch.cuda.device(pos.device):
             stream = torch.cuda.current_stream(pos.device).cuda_stream
-            _capi.check(lib.vp3d_projected_mpjpe_fwd_bwd(
+            _capi.check(lib.vp3d_projected_mpjpe_fwd_bwd_ex(
                 pos_c.data_ptr(), traj_c.data_ptr(), cam_c.data_ptr(), tgt_c.data_ptr(), n, frames,
                 joints, int(bool(linear)), loss.data_ptr(),
                 dpos.data_ptr() if need_grad else None, dtraj.data_ptr() if need_grad else None,
-                stream), "vp3d_projected_mpjpe_fwd_bwd")
+                _ptr(scratch), _numel(scratch), stream), "vp3d_projected_mpjpe_fwd_bwd_ex")
         ctx.grads = (dpos, dtraj)
         return loss
 
@@ -116,9 +132,24 @@ def projected_mpjpe(predicted_pos, predicted_traj, camera_params, target_2d, lin
     return _ProjectedMpjpe.apply(predicted_pos, predicted_traj, camera_params, target_2d, linear)
 
 
+def _checked_parents(parents, joints):
+    """The skeleton's parent list as ints; every entry after the root must index the pose, because
+    the kernel reads pos[parent] unchecked.  The root's parent (-1 in the reference's list) is
+    never read: bones start at joint 1."""
+    plist = [int(p) for p in parents]
+    bad = [(j, p) for j, p in enumerate(plist) if j >= 1 and not 0 <= p < joints]
+    if len(plist) != joints or bad:
+        raise ValueError(f"videopose3d_b200.loss: parents must give each of the {joints} joints after "
+                         f"the root a parent in [0, {joints}) (got {len(plist)} entries; out of range "
+                         f"(joint, parent): {bad[:4]})")
+    return plist
+
+
 class _SemiLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pos, traj, target_3d, cam, target_2d, parents, n_labeled, linear, terms, which):
+        if terms & _capi.VP3D_SEMI_BONE:
+            parents = _checked_parents(parents, pos.shape[2])
         for t, what in ((pos, "predicted_3d_pos"), (traj, "predicted_traj")):
             if not (t.is_cuda and t.dtype == torch.float32):
                 raise RuntimeError(f"videopose3d_b200.loss: {what} must be a CUDA float32 tensor "
@@ -140,9 +171,7 @@ class _SemiLoss(torch.autograd.Function):
         tgt2 = prep(target_2d, (n_unl, frames, joints, 2), "target_2d")
         par = None
         if terms & _capi.VP3D_SEMI_BONE:
-            # the root's parent is -1 in the reference's list and never read (bones start at joint 1)
-            par = torch.as_tensor(list(parents), dtype=torch.int32).clamp_min(0).to(dev)
-            assert par.numel() == joints
+            par = torch.as_tensor(parents, dtype=torch.int32).clamp_min(0).to(dev)
         lib = _capi.load()
         pos_c, traj_c = pos.contiguous(), traj.contiguous()
         losses = torch.empty(5, dtype=torch.float32, device=dev)
@@ -150,13 +179,12 @@ class _SemiLoss(torch.autograd.Function):
         dpos = torch.empty_like(pos_c) if need_grad else None
         dtraj = torch.empty_like(traj_c) if need_grad else None
         scratch = torch.empty(lib.vp3d_semi_loss_scratch_bytes(), dtype=torch.uint8, device=dev)
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
             _capi.check(lib.vp3d_semi_loss_fwd_bwd(
-                pos_c.data_ptr(), traj_c.data_ptr(), ptr(tgt3), ptr(cam_c), ptr(tgt2), ptr(par),
+                pos_c.data_ptr(), traj_c.data_ptr(), _ptr(tgt3), _ptr(cam_c), _ptr(tgt2), _ptr(par),
                 n_labeled, n_unl, frames, joints, int(bool(linear)), int(terms), losses.data_ptr(),
-                ptr(dpos), ptr(dtraj), scratch.data_ptr(), scratch.numel(), stream),
+                _ptr(dpos), _ptr(dtraj), scratch.data_ptr(), scratch.numel(), stream),
                 "vp3d_semi_loss_fwd_bwd")
         ctx.grads = (dpos, dtraj)
         ctx.mark_non_differentiable(losses)
