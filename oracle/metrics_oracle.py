@@ -1,4 +1,4 @@
-"""float64 NumPy statement of the evaluation metrics (TEST ORACLE for csrc/eval_metrics.cu).
+"""float64 NumPy statement of the evaluation metrics (TEST ORACLE for the metrics of csrc/pose_loss.cu).
 
 Written from the definitions, not from the reference's code:
   * P1, MPJPE: mean over frames and joints of the Euclidean distance;

@@ -1,4 +1,4 @@
-"""GPU: the evaluation-metric kernel (csrc/eval_metrics.cu, videopose3d_b200.metrics) against the
+"""GPU: the evaluation metrics (csrc/pose_loss.cu, videopose3d_b200.metrics) against the
 reference's values stored in tests/golden/metrics, against the float64 oracle on a large random
 input, bit for bit against the torch flip-average expression of run.py:677-680, run to run, and
 end to end: `metrics.evaluate()` against run.py's evaluate() loop, and run.py itself with the

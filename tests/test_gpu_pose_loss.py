@@ -1,6 +1,6 @@
 """GPU: the differentiable pose losses (`vp3d_pose_loss_fwd_bwd`, csrc/pose_loss.cu) against the
 reference's values and the float64 oracles: every golden term by term and combined (values within
-1e-6 relative, gradients within 1e-5 of max |g|), the forward against the float64 evaluation
+1e-6 relative, gradients within 1e-5 of max |g|), the forward equal to the float64 evaluation
 metrics rounded to fp32, reproducible bits, the degenerate-rotation rule, NaN where the reference
 gives NaN, retain_graph, non-contiguous inputs, three training steps of a TemporalModel against a
 torch-expression loss, and a velocity prior on the 2-D input of a frozen model."""
@@ -82,6 +82,10 @@ def test_each_term_matches_golden(cuda_device, name, k):
 @pytest.mark.parametrize("name", [n for n in NAMES if n.startswith("seq_") or n.startswith("mirrored")
                                   or n.startswith("batch_n4")])
 def test_forward_equals_float64_metrics_rounded(cuda_device, name):
+    # The loss and the metrics are two instances of one kernel with the same per-pose code, so the
+    # fp32 loss term is the fp64 metric rounded once, bit for bit, when both launches use the same
+    # grid.  That holds here: every case has at most 972 poses, i.e. at most 122 blocks of 8 poses,
+    # below both grid caps on a 132-SM H100 (one loss block or two metric blocks per SM).
     _, case = load_case(name)
     p = torch.from_numpy(case["pred"]).to(cuda_device)
     t = torch.from_numpy(case["target"]).to(cuda_device)
@@ -96,7 +100,7 @@ def test_forward_equals_float64_metrics_rounded(cuda_device, name):
         if np.isnan(ref32):
             assert np.isnan(float(ours))
             continue
-        assert abs(np.float32(float(ours)) - ref32) <= np.spacing(ref32), (float(ours), float(ref))
+        assert np.float32(float(ours)) == ref32, (float(ours), float(ref))
 
 
 def test_two_runs_give_identical_bits(cuda_device):

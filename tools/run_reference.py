@@ -11,7 +11,7 @@ symbols `run.py` picks up with `from common.model import *` (run.py:21), `from c
 No file of the reference is modified.
   model   TemporalModel, TemporalModelOptimized1f -> videopose3d_b200 (CUDA only)
   loss    mpjpe, weighted_mpjpe                   -> fused kernels
-  metrics n_mpjpe, p_mpjpe, mean_velocity_error   -> the evaluation kernel (csrc/eval_metrics.cu).
+  metrics n_mpjpe, p_mpjpe, mean_velocity_error   -> the metrics instance of csrc/pose_loss.cu.
           run.py hands p_mpjpe / mean_velocity_error NumPy arrays (run.py:697-704): the shims
           upload them (a few hundred kB per sequence), run the kernel and return a float, in place
           of the per-frame LAPACK SVDs

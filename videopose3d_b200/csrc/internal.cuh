@@ -74,7 +74,7 @@ inline const float* conv_weight(const vp3d_weights* w, int src) {
 // One coordinate of the test-time flip average (run.py:677-680): p0 from the plain copy, p1 from the
 // mirrored copy (its joints already swapped back), axis 0 negated back.  Rounded as torch rounds
 // `torch.mean(stack(p0, mirror(p1)), dim=0)`: one fp32 add, then the exact * 0.5.  The one
-// definition of run.py's averaging, shared by eval_metrics.cu and stream.cu.
+// definition of run.py's averaging, shared by the metrics of pose_loss.cu and stream.cu.
 __device__ __forceinline__ float flip_average(float p0, float p1, int axis) {
   return __fmul_rn(__fadd_rn(p0, axis == 0 ? -p1 : p1), 0.5f);
 }

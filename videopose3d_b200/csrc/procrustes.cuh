@@ -1,9 +1,9 @@
-// Per-pose similarity Procrustes (common/loss.py:34-66) in Horn's quaternion form, fp64, shared by
-// eval_metrics.cu (the P-MPJPE metric) and pose_loss.cu (P-MPJPE as a differentiable loss).
+// Per-pose similarity Procrustes (common/loss.py:34-66) in Horn's quaternion form, fp64, for
+// pose_loss.cu's P-MPJPE (the metric and the differentiable loss).
 // H = X0^T Y0 of the centred, normalised target X0 and prediction Y0.  The symmetric 4x4 N(H)
 // (Horn 1987) has as its largest eigenvalue the reference's optimal trace s1 + s2 + sign(det H) s3
 // of the SVD, and as its eigenvector the unit quaternion of the rotation.  The eigen-decomposition
-// is cyclic Jacobi; all four eigenpairs come out of the sweeps (pose_loss.cu's backward needs them).
+// is cyclic Jacobi; all four eigenpairs come out of the sweeps (the loss's backward needs them).
 #pragma once
 
 namespace vp3d {
@@ -68,26 +68,6 @@ __device__ __forceinline__ void quat_rotation(double w, double x, double y, doub
   Q[0][0] = w * w + x * x - y * y - z * z; Q[0][1] = 2.0 * (x * y - w * z); Q[0][2] = 2.0 * (x * z + w * y);
   Q[1][0] = 2.0 * (x * y + w * z); Q[1][1] = w * w - x * x + y * y - z * z; Q[1][2] = 2.0 * (y * z - w * x);
   Q[2][0] = 2.0 * (x * z - w * y); Q[2][1] = 2.0 * (y * z + w * x); Q[2][2] = w * w - x * x - y * y + z * z;
-}
-
-// Rotation (row-major, applied as Q y to column vectors) and optimal trace for the normalised,
-// centred H = X0^T Y0.  The reference aligns `predicted @ R`, i.e. R = Q^T.
-__device__ void procrustes(const double (&H)[3][3], double (&Q)[3][3], double* trace) {
-  double A[4][4], V[4][4];
-  horn_eigen(H, A, V);
-  int k = 0;
-  double lam = A[0][0];
-  if (A[1][1] > lam) { lam = A[1][1]; k = 1; }
-  if (A[2][2] > lam) { lam = A[2][2]; k = 2; }
-  if (A[3][3] > lam) { lam = A[3][3]; k = 3; }
-  double w = V[0][0], x = V[1][0], y = V[2][0], z = V[3][0];
-  if (k == 1) { w = V[0][1]; x = V[1][1]; y = V[2][1]; z = V[3][1]; }
-  if (k == 2) { w = V[0][2]; x = V[1][2]; y = V[2][2]; z = V[3][2]; }
-  if (k == 3) { w = V[0][3]; x = V[1][3]; y = V[2][3]; z = V[3][3]; }
-  const double n = rsqrt(w * w + x * x + y * y + z * z);
-  w *= n; x *= n; y *= n; z *= n;
-  quat_rotation(w, x, y, z, Q);
-  *trace = lam;
 }
 
 }  // namespace

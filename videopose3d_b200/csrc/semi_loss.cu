@@ -14,6 +14,7 @@
 #include <cooperative_groups.h>
 
 #include "internal.cuh"
+#include "camera.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -112,51 +113,22 @@ __global__ void __launch_bounds__(kThreads) semi_loss_kernel(const SemiArgs a) {
   for (long long v = first; v < unl_units; v += stride) {
     const long long u = lab_units + v;
     const float* p = a.pos + u * J * 3;
-    const bool have_cam = a.cam != nullptr && a.target_2d != nullptr;
-    const float* cp = have_cam ? a.cam + (v / F) * 9 : nullptr;
-    const float fx = have_cam ? cp[0] : 0.0f, fy = have_cam ? cp[1] : 0.0f;
-    const float cx = have_cam ? cp[2] : 0.0f, cy = have_cam ? cp[3] : 0.0f;
-    const float k0 = have_cam ? cp[4] : 0.0f, k1 = have_cam ? cp[5] : 0.0f, k2 = have_cam ? cp[6] : 0.0f;
-    const float p0 = have_cam ? cp[7] : 0.0f, p1 = have_cam ? cp[8] : 0.0f;
+    const bool have_cam = a.cam != nullptr && a.target_2d != nullptr;   // else intrinsics and target read as 0
+    const Camera c = have_cam ? load_camera(a.cam + (v / F) * 9) : Camera{};
     const float tx = a.traj[u * 3], ty = a.traj[u * 3 + 1], tz = a.traj[u * 3 + 2];
     float gtx = 0.0f, gty = 0.0f, gtz = 0.0f;
     for (int j = 0; j < J; ++j) {
       const float px = p[j * 3], py = p[j * 3 + 1], pz = p[j * 3 + 2];
-      const float x = px + tx, y = py + ty, z = pz + tz;
-      const float uu = x / z, vv = y / z;
-      const float xx = fminf(fmaxf(uu, -1.0f), 1.0f), yy = fminf(fmaxf(vv, -1.0f), 1.0f);
-      float ox, oy, s = 1.0f, rp = 0.0f;
-      if (a.linear) {
-        ox = xx; oy = yy;
-      } else {
-        const float r2 = xx * xx + yy * yy;
-        const float radial = 1.0f + r2 * (k0 + r2 * (k1 + r2 * k2));
-        rp = k0 + r2 * (2.0f * k1 + 3.0f * k2 * r2);
-        s = radial + (p0 * xx + p1 * yy);
-        ox = xx * s + p0 * r2;
-        oy = yy * s + p1 * r2;
-      }
+      const Projection P = project(c, px + tx, py + ty, pz + tz, a.linear);
       const float* tg = have_cam ? a.target_2d + (v * J + j) * 2 : nullptr;
-      const float ex = have_cam ? fx * ox + cx - tg[0] : 0.0f, ey = have_cam ? fy * oy + cy - tg[1] : 0.0f;
+      const float ex = have_cam ? P.x - tg[0] : 0.0f, ey = have_cam ? P.y - tg[1] : 0.0f;
       const float d = sqrtf(ex * ex + ey * ey);
       acc_rec += d;
       if (grads) {
-        const float inv = d > 0.0f ? w_rec_g / d : 0.0f;
-        const float ga = fx * ex * inv, gb = fy * ey * inv;
-        float gxx, gyy;
-        if (a.linear) {
-          gxx = ga; gyy = gb;
-        } else {
-          const float sx = rp * 2.0f * xx + p0, sy = rp * 2.0f * yy + p1;
-          gxx = ga * (s + xx * sx + p0 * 2.0f * xx) + gb * (yy * sx + p1 * 2.0f * xx);
-          gyy = ga * (xx * sy + p0 * 2.0f * yy) + gb * (s + yy * sy + p1 * 2.0f * yy);
-        }
-        const float gu = (uu >= -1.0f && uu <= 1.0f) ? gxx : 0.0f;
-        const float gv = (vv >= -1.0f && vv <= 1.0f) ? gyy : 0.0f;
-        const float gx = gu / z, gy = gv / z, gz = -(gu * uu + gv * vv) / z;
+        const float3 gp = project_backward(c, P, ex, ey, d > 0.0f ? w_rec_g / d : 0.0f, a.linear);
         float* g = a.dpos + (u * J + j) * 3;
-        g[0] = gx; g[1] = gy; g[2] = gz;
-        gtx += gx; gty += gy; gtz += gz;
+        g[0] = gp.x; g[1] = gp.y; g[2] = gp.z;
+        gtx += gp.x; gty += gp.y; gtz += gp.z;
       }
       if (j > 0 && a.use_bone) {
         const int pa = a.parents[j];

@@ -9,6 +9,7 @@
 //    gradient w.r.t. the prediction in one launch.  The loss is summed in block order (no
 //    floating-point atomics): the same input gives the same bits.
 #include "internal.cuh"
+#include "camera.cuh"
 
 namespace vp3d {
 namespace {
@@ -246,8 +247,7 @@ mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ target,
 // ---- re-projection loss (semi-supervised branch) -------------------------------------------------
 
 // One thread per frame (n, t): for each joint X = pos + traj, project with the camera of sample n
-// (camera.py:37-67: perspective divide clamped to [-1, 1], radial k1..k3 and tangential p1, p2
-// distortion, focal length, principal point; or only the linear part, :69-88), accumulate the 2-D
+// (camera.cuh: camera.py:37-88, distortion-aware or linear), accumulate the 2-D
 // distance to the target, and write d loss / d pos per joint and d loss / d traj per frame (the
 // joint sum -- no atomics needed since the frame's joints live in one thread).  Frames are
 // grid-strided; the loss is summed as in mpjpe_kernel.
@@ -262,54 +262,24 @@ projected_mpjpe_kernel(const float* __restrict__ pos, const float* __restrict__ 
   float acc = 0.0f;
   for (long long fr = (long long)blockIdx.x * kLossThreads + threadIdx.x; fr < frames_total;
        fr += (long long)gridDim.x * kLossThreads) {
-    const float* cp = cam + (fr / frames_per_sample) * 9;
-    const float fx = cp[0], fy = cp[1], cx = cp[2], cy = cp[3];
-    const float k0 = cp[4], k1 = cp[5], k2 = cp[6], p0 = cp[7], p1 = cp[8];
+    const Camera c = load_camera(cam + (fr / frames_per_sample) * 9);
     const float tx = traj[fr * 3 + 0], ty = traj[fr * 3 + 1], tz = traj[fr * 3 + 2];
     float gtx = 0.0f, gty = 0.0f, gtz = 0.0f;
     for (int j = 0; j < joints; ++j) {
       const long long e = fr * joints + j;
-      const float x = pos[e * 3 + 0] + tx, y = pos[e * 3 + 1] + ty, z = pos[e * 3 + 2] + tz;
-      const float u = x / z, v = y / z;
-      const float xx = fminf(fmaxf(u, -1.0f), 1.0f), yy = fminf(fmaxf(v, -1.0f), 1.0f);
-      float ox, oy;           // projected point before focal length / principal point
-      float s = 1.0f, rp = 0.0f, r2 = 0.0f;
-      if (linear) {
-        ox = xx;
-        oy = yy;
-      } else {
-        r2 = xx * xx + yy * yy;
-        const float radial = 1.0f + r2 * (k0 + r2 * (k1 + r2 * k2));
-        rp = k0 + r2 * (2.0f * k1 + 3.0f * k2 * r2);  // d radial / d r2
-        s = radial + (p0 * xx + p1 * yy);
-        ox = xx * s + p0 * r2;
-        oy = yy * s + p1 * r2;
-      }
-      const float ex = fx * ox + cx - target[e * 2 + 0];
-      const float ey = fy * oy + cy - target[e * 2 + 1];
+      const Projection P = project(c, pos[e * 3 + 0] + tx, pos[e * 3 + 1] + ty, pos[e * 3 + 2] + tz, linear);
+      const float ex = P.x - target[e * 2 + 0];
+      const float ey = P.y - target[e * 2 + 1];
       const float d = sqrtf(ex * ex + ey * ey);
       acc += d;
       if (dpos != nullptr) {
-        const float inv = d > 0.0f ? weight / d : 0.0f;
-        const float a = fx * ex * inv, b = fy * ey * inv;  // d loss / d (ox, oy)
-        float gxx, gyy;
-        if (linear) {
-          gxx = a;
-          gyy = b;
-        } else {
-          const float sx = rp * 2.0f * xx + p0, sy = rp * 2.0f * yy + p1;  // d s / d (xx, yy)
-          gxx = a * (s + xx * sx + p0 * 2.0f * xx) + b * (yy * sx + p1 * 2.0f * xx);
-          gyy = a * (xx * sy + p0 * 2.0f * yy) + b * (s + yy * sy + p1 * 2.0f * yy);
-        }
-        const float gu = (u >= -1.0f && u <= 1.0f) ? gxx : 0.0f;  // clamp passes gradient inside
-        const float gv = (v >= -1.0f && v <= 1.0f) ? gyy : 0.0f;
-        const float gx = gu / z, gy = gv / z, gz = -(gu * u + gv * v) / z;
-        dpos[e * 3 + 0] = gx;
-        dpos[e * 3 + 1] = gy;
-        dpos[e * 3 + 2] = gz;
-        gtx += gx;
-        gty += gy;
-        gtz += gz;
+        const float3 g = project_backward(c, P, ex, ey, d > 0.0f ? weight / d : 0.0f, linear);
+        dpos[e * 3 + 0] = g.x;
+        dpos[e * 3 + 1] = g.y;
+        dpos[e * 3 + 2] = g.z;
+        gtx += g.x;
+        gty += g.y;
+        gtz += g.z;
       }
     }
     if (dtraj != nullptr) {

@@ -3,7 +3,7 @@
 The reference computes its four evaluation protocols per test sequence with an `.item()` sync for
 each torch metric, a copy of prediction and target to the host, and NumPy for Protocol #2 (batched
 3x3 SVD per frame) and the velocity error.  Here one launch (`vp3d_pose_errors`,
-csrc/eval_metrics.cu) flip-averages the test-time-augmented prediction and produces all four
+csrc/pose_loss.cu) flip-averages the test-time-augmented prediction and produces all four
 per-sequence means in float64; `evaluate()` keeps the frame-weighted sums on the device and syncs
 once at the end.
 
