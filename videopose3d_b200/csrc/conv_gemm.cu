@@ -12,6 +12,9 @@
 //                   (coalesced 128-byte rows, clipped at the tensor edge by the map)
 // The operand pipeline keeps running across tiles: the producer fills the stages of the next tile
 // while the consumers are in the epilogue of the current one.
+// Lean inference launches with more tiles than CTAs use the ping-pong instances instead: each
+// consumer warpgroup computes all 128 rows of every other tile, so that one warpgroup's epilogue
+// runs under the other's MMAs.
 #include "conv_gemm.cuh"
 
 #include <stdlib.h>
@@ -24,23 +27,29 @@ namespace vp3d {
 // OUT2: two output planes (hi, lo) -> two staging planes per buffer.
 // LEAN (inference layers: affine + ReLU [+ one-plane TMA residual] -> one 16-bit plane): the same
 // epilogue with every option resolved at compile time.
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN>
+// PP (lean only): ping-pong schedule, each consumer warpgroup computes whole tiles (see the kernel).
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool PP = false>
 struct GemmCfg {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma tiles are 64 or 128 columns wide");
   static_assert(!(LEAN && (OUT2 || TRAIN)), "the lean epilogue is inference-only, one plane");
+  static_assert(LEAN || !PP, "only the lean instances run the ping-pong schedule");
   static constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
   static constexpr uint32_t kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kTileBytes = kBlockM * 64 * 2;   // one 128 x 64 16-bit tile (16 KiB)
   static constexpr uint32_t kHalfBytes = 64 * 64 * 2;        // one warpgroup's 64 x 64 slice
-  // staging: 2 warpgroups x 2 alternating buffers x (hi[, lo])
-  static constexpr uint32_t kStagingBytes = 2 * 2 * (OUT2 ? 2 : 1) * kHalfBytes;
+  // staging: 2 warpgroups x 2 alternating buffers x (hi[, lo]).  Ping-pong: one 128 x 64 tile per
+  // warpgroup; the residual instance stores in place from the residual's landing tile instead.
+  static constexpr uint32_t kStagingBytes =
+      PP ? (RES ? 0 : 2 * kTileBytes) : 2 * 2 * (OUT2 ? 2 : 1) * kHalfBytes;
   // auxiliary (residual / Z) landing tiles: four, so that two-tile store blocks (hi+lo residual,
-  // or residual + Z) still get two stages in flight
+  // or residual + Z) still get two stages in flight.  Ping-pong: two per warpgroup.
   static constexpr int kResSlots = RES ? 4 : 0;
   static constexpr uint32_t kFixedBytes = kStagingBytes + kResSlots * kTileBytes;
-  // per-channel affine (scale, shift) of the current N block: 2 x BLOCK_N floats
-  static constexpr uint32_t kAffineBytes = 2 * BLOCK_N * 4;
+  // per-channel affine (scale, shift) of the current N block: 2 x BLOCK_N floats.  Ping-pong reads
+  // it through L1 instead: the two warpgroups may hold different N blocks, and a copy per
+  // warpgroup would cost the 128-wide instance an operand stage.
+  static constexpr uint32_t kAffineBytes = PP ? 0 : 2 * BLOCK_N * 4;
   // training: per-column (sum, sumsq) of one warp of every 32-row slab pair, 4 slabs x 2 x 64
   static constexpr uint32_t kPairBytes = TRAIN ? 4 * 2 * 64 * 4 : 0;
   static constexpr uint32_t kBarBytesMax = (2 * 8 + 8 + 1) * 8 + 32;
@@ -164,7 +173,9 @@ __device__ __forceinline__ void tl_stamp(const ConvGemmArgs& p, int ev) {
 // value, fused BatchNorm-backward reductions); eval launches use the leaner TRAIN = false build.
 // F16 (LEAN only): the operand / storage format at compile time (fp16, else bf16), so that each
 // k-block is one branch-free group of wgmma; the other instances read it from p.f16.
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false>
+// PP (LEAN only): the ping-pong schedule for launches where CTAs get more than one tile (see the
+// consumer branches below); the cooperative schedule otherwise.
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false, bool PP = false>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_w,
@@ -172,7 +183,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_res,
                  const __grid_constant__ CUtensorMap tmap_z, const ConvGemmArgs p) {
   static_assert(LEAN || !F16, "only the lean instances fix the operand format at compile time");
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN>;
+  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBlocksPerTile = BLOCK_N / 64;
   constexpr int kFrag = BLOCK_N / 2;   // accumulator floats per consumer thread
@@ -221,11 +232,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar + s * 8, 1);
-      mbar_init(empty_bar + s * 8, 8);   // lane 0 of each of the 8 consumer warps
+      // lane 0 of each consumer warp that reads the stage: all 8, or the 4 of one ping-pong warpgroup
+      mbar_init(empty_bar + s * 8, PP ? 4 : 8);
     }
     for (int s = 0; s < 4; ++s) {
       mbar_init(rfull_bar + s * 8, 1);
-      mbar_init(rempty_bar + s * 8, 256);   // every consumer thread reads its rows of the stage
+      // every consumer thread reads its rows of the stage; ping-pong: the thread that issued the
+      // stores from the tile, once they have read it
+      mbar_init(rempty_bar + s * 8, PP ? 1 : 256);
     }
     mbar_init(dep_bar, 1);
     fence_mbar_init();
@@ -311,7 +325,27 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     }
   } else if (warp == 1) {
     // ------------------------------------------------------------ auxiliary-tile producer
-    if (RES && lane == 0) {
+    if (PP && RES && lane == 0) {
+      // ping-pong: the residual tiles in tile order; tile j goes to warpgroup j & 1, whose two
+      // landing slots (2 g, 2 g + 1) form a ring of their own
+      uint32_t filled[2] = {0u, 0u};   // residual tiles sent to warpgroup 0 / 1 so far
+      for (int j = 0, w = blockIdx.x; w < total_tiles; ++j, w += gridDim.x) {
+        int n_blk, sample, row0;
+        tile_coords(p, w, n_blk, sample, row0);
+        const int g = j & 1;
+        for (int sb = 0; sb < kBlocksPerTile; ++sb) {
+          const uint32_t n = g ? filled[1] : filled[0];
+          const uint32_t slot = 2u * g + (n & 1u);
+          mbar_wait(rempty_bar + slot * 8, ((n >> 1) & 1u) ^ 1u);
+          mbar_expect_tx(rfull_bar + slot * 8, Cfg::kTileBytes);
+          tma_load_4d(&tmap_res, rfull_bar + slot * 8, smem_res + slot * Cfg::kTileBytes,
+                      n_blk * BLOCK_N + sb * 64 + p.res_tma_col_off, row0 + p.res_tma_row_off,
+                      sample, 0);
+          if (g) ++filled[1];
+          else ++filled[0];
+        }
+      }
+    } else if (!PP && RES && lane == 0) {
       uint32_t rs = 0, rphase = 0;
       for (int w = blockIdx.x; w < total_tiles; w += gridDim.x) {
         int n_blk, sample, row0;
@@ -335,7 +369,134 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         }
       }
     }
-  } else if (warp >= 4) {
+  } else if (PP && warp >= 4) {
+    // ------------------------------------------------------------ ping-pong MMA + lean epilogue
+    // Warpgroup g computes all 128 rows of the CTA's tiles j = g, g + 2, ... (w = blockIdx.x +
+    // j gridDim.x): per k16 step one m64 wgmma per 64-row half of the A stage, into acc[0] and
+    // acc[1].  The warpgroups issue their k-loops in tile order, taking turns through two named
+    // barriers (8 + g: "warpgroup g may issue"), so that one warpgroup's epilogue runs under the
+    // other's MMAs.  Because the k-loops are ordered, every earlier fill of a stage has been
+    // consumed before a warpgroup waits on it, and the parity wait is exact.
+    const int wg = (warp - 4) >> 2;
+    const int wq = warp & 3;
+    const int tid = (int)threadIdx.x - 128 - 128 * wg;
+    const int rl0 = 16 * wq + (lane >> 2);   // this thread's rows in each 64-row half: rl0, rl0 + 8
+    const int cq = 2 * (lane & 3);
+    const uint32_t bar_wg = 2u + (uint32_t)wg;
+    const uint32_t bar_mine = 8u + (uint32_t)wg, bar_other = 9u - (uint32_t)wg;
+    const uint32_t staging = smem_store + wg * Cfg::kTileBytes;   // (no-residual instance)
+    uint32_t res_seen = 0;            // residual tiles this warpgroup has received
+    float acc[2][kFrag];
+#pragma unroll
+    for (int i = 0; i < kFrag; ++i) acc[0][i] = acc[1][i] = 0.0f;
+
+    for (int j = wg, w = blockIdx.x + wg * gridDim.x; w < total_tiles; j += 2, w += 2 * gridDim.x) {
+      int n_blk, sample, row0;
+      tile_coords(p, w, n_blk, sample, row0);
+
+      // ---- main loop: k-block it of tile j sits in the producer's (j k_iters + it)-th fill
+      const uint32_t fill = (uint32_t)j * (uint32_t)k_iters;
+      uint32_t stage = fill % kStages, phase = (fill / kStages) & 1u;
+      if (j > 0) named_bar_sync(bar_mine, 256);   // tile j - 1's k-loop has been issued
+      uint32_t prev_stage = 0;
+      for (int it = 0; it < k_iters; ++it) {
+        mbar_wait(full_bar + stage * 8, phase);
+#ifdef VP3D_TIMELINE
+        if (warp == 4 && lane == 0 && w == (int)blockIdx.x && it == 0) TL(4);
+#endif
+        const uint32_t a_st = smem_a + stage * Cfg::kABytes;
+        const uint64_t da0 = make_gmma_desc_sw128(a_st, 16, 1024);
+        const uint64_t da1 = make_gmma_desc_sw128(a_st + 64 * 128, 16, 1024);   // rows 64..127
+        const uint64_t db = make_gmma_desc_sw128(smem_b + stage * Cfg::kBBytes, 16, 1024);
+        wgmma_fence_operands(acc[0]);
+        wgmma_fence_operands(acc[1]);
+        wgmma_fence();
+        wgmma_kblock<BLOCK_N, F16>(acc[0], da0, db, it == 0);
+        wgmma_kblock<BLOCK_N, F16>(acc[1], da1, db, it == 0);
+        wgmma_commit();
+        wgmma_fence_operands(acc[0]);
+        wgmma_fence_operands(acc[1]);
+        if (it > 0) {
+          wgmma_wait<1>();
+          wgmma_fence_operands(acc[0]);
+          wgmma_fence_operands(acc[1]);
+          if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+        }
+        prev_stage = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      if (w + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);   // tile j + 1 may issue
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc[0]);
+      wgmma_fence_operands(acc[1]);
+      if (k_iters > 0 && lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+#ifdef VP3D_TIMELINE
+      if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(7); TL(8); }
+#endif
+
+      const float* scale = p.scale + n_blk * BLOCK_N;
+      const float* shift = p.shift + n_blk * BLOCK_N;
+#pragma unroll
+      for (int sb = 0; sb < kBlocksPerTile; ++sb) {
+        const int cb = n_blk * BLOCK_N + sb * 64;   // first column of the store block
+        uint32_t tile_smem;
+        if constexpr (RES) {
+          // in place: every thread overwrites the residual elements it adds with its results
+          const uint32_t slot = 2u * wg + (res_seen & 1u);
+          mbar_wait(rfull_bar + slot * 8, (res_seen >> 1) & 1u);
+          ++res_seen;
+          tile_smem = smem_res + slot * Cfg::kTileBytes;
+        } else {
+          // the staging tile must have been read out by the bulk stores issued from it last
+          if (tid == 0) tma_store_wait_read<0>();
+          named_bar_sync(bar_wg, 128);
+          tile_smem = staging;
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j4 = 4 * (sb * 8 + jj);
+          const int cl = sb * 64 + jj * 8 + cq;   // column inside the N block
+          const float2 sc = __ldg(reinterpret_cast<const float2*>(scale + cl));
+          const float2 sh = __ldg(reinterpret_cast<const float2*>(shift + cl));
+#pragma unroll
+          for (int h2 = 0; h2 < 2; ++h2) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = fmaxf(fmaf(acc[h2][j4 + 2 * h], sc.x, sh.x), 0.0f);
+              float v1 = fmaxf(fmaf(acc[h2][j4 + 2 * h + 1], sc.y, sh.y), 0.0f);
+              const uint32_t off = sw128_off(64 * h2 + rl0 + 8 * h, jj * 8 + cq);
+              if (RES) add_pair(v0, v1, ld_shared_u32(tile_smem + off), F16);
+              st_shared_u32(tile_smem + off, F16 ? pack_f16x2(v0, v1) : pack_bf16x2(v0, v1));
+            }
+          }
+        }
+        fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA engine
+        named_bar_sync(bar_wg, 128);
+        if (tid == 0) {
+          // four 32-row boxes: 4 KiB-aligned quarters of the tile, same swizzle phase as written
+#pragma unroll
+          for (int hb = 0; hb < 4; ++hb)
+            tma_store_4d(&tmap_out, tile_smem + hb * 4096u, cb, row0 + 32 * hb, sample, 0);
+          tma_store_commit();
+        }
+      }
+      if (RES && tid == 0) {
+        // the landing tiles go back to the auxiliary producer once the stores have read them
+        tma_store_wait_read<0>();
+#pragma unroll
+        for (int sb = 0; sb < kBlocksPerTile; ++sb)
+          mbar_arrive(rempty_bar + (2u * wg + ((res_seen - kBlocksPerTile + sb) & 1u)) * 8);
+      }
+#ifdef VP3D_TIMELINE
+      if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(9); TL(10); }
+#endif
+    }
+    // the staging tiles must outlive every bulk store that reads them
+    if (tid == 0) tma_store_wait_all<0>();
+#ifdef VP3D_TIMELINE
+    if (warp == 4 && lane == 0) TL(11);
+#endif
+  } else if (!PP && warp >= 4) {
     // ------------------------------------------------------------ MMA + epilogue (two warpgroups)
     const int wg = (warp - 4) >> 2;   // rows [64 wg, 64 wg + 64) of the tile
     const int wq = warp & 3;          // warp inside the warpgroup: 16 rows each
@@ -628,13 +789,19 @@ static bool pdl_enabled() {
 void conv_gemm_set_pdl(int on) { g_pdl = on ? 1 : 0; }
 bool conv_gemm_pdl_enabled() { return pdl_enabled(); }
 
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false, bool F16 = false>
+static int conv_tiles(const ConvGemmArgs& a) {
+  const int m_tiles = a.dilated ? a.samples * a.tiles_per_sample : a.tiles_per_sample;
+  return m_tiles * a.n_tiles;
+}
+
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false, bool F16 = false,
+          bool PP = false>
 static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                                const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                                const CUtensorMap& tmap_z, const ConvGemmArgs& args, int num_sms,
                                cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN>;
-  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16>;
+  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP>;
+  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16, PP>;
   // the dynamic shared memory opt-in is a per-device attribute
   static bool attr_set[kMaxDevices] = {};
   int dev = 0;
@@ -646,8 +813,7 @@ static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tma
     if (e != cudaSuccess) return e;
     attr_set[dev] = true;
   }
-  const int m_tiles = args.dilated ? args.samples * args.tiles_per_sample : args.tiles_per_sample;
-  const int total = m_tiles * args.n_tiles;
+  const int total = conv_tiles(args);
   if (total <= 0) return cudaSuccess;
   const int workers = total < num_sms ? total : num_sms;
   cudaLaunchConfig_t cfg;
@@ -692,9 +858,15 @@ static cudaError_t launch_train(const CUtensorMap& a, const CUtensorMap& w, cons
   if ((args.flags & kEpiStats) || args.bnb)
     return launch_impl<BLOCK_N, RES, OUT2, true>(a, w, o, r, z, args, num_sms, stream);
   if constexpr (!OUT2) {
-    if (lean_ok(args, RES))
+    if (lean_ok(args, RES)) {
+      // Ping-pong pays only where a CTA gets a second tile whose MMAs can run under the first
+      // tile's epilogue; with one tile per CTA both warpgroups share it (cooperative).
+      if (conv_tiles(args) > num_sms)
+        return args.f16 ? launch_impl<BLOCK_N, RES, false, false, true, true, true>(a, w, o, r, z, args, num_sms, stream)
+                        : launch_impl<BLOCK_N, RES, false, false, true, false, true>(a, w, o, r, z, args, num_sms, stream);
       return args.f16 ? launch_impl<BLOCK_N, RES, false, false, true, true>(a, w, o, r, z, args, num_sms, stream)
                       : launch_impl<BLOCK_N, RES, false, false, true, false>(a, w, o, r, z, args, num_sms, stream);
+    }
   }
   return launch_impl<BLOCK_N, RES, OUT2, false>(a, w, o, r, z, args, num_sms, stream);
 }

@@ -105,6 +105,10 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// arrive on a named barrier without waiting for it (the other side waits with named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format"): bits [0,14)
