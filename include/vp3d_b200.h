@@ -46,11 +46,18 @@ typedef enum {
   VP3D_PRECISION_MIXED = 2,  /* bf16 residual blocks, split-bf16 expand and shrink (and blocks below
                                 0.5% of the FLOPs), residual stream kept in hi+lo planes; ~1e-3 of
                                 fp32 (<= 2e-3) close to bf16 cost */
-  VP3D_PRECISION_FP16 = 3    /* eval default: IEEE fp16 operands and activations (11-bit significand,
+  VP3D_PRECISION_FP16 = 3,   /* eval default: IEEE fp16 operands and activations (11-bit significand,
                                 single plane), fp32 accumulate -- the tensor rate of bf16 at 1/8 of
                                 its rounding error: ~4e-4 of fp32 on cfg2, inside north_star's 1e-3.
                                 Stores saturate at +-65504.  Inference only (training runs bf16 /
                                 bf16x3: gradients need the bf16 exponent range) */
+  VP3D_PRECISION_INT8 = 4    /* eval only: the two convs of every residual block multiply u8
+                                activations by s8 weights into exact int32 sums (one activation scale
+                                s = amax / 255 per quantised tensor from vp3d_calibrate_int8, weight
+                                scale max|W| / 127 per output channel, folded into the BatchNorm
+                                affine); expand, shrink and the residual stream are fp16 as in FP16.
+                                Needs vp3d_set_int8_scales before its vp3d_set_weights.  Not for
+                                streaming or training.  Op level: u8 A, s8 W, k_per_tap % 128 == 0 */
 } vp3d_precision;
 
 /* Constructor arguments of TemporalModel / TemporalModelOptimized1f (model.py:85-86, :151-152). */
@@ -128,6 +135,27 @@ size_t vp3d_workspace_bytes(const vp3d_plan* plan, int N, int T);
  * Asynchronous on `stream`. */
 int vp3d_forward_eval(vp3d_plan* plan, const float* x, float* y, int N, int T, void* workspace,
                       size_t workspace_bytes, void* stream);
+
+/* Activation calibration of the int8 eval mode: runs the fp16 eval chain of `fp16_plan` (a
+ * VP3D_PRECISION_FP16 plan with its weights set; no shrink) on x (N, T, J_in, F), and after each GEMM
+ * whose output an int8 plan quantises reads the stored fp16 plane and folds its maximum into
+ * amax[2B] (device fp32, B residual blocks): amax[2(i-1)] = max X_{i-1} (the input of block i's
+ * first conv; X_0 is the expand output), amax[2(i-1)+1] = max H_i (the input of its 1x1 conv).  The
+ * fold is an integer atomicMax on the fp32 bits (every value is >= 0): order-independent and
+ * reproducible.  Calls accumulate (zero amax before the first batch). */
+int vp3d_calibrate_int8(vp3d_plan* fp16_plan, const float* x, int N, int T, void* workspace,
+                        size_t workspace_bytes, float* amax, void* stream);
+/* Stores the activation scales of an int8 plan from n = 2B HOST amax values (as above): s = amax /
+ * 255 in fp32 (1 when amax is 0), 1 / s in fp32.  The next vp3d_set_weights that leaves both the
+ * conv and the BatchNorm packs current folds them into the int8 affine; until then vp3d_forward_eval
+ * returns VP3D_ERR_STATE. */
+int vp3d_set_int8_scales(vp3d_plan* int8_plan, const float* amax_host, int n);
+/* Copies the int8 packs of layers_conv[layer] of an int8 plan (as its last vp3d_set_weights left
+ * them) to DEVICE buffers, each may be NULL: w_s8 [taps][n_pad][k_pad] s8 with n_pad = channels
+ * rounded up to 64 and k_pad = n_pad rounded up to 128; w_scale and q_scale [n_pad] fp32 (q_scale
+ * as last folded; VP3D_ERR_STATE before the first fold).  For checking the packs. */
+int vp3d_int8_packs(const vp3d_plan* int8_plan, int layer, void* w_s8, float* w_scale,
+                    float* q_scale, void* stream);
 
 /* Same computation with HOST buffers (the call run.py makes: numpy batch -> .cuda() -> model ->
  * .cpu(), run.py:663-672): copies x host->device, runs the forward, copies y device->host and
@@ -317,6 +345,12 @@ typedef struct {
   /* elements between the A planes; 0 = samples * a_rows * a_ld (A is exactly its planes).  Set when
    * the A rows are a window into a larger buffer, such as a streaming history ring. */
   long long a_plane_stride;
+  /* u8 copy of the output (precision FP16 or INT8, affine + ReLU [+ residual] launches only):
+   * out_u8[row][c] = cvt.rni.sat.u8.f32(v * out_u8_inv_scale) of the fp32 value v that the fp16 store
+   * rounds, rows as in `out`.  With INT8 and no residual `out` must be NULL (u8 only); NULL = off. */
+  void* out_u8;
+  int out_u8_ld;        /* >= n_pad, a multiple of 16 (out_u8 16-byte aligned) */
+  float out_u8_inv_scale;
 } vp3d_conv_desc;
 
 int vp3d_conv_gemm(const vp3d_conv_desc* d, void* stream);

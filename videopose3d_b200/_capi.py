@@ -17,6 +17,7 @@ VP3D_PRECISION_BF16 = 0
 VP3D_PRECISION_BF16X3 = 1
 VP3D_PRECISION_MIXED = 2
 VP3D_PRECISION_FP16 = 3
+VP3D_PRECISION_INT8 = 4
 VP3D_PACK_CONV = 1
 VP3D_PACK_BN_EVAL = 2
 VP3D_PACK_CONV_T = 4
@@ -158,6 +159,9 @@ class ConvDesc(ctypes.Structure):
         ("lo_row_begin", ctypes.c_int),
         ("lo_row_end", ctypes.c_int),
         ("a_plane_stride", ctypes.c_longlong),
+        ("out_u8", ctypes.c_void_p),
+        ("out_u8_ld", ctypes.c_int),
+        ("out_u8_inv_scale", ctypes.c_float),
     ]
 
 
@@ -206,6 +210,13 @@ SIGNATURES = {
     "vp3d_forward_eval": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                          ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_size_t, ctypes.c_void_p]),
+    "vp3d_calibrate_int8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                           ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                           ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_set_int8_scales": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
+                                            ctypes.c_int]),
+    "vp3d_int8_packs": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_forward_eval_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                               ctypes.c_int, ctypes.c_int]),
     "vp3d_forward_eval_host_submit": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p,

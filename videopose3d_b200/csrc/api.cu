@@ -50,17 +50,18 @@ static EncodeTiledFn get_encode_fn() {
 namespace vp3d {
 int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows,
                        uint64_t row_stride, uint64_t samples, uint64_t sample_stride,
-                       uint64_t planes, uint64_t plane_stride, uint32_t box_rows) {
+                       uint64_t planes, uint64_t plane_stride, uint32_t box_rows, int elem_bytes) {
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (row_stride * 2) % 16 || (sample_stride * 2) % 16 ||
-      (plane_stride * 2) % 16)
+  const uint64_t eb = (uint64_t)elem_bytes;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (row_stride * eb) % 16 || (sample_stride * eb) % 16 ||
+      (plane_stride * eb) % 16)
     return fail(VP3D_ERR_INVALID, "tensor map operand not 16-byte aligned");
   cuuint64_t dims[4] = {inner, rows, samples, planes};
-  cuuint64_t strides[3] = {row_stride * 2, sample_stride * 2, plane_stride * 2};
-  cuuint32_t box[4] = {(cuuint32_t)kBlockK, box_rows, 1, 1};
+  cuuint64_t strides[3] = {row_stride * eb, sample_stride * eb, plane_stride * eb};
+  cuuint32_t box[4] = {(cuuint32_t)(elem_bytes == 1 ? kBlockK8 : kBlockK), box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides,
+  CUresult r = enc(m, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -76,14 +77,14 @@ int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows,
 
 // 2-D bf16 map (k, row), box (64, box_rows), 128-byte swizzle.
 int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows,
-                       uint32_t box_rows) {
+                       uint32_t box_rows, int elem_bytes) {
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t dims[2] = {inner, rows};
-  cuuint64_t strides[1] = {inner * 2};
-  cuuint32_t box[2] = {(cuuint32_t)kBlockK, box_rows};
+  cuuint64_t strides[1] = {inner * (uint64_t)elem_bytes};
+  cuuint32_t box[2] = {(cuuint32_t)(elem_bytes == 1 ? kBlockK8 : kBlockK), box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides,
+  CUresult r = enc(m, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -127,9 +128,24 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   if (d->out_rows == 0) return VP3D_OK;
   const int a_planes = d->a_planes > 0 ? d->a_planes : 1;
   const int pairs = d->precision == VP3D_PRECISION_BF16X3 ? 3 : 1;
-  const int f16 = d->precision == VP3D_PRECISION_FP16 ? 1 : 0;
+  const int i8 = d->precision == VP3D_PRECISION_INT8 ? 1 : 0;
+  const int f16 = (d->precision == VP3D_PRECISION_FP16 || i8) ? 1 : 0;   // (int8: fp16 res / out)
   if (f16 && (a_planes != 1 || d->out_planes > 1 || d->stats || d->bnb_z))
     return fail(VP3D_ERR_INVALID, "conv_gemm: fp16 is a single-plane, inference-only format");
+  if (i8 && (d->k_per_tap % kBlockK8 || d->tap_col_step != 0))
+    return fail(VP3D_ERR_INVALID, "conv_gemm: int8 needs k_per_tap %% 128 == 0 and taps that step "
+                "rows (tap_col_step 0)");
+  if (d->out_u8 && (!f16 || d->out_u8_ld % 16 || d->out_u8_ld < d->n_pad ||
+                    reinterpret_cast<uintptr_t>(d->out_u8) % 16))
+    return fail(VP3D_ERR_INVALID, "conv_gemm: a u8 output needs fp16 or int8, a 16-byte aligned "
+                "pointer and out_u8_ld >= n_pad, a multiple of 16");
+  if ((i8 || d->out_u8) &&
+      (!d->scale || !d->shift || !d->relu || d->out_f32 || d->res_col_begin || d->res_cols ||
+       (i8 && d->res && !d->out) || (i8 && !d->res && (d->out || !d->out_u8)) ||
+       (!i8 && (!d->out || d->res))))
+    return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm: int8 and u8 outputs exist for affine + ReLU "
+                "[+ residual] launches: int8 writes u8 alone or, with a residual, fp16 [+ u8]; fp16 "
+                "without a residual writes fp16 + u8");
   if (pairs == 3 && a_planes != 2)
     return fail(VP3D_ERR_INVALID, "conv_gemm: bf16x3 needs hi/lo planes of A");
   const int w_planes = pairs == 3 ? 2 : 1;
@@ -150,7 +166,7 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   const uint64_t plane_stride = d->a_plane_stride > 0 ? (uint64_t)d->a_plane_stride
                                                       : (uint64_t)d->samples * a_rows * a_ld;
   VP3D_TRY(make_map_4d(&ma, d->a, a_ld, a_rows, a_ld, d->samples, a_rows * a_ld, a_planes,
-                       plane_stride, kBlockM));
+                       plane_stride, kBlockM, i8 ? 1 : 2));
   ConvGemmArgs g;
   memset(&g, 0, sizeof(g));
   g.dilated = d->per_sample_tiles ? 1 : 0;
@@ -158,7 +174,7 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   g.out_rows = d->out_rows;
   g.tiles_per_sample = (d->out_rows + kBlockM - 1) / kBlockM;
   g.taps = d->taps;
-  g.kblocks_per_tap = d->k_per_tap / kBlockK;
+  g.kblocks_per_tap = d->k_per_tap / (i8 ? kBlockK8 : kBlockK);
   g.tap_row_step = d->tap_row_step;
   g.tap_col_step = d->tap_col_step;
   g.n_pad = d->n_pad;
@@ -194,7 +210,10 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   g.stats = d->stats;
   g.lo_row_begin = d->lo_row_end > 0 ? d->lo_row_begin : 0;
   g.lo_row_end = d->lo_row_end > 0 ? d->lo_row_end : 0x7fffffff;
-  if (!d->out && !d->out_f32) return fail(VP3D_ERR_INVALID, "conv_gemm: no output");
+  g.i8 = i8;
+  g.out_u8 = static_cast<uint8_t*>(d->out_u8);
+  g.u8_inv_s = d->out_u8_inv_scale;
+  if (!d->out && !d->out_f32 && !d->out_u8) return fail(VP3D_ERR_INVALID, "conv_gemm: no output");
   if (d->out && (d->out_ld % 8)) return fail(VP3D_ERR_INVALID, "conv_gemm: out_ld % 8 != 0");
   if (d->res && (d->res_ld % 8)) return fail(VP3D_ERR_INVALID, "conv_gemm: res_ld % 8 != 0");
   CUtensorMap mo = ma;
@@ -267,7 +286,26 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
     g.bnb_seed_hi = (unsigned)(d->bnb_seed >> 32);
     g.bnb_layer = (unsigned)d->bnb_layer;
   }
-  VP3D_TRY(make_map_2d(&mw, d->w, d->k_per_tap, (uint64_t)w_planes * d->taps * d->n_pad, block_n));
+  if (d->out_u8) {
+    // the u8 output rides the auxiliary map slot (u8 launches have no BatchNorm-backward Z)
+    EncodeTiledFn enc = get_encode_fn();
+    if (!enc) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
+    const uint64_t rows = d->out_rows, ld = d->out_u8_ld;
+    const uint64_t smp = d->per_sample_tiles ? d->samples : 1;
+    cuuint64_t dims[4] = {(cuuint64_t)d->n_pad, rows, smp, 1};
+    cuuint64_t strides[3] = {ld, rows * ld, smp * rows * ld};
+    cuuint32_t box[4] = {64, 32, 1, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUresult r = enc(&mz, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, d->out_u8, dims, strides, box,
+                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled(u8 out) failed: %d", (int)r);
+  }
+  if ((i8 || d->out_u8) && d->res && !g.res_tma)
+    return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm: int8 / u8-output launches need a residual that "
+                "TMA can load (one box of a strided row view)");
+  VP3D_TRY(make_map_2d(&mw, d->w, d->k_per_tap, (uint64_t)w_planes * d->taps * d->n_pad, block_n,
+                       i8 ? 1 : 2));
   CUDA_TRY(launch_conv_gemm(ma, mw, mo, mr, mz, g, block_n, num_sms(), stream));
   return VP3D_OK;
 }
@@ -295,7 +333,10 @@ static void plan_packs(vp3d_plan* p) {
   auto layer_taps = [p](int l) { return l % 2 == 0 ? p->taps[l / 2 + 1] : 1; };
   p->expand_dil = add(kSrcExpand, cr, p->c_in_raw, w0, false, false, C, p->c_in_pad);
   p->expand_flat = add(kSrcExpand, cr, p->c_in_raw, w0, false, true, C, p->k0_pad);
-  for (int l = 0; l < 2 * p->nb; ++l) p->conv[l] = add(l, cr, cr, layer_taps(l), false, false, C, C);
+  // (int8 block convs: 128-element k-blocks, the K per tap padded to 128 with zero weights)
+  const int k_conv = p->int8 ? round_up(C, kBlockK8) : C;
+  for (int l = 0; l < 2 * p->nb; ++l)
+    p->conv[l] = add(l, cr, cr, layer_taps(l), false, false, C, k_conv);
   p->shrink = add(kSrcShrink, p->c_out_raw, cr, 1, false, false, p->c_out_pad, C);
   for (int l = 0; l < 2 * p->nb; ++l) p->conv_t[l] = add(l, cr, cr, layer_taps(l), true, false, C, C);
   // K of the shrink data gradient (dY's columns) padded to 128: also the row pitch of the padded dY
@@ -321,7 +362,10 @@ int pack_weight(const vp3d_plan* p, const PackedConv& k, const vp3d_weights* w, 
                 const PackedConv* fwd) {
   const float* src = nullptr;
   VP3D_TRY(pack_source(k, w, &src));
-  if (k.transposed)
+  if (pack_is_s8(p, k))
+    CUDA_TRY(launch_pack_conv_weight_s8(src, reinterpret_cast<int8_t*>(k.w), k.w_scale, k.c_out,
+                                        k.c_in, k.taps, k.n_pad, k.k_pad, stream));
+  else if (k.transposed)
     CUDA_TRY(launch_pack_conv_weight_t(src, k.w, p->planes, k.c_out, k.c_in, k.taps, k.n_pad, k.k_pad,
                                        stream, fwd ? fwd->w : nullptr, fwd ? fwd->n_pad : 0,
                                        fwd ? fwd->k_pad : 0, k.merged));
@@ -377,7 +421,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
     return fail(VP3D_ERR_INVALID, "plan_create: joint / feature counts must be positive");
   if (cfg->channels < 1)
     return fail(VP3D_ERR_INVALID, "channels must be positive (got %d)", cfg->channels);
-  if (cfg->precision < VP3D_PRECISION_BF16 || cfg->precision > VP3D_PRECISION_FP16)
+  if (cfg->precision < VP3D_PRECISION_BF16 || cfg->precision > VP3D_PRECISION_INT8)
     return fail(VP3D_ERR_INVALID, "plan_create: unknown precision %d", cfg->precision);
   if (cfg->variant != VP3D_VARIANT_DILATED && cfg->variant != VP3D_VARIANT_STRIDED)
     return fail(VP3D_ERR_INVALID, "plan_create: unknown variant %d", cfg->variant);
@@ -400,7 +444,8 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
   p->c_in_pad = round_up(p->c_in_raw, 64);
   p->k0_pad = round_up(p->c_in_raw * cfg->filter_widths[0], 64);
   p->c_out_pad = round_up(p->c_out_raw, 64);
-  p->f16 = cfg->precision == VP3D_PRECISION_FP16 ? 1 : 0;
+  p->int8 = cfg->precision == VP3D_PRECISION_INT8 ? 1 : 0;
+  p->f16 = (cfg->precision == VP3D_PRECISION_FP16 || p->int8) ? 1 : 0;
   p->planes = (cfg->precision == VP3D_PRECISION_BF16 || p->f16) ? 1 : 2;
   // model.py:31, 107-121 / :172-184
   p->pad[0] = cfg->filter_widths[0] / 2;
@@ -416,6 +461,17 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
     p->dilation[i] = cfg->dense ? 1 : next_dilation;
     p->taps[i] = cfg->dense ? 2 * p->pad[i] + 1 : w;
     next_dilation *= w;
+  }
+
+  // int8: every int32 sum is bounded by K * 255 * 127 (K = taps * channels); reject a plan where
+  // that could overflow (only the dense ablation's widest blocks reach it)
+  for (int i = 1; p->int8 && i <= p->nb; ++i) {
+    if ((long long)p->taps[i] * p->c_real * 255 * 127 >= (1ll << 31)) {
+      const int taps = p->taps[i];
+      vp3d_plan_destroy(p);
+      return fail(VP3D_ERR_UNSUPPORTED, "int8: block %d has K = %d x %d, whose int32 sums could "
+                  "overflow (K * 255 * 127 >= 2^31)", i, taps, cfg->channels);
+    }
   }
 
   plan_packs(p);
@@ -438,6 +494,15 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
     }
     p->shrink->scale = aff + (size_t)(2 * p->nb + 1) * 2 * p->C;
     p->shrink->shift = p->shrink->scale + p->c_out_pad;
+    if (p->int8 && p->nb > 0) {
+      float* q = nullptr;
+      if ((st = plan_alloc(p, reinterpret_cast<void**>(&q), (size_t)4 * p->nb * p->C * sizeof(float))))
+        break;
+      for (int l = 0; l < 2 * p->nb; ++l) {
+        p->conv[l]->w_scale = q + (size_t)l * 2 * p->C;
+        p->conv[l]->q_scale = p->conv[l]->w_scale + p->C;
+      }
+    }
   } while (0);
   if (st) {
     vp3d_plan_destroy(p);
@@ -517,6 +582,16 @@ extern "C" __attribute__((visibility("default"))) int vp3d_set_weights(vp3d_plan
                                 p->c_out_pad, stream));
     p->bn_packed = true;
   }
+  if (p->int8 && (what & (VP3D_PACK_CONV | VP3D_PACK_BN_EVAL))) {
+    // the int8 affine: the BatchNorm scale times both dequantisation factors
+    p->int8_folded = false;
+    if (p->int8_scales && p->conv_packed && p->bn_packed) {
+      for (int l = 0; l < 2 * p->nb; ++l)
+        CUDA_TRY(launch_int8_fold(p->conv[l]->scale, p->conv[l]->w_scale, p->act_scale[l],
+                                  p->conv[l]->q_scale, p->C, stream));
+      p->int8_folded = true;
+    }
+  }
   if ((what & VP3D_PACK_CONV_T) && p->f16)
     return fail(VP3D_ERR_UNSUPPORTED, "fp16 plans are inference-only (train with bf16 / bf16x3)");
   if (what & VP3D_PACK_CONV_T)
@@ -587,7 +662,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_output_frames(const v
 }
 
 struct WsLayout {
-  size_t a0 = 0, x0 = 0, x1 = 0, h = 0, total = 0;
+  size_t a0 = 0, x0 = 0, x1 = 0, h = 0, q = 0, total = 0;
   size_t a0_plane = 0, x_plane = 0, h_plane = 0;  // elements per plane
 };
 
@@ -603,6 +678,9 @@ static WsLayout ws_layout(const vp3d_plan* p, int N, int T, bool strided, const 
   w.x0 = off; off = align_up(off + w.x_plane * p->planes * 2, 1024);
   w.x1 = off; off = align_up(off + w.h_plane * p->planes * 2, 1024);  // block outputs are <= L[1] rows
   w.h = off;  off = align_up(off + w.h_plane * p->planes * 2, 1024);
+  // int8: H is stored as u8 only (in the fp16 H buffer), and one u8 buffer holds Q_i: block i + 1's
+  // first conv reads it before its 1x1 conv writes Q_{i+1} (the next kernel of the stream)
+  if (p->int8) { w.q = off; off = align_up(off + w.x_plane, 1024); }
   w.total = off + 1024;
   return w;
 }
@@ -652,6 +730,11 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
     ++*launches;
     return VP3D_OK;
   };
+  // calibration: fold the maximum of a stored fp16 plane into amax[l]
+  auto amax = [&](int l, const __nv_bfloat16* x, long long n) -> int {
+    if (c.amax) CUDA_TRY(launch_amax_f16(x, n, c.amax + l, stream));
+    return VP3D_OK;
+  };
   for (int i = 0; i < c.stages; ++i) {
     const ChainStage& s = c.st[i];
     // the planes of a stage's input lie where its producer wrote them, and must hold its rows
@@ -659,6 +742,28 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
     const int in_ld = i == 0 ? c.expand->k_pad : C;
     if (in_plane < (long long)c.samples * s.in_rows * in_ld)
       return fail(VP3D_ERR_STATE, "internal: activation plane mismatch in block %d", i);
+    if (i > 0 && c.precision[i] == VP3D_PRECISION_INT8) {
+      // u8 x s8 block: Q_{i-1} -> H (u8 only) -> X_i (fp16, residual X_{i-1}) [+ Q_i]
+      const PackedConv& k1 = *p->conv[2 * (i - 1)];
+      const PackedConv& k2 = *p->conv[2 * (i - 1) + 1];
+      if (!c.st[i - 1].q_out || !c.hq) return fail(VP3D_ERR_STATE, "internal: int8 block %d has no u8 input", i);
+      vp3d_conv_desc d = conv(i, k1, nullptr, 0, s.in_rows, C);
+      d.a = c.st[i - 1].q_out;
+      d.tap_row_step = s.tap_row_step;
+      d.scale = k1.q_scale;
+      d.out_u8 = c.hq; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[2 * (i - 1) + 1];
+      VP3D_TRY(launch(d));
+      d = conv(i, k2, nullptr, 0, s.out_rows, C);
+      d.a = c.hq;
+      d.scale = k2.q_scale;
+      d.res = s.in; d.res_plane_stride = in_plane; d.res_ld = C; d.res_row_step = 1;
+      d.res_row_off = s.res_row_off;
+      d.res_rows_per_sample = c.per_sample_tiles ? s.in_rows : 0;
+      d.out = s.out; d.out_plane_stride = s.out_plane;
+      if (s.q_out) { d.out_u8 = s.q_out; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[2 * i]; }
+      VP3D_TRY(launch(d));
+      continue;
+    }
     // the k-tap conv: the expand conv writes X_0, a block's first conv H
     vp3d_conv_desc d = conv(i, i == 0 ? *c.expand : *p->conv[2 * (i - 1)], s.in, in_plane,
                             s.in_rows, in_ld);
@@ -668,6 +773,7 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
       const int h_planes = c.precision[i] == VP3D_PRECISION_BF16X3 ? 2 : 1;
       d.out_planes = h_planes; d.out = c.h; d.out_plane_stride = s.h_plane;
       VP3D_TRY(launch(d));
+      VP3D_TRY(amax(2 * (i - 1) + 1, c.h, (long long)c.samples * s.out_rows * C));
       // second conv: 1x1 + the block input's centre (causal: newest) tap as residual; with
       // per-sample tiles the residual rows of a tile are then one TMA box of the block input
       d = conv(i, *p->conv[2 * (i - 1) + 1], c.h, s.h_plane, s.out_rows, C);
@@ -678,7 +784,9 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
     }
     d.out = s.out; d.out_plane_stride = s.out_plane;
     d.lo_row_begin = s.lo_row_begin; d.lo_row_end = s.lo_row_end;
+    if (s.q_out) { d.out_u8 = s.q_out; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[2 * i]; }
     VP3D_TRY(launch(d));
+    if (i < p->nb) VP3D_TRY(amax(2 * i, s.out, (long long)c.samples * s.out_rows * C));
   }
   if (!c.y) return VP3D_OK;
   // shrink: one flat GEMM over all rows of the last stage, the bias as its affine, fp32 out
@@ -726,13 +834,16 @@ static void dilated_chain(const vp3d_plan* p, int N, int T, const int* L, InferC
   }
 }
 
-extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
-                                 size_t ws_bytes, void* stream_) {
-  if (!p || !x || !y) return fail(VP3D_ERR_INVALID, "forward_eval: null argument");
+// The offline eval forward (y != null) or, with `amax`, the calibration pass of vp3d_calibrate_int8
+// (the chain without shrink, every quantised activation's maximum folded into amax).
+static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
+                        size_t ws_bytes, cudaStream_t stream, unsigned* amax) {
   if (N < 1) return fail(VP3D_ERR_INVALID, "forward_eval: batch must be >= 1");
   if (!p->conv_packed || !p->bn_packed)
     return fail(VP3D_ERR_STATE, "forward_eval: vp3d_set_weights has not been called");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (p->int8 && !p->int8_folded)
+    return fail(VP3D_ERR_STATE, "forward_eval: int8 plan without activation scales (call "
+                "vp3d_set_int8_scales, then vp3d_set_weights)");
   const bool strided = use_strided(p, T);
   int L[VP3D_MAX_WIDTHS];
   if (!layer_rows(p, T, strided, L))
@@ -755,11 +866,14 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   c.h = bf(wl.h);
   c.y = y;
   c.profile = true;
+  c.amax = amax;
+  if (p->int8) c.hq = base + wl.h;
   for (int i = 0; i <= p->nb; ++i) {
     ChainStage& s = c.st[i];
     s.in = i == 0 ? bf(wl.a0) : c.st[i - 1].out;
     s.out = bf(i % 2 ? wl.x1 : wl.x0);
     s.out_plane = s.h_plane = (long long)N * L[i] * C;
+    if (p->int8 && i < p->nb) s.q_out = base + wl.q;
   }
 
   // Per-layer operand precision.  index 0 = expand, 1..nb = residual blocks, nb+1 = shrink.
@@ -769,6 +883,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   //            split-bf16 (they carry most of the bf16 error, tools/precision_study.py),
   //            residual blocks run plain bf16 on the hi plane unless they hold < 0.5% of the
   //            forward FLOPs (negligible even at the narrow-tile rate of such layers).
+  //   int8   : residual blocks u8 x s8, expand and shrink fp16.
   {
     double fl[VP3D_MAX_WIDTHS + 1], total = 0.0;
     fl[0] = (double)N * L[0] * p->c_in_raw * fw[0] * C;
@@ -777,8 +892,11 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
     for (int i = 0; i <= p->nb + 1; ++i) total += fl[i];
     for (int i = 0; i <= p->nb + 1; ++i) {
       const bool x3 = i == 0 || i == p->nb + 1 || fl[i] < 0.005 * total;
-      c.precision[i] = p->cfg.precision != VP3D_PRECISION_MIXED ? p->cfg.precision
-                       : x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16;
+      const bool edge = i == 0 || i == p->nb + 1;
+      c.precision[i] = p->cfg.precision == VP3D_PRECISION_MIXED
+                           ? (x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16)
+                       : p->cfg.precision == VP3D_PRECISION_INT8 && edge ? VP3D_PRECISION_FP16
+                                                                         : p->cfg.precision;
     }
   }
 
@@ -815,6 +933,64 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
   ++launches;
   VP3D_TRY(run_infer_chain(p, c, stream, &launches));
   p->last_launches = launches;
+  return VP3D_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
+                                 size_t ws_bytes, void* stream_) {
+  if (!p || !x || !y) return fail(VP3D_ERR_INVALID, "forward_eval: null argument");
+  return eval_forward(p, x, y, N, T, ws, ws_bytes, static_cast<cudaStream_t>(stream_), nullptr);
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_calibrate_int8(
+    vp3d_plan* p, const float* x, int N, int T, void* ws, size_t ws_bytes, float* amax,
+    void* stream_) {
+  if (!p || !x || !amax) return fail(VP3D_ERR_INVALID, "calibrate_int8: null argument");
+  if (p->cfg.precision != VP3D_PRECISION_FP16)
+    return fail(VP3D_ERR_INVALID, "calibrate_int8: needs an fp16 plan (the activations it measures "
+                "are the fp16 forward's)");
+  if (reinterpret_cast<uintptr_t>(amax) % 4)
+    return fail(VP3D_ERR_INVALID, "calibrate_int8: amax not 4-byte aligned");
+  // (fp32 values >= 0: their bit patterns order like the values)
+  return eval_forward(p, x, nullptr, N, T, ws, ws_bytes, static_cast<cudaStream_t>(stream_),
+                      reinterpret_cast<unsigned*>(amax));
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_int8_packs(
+    const vp3d_plan* p, int layer, void* w_s8, float* w_scale, float* q_scale, void* stream_) {
+  if (!p || !p->int8) return fail(VP3D_ERR_INVALID, "int8_packs: not an int8 plan");
+  if (layer < 0 || layer >= 2 * p->nb) return fail(VP3D_ERR_INVALID, "int8_packs: no layer %d", layer);
+  if (!p->conv_packed) return fail(VP3D_ERR_STATE, "int8_packs: weights not packed yet");
+  if (q_scale && !p->int8_folded) return fail(VP3D_ERR_STATE, "int8_packs: scales not folded yet");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const PackedConv& k = *p->conv[layer];
+  if (w_s8) CUDA_TRY(cudaMemcpyAsync(w_s8, k.w, pack_bytes(p, k), cudaMemcpyDeviceToDevice, stream));
+  if (w_scale)
+    CUDA_TRY(cudaMemcpyAsync(w_scale, k.w_scale, k.n_pad * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  if (q_scale)
+    CUDA_TRY(cudaMemcpyAsync(q_scale, k.q_scale, k.n_pad * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  return VP3D_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_set_int8_scales(vp3d_plan* p,
+                                                                          const float* amax_host,
+                                                                          int n) {
+  if (!p || !amax_host) return fail(VP3D_ERR_INVALID, "set_int8_scales: null argument");
+  if (!p->int8) return fail(VP3D_ERR_INVALID, "set_int8_scales: not an int8 plan");
+  if (n != 2 * p->nb)
+    return fail(VP3D_ERR_INVALID, "set_int8_scales: expected %d amax values, got %d", 2 * p->nb, n);
+  for (int l = 0; l < n; ++l)
+    if (!(amax_host[l] >= 0.0f) || !(amax_host[l] <= 3.0e38f))
+      return fail(VP3D_ERR_INVALID, "set_int8_scales: amax[%d] = %g is not a finite value >= 0", l,
+                  (double)amax_host[l]);
+  for (int l = 0; l < n; ++l) {
+    // s = amax / 255 and 1 / s, both in fp32 (round to nearest)
+    const float s = amax_host[l] > 0.0f ? amax_host[l] / 255.0f : 1.0f;
+    p->act_scale[l] = s;
+    p->act_inv[l] = 1.0f / s;
+  }
+  p->int8_scales = true;
+  p->int8_folded = false;
   return VP3D_OK;
 }
 

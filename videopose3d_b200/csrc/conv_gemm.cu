@@ -15,10 +15,14 @@
 // Lean inference launches with more tiles than CTAs use the ping-pong instances instead: each
 // consumer warpgroup computes all 128 rows of every other tile, so that one warpgroup's epilogue
 // runs under the other's MMAs.
+// The int8 eval instances (I8) run the same pipeline on u8 A / s8 W tiles of 128 x 128 bytes per
+// k-block (int32 accumulators, k32 MMAs), and may store a u8 copy of their output (U8).
 #include "conv_gemm.cuh"
 
 #include <stdlib.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "ptx.cuh"
 
@@ -28,7 +32,9 @@ namespace vp3d {
 // LEAN (inference layers: affine + ReLU [+ one-plane TMA residual] -> one 16-bit plane): the same
 // epilogue with every option resolved at compile time.
 // PP (lean only): ping-pong schedule, each consumer warpgroup computes whole tiles (see the kernel).
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool PP = false>
+// U8 == 1: a u8 copy next to the 16-bit plane gets staging tiles of its own (U8 == 2 stages its
+// u8 tiles in the unused 16-bit staging).
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool PP = false, int U8 = 0>
 struct GemmCfg {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma tiles are 64 or 128 columns wide");
   static_assert(!(LEAN && (OUT2 || TRAIN)), "the lean epilogue is inference-only, one plane");
@@ -45,7 +51,10 @@ struct GemmCfg {
   // auxiliary (residual / Z) landing tiles: four, so that two-tile store blocks (hi+lo residual,
   // or residual + Z) still get two stages in flight.  Ping-pong: two per warpgroup.
   static constexpr int kResSlots = RES ? 4 : 0;
-  static constexpr uint32_t kFixedBytes = kStagingBytes + kResSlots * kTileBytes;
+  // u8 staging (64 columns of 64 bytes per row): ping-pong one 128-row tile per warpgroup,
+  // cooperative two alternating 64-row halves per warpgroup -- 16 KiB either way
+  static constexpr uint32_t kU8Bytes = U8 == 1 ? 2 * kBlockM * 64 : 0;
+  static constexpr uint32_t kFixedBytes = kStagingBytes + kResSlots * kTileBytes + kU8Bytes;
   // per-channel affine (scale, shift) of the current N block: 2 x BLOCK_N floats.  Ping-pong reads
   // it through L1 instead: the two warpgroups may hold different N blocks, and a copy per
   // warpgroup would cost the 128-wide instance an operand stage.
@@ -114,6 +123,25 @@ __device__ __forceinline__ void wgmma_kblock(float (&acc)[BLOCK_N / 2], uint64_t
   }
 }
 
+// one k-block of u8 x s8: the same 128-byte swizzle row holds 128 elements, four k32 steps of 32 B
+// (the same +2 descriptor advance per step as the 16-bit k16 steps)
+template <int BLOCK_N>
+__device__ __forceinline__ void wgmma_kblock_i8(int (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db,
+                                                bool first) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
+    if constexpr (BLOCK_N == 128) wgmma_m64n128k32_u8s8(acc, da + 2 * k, db + 2 * k, accumulate);
+    else wgmma_m64n64k32_u8s8(acc, da + 2 * k, db + 2 * k, accumulate);
+  }
+}
+
+// the u8 pair (columns c, c + 1) at byte `off` of a u8 staging tile (rows of 64 bytes, no swizzle)
+__device__ __forceinline__ void st_u8_pair(uint32_t addr, float v0, float v1, float inv_s) {
+  const uint32_t q = quant_u8(v0, inv_s) | (quant_u8(v1, inv_s) << 8);
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)q) : "memory");
+}
+
 // Per-column sums over the 16 rows a warp holds of one 64-column store block (values v[jj][0..3]
 // in the wgmma layout), then over the two warps of a 32-row slab (in a fixed order: the even warp's
 // partial plus the odd warp's).  Lane l < 4 of the even warp ends up with the slab sums of columns
@@ -175,7 +203,12 @@ __device__ __forceinline__ void tl_stamp(const ConvGemmArgs& p, int ev) {
 // k-block is one branch-free group of wgmma; the other instances read it from p.f16.
 // PP (LEAN only): the ping-pong schedule for launches where CTAs get more than one tile (see the
 // consumer branches below); the cooperative schedule otherwise.
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false, bool PP = false>
+// I8 (LEAN + F16 only): u8 A times s8 W into int32 accumulators, 128-element k-blocks; the
+// residual and the 16-bit output stay fp16.
+// U8 (LEAN only): 1 = also store the u8 quantisation of every stored value (ConvGemmArgs::out_u8),
+// 2 = store only that u8 plane (no 16-bit output, no staging).
+template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false, bool PP = false,
+          bool I8 = false, int U8 = 0>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_w,
@@ -183,10 +216,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_res,
                  const __grid_constant__ CUtensorMap tmap_z, const ConvGemmArgs p) {
   static_assert(LEAN || !F16, "only the lean instances fix the operand format at compile time");
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP>;
+  static_assert((!I8 && U8 == 0) || (LEAN && F16), "int8 and u8 outputs are lean fp16 instances");
+  static_assert(!(RES && U8 == 2), "a residual instance stores its 16-bit plane");
+  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP, U8>;
+  using Acc = std::conditional_t<I8, int, float>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBlocksPerTile = BLOCK_N / 64;
-  constexpr int kFrag = BLOCK_N / 2;   // accumulator floats per consumer thread
+  constexpr int kFrag = BLOCK_N / 2;   // accumulator registers per consumer thread
+  constexpr int kBK = I8 ? kBlockK8 : kBlockK;   // elements per k-block (128 bytes either way)
+  constexpr bool kStore16 = U8 != 2;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -197,7 +235,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const uint32_t smem_b = base + kStages * Cfg::kABytes;
   const uint32_t smem_store = base + kStages * Cfg::kStageBytes;
   const uint32_t smem_res = smem_store + Cfg::kStagingBytes;
-  const uint32_t bar_base = smem_res + Cfg::kResSlots * Cfg::kTileBytes;
+  const uint32_t smem_u8 = smem_res + Cfg::kResSlots * Cfg::kTileBytes;   // (U8 == 1)
+  const uint32_t bar_base = smem_u8 + Cfg::kU8Bytes;
   const uint32_t full_bar = bar_base;
   const uint32_t empty_bar = bar_base + kStages * 8;
   const uint32_t rfull_bar = bar_base + 2 * kStages * 8;   // up to 4 auxiliary stages
@@ -228,6 +267,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     tma_prefetch_desc(&tmap_out);
     if (RES) tma_prefetch_desc(&tmap_res);
     if (RES && bnb) tma_prefetch_desc(&tmap_z);
+    if (U8 != 0) tma_prefetch_desc(&tmap_z);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
@@ -290,11 +330,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
             mbar_wait(empty_bar + stage * 8, phase ^ 1);
             mbar_expect_tx(fb, Cfg::kStageBytes);
             const int w_row = (w_plane * p.taps + tap) * p.n_pad + n_blk * BLOCK_N;
-            tma_load_2d(&tmap_w, fb, smem_b + stage * Cfg::kBBytes, kb * kBlockK, w_row);
+            tma_load_2d(&tmap_w, fb, smem_b + stage * Cfg::kBBytes, kb * kBK, w_row);
           }
           if (mode != 0) {
             const int a_row = row0 + tap * p.tap_row_step;
-            const int a_col = tap * p.tap_col_step + kb * kBlockK;
+            const int a_col = tap * p.tap_col_step + kb * kBK;
             tma_load_4d(&tmap_a, fb, smem_a + stage * Cfg::kABytes, a_col, a_row, sample, a_plane);
 #ifdef VP3D_TIMELINE
             if (w == (int)blockIdx.x && it == 0) TL(3);
@@ -386,7 +426,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const uint32_t bar_mine = 8u + (uint32_t)wg, bar_other = 9u - (uint32_t)wg;
     const uint32_t staging = smem_store + wg * Cfg::kTileBytes;   // (no-residual instance)
     uint32_t res_seen = 0;            // residual tiles this warpgroup has received
-    float acc[2][kFrag];
+    Acc acc[2][kFrag];
 #pragma unroll
     for (int i = 0; i < kFrag; ++i) acc[0][i] = acc[1][i] = 0.0f;
 
@@ -411,8 +451,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         wgmma_fence_operands(acc[0]);
         wgmma_fence_operands(acc[1]);
         wgmma_fence();
-        wgmma_kblock<BLOCK_N, F16>(acc[0], da0, db, it == 0);
-        wgmma_kblock<BLOCK_N, F16>(acc[1], da1, db, it == 0);
+        if constexpr (I8) {
+          wgmma_kblock_i8<BLOCK_N>(acc[0], da0, db, it == 0);
+          wgmma_kblock_i8<BLOCK_N>(acc[1], da1, db, it == 0);
+        } else {
+          wgmma_kblock<BLOCK_N, F16>(acc[0], da0, db, it == 0);
+          wgmma_kblock<BLOCK_N, F16>(acc[1], da1, db, it == 0);
+        }
         wgmma_commit();
         wgmma_fence_operands(acc[0]);
         wgmma_fence_operands(acc[1]);
@@ -446,12 +491,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           mbar_wait(rfull_bar + slot * 8, (res_seen >> 1) & 1u);
           ++res_seen;
           tile_smem = smem_res + slot * Cfg::kTileBytes;
+          if constexpr (U8 != 0) {
+            // the u8 tile must have been read out by the bulk stores issued from it last
+            if (tid == 0) tma_store_wait_read<0>();
+            named_bar_sync(bar_wg, 128);
+          }
         } else {
           // the staging tile must have been read out by the bulk stores issued from it last
           if (tid == 0) tma_store_wait_read<0>();
           named_bar_sync(bar_wg, 128);
           tile_smem = staging;
         }
+        // u8 tile of this warpgroup: 128 rows of 64 bytes (U8 == 2: inside the 16-bit staging)
+        const uint32_t u8_tile = U8 == 2 ? staging : smem_u8 + (uint32_t)wg * (kBlockM * 64);
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j4 = 4 * (sb * 8 + jj);
@@ -462,11 +514,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           for (int h2 = 0; h2 < 2; ++h2) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              float v0 = fmaxf(fmaf(acc[h2][j4 + 2 * h], sc.x, sh.x), 0.0f);
-              float v1 = fmaxf(fmaf(acc[h2][j4 + 2 * h + 1], sc.y, sh.y), 0.0f);
+              float v0 = fmaxf(fmaf(static_cast<float>(acc[h2][j4 + 2 * h]), sc.x, sh.x), 0.0f);
+              float v1 = fmaxf(fmaf(static_cast<float>(acc[h2][j4 + 2 * h + 1]), sc.y, sh.y), 0.0f);
               const uint32_t off = sw128_off(64 * h2 + rl0 + 8 * h, jj * 8 + cq);
               if (RES) add_pair(v0, v1, ld_shared_u32(tile_smem + off), F16);
-              st_shared_u32(tile_smem + off, F16 ? pack_f16x2(v0, v1) : pack_bf16x2(v0, v1));
+              if constexpr (kStore16)
+                st_shared_u32(tile_smem + off, F16 ? pack_f16x2(v0, v1) : pack_bf16x2(v0, v1));
+              if constexpr (U8 != 0)
+                st_u8_pair(u8_tile + (uint32_t)(64 * h2 + rl0 + 8 * h) * 64u + jj * 8 + cq, v0, v1,
+                           p.u8_inv_s);
             }
           }
         }
@@ -475,8 +531,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         if (tid == 0) {
           // four 32-row boxes: 4 KiB-aligned quarters of the tile, same swizzle phase as written
 #pragma unroll
-          for (int hb = 0; hb < 4; ++hb)
-            tma_store_4d(&tmap_out, tile_smem + hb * 4096u, cb, row0 + 32 * hb, sample, 0);
+          for (int hb = 0; hb < 4; ++hb) {
+            if constexpr (kStore16)
+              tma_store_4d(&tmap_out, tile_smem + hb * 4096u, cb, row0 + 32 * hb, sample, 0);
+            // (u8 instances are lean, never BatchNorm-backward: tmap_z maps the u8 plane)
+            if constexpr (U8 != 0)
+              tma_store_4d(&tmap_z, u8_tile + hb * 2048u, cb, row0 + 32 * hb, sample, 0);
+          }
           tma_store_commit();
         }
       }
@@ -518,7 +579,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     uint32_t ablock = 0;              // auxiliary stages seen so far
     uint32_t sbuf = 0;                // staging buffer of the next store block
     int aff_n_blk = -1;               // N block whose scale / shift sit in shared memory
-    float acc[kFrag];
+    Acc acc[kFrag];
 #pragma unroll
     for (int i = 0; i < kFrag; ++i) acc[i] = 0.0f;
 
@@ -539,7 +600,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const uint64_t db = make_gmma_desc_sw128(smem_b + stage * Cfg::kBBytes, 16, 1024);
         wgmma_fence_operands(acc);
         wgmma_fence();
-        if constexpr (LEAN) wgmma_kblock<BLOCK_N, F16>(acc, da, db, it == 0);
+        if constexpr (I8) wgmma_kblock_i8<BLOCK_N>(acc, da, db, it == 0);
+        else if constexpr (LEAN) wgmma_kblock<BLOCK_N, F16>(acc, da, db, it == 0);
         else if (f16) wgmma_kblock<BLOCK_N, true>(acc, da, db, it == 0);
         else wgmma_kblock<BLOCK_N, false>(acc, da, db, it == 0);
         wgmma_commit();
@@ -615,6 +677,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const uint32_t aux0 = smem_res + (rs * aux_tiles) * Cfg::kTileBytes;
         // this warpgroup's staging slice(s): [hi] or [hi, lo], 64 rows x 128 B each
         const uint32_t my_store = smem_store + (wg * 2 + sbuf) * (OUT2 ? 2 : 1) * Cfg::kHalfBytes;
+        // its u8 slice: 64 rows of 64 bytes (U8 == 2: inside the 16-bit slice)
+        const uint32_t my_u8 = U8 == 2 ? my_store : smem_u8 + (uint32_t)(wg * 2 + sbuf) * (64 * 64);
         if (!do_f32) {
           // The slice must have been read out by the bulk store issued from it two blocks ago.
           if (tid == 0) tma_store_wait_read<1>();
@@ -626,7 +690,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           const int j = sb * 8 + jj;
           const int cl = sb * 64 + jj * 8 + cq;   // column inside the N block
           const int c = cb + jj * 8 + cq;         // output column
-          float v[2][2] = {{acc[4 * j], acc[4 * j + 1]}, {acc[4 * j + 2], acc[4 * j + 3]}};
+          float v[2][2] = {{static_cast<float>(acc[4 * j]), static_cast<float>(acc[4 * j + 1])},
+                           {static_cast<float>(acc[4 * j + 2]), static_cast<float>(acc[4 * j + 3])}};
           if (do_affine) {
             const float2 sc = *reinterpret_cast<const float2*>(s_affine + cl);
             const float2 sh = *reinterpret_cast<const float2*>(s_affine + BLOCK_N + cl);
@@ -673,8 +738,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
               if (c + 1 < p.n_valid) op[1] = v[h][1];
             }
           } else {
+            if constexpr (U8 != 0) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
+              for (int h = 0; h < 2; ++h)
+                st_u8_pair(my_u8 + (uint32_t)(rl0 + 8 * h) * 64u + jj * 8 + cq, v[h][0], v[h][1],
+                           p.u8_inv_s);
+            }
+#pragma unroll
+            for (int h = 0; h < 2 && kStore16; ++h) {
               const uint32_t hi = f16 ? pack_f16x2(v[h][0], v[h][1]) : pack_bf16x2(v[h][0], v[h][1]);
               const uint32_t off = sw128_off(rl0 + 8 * h, jj * 8 + cq);
               st_shared_u32(my_store + off, hi);
@@ -755,7 +826,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
             for (int hb = 0; hb < 2; ++hb) {
               const int r = row0 + 64 * wg + 32 * hb;
-              tma_store_4d(&tmap_out, my_store + hb * 4096u, cb, r, sample, 0);
+              if constexpr (kStore16) tma_store_4d(&tmap_out, my_store + hb * 4096u, cb, r, sample, 0);
+              // (u8 instances are lean, never BatchNorm-backward: tmap_z maps the u8 plane)
+              if constexpr (U8 != 0) tma_store_4d(&tmap_z, my_u8 + hb * 2048u, cb, r, sample, 0);
               if (two_planes_t) tma_store_4d(&tmap_out, my_store + Cfg::kHalfBytes + hb * 4096u, cb, r, sample, 1);
             }
             tma_store_commit();
@@ -795,13 +868,13 @@ static int conv_tiles(const ConvGemmArgs& a) {
 }
 
 template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false, bool F16 = false,
-          bool PP = false>
+          bool PP = false, bool I8 = false, int U8 = 0>
 static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                                const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                                const CUtensorMap& tmap_z, const ConvGemmArgs& args, int num_sms,
                                cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP>;
-  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16, PP>;
+  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP, U8>;
+  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16, PP, I8, U8>;
   // the dynamic shared memory opt-in is a per-device attribute
   static bool attr_set[kMaxDevices] = {};
   int dev = 0;
@@ -871,6 +944,42 @@ static cudaError_t launch_train(const CUtensorMap& a, const CUtensorMap& w, cons
   return launch_impl<BLOCK_N, RES, OUT2, false>(a, w, o, r, z, args, num_sms, stream);
 }
 
+// The int8 eval instances and the fp16 ones with a u8 second output: always the lean epilogue (they
+// have no general counterpart), ping-pong by the same rule as the 16-bit lean launches.
+template <int BLOCK_N, bool RES, bool I8, int U8>
+static cudaError_t launch_quant(const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
+                                const CUtensorMap& r, const CUtensorMap& z, const ConvGemmArgs& args,
+                                int num_sms, cudaStream_t stream) {
+  if (conv_tiles(args) > num_sms)
+    return launch_impl<BLOCK_N, RES, false, false, true, true, true, I8, U8>(a, w, o, r, z, args, num_sms, stream);
+  return launch_impl<BLOCK_N, RES, false, false, true, true, false, I8, U8>(a, w, o, r, z, args, num_sms, stream);
+}
+
+template <int BLOCK_N>
+static cudaError_t launch_quant_variants(const CUtensorMap& a, const CUtensorMap& w,
+                                         const CUtensorMap& o, const CUtensorMap& r,
+                                         const CUtensorMap& z, const ConvGemmArgs& args,
+                                         int num_sms, cudaStream_t stream) {
+  const bool res = args.res_tma != 0;
+  const bool u8 = args.out_u8 != nullptr;
+  // what the int8 chain runs: H (u8 only), X_i (fp16 [+ u8]), and the fp16 expand with Q_0
+  if (!args.f16 || args.bnb || args.out_planes != 1 ||
+      args.flags != (kEpiAffine | kEpiRelu | (res ? kEpiResidual : 0)) ||
+      (res && (args.res_planes != 1 || args.res_col_begin != 0 || args.res_cols < args.n_pad)))
+    return cudaErrorInvalidValue;
+  if (args.i8) {
+    if (res) {
+      if (!args.out) return cudaErrorInvalidValue;
+      return u8 ? launch_quant<BLOCK_N, true, true, 1>(a, w, o, r, z, args, num_sms, stream)
+                : launch_quant<BLOCK_N, true, true, 0>(a, w, o, r, z, args, num_sms, stream);
+    }
+    if (args.out || !u8) return cudaErrorInvalidValue;
+    return launch_quant<BLOCK_N, false, true, 2>(a, w, o, r, z, args, num_sms, stream);
+  }
+  if (res || !u8 || !args.out) return cudaErrorInvalidValue;
+  return launch_quant<BLOCK_N, false, false, 1>(a, w, o, r, z, args, num_sms, stream);
+}
+
 template <int BLOCK_N, bool RES>
 static cudaError_t launch_planes(const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
                                  const CUtensorMap& r, const CUtensorMap& z, const ConvGemmArgs& args,
@@ -901,6 +1010,11 @@ cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_
 #else
   const ConvGemmArgs& args = args_in;
 #endif
+  if (args.i8 || args.out_u8) {
+    if (block_n == 128) return launch_quant_variants<128>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
+    if (block_n == 64) return launch_quant_variants<64>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
+    return cudaErrorInvalidValue;
+  }
   const bool res = args.res_tma != 0 || args.bnb != 0;
   switch (block_n) {
     case 128:

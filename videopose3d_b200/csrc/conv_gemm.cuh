@@ -26,6 +26,7 @@ namespace vp3d {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;   // 64 bf16 = one 128-byte swizzle row
+constexpr int kBlockK8 = 128; // the same row holds 128 one-byte (int8) elements
 constexpr int kUmmaK = 16;
 constexpr int kMaxDevices = 64;  // per-device caches (function attributes, SM counts)
 
@@ -97,6 +98,13 @@ struct ConvGemmArgs {
   // two output planes: the lo plane is only produced for tiles that intersect rows
   // [lo_row_begin, lo_row_end) (flat tiling; the rows a later residual add / split-bf16 GEMM reads)
   int lo_row_begin, lo_row_end;
+  // ---- int8 inference (lean instances only)
+  int i8;                      // 1: A is u8 and W s8, k-blocks of 128 one-byte elements, int32 acc
+  // u8 copy of the stored value, q = cvt.rni.sat.u8(v * u8_inv_s), rows as in `out`: staged in
+  // shared memory and TMA-stored through tmap_z (64 x 32 byte boxes, no swizzle); next to the
+  // 16-bit plane, or alone when `out` is null.  out_u8 (non-null) selects the u8 instances.
+  uint8_t* out_u8;
+  float u8_inv_s;
 #ifdef VP3D_TIMELINE
   // debug build (`make dbg`): per-launch time stamps of the first and the last CTA
   unsigned long long* timeline;   // [2 CTAs][32 events][globaltimer ns, clock64] or null
@@ -112,6 +120,8 @@ void conv_gemm_debug_set_timeline(unsigned long long* buf, int max_launches);
 // tmap_res: 4-D (channel, row, sample, plane) over the residual's row view, box (64, 128, 1, 1); used
 // only when args.res_tma is set.
 // tmap_z: same geometry as tmap_out over the Z tensor of the layer below; used only when args.bnb.
+// With args.out_u8 it maps the u8 output instead: 4-D (channel, row, sample, 1) bytes, box
+// (64, 32, 1, 1), no swizzle.
 // tmap_w: box rows = block_n.  block_n is 128 or 64.
 void conv_gemm_set_pdl(int on);   // programmatic dependent launch of the GEMM kernels (default on)
 bool conv_gemm_pdl_enabled();     // (also honoured by the small kernels between the GEMMs, launch.cuh)

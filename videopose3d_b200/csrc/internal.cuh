@@ -29,12 +29,14 @@ int fail(int code, const char* fmt, ...);
     if (_s != VP3D_OK) return _s; \
   } while (0)
 
-// 4-D bf16 map (k, row, sample, plane), box (64, box_rows, 1, 1), 128-byte swizzle.
+// 4-D bf16 map (k, row, sample, plane), box (64, box_rows, 1, 1), 128-byte swizzle; with
+// elem_bytes = 1 a byte map (u8 / s8 operands) whose box is 128 elements wide (the same 128 bytes).
 int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint64_t row_stride,
                 uint64_t samples, uint64_t sample_stride, uint64_t planes, uint64_t plane_stride,
-                uint32_t box_rows);
-// 2-D bf16 map (k, row), box (64, box_rows), 128-byte swizzle.
-int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint32_t box_rows);
+                uint32_t box_rows, int elem_bytes = 2);
+// 2-D bf16 map (k, row), box (64, box_rows), 128-byte swizzle; elem_bytes as above.
+int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint32_t box_rows,
+                int elem_bytes = 2);
 
 int pick_block_n(int n_pad);
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
@@ -63,6 +65,11 @@ struct PackedConv {
   __nv_bfloat16* w = nullptr;  // transposed packs: allocated with the training state
   float* scale = nullptr;      // forward packs: eval affine of the conv's output [n_pad]
   float* shift = nullptr;
+  // int8 plans, residual-block convs: w holds s8 [taps][n_pad][k_pad] (k_pad a multiple of 128),
+  // w_scale its per-channel weight scales and q_scale the affine scale with both dequantisation
+  // factors folded in (launch_int8_fold), both [n_pad]
+  float* w_scale = nullptr;
+  float* q_scale = nullptr;
 };
 constexpr int kMaxPacks = 2 * VP3D_MAX_LAYERS + 5;
 
@@ -112,7 +119,12 @@ struct vp3d_plan {
   int c_real = 0;   // the model's `channels` argument (any positive value, model.py:85-86)
   int c_in_raw = 0, c_out_raw = 0, c_in_pad = 0, k0_pad = 0, c_out_pad = 0;
   int planes = 1;
-  int f16 = 0;  // VP3D_PRECISION_FP16: 16-bit stores hold IEEE fp16
+  int f16 = 0;  // VP3D_PRECISION_FP16 (and INT8): 16-bit stores hold IEEE fp16
+  int int8 = 0; // VP3D_PRECISION_INT8: the residual blocks' convs run u8 x s8
+  // int8: activation scale s and 1 / s of every block conv's input (vp3d_set_int8_scales), and
+  // whether the packs' q_scale vectors have been folded from the current scales
+  bool int8_scales = false, int8_folded = false;
+  float act_scale[VP3D_MAX_LAYERS] = {}, act_inv[VP3D_MAX_LAYERS] = {};
   int pad[VP3D_MAX_WIDTHS];
   int shift_dil[VP3D_MAX_WIDTHS];  // causal shift in frames (TemporalModel, model.py:111)
   int shift_str[VP3D_MAX_WIDTHS];  // causal shift in strided units (Optimized1f, model.py:176)
@@ -163,8 +175,13 @@ bool use_strided(const vp3d_plan* p, int T);
 // rows per sample after each stage: L[0] = rows out of expand, L[i] = rows out of block i
 int layer_rows(const vp3d_plan* p, int T, bool strided, int* L);
 int strided_trim(const vp3d_plan* p, int* L);
+// int8 plans keep the residual-block convs' forward packs in s8
+inline bool pack_is_s8(const vp3d_plan* p, const PackedConv& k) {
+  return p->int8 && !k.transposed && k.src >= 0;
+}
 inline size_t pack_bytes(const vp3d_plan* p, const PackedConv& k) {
-  return (size_t)p->planes * k.stored_taps * k.n_pad * k.k_pad * sizeof(__nv_bfloat16);
+  return (size_t)p->planes * k.stored_taps * k.n_pad * k.k_pad *
+         (pack_is_s8(p, k) ? 1 : sizeof(__nv_bfloat16));
 }
 // packs k from its fp32 weight in w; a transposed pack given `fwd` writes that forward pack of the
 // same conv in the same pass
@@ -197,6 +214,7 @@ struct ChainStage {
   int out_rows;              // per sample (per-sample tiles) or in all (flat)
   int tap_row_step, res_row_off;
   int lo_row_begin, lo_row_end;   // as in vp3d_conv_desc, of the GEMM that writes X_i
+  uint8_t* q_out;            // int8 chain: the u8 copy Q_i of X_i that block i + 1 reads, or null
 };
 // The geometry of one run of the chain: what the offline forward (strided, dilated), the streaming
 // push and its start pass differ in.  run_infer_chain makes every GEMM descriptor from it.
@@ -211,6 +229,10 @@ struct InferChain {
   float* y;                    // fp32 rows shrink writes from the last stage's output; null: no shrink
   int precision[VP3D_MAX_WIDTHS + 1];   // operands of expand, of block i, of shrink (nb + 1)
   bool profile;                // honour vp3d_profile_launch
+  uint8_t* hq;                 // int8 blocks: H as u8 [rows][C]
+  // calibration (vp3d_calibrate_int8): fp32 bits of amax[2B], folded after every GEMM whose output
+  // an int8 plan quantises; null otherwise
+  unsigned* amax;
 };
 // runs the chain on `stream` and adds its launches to *launches
 int run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream, int* launches);

@@ -166,6 +166,91 @@ cudaError_t launch_pack_conv_weight(const float* w, __nv_bfloat16* out, int plan
   return cudaGetLastError();
 }
 
+// one block per output channel: the channel's |w| maximum, then its s8 row of every tap
+__global__ void __launch_bounds__(256)
+pack_conv_weight_s8_kernel(const float* __restrict__ w, int8_t* __restrict__ out,
+                           float* __restrict__ w_scale, int c_out, int c_in, int taps, int n_pad,
+                           int k_pad) {
+  __shared__ float s_max[8];
+  const int co = blockIdx.x;
+  const float* src = w + (long long)co * c_in * taps;
+  const int n = co < c_out ? c_in * taps : 0;
+  float m = 0.0f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(__ldg(src + i)));
+  for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+  if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = 0.0f;
+  for (int i = 0; i < 8; ++i) m = fmaxf(m, s_max[i]);
+  const float s = m > 0.0f ? __fdiv_rn(m, 127.0f) : 1.0f;
+  if (threadIdx.x == 0) w_scale[co] = s;
+  for (int tap = 0; tap < taps; ++tap) {
+    int8_t* row = out + ((long long)tap * n_pad + co) * k_pad;
+    for (int k = threadIdx.x; k < k_pad; k += blockDim.x) {
+      float q = 0.0f;
+      if (k < c_in && co < c_out)
+        q = fminf(fmaxf(rintf(__fdiv_rn(__ldg(src + (long long)k * taps + tap), s)), -127.0f), 127.0f);
+      row[k] = (int8_t)(int)q;
+    }
+  }
+}
+
+cudaError_t launch_pack_conv_weight_s8(const float* w, int8_t* out, float* w_scale, int c_out,
+                                       int c_in, int taps, int n_pad, int k_pad,
+                                       cudaStream_t stream) {
+  pack_conv_weight_s8_kernel<<<n_pad, 256, 0, stream>>>(w, out, w_scale, c_out, c_in, taps, n_pad,
+                                                        k_pad);
+  return cudaGetLastError();
+}
+
+__global__ void int8_fold_kernel(const float* __restrict__ bn_scale, const float* __restrict__ w_scale,
+                                 float s_in, float* __restrict__ q_scale, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) q_scale[i] = __fmul_rn(bn_scale[i], __fmul_rn(w_scale[i], s_in));
+}
+
+cudaError_t launch_int8_fold(const float* bn_scale, const float* w_scale, float s_in, float* q_scale,
+                             int n, cudaStream_t stream) {
+  int8_fold_kernel<<<(n + 255) / 256, 256, 0, stream>>>(bn_scale, w_scale, s_in, q_scale, n);
+  return cudaGetLastError();
+}
+
+// fp16 bits of values >= 0 order like the values; -0 (0x8000) is mapped to 0
+__global__ void __launch_bounds__(256)
+amax_f16_kernel(const uint4* __restrict__ x, long long n8, unsigned* __restrict__ amax_bits) {
+  __shared__ unsigned s_max[8];
+  unsigned m = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8;
+       i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = __ldg(x + i);
+    const unsigned u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const unsigned lo = u[k] & 0xFFFFu, hi = u[k] >> 16;
+      m = max(m, (lo & 0x8000u) ? 0u : lo);
+      m = max(m, (hi & 0x8000u) ? 0u : hi);
+    }
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < 8; ++i) m = max(m, s_max[i]);
+    const float f = __half2float(__ushort_as_half((unsigned short)m));
+    atomicMax(amax_bits, __float_as_uint(f));
+  }
+}
+
+cudaError_t launch_amax_f16(const void* x, long long n, unsigned* amax_bits, cudaStream_t stream) {
+  if (n % 8 || reinterpret_cast<uintptr_t>(x) % 16) return cudaErrorInvalidValue;
+  const long long n8 = n / 8;
+  if (n8 == 0) return cudaSuccess;
+  long long blocks = (n8 + 255) / 256;
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  amax_f16_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), n8, amax_bits);
+  return cudaGetLastError();
+}
+
 __global__ void bn_fold_kernel(const float* __restrict__ gamma, const float* __restrict__ beta,
                                const float* __restrict__ mean, const float* __restrict__ var,
                                float eps, float* __restrict__ scale, float* __restrict__ shift,

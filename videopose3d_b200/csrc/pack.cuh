@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <stdint.h>
 
 namespace vp3d {
 
@@ -65,6 +66,21 @@ cudaError_t launch_pack_input(const float* x, __nv_bfloat16* out, int planes, in
 cudaError_t launch_pack_conv_weight(const float* w, __nv_bfloat16* out, int planes, int c_out,
                                     int c_in, int taps, int n_pad, int k_pad, int merge_taps,
                                     cudaStream_t stream, int f16 = 0);
+
+// int8 eval weights, per output channel co (fp32 throughout, IEEE division and rint):
+//   w_scale[co] = max_{ci, tap} |w[co][ci][tap]| / 127   (1 for an all-zero or padding channel)
+//   out[tap][co][ci] = clamp(rint(w[co][ci][tap] / w_scale[co]), -127, 127)   (s8, zero padded)
+// out: s8 [taps][n_pad][k_pad]; w_scale: [n_pad].
+cudaError_t launch_pack_conv_weight_s8(const float* w, int8_t* out, float* w_scale, int c_out,
+                                       int c_in, int taps, int n_pad, int k_pad,
+                                       cudaStream_t stream);
+// The int8 dequantisation folded into the eval affine: q_scale[c] = bn_scale[c] * (w_scale[c] * s_in)
+// (two fp32 roundings in this order), c < n.
+cudaError_t launch_int8_fold(const float* bn_scale, const float* w_scale, float s_in, float* q_scale,
+                             int n, cudaStream_t stream);
+// amax_bits = max(amax_bits, fp32 bits of max(x)) over n fp16 values >= 0 (n % 8 == 0, x 16-byte
+// aligned; -0 counts as 0), one integer atomicMax per block.
+cudaError_t launch_amax_f16(const void* x, long long n, unsigned* amax_bits, cudaStream_t stream);
 
 // Eval-mode BatchNorm1d (model.py:32,117,119; eps = 1e-5) as y = x*scale + shift.
 // gamma/beta/mean/var: [c]; scale/shift: [c_pad] (padding: scale 0, shift 0).  mean_out /

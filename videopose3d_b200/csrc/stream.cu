@@ -531,6 +531,8 @@ static int stream_supported(const vp3d_plan* p, const char* what) {
                 what);
   if (p->cfg.precision == VP3D_PRECISION_MIXED)
     return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'mixed' is not supported for streaming", what);
+  if (p->cfg.precision == VP3D_PRECISION_INT8)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'int8' is not supported for streaming", what);
   return VP3D_OK;
 }
 

@@ -248,6 +248,10 @@ class StreamingSession:
             raise NotImplementedError(
                 "precision 'mixed' cannot stream: its per-layer split choice depends on the "
                 "sequence length; use 'fp16', 'bf16' or 'bf16x3'")
+        if model.precision == "int8":
+            raise NotImplementedError(
+                "precision 'int8' cannot stream (the offline eval forward only); use 'fp16', "
+                "'bf16' or 'bf16x3'")
         if model.training:
             raise RuntimeError("streaming is an eval-mode computation: call model.eval() first")
         streams, max_frames = int(streams), int(max_frames)

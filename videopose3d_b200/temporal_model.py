@@ -19,7 +19,8 @@ import torch.nn as nn
 from . import _capi
 
 _PRECISIONS = {"bf16": _capi.VP3D_PRECISION_BF16, "bf16x3": _capi.VP3D_PRECISION_BF16X3,
-               "mixed": _capi.VP3D_PRECISION_MIXED, "fp16": _capi.VP3D_PRECISION_FP16}
+               "mixed": _capi.VP3D_PRECISION_MIXED, "fp16": _capi.VP3D_PRECISION_FP16,
+               "int8": _capi.VP3D_PRECISION_INT8}
 
 
 # id(parameter) -> weakref(owning model): lets optim.FusedAdam find the model whose packed bf16
@@ -43,14 +44,17 @@ class _Plan:
     VP3D_PACK_BN_EVAL), ``train`` (VP3D_PACK_CONV | VP3D_PACK_CONV_T) and ``expand_t``
     (VP3D_PACK_EXPAND_T, the expand conv weight's entry only).  ``bn_sync`` is (reducer, ctypes
     exchange callback) while the plan's synchronized BatchNorm is on (vp3d_set_bn_sync): the plan
-    holds the callback as long as it may call it."""
+    holds the callback as long as it may call it.  ``int8`` is the calibration (the module's
+    ``_int8`` tuple) whose scales an int8 plan holds, None before any."""
 
-    __slots__ = ("handle", "eval", "train", "expand_t", "bn_sync")
+    __slots__ = ("handle", "precision", "eval", "train", "expand_t", "bn_sync", "int8")
 
-    def __init__(self, handle):
+    def __init__(self, handle, precision):
         self.handle = handle
+        self.precision = precision
         self.eval = self.train = self.expand_t = None
         self.bn_sync = None
+        self.int8 = None
 
     @property
     def _as_parameter_(self):
@@ -74,7 +78,7 @@ class _EngineState:
         self._finalizer = weakref.finalize(self, _EngineState._destroy, self._handles)
 
     def add(self, key, handle):
-        self.plans[key] = plan = _Plan(handle)
+        self.plans[key] = plan = _Plan(handle, key[1])
         self._handles.append(handle)
         return plan
 
@@ -145,6 +149,8 @@ class TemporalModelBase(nn.Module):
         self._stats_epoch = 0      # bumped by every training forward (running stats changed)
         self._fwd_token = 0        # identifies the most recent training forward
         self._grad_reducer = None  # data_parallel.GradientReducer, set by its attach()
+        # int8 calibration: (amax CPU float tensor [2B], parameter versions it belongs to), or None
+        self._int8 = None
 
     def _build_layers(self, strided):
         """Create the parameter containers with the reference's names, shapes and default init.
@@ -223,8 +229,12 @@ class TemporalModelBase(nn.Module):
         """Eval-mode operand format.  'fp16' (default): IEEE fp16 operands and activations, fp32
         accumulate -- ~4e-4 of the fp32 reference at the tensor rate of bf16; 'bf16x3': every GEMM
         split-bf16 (fp32-faithful, ~1e-5); 'mixed': bf16 residual blocks on a hi+lo residual
-        stream, split-bf16 expand / shrink (~1e-3); 'bf16': every GEMM plain bf16 (~3e-3).  Not in
-        the reference."""
+        stream, split-bf16 expand / shrink (~1e-3); 'bf16': every GEMM plain bf16 (~3e-3);
+        'int8': the residual blocks' convs on u8 activations times s8 weights (exact int32 sums),
+        the rest as 'fp16' -- about 0.73x the fp16 forward time on the bench model (H100), at
+        ~5e-3 of fp32 on a random-init model (ten times fp16's error; trained checkpoints not
+        measured).  Needs ``calibrate_int8`` or ``load_int8_calibration`` first.  Not in the
+        reference."""
         if precision not in _PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(_PRECISIONS)}")
         self._precision = precision
@@ -241,7 +251,88 @@ class TemporalModelBase(nn.Module):
         automatically through ``tensor._version``.  Not in the reference."""
         for plan in self._engine.plans.values():
             plan.eval = plan.train = plan.expand_t = None
+        if self._int8 is not None:
+            self._int8 = (self._int8[0], None)   # stale: recalibrate or load a calibration
         return self
+
+    # ------------------------------------------------------------------ int8 calibration
+    def calibrate_int8(self, inputs):
+        """Measure the activation ranges of the 'int8' eval mode: runs the fp16 eval forward
+        (without shrink) on `inputs` -- one CUDA float32 (N, T, J, F) tensor, a list of them, or an
+        ``UnchunkedGenerator`` on the device (every batch of one epoch) -- and keeps, for every
+        residual-block conv, the maximum of its input over all of them.  Recorded with the current
+        parameter versions: after any parameter change an int8 forward raises until the model is
+        recalibrated or a calibration is loaded.  Not in the reference."""
+        if hasattr(inputs, "next_epoch"):
+            inputs = [batch[-1] for batch in inputs.next_epoch()]
+        elif torch.is_tensor(inputs):
+            inputs = [inputs]
+        inputs = list(inputs)
+        if not inputs:
+            raise ValueError("calibrate_int8 needs at least one input batch")
+        lib = _capi.load()
+        device = self.expand_conv.weight.device
+        if device.type != "cuda":
+            raise RuntimeError("module parameters must be on a CUDA device")
+        amax = torch.zeros(len(self.layers_conv), dtype=torch.float32, device=device)
+        with torch.cuda.device(device):
+            plan = self._get_plan(device, "fp16")
+            stream = torch.cuda.current_stream(device).cuda_stream
+            self._sync_weights(plan, stream)
+            for x in inputs:
+                if not (torch.is_tensor(x) and x.is_cuda and x.device == device
+                        and x.dtype == torch.float32 and x.dim() == 4
+                        and x.shape[-2] == self.num_joints_in and x.shape[-1] == self.in_features):
+                    raise ValueError("calibrate_int8 takes CUDA float32 (N, T, J, F) tensors on the "
+                                     "model's device")
+                x = x.contiguous()
+                N, T = int(x.shape[0]), int(x.shape[1])
+                nbytes = lib.vp3d_workspace_bytes(plan, N, T)
+                if nbytes == 0:
+                    raise ValueError(f"input of {T} frames is shorter than the receptive field "
+                                     f"({self.receptive_field()})")
+                ws = self._get_workspace(nbytes, device)
+                _capi.check(lib.vp3d_calibrate_int8(plan, x.data_ptr(), N, T, ws.data_ptr(),
+                                                    ws.numel(), amax.data_ptr(), stream),
+                            "vp3d_calibrate_int8")
+        self._int8 = (amax.cpu(), self._versions())
+        return self
+
+    def int8_calibration(self):
+        """The activation maxima of the last calibration as a CPU float32 tensor of 2B values
+        (block i's first-conv input, then its 1x1-conv input, for i = 1..B); None before any.  Kept
+        out of the state_dict: checkpoints keep the reference's layout.  Not in the reference."""
+        return None if self._int8 is None else self._int8[0].clone()
+
+    def load_int8_calibration(self, amax):
+        """Use a calibration saved with ``int8_calibration`` for the current parameters.  Not in the
+        reference."""
+        amax = torch.as_tensor(amax, dtype=torch.float32).detach().cpu().contiguous()
+        if amax.shape != (len(self.layers_conv),):
+            raise ValueError(f"expected {len(self.layers_conv)} amax values, got shape "
+                             f"{tuple(amax.shape)}")
+        if not bool(torch.isfinite(amax).all()) or bool((amax < 0).any()):
+            raise ValueError("amax values must be finite and >= 0")
+        self._int8 = (amax.clone(), self._versions())
+        return self
+
+    def _sync_int8(self, plan):
+        """Give an int8 plan the scales of the current calibration (its next weight sync folds
+        them); raises when there is none or the parameters changed since it was taken."""
+        if self._int8 is None:
+            raise RuntimeError("precision 'int8' needs calibrate_int8(inputs) or "
+                               "load_int8_calibration(amax) first")
+        amax, versions = self._int8
+        if versions != self._versions():
+            raise RuntimeError("the int8 calibration is stale: the parameters changed since it was "
+                               "taken; call calibrate_int8 again or load_int8_calibration")
+        if plan.int8 is self._int8:
+            return
+        vals = (_capi.ctypes.c_float * amax.numel())(*amax.tolist())
+        _capi.check(_capi.load().vp3d_set_int8_scales(plan, vals, amax.numel()),
+                    "vp3d_set_int8_scales")
+        plan.eval = None   # the next sync re-packs and folds the scales in
+        plan.int8 = self._int8
 
     # copies / replicas never share engine state with the original (the handles point into one
     # device allocation each; sharing them made a collected copy free the original's plans)
@@ -360,6 +451,8 @@ class TemporalModelBase(nn.Module):
     def _sync_weights(self, plan, stream, training=False):
         """Re-pack whatever changed since `plan`'s eval (or training) packs last saw the parameters
         (optimizer.step, load_state_dict, in-place edits).  Returns whether it packed."""
+        if not training and plan.precision == "int8":
+            self._sync_int8(plan)
         versions = self._versions()
         seen = plan.train if training else plan.eval
         what = 0
