@@ -277,3 +277,52 @@ def test_training_operator_entries_validate_before_launching():
                              0, None) == -1            # channels not a multiple of 64
     assert lib.vp3d_bn_bwd_apply(fake, 0, fake, 0, fake, 0, 1, 10, 64, fake, fake, None, None, 0.0,
                                  0, 0, None, None, None, 64, 0, None) == -1   # sums needed unless frozen
+
+
+@pytest.mark.parametrize("precision,changes,code,word", [
+    # fp16 (and int8, whose residual and 16-bit output are fp16): one plane, inference only
+    ("fp16", dict(a_planes=2), -1, b"single-plane"),
+    ("fp16", dict(out_planes=2), -1, b"single-plane"),
+    ("fp16", dict(stats=1 << 20), -1, b"inference-only"),
+    ("int8", dict(bnb_z=1 << 20), -1, b"inference-only"),
+    # int8 k-blocks are 128 one-byte elements, and taps step rows
+    ("int8", dict(k_per_tap=64), -1, b"k_per_tap"),
+    ("int8", dict(tap_col_step=128), -1, b"tap_col_step"),
+    # a u8 output: fp16 or int8, 16-byte aligned rows covering n_pad
+    ("bf16", dict(res=None, out_u8=1 << 20), -1, b"u8 output"),
+    ("int8", dict(out_u8_ld=48), -1, b"out_u8_ld"),
+    ("int8", dict(out_u8_ld=72), -1, b"out_u8_ld"),
+    ("int8", dict(out_u8=(1 << 20) + 8), -1, b"aligned"),
+    # int8 / u8 launches are affine + ReLU [+ a one-plane residual over every column]
+    ("int8", dict(relu=0), -2, b"affine + ReLU"),
+    ("int8", dict(shift=None), -2, b"affine + ReLU"),
+    ("int8", dict(out_f32=1 << 20), -2, b"affine + ReLU"),
+    ("int8", dict(res_col_begin=64), -2, b"every column"),
+    ("int8", dict(res_cols=64), -2, b"every column"),
+    ("int8", dict(res_planes=2), -2, b"one-plane residual"),
+    # int8 writes u8 alone, or with a residual fp16 [+ u8]; fp16 + u8 has no residual
+    ("int8", dict(out=None), -2, b"with a residual, fp16"),
+    ("int8", dict(res=None), -2, b"int8 writes u8 alone"),
+    ("int8", dict(res=None, out_u8=None), -2, b"int8 writes u8 alone"),
+    ("fp16", dict(), -2, b"without a residual"),
+    ("fp16", dict(res=None, out=None), -2, b"fp16 without a residual writes fp16 + u8"),
+])
+def test_conv_gemm_rejects_unsupported_int8_u8_fp16_launches(precision, changes, code, word):
+    """vp3d_conv_gemm checks every int8 / u8 / fp16 condition before touching a device (the pointers
+    below are never dereferenced)."""
+    ct = _capi.ctypes
+    lib = _capi.load()
+    fake = 1 << 20
+    d = _capi.ConvDesc()
+    d.a = d.w = d.scale = d.shift = d.res = d.out = d.out_u8 = fake
+    d.samples, d.a_rows, d.a_ld, d.taps, d.k_per_tap, d.n_pad = 1, 130, 128, 3, 128, 128
+    d.per_sample_tiles, d.tap_row_step, d.out_rows = 1, 1, 128
+    d.precision = {"bf16": 0, "fp16": 3, "int8": 4}[precision]
+    d.relu = 1
+    d.res_ld = d.out_ld = d.out_u8_ld = 128
+    d.res_rows_per_sample, d.res_row_step, d.res_row_off = 130, 1, 1
+    for k, v in changes.items():
+        assert k in dict(d._fields_)
+        setattr(d, k, v)
+    assert lib.vp3d_conv_gemm(ct.byref(d), None) == code
+    assert word in lib.vp3d_last_error()

@@ -46,11 +46,11 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 4-D bf16 map (k, row, sample, plane), box (64, box_rows, 1, 1), 128-byte swizzle.
 namespace vp3d {
 int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows,
                        uint64_t row_stride, uint64_t samples, uint64_t sample_stride,
-                       uint64_t planes, uint64_t plane_stride, uint32_t box_rows, int elem_bytes) {
+                       uint64_t planes, uint64_t plane_stride, uint32_t box_rows, int elem_bytes,
+                       uint32_t box_bytes, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   const uint64_t eb = (uint64_t)elem_bytes;
@@ -59,10 +59,10 @@ int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows,
     return fail(VP3D_ERR_INVALID, "tensor map operand not 16-byte aligned");
   cuuint64_t dims[4] = {inner, rows, samples, planes};
   cuuint64_t strides[3] = {row_stride * eb, sample_stride * eb, plane_stride * eb};
-  cuuint32_t box[4] = {(cuuint32_t)(elem_bytes == 1 ? kBlockK8 : kBlockK), box_rows, 1, 1};
+  cuuint32_t box[4] = {box_bytes / (cuuint32_t)elem_bytes, box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(m, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides,
-                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(VP3D_ERR_CUDA,
@@ -141,11 +141,11 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
                 "pointer and out_u8_ld >= n_pad, a multiple of 16");
   if ((i8 || d->out_u8) &&
       (!d->scale || !d->shift || !d->relu || d->out_f32 || d->res_col_begin || d->res_cols ||
-       (i8 && d->res && !d->out) || (i8 && !d->res && (d->out || !d->out_u8)) ||
-       (!i8 && (!d->out || d->res))))
+       (d->res && d->res_planes > 1) || (i8 && d->res && !d->out) ||
+       (i8 && !d->res && (d->out || !d->out_u8)) || (!i8 && (!d->out || d->res))))
     return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm: int8 and u8 outputs exist for affine + ReLU "
-                "[+ residual] launches: int8 writes u8 alone or, with a residual, fp16 [+ u8]; fp16 "
-                "without a residual writes fp16 + u8");
+                "[+ one-plane residual over every column] launches: int8 writes u8 alone or, with a "
+                "residual, fp16 [+ u8]; fp16 without a residual writes fp16 + u8");
   if (pairs == 3 && a_planes != 2)
     return fail(VP3D_ERR_INVALID, "conv_gemm: bf16x3 needs hi/lo planes of A");
   const int w_planes = pairs == 3 ? 2 : 1;
@@ -287,19 +287,12 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
     g.bnb_layer = (unsigned)d->bnb_layer;
   }
   if (d->out_u8) {
-    // the u8 output rides the auxiliary map slot (u8 launches have no BatchNorm-backward Z)
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
+    // the u8 output rides the auxiliary map slot (u8 launches have no BatchNorm-backward Z):
+    // 64 x 32 byte boxes, unswizzled like the kernel's u8 staging tiles
     const uint64_t rows = d->out_rows, ld = d->out_u8_ld;
     const uint64_t smp = d->per_sample_tiles ? d->samples : 1;
-    cuuint64_t dims[4] = {(cuuint64_t)d->n_pad, rows, smp, 1};
-    cuuint64_t strides[3] = {ld, rows * ld, smp * rows * ld};
-    cuuint32_t box[4] = {64, 32, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = enc(&mz, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, d->out_u8, dims, strides, box,
-                           estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(VP3D_ERR_CUDA, "cuTensorMapEncodeTiled(u8 out) failed: %d", (int)r);
+    VP3D_TRY(make_map_4d(&mz, d->out_u8, d->n_pad, rows, ld, smp, rows * ld, 1, smp * rows * ld, 32,
+                         1, 64, CU_TENSOR_MAP_SWIZZLE_NONE));
   }
   if ((i8 || d->out_u8) && d->res && !g.res_tma)
     return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm: int8 / u8-output launches need a residual that "

@@ -2,7 +2,7 @@
 //
 // CTA = 384 threads (three warpgroups), persistent over output tiles (128 rows x BLOCK_N channels):
 //   warp 0 lane 0 : TMA producer  (A tile 128x64 + W tile BLOCK_Nx64 16-bit per k-block)
-//   warp 1 lane 0 : auxiliary producer (RES variant): TMA-loads the 128x64 residual tile(s) / the Z
+//   warp 1 lane 0 : auxiliary producer (residual instances): TMA-loads the 128x64 residual tile(s) / the Z
 //                   tile of every 64-column store block into shared memory ahead of the epilogue
 //   warps 4..11   : two consumer warpgroups; warpgroup g owns rows [64 g, 64 g + 64) of every tile.
 //                   Each issues the m64 x BLOCK_N x k16 wgmma stream of its rows (fp32 accumulators
@@ -15,8 +15,8 @@
 // Lean inference launches with more tiles than CTAs use the ping-pong instances instead: each
 // consumer warpgroup computes all 128 rows of every other tile, so that one warpgroup's epilogue
 // runs under the other's MMAs.
-// The int8 eval instances (I8) run the same pipeline on u8 A / s8 W tiles of 128 x 128 bytes per
-// k-block (int32 accumulators, k32 MMAs), and may store a u8 copy of their output (U8).
+// The int8 eval instances run the same pipeline on u8 A / s8 W tiles of 128 x 128 bytes per
+// k-block (int32 accumulators, k32 MMAs), and may store a u8 copy of their output.
 #include "conv_gemm.cuh"
 
 #include <stdlib.h>
@@ -28,17 +28,63 @@
 
 namespace vp3d {
 
-// OUT2: two output planes (hi, lo) -> two staging planes per buffer.
-// LEAN (inference layers: affine + ReLU [+ one-plane TMA residual] -> one 16-bit plane): the same
-// epilogue with every option resolved at compile time.
-// PP (lean only): ping-pong schedule, each consumer warpgroup computes whole tiles (see the kernel).
-// U8 == 1: a u8 copy next to the 16-bit plane gets staging tiles of its own (U8 == 2 stages its
-// u8 tiles in the unused 16-bit staging).
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool PP = false, int U8 = 0>
-struct GemmCfg {
-  static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma tiles are 64 or 128 columns wide");
-  static_assert(!(LEAN && (OUT2 || TRAIN)), "the lean epilogue is inference-only, one plane");
-  static_assert(LEAN || !PP, "only the lean instances run the ping-pong schedule");
+// What a kernel instance fixes at compile time.
+// Epilogue: kTrain compiles in the training-only paths (BatchNorm batch statistics of the stored
+// value, fused BatchNorm-backward reductions); kGeneral reads every option from ConvGemmArgs;
+// kLean serves the inference layers, exactly affine + ReLU [+ a one-plane TMA residual over every
+// column] into one 16-bit plane [+ its u8 copy], with every option resolved at compile time.
+enum class Epi { kTrain, kGeneral, kLean };
+// Operand / storage format: the lean instances fix it (so that each k-block is one branch-free
+// group of wgmma), the others read p.f16.  kI8: u8 A times s8 W into int32 accumulators,
+// 128-element k-blocks; the residual and the 16-bit output stay fp16.
+enum class Fmt { kRuntime, kBf16, kF16, kI8 };
+// kPingPong: each consumer warpgroup computes whole tiles (see the kernel's consumer branches).
+enum class Sched { kCooperative, kPingPong };
+// u8 quantisation of every stored value (ConvGemmArgs::out_u8): beside the 16-bit plane, with
+// staging tiles of its own, or alone (no 16-bit output; staged in the unused 16-bit staging).
+enum class U8Out { kNone, kBeside, kAlone };
+
+struct InstKey {
+  int block_n;
+  Epi epi;
+  Fmt fmt;
+  Sched sched;
+  bool res;    // auxiliary TMA tiles: the residual and / or the BatchNorm-backward Z
+  bool out2;   // two output planes (hi, lo) -> two staging planes per buffer
+  U8Out u8;
+  constexpr bool operator==(const InstKey& o) const {
+    return block_n == o.block_n && epi == o.epi && fmt == o.fmt && sched == o.sched &&
+           res == o.res && out2 == o.out2 && u8 == o.u8;
+  }
+};
+
+// One kernel instance: its compile-time options and its shared-memory layout.
+template <int BLOCK_N, Epi EPI, Fmt FMT, Sched SCHED, bool RES, bool OUT2 = false,
+          U8Out U8 = U8Out::kNone>
+struct Inst {
+  static_assert((BLOCK_N == 64 || BLOCK_N == 128) &&             // wgmma tiles are 64 or 128 wide
+                    (EPI == Epi::kLean) == (FMT != Fmt::kRuntime) &&
+                    !(EPI == Epi::kLean && OUT2) &&                 // lean: one output plane
+                    (SCHED == Sched::kCooperative || EPI == Epi::kLean) &&
+                    (U8 == U8Out::kNone || FMT == Fmt::kF16 || FMT == Fmt::kI8) &&
+                    !(RES && U8 == U8Out::kAlone),                  // a residual stores 16 bits
+                "not a conv GEMM instance");
+  static constexpr InstKey kKey = {BLOCK_N, EPI, FMT, SCHED, RES, OUT2, U8};
+  static constexpr int kBlockN = BLOCK_N;
+  static constexpr Fmt kFmt = FMT;
+  static constexpr bool kTrain = EPI == Epi::kTrain;
+  static constexpr bool kLean = EPI == Epi::kLean;
+  static constexpr bool kF16 = FMT == Fmt::kF16 || FMT == Fmt::kI8;
+  static constexpr bool kI8 = FMT == Fmt::kI8;
+  static constexpr bool kPP = SCHED == Sched::kPingPong;
+  static constexpr bool kRes = RES;
+  static constexpr bool kOut2 = OUT2;
+  static constexpr bool kU8 = U8 != U8Out::kNone;
+  static constexpr bool kU8Beside = U8 == U8Out::kBeside;
+  static constexpr bool kU8Alone = U8 == U8Out::kAlone;
+  static constexpr bool kStore16 = !kU8Alone;
+  using Acc = std::conditional_t<kI8, int, float>;
+
   static constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
   static constexpr uint32_t kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
@@ -47,20 +93,20 @@ struct GemmCfg {
   // staging: 2 warpgroups x 2 alternating buffers x (hi[, lo]).  Ping-pong: one 128 x 64 tile per
   // warpgroup; the residual instance stores in place from the residual's landing tile instead.
   static constexpr uint32_t kStagingBytes =
-      PP ? (RES ? 0 : 2 * kTileBytes) : 2 * 2 * (OUT2 ? 2 : 1) * kHalfBytes;
+      kPP ? (RES ? 0 : 2 * kTileBytes) : 2 * 2 * (OUT2 ? 2 : 1) * kHalfBytes;
   // auxiliary (residual / Z) landing tiles: four, so that two-tile store blocks (hi+lo residual,
   // or residual + Z) still get two stages in flight.  Ping-pong: two per warpgroup.
   static constexpr int kResSlots = RES ? 4 : 0;
   // u8 staging (64 columns of 64 bytes per row): ping-pong one 128-row tile per warpgroup,
   // cooperative two alternating 64-row halves per warpgroup -- 16 KiB either way
-  static constexpr uint32_t kU8Bytes = U8 == 1 ? 2 * kBlockM * 64 : 0;
+  static constexpr uint32_t kU8Bytes = kU8Beside ? 2 * kBlockM * 64 : 0;
   static constexpr uint32_t kFixedBytes = kStagingBytes + kResSlots * kTileBytes + kU8Bytes;
   // per-channel affine (scale, shift) of the current N block: 2 x BLOCK_N floats.  Ping-pong reads
   // it through L1 instead: the two warpgroups may hold different N blocks, and a copy per
   // warpgroup would cost the 128-wide instance an operand stage.
-  static constexpr uint32_t kAffineBytes = PP ? 0 : 2 * BLOCK_N * 4;
+  static constexpr uint32_t kAffineBytes = kPP ? 0 : 2 * BLOCK_N * 4;
   // training: per-column (sum, sumsq) of one warp of every 32-row slab pair, 4 slabs x 2 x 64
-  static constexpr uint32_t kPairBytes = TRAIN ? 4 * 2 * 64 * 4 : 0;
+  static constexpr uint32_t kPairBytes = kTrain ? 4 * 2 * 64 * 4 : 0;
   static constexpr uint32_t kBarBytesMax = (2 * 8 + 8 + 1) * 8 + 32;
   // as many operand stages as fit into the 227 KiB a CTA may use (less 1 KiB of alignment slack),
   // at most 8
@@ -103,37 +149,6 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int c) {
 __device__ __forceinline__ void add_pair(float& a, float& b, uint32_t u, bool f16) {
   if (f16) { a += f16_lo_to_f(u); b += f16_hi_to_f(u); }
   else { a += bf16_lo_to_f(u); b += bf16_hi_to_f(u); }
-}
-
-// one 64-deep k-block: four k16 steps (16 elements = 32 B along K inside the 128 B swizzle row:
-// +2 in the descriptor's address >> 4)
-template <int BLOCK_N, bool F16>
-__device__ __forceinline__ void wgmma_kblock(float (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db,
-                                             bool first) {
-#pragma unroll
-  for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-    const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
-    if constexpr (BLOCK_N == 128) {
-      if constexpr (F16) wgmma_m64n128_f16(acc, da + 2 * k, db + 2 * k, accumulate);
-      else wgmma_m64n128_bf16(acc, da + 2 * k, db + 2 * k, accumulate);
-    } else {
-      if constexpr (F16) wgmma_m64n64_f16(acc, da + 2 * k, db + 2 * k, accumulate);
-      else wgmma_m64n64_bf16(acc, da + 2 * k, db + 2 * k, accumulate);
-    }
-  }
-}
-
-// one k-block of u8 x s8: the same 128-byte swizzle row holds 128 elements, four k32 steps of 32 B
-// (the same +2 descriptor advance per step as the 16-bit k16 steps)
-template <int BLOCK_N>
-__device__ __forceinline__ void wgmma_kblock_i8(int (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db,
-                                                bool first) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
-    if constexpr (BLOCK_N == 128) wgmma_m64n128k32_u8s8(acc, da + 2 * k, db + 2 * k, accumulate);
-    else wgmma_m64n64k32_u8s8(acc, da + 2 * k, db + 2 * k, accumulate);
-  }
 }
 
 // the u8 pair (columns c, c + 1) at byte `off` of a u8 staging tile (rows of 64 bytes, no swizzle)
@@ -197,34 +212,94 @@ __device__ __forceinline__ void tl_stamp(const ConvGemmArgs& p, int ev) {
 #define TL(ev) ((void)0)
 #endif
 
-// TRAIN compiles in the training-only epilogue paths (BatchNorm batch statistics of the stored
-// value, fused BatchNorm-backward reductions); eval launches use the leaner TRAIN = false build.
-// F16 (LEAN only): the operand / storage format at compile time (fp16, else bf16), so that each
-// k-block is one branch-free group of wgmma; the other instances read it from p.f16.
-// PP (LEAN only): the ping-pong schedule for launches where CTAs get more than one tile (see the
-// consumer branches below); the cooperative schedule otherwise.
-// I8 (LEAN + F16 only): u8 A times s8 W into int32 accumulators, 128-element k-blocks; the
-// residual and the 16-bit output stay fp16.
-// U8 (LEAN only): 1 = also store the u8 quantisation of every stored value (ConvGemmArgs::out_u8),
-// 2 = store only that u8 plane (no 16-bit output, no staging).
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN, bool F16 = false, bool PP = false,
-          bool I8 = false, int U8 = 0>
+// One k-block (one 128-byte swizzle row of K) of m64 x BLOCK_N MMAs into each of the H accumulator
+// halves in turn, half h reading the A rows of descriptor da[h]: four k16 steps of 16 elements, or
+// for int8 (u8 x s8) four k32 steps of 32 elements -- 32 B each, +2 in the descriptors' address >> 4.
+template <int BLOCK_N, Fmt FMT, int H, class Acc>
+__device__ __forceinline__ void wgmma_kblock(Acc (&acc)[H][BLOCK_N / 2], const uint64_t (&da)[H],
+                                             uint64_t db, bool first) {
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
+      if constexpr (FMT == Fmt::kI8) {
+        if constexpr (BLOCK_N == 128) wgmma_m64n128k32_u8s8(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n64k32_u8s8(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+      } else if constexpr (BLOCK_N == 128) {
+        if constexpr (FMT == Fmt::kF16) wgmma_m64n128_f16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n128_bf16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+      } else {
+        if constexpr (FMT == Fmt::kF16) wgmma_m64n64_f16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n64_bf16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+      }
+    }
+  }
+}
+
+// The MMA main loop of one tile, over H 64-row halves of every A stage from byte a_off on (the
+// cooperative schedule: H = 1, this warpgroup's rows; ping-pong: H = 2, the whole tile).  The tile's
+// first k-block sits in pipeline stage `stage` of parity `phase`; both are left at the next fill.
+// Each k-block is one wgmma group; a stage is released once wait_group 1 shows the group reading it
+// has retired.  `issued()` runs after the last group is issued, before the wait for it.
+// The runtime format test of the general instances stays outside the k16 steps: a branch inside a
+// group makes ptxas close it with an extra null HGMMA (DESIGN.md section 4).
+template <class I, int H, class Issued>
+__device__ __forceinline__ void mma_tile(typename I::Acc (&acc)[H][I::kBlockN / 2],
+                                         const ConvGemmArgs& p, bool f16, uint32_t smem_a,
+                                         uint32_t a_off, uint32_t smem_b, uint32_t full_bar,
+                                         uint32_t empty_bar, uint32_t& stage_io, uint32_t& phase_io,
+                                         int k_iters, int lane, bool tl_first, Issued issued) {
+  uint32_t stage = stage_io, phase = phase_io;
+  uint32_t prev_stage = 0;
+  for (int it = 0; it < k_iters; ++it) {
+    mbar_wait(full_bar + stage * 8, phase);
+#ifdef VP3D_TIMELINE
+    if (tl_first && it == 0) TL(4);
+#endif
+    const uint32_t a_st = smem_a + stage * I::kABytes + a_off;
+    uint64_t da[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) da[h] = make_gmma_desc_sw128(a_st + h * 64 * 128, 16, 1024);
+    const uint64_t db = make_gmma_desc_sw128(smem_b + stage * I::kBBytes, 16, 1024);
+#pragma unroll
+    for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
+    wgmma_fence();
+    if constexpr (I::kFmt != Fmt::kRuntime) wgmma_kblock<I::kBlockN, I::kFmt>(acc, da, db, it == 0);
+    else if (f16) wgmma_kblock<I::kBlockN, Fmt::kF16>(acc, da, db, it == 0);
+    else wgmma_kblock<I::kBlockN, Fmt::kBf16>(acc, da, db, it == 0);
+    wgmma_commit();
+#pragma unroll
+    for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
+    if (it > 0) {
+      // the previous k-block's MMAs have retired: its stage may be refilled
+      wgmma_wait<1>();
+#pragma unroll
+      for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
+      if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+    }
+    prev_stage = stage;
+    if (++stage == I::kStages) { stage = 0; phase ^= 1; }
+  }
+  stage_io = stage; phase_io = phase;
+  issued();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
+  if (k_iters > 0 && lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+}
+
+template <class I>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ CUtensorMap tmap_out,
                  const __grid_constant__ CUtensorMap tmap_res,
                  const __grid_constant__ CUtensorMap tmap_z, const ConvGemmArgs p) {
-  static_assert(LEAN || !F16, "only the lean instances fix the operand format at compile time");
-  static_assert((!I8 && U8 == 0) || (LEAN && F16), "int8 and u8 outputs are lean fp16 instances");
-  static_assert(!(RES && U8 == 2), "a residual instance stores its 16-bit plane");
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP, U8>;
-  using Acc = std::conditional_t<I8, int, float>;
-  constexpr int kStages = Cfg::kStages;
-  constexpr int kBlocksPerTile = BLOCK_N / 64;
-  constexpr int kFrag = BLOCK_N / 2;   // accumulator registers per consumer thread
-  constexpr int kBK = I8 ? kBlockK8 : kBlockK;   // elements per k-block (128 bytes either way)
-  constexpr bool kStore16 = U8 != 2;
+  using Acc = typename I::Acc;
+  constexpr int kBlocksPerTile = I::kBlockN / 64;
+  constexpr int kFrag = I::kBlockN / 2;   // accumulator registers per consumer thread
+  constexpr int kBK = I::kI8 ? kBlockK8 : kBlockK;   // elements per k-block (128 bytes either way)
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -232,19 +307,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   uint8_t* smem = smem_raw + (base - raw_addr);
 
   const uint32_t smem_a = base;
-  const uint32_t smem_b = base + kStages * Cfg::kABytes;
-  const uint32_t smem_store = base + kStages * Cfg::kStageBytes;
-  const uint32_t smem_res = smem_store + Cfg::kStagingBytes;
-  const uint32_t smem_u8 = smem_res + Cfg::kResSlots * Cfg::kTileBytes;   // (U8 == 1)
-  const uint32_t bar_base = smem_u8 + Cfg::kU8Bytes;
+  const uint32_t smem_b = base + I::kStages * I::kABytes;
+  const uint32_t smem_store = base + I::kStages * I::kStageBytes;
+  const uint32_t smem_res = smem_store + I::kStagingBytes;
+  const uint32_t smem_u8 = smem_res + I::kResSlots * I::kTileBytes;   // (u8 beside the 16-bit plane)
+  const uint32_t bar_base = smem_u8 + I::kU8Bytes;
   const uint32_t full_bar = bar_base;
-  const uint32_t empty_bar = bar_base + kStages * 8;
-  const uint32_t rfull_bar = bar_base + 2 * kStages * 8;   // up to 4 auxiliary stages
+  const uint32_t empty_bar = bar_base + I::kStages * 8;
+  const uint32_t rfull_bar = bar_base + 2 * I::kStages * 8;   // up to 4 auxiliary stages
   const uint32_t rempty_bar = rfull_bar + 32;
   const uint32_t dep_bar = rempty_bar + 32;     // "the dependency wait has returned" (see the producer)
-  const uint32_t affine_off = (dep_bar + 8 - base + 15u) & ~15u;   // [scale | shift][BLOCK_N]
+  const uint32_t affine_off = (dep_bar + 8 - base + 15u) & ~15u;   // [scale | shift][kBlockN]
   float* s_affine = reinterpret_cast<float*>(smem + affine_off);
-  float* s_pairs = reinterpret_cast<float*>(smem + affine_off + Cfg::kAffineBytes);
+  float* s_pairs = reinterpret_cast<float*>(smem + affine_off + I::kAffineBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -256,30 +331,30 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   // auxiliary tiles per 64-column store block: the residual plane(s) and, for the fused
   // BatchNorm-backward reductions, the Z tile.  kResSlots / tiles stages are in flight.
   const bool has_res = (p.flags & kEpiResidual) != 0;
-  const bool bnb = TRAIN && p.bnb != 0;
+  const bool bnb = I::kTrain && p.bnb != 0;
   const int aux_tiles = (has_res ? p.res_planes : 0) + (bnb ? 1 : 0);
   const int res_stages =
-      (aux_tiles > 0 && Cfg::kResSlots >= aux_tiles) ? Cfg::kResSlots / aux_tiles : 1;
+      (aux_tiles > 0 && I::kResSlots >= aux_tiles) ? I::kResSlots / aux_tiles : 1;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_out);
-    if (RES) tma_prefetch_desc(&tmap_res);
-    if (RES && bnb) tma_prefetch_desc(&tmap_z);
-    if (U8 != 0) tma_prefetch_desc(&tmap_z);
+    if (I::kRes) tma_prefetch_desc(&tmap_res);
+    if (I::kRes && bnb) tma_prefetch_desc(&tmap_z);
+    if (I::kU8) tma_prefetch_desc(&tmap_z);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) {
+    for (int s = 0; s < I::kStages; ++s) {
       mbar_init(full_bar + s * 8, 1);
       // lane 0 of each consumer warp that reads the stage: all 8, or the 4 of one ping-pong warpgroup
-      mbar_init(empty_bar + s * 8, PP ? 4 : 8);
+      mbar_init(empty_bar + s * 8, I::kPP ? 4 : 8);
     }
     for (int s = 0; s < 4; ++s) {
       mbar_init(rfull_bar + s * 8, 1);
       // every consumer thread reads its rows of the stage; ping-pong: the thread that issued the
       // stores from the tile, once they have read it
-      mbar_init(rempty_bar + s * 8, PP ? 1 : 256);
+      mbar_init(rempty_bar + s * 8, I::kPP ? 1 : 256);
     }
     mbar_init(dep_bar, 1);
     fence_mbar_init();
@@ -310,10 +385,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       // optimiser step, always at least one full kernel boundary (the input pack) before any conv
       // kernel of a forward, so they are safe to read while the previous layer is still running.
       // Training kernels keep the plain order (their weight packs change every step).
-      constexpr bool kEarlyW = !TRAIN;
+      constexpr bool kEarlyW = !I::kTrain;
       if (!kEarlyW) mbar_wait(dep_bar, 0);
       // mode 0: W only (before the wait), 1: the A tiles of those same stages, 2: steady state
-      const int n_pre = kEarlyW ? (k_iters < kStages ? k_iters : kStages) : 0;
+      const int n_pre = kEarlyW ? (k_iters < I::kStages ? k_iters : I::kStages) : 0;
       int mode = n_pre > 0 ? 0 : 2;
       if (kEarlyW && mode == 2) mbar_wait(dep_bar, 0);
       int w = blockIdx.x;
@@ -328,19 +403,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           const uint32_t fb = full_bar + stage * 8;
           if (mode != 1) {
             mbar_wait(empty_bar + stage * 8, phase ^ 1);
-            mbar_expect_tx(fb, Cfg::kStageBytes);
-            const int w_row = (w_plane * p.taps + tap) * p.n_pad + n_blk * BLOCK_N;
-            tma_load_2d(&tmap_w, fb, smem_b + stage * Cfg::kBBytes, kb * kBK, w_row);
+            mbar_expect_tx(fb, I::kStageBytes);
+            const int w_row = (w_plane * p.taps + tap) * p.n_pad + n_blk * I::kBlockN;
+            tma_load_2d(&tmap_w, fb, smem_b + stage * I::kBBytes, kb * kBK, w_row);
           }
           if (mode != 0) {
             const int a_row = row0 + tap * p.tap_row_step;
             const int a_col = tap * p.tap_col_step + kb * kBK;
-            tma_load_4d(&tmap_a, fb, smem_a + stage * Cfg::kABytes, a_col, a_row, sample, a_plane);
+            tma_load_4d(&tmap_a, fb, smem_a + stage * I::kABytes, a_col, a_row, sample, a_plane);
 #ifdef VP3D_TIMELINE
             if (w == (int)blockIdx.x && it == 0) TL(3);
 #endif
           }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          if (++stage == I::kStages) { stage = 0; phase ^= 1; }
           ++it;
           if (++kb == p.kblocks_per_tap) {
             kb = 0;
@@ -365,7 +440,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     }
   } else if (warp == 1) {
     // ------------------------------------------------------------ auxiliary-tile producer
-    if (PP && RES && lane == 0) {
+    if (I::kPP && I::kRes && lane == 0) {
       // ping-pong: the residual tiles in tile order; tile j goes to warpgroup j & 1, whose two
       // landing slots (2 g, 2 g + 1) form a ring of their own
       uint32_t filled[2] = {0u, 0u};   // residual tiles sent to warpgroup 0 / 1 so far
@@ -377,39 +452,39 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           const uint32_t n = g ? filled[1] : filled[0];
           const uint32_t slot = 2u * g + (n & 1u);
           mbar_wait(rempty_bar + slot * 8, ((n >> 1) & 1u) ^ 1u);
-          mbar_expect_tx(rfull_bar + slot * 8, Cfg::kTileBytes);
-          tma_load_4d(&tmap_res, rfull_bar + slot * 8, smem_res + slot * Cfg::kTileBytes,
-                      n_blk * BLOCK_N + sb * 64 + p.res_tma_col_off, row0 + p.res_tma_row_off,
+          mbar_expect_tx(rfull_bar + slot * 8, I::kTileBytes);
+          tma_load_4d(&tmap_res, rfull_bar + slot * 8, smem_res + slot * I::kTileBytes,
+                      n_blk * I::kBlockN + sb * 64 + p.res_tma_col_off, row0 + p.res_tma_row_off,
                       sample, 0);
           if (g) ++filled[1];
           else ++filled[0];
         }
       }
-    } else if (!PP && RES && lane == 0) {
+    } else if (!I::kPP && I::kRes && lane == 0) {
       uint32_t rs = 0, rphase = 0;
       for (int w = blockIdx.x; w < total_tiles; w += gridDim.x) {
         int n_blk, sample, row0;
         tile_coords(p, w, n_blk, sample, row0);
         for (int sb = 0; sb < kBlocksPerTile; ++sb) {
-          const int col = n_blk * BLOCK_N + sb * 64;
+          const int col = n_blk * I::kBlockN + sb * 64;
           const bool res_here = has_res && col >= p.res_col_begin && col < p.res_col_begin + p.res_cols;
           if (!res_here && !bnb) continue;
           const int n_res = res_here ? p.res_planes : 0;
           mbar_wait(rempty_bar + rs * 8, rphase ^ 1);
-          mbar_expect_tx(rfull_bar + rs * 8, (n_res + (bnb ? 1 : 0)) * Cfg::kTileBytes);
-          const uint32_t slot0 = smem_res + rs * aux_tiles * Cfg::kTileBytes;
+          mbar_expect_tx(rfull_bar + rs * 8, (n_res + (bnb ? 1 : 0)) * I::kTileBytes);
+          const uint32_t slot0 = smem_res + rs * aux_tiles * I::kTileBytes;
           for (int pl = 0; pl < n_res; ++pl)
-            tma_load_4d(&tmap_res, rfull_bar + rs * 8, slot0 + pl * Cfg::kTileBytes,
+            tma_load_4d(&tmap_res, rfull_bar + rs * 8, slot0 + pl * I::kTileBytes,
                         col - p.res_col_begin + p.res_tma_col_off, row0 + p.res_tma_row_off, sample,
                         pl);
           if (bnb)  // the Z tile always sits in the last slot of the stage
-            tma_load_4d(&tmap_z, rfull_bar + rs * 8, slot0 + (aux_tiles - 1) * Cfg::kTileBytes, col,
+            tma_load_4d(&tmap_z, rfull_bar + rs * 8, slot0 + (aux_tiles - 1) * I::kTileBytes, col,
                         row0, sample, 0);
           if (++rs == (uint32_t)res_stages) { rs = 0; rphase ^= 1; }
         }
       }
     }
-  } else if (PP && warp >= 4) {
+  } else if (I::kPP && warp >= 4) {
     // ------------------------------------------------------------ ping-pong MMA + lean epilogue
     // Warpgroup g computes all 128 rows of the CTA's tiles j = g, g + 2, ... (w = blockIdx.x +
     // j gridDim.x): per k16 step one m64 wgmma per 64-row half of the A stage, into acc[0] and
@@ -424,7 +499,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const int cq = 2 * (lane & 3);
     const uint32_t bar_wg = 2u + (uint32_t)wg;
     const uint32_t bar_mine = 8u + (uint32_t)wg, bar_other = 9u - (uint32_t)wg;
-    const uint32_t staging = smem_store + wg * Cfg::kTileBytes;   // (no-residual instance)
+    const uint32_t staging = smem_store + wg * I::kTileBytes;   // (no-residual instance)
     uint32_t res_seen = 0;            // residual tiles this warpgroup has received
     Acc acc[2][kFrag];
 #pragma unroll
@@ -436,62 +511,30 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
       // ---- main loop: k-block it of tile j sits in the producer's (j k_iters + it)-th fill
       const uint32_t fill = (uint32_t)j * (uint32_t)k_iters;
-      uint32_t stage = fill % kStages, phase = (fill / kStages) & 1u;
+      uint32_t stage = fill % I::kStages, phase = (fill / I::kStages) & 1u;
       if (j > 0) named_bar_sync(bar_mine, 256);   // tile j - 1's k-loop has been issued
-      uint32_t prev_stage = 0;
-      for (int it = 0; it < k_iters; ++it) {
-        mbar_wait(full_bar + stage * 8, phase);
-#ifdef VP3D_TIMELINE
-        if (warp == 4 && lane == 0 && w == (int)blockIdx.x && it == 0) TL(4);
-#endif
-        const uint32_t a_st = smem_a + stage * Cfg::kABytes;
-        const uint64_t da0 = make_gmma_desc_sw128(a_st, 16, 1024);
-        const uint64_t da1 = make_gmma_desc_sw128(a_st + 64 * 128, 16, 1024);   // rows 64..127
-        const uint64_t db = make_gmma_desc_sw128(smem_b + stage * Cfg::kBBytes, 16, 1024);
-        wgmma_fence_operands(acc[0]);
-        wgmma_fence_operands(acc[1]);
-        wgmma_fence();
-        if constexpr (I8) {
-          wgmma_kblock_i8<BLOCK_N>(acc[0], da0, db, it == 0);
-          wgmma_kblock_i8<BLOCK_N>(acc[1], da1, db, it == 0);
-        } else {
-          wgmma_kblock<BLOCK_N, F16>(acc[0], da0, db, it == 0);
-          wgmma_kblock<BLOCK_N, F16>(acc[1], da1, db, it == 0);
-        }
-        wgmma_commit();
-        wgmma_fence_operands(acc[0]);
-        wgmma_fence_operands(acc[1]);
-        if (it > 0) {
-          wgmma_wait<1>();
-          wgmma_fence_operands(acc[0]);
-          wgmma_fence_operands(acc[1]);
-          if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
-        }
-        prev_stage = stage;
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      if (w + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);   // tile j + 1 may issue
-      wgmma_wait<0>();
-      wgmma_fence_operands(acc[0]);
-      wgmma_fence_operands(acc[1]);
-      if (k_iters > 0 && lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+      mma_tile<I>(acc, p, I::kF16, smem_a, 0u, smem_b, full_bar, empty_bar, stage, phase, k_iters,
+                  lane, warp == 4 && lane == 0 && w == (int)blockIdx.x, [&] {
+                    // tile j + 1 may issue
+                    if (w + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);
+                  });
 #ifdef VP3D_TIMELINE
       if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(7); TL(8); }
 #endif
 
-      const float* scale = p.scale + n_blk * BLOCK_N;
-      const float* shift = p.shift + n_blk * BLOCK_N;
+      const float* scale = p.scale + n_blk * I::kBlockN;
+      const float* shift = p.shift + n_blk * I::kBlockN;
 #pragma unroll
       for (int sb = 0; sb < kBlocksPerTile; ++sb) {
-        const int cb = n_blk * BLOCK_N + sb * 64;   // first column of the store block
+        const int cb = n_blk * I::kBlockN + sb * 64;   // first column of the store block
         uint32_t tile_smem;
-        if constexpr (RES) {
+        if constexpr (I::kRes) {
           // in place: every thread overwrites the residual elements it adds with its results
           const uint32_t slot = 2u * wg + (res_seen & 1u);
           mbar_wait(rfull_bar + slot * 8, (res_seen >> 1) & 1u);
           ++res_seen;
-          tile_smem = smem_res + slot * Cfg::kTileBytes;
-          if constexpr (U8 != 0) {
+          tile_smem = smem_res + slot * I::kTileBytes;
+          if constexpr (I::kU8) {
             // the u8 tile must have been read out by the bulk stores issued from it last
             if (tid == 0) tma_store_wait_read<0>();
             named_bar_sync(bar_wg, 128);
@@ -502,8 +545,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           named_bar_sync(bar_wg, 128);
           tile_smem = staging;
         }
-        // u8 tile of this warpgroup: 128 rows of 64 bytes (U8 == 2: inside the 16-bit staging)
-        const uint32_t u8_tile = U8 == 2 ? staging : smem_u8 + (uint32_t)wg * (kBlockM * 64);
+        // u8 tile of this warpgroup: 128 rows of 64 bytes (u8 alone: inside the 16-bit staging)
+        const uint32_t u8_tile = I::kU8Alone ? staging : smem_u8 + (uint32_t)wg * (kBlockM * 64);
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j4 = 4 * (sb * 8 + jj);
@@ -517,10 +560,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
               float v0 = fmaxf(fmaf(static_cast<float>(acc[h2][j4 + 2 * h]), sc.x, sh.x), 0.0f);
               float v1 = fmaxf(fmaf(static_cast<float>(acc[h2][j4 + 2 * h + 1]), sc.y, sh.y), 0.0f);
               const uint32_t off = sw128_off(64 * h2 + rl0 + 8 * h, jj * 8 + cq);
-              if (RES) add_pair(v0, v1, ld_shared_u32(tile_smem + off), F16);
-              if constexpr (kStore16)
-                st_shared_u32(tile_smem + off, F16 ? pack_f16x2(v0, v1) : pack_bf16x2(v0, v1));
-              if constexpr (U8 != 0)
+              if (I::kRes) add_pair(v0, v1, ld_shared_u32(tile_smem + off), I::kF16);
+              if constexpr (I::kStore16)
+                st_shared_u32(tile_smem + off, I::kF16 ? pack_f16x2(v0, v1) : pack_bf16x2(v0, v1));
+              if constexpr (I::kU8)
                 st_u8_pair(u8_tile + (uint32_t)(64 * h2 + rl0 + 8 * h) * 64u + jj * 8 + cq, v0, v1,
                            p.u8_inv_s);
             }
@@ -532,16 +575,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           // four 32-row boxes: 4 KiB-aligned quarters of the tile, same swizzle phase as written
 #pragma unroll
           for (int hb = 0; hb < 4; ++hb) {
-            if constexpr (kStore16)
+            if constexpr (I::kStore16)
               tma_store_4d(&tmap_out, tile_smem + hb * 4096u, cb, row0 + 32 * hb, sample, 0);
             // (u8 instances are lean, never BatchNorm-backward: tmap_z maps the u8 plane)
-            if constexpr (U8 != 0)
+            if constexpr (I::kU8)
               tma_store_4d(&tmap_z, u8_tile + hb * 2048u, cb, row0 + 32 * hb, sample, 0);
           }
           tma_store_commit();
         }
       }
-      if (RES && tid == 0) {
+      if (I::kRes && tid == 0) {
         // the landing tiles go back to the auxiliary producer once the stores have read them
         tma_store_wait_read<0>();
 #pragma unroll
@@ -557,7 +600,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #ifdef VP3D_TIMELINE
     if (warp == 4 && lane == 0) TL(11);
 #endif
-  } else if (!PP && warp >= 4) {
+  } else if (!I::kPP && warp >= 4) {
     // ------------------------------------------------------------ MMA + epilogue (two warpgroups)
     const int wg = (warp - 4) >> 2;   // rows [64 wg, 64 wg + 64) of the tile
     const int wq = warp & 3;          // warp inside the warpgroup: 16 rows each
@@ -568,56 +611,30 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const uint32_t bar_slab = 4u + (uint32_t)(wg * 2 + (wq >> 1));   // the two warps of a slab
     float* s_pair = s_pairs + (wg * 2 + (wq >> 1)) * 128;
     // IEEE fp16 operands / storage instead of bf16 (eval fp16 mode)
-    const bool f16 = LEAN ? F16 : p.f16 != 0;
-    const bool do_relu = LEAN || (p.flags & kEpiRelu);
-    const bool do_res = LEAN ? RES : (p.flags & kEpiResidual) != 0;
-    const bool do_stats = TRAIN && (p.flags & kEpiStats);
-    const bool do_f32 = !LEAN && (p.flags & kEpiOutF32);
-    const bool do_affine = LEAN || (p.flags & kEpiAffine);
-    const bool two_planes = OUT2 && p.out_planes == 2;
+    const bool f16 = I::kLean ? I::kF16 : p.f16 != 0;
+    const bool do_relu = I::kLean || (p.flags & kEpiRelu);
+    const bool do_res = I::kLean ? I::kRes : (p.flags & kEpiResidual) != 0;
+    const bool do_stats = I::kTrain && (p.flags & kEpiStats);
+    const bool do_f32 = !I::kLean && (p.flags & kEpiOutF32);
+    const bool do_affine = I::kLean || (p.flags & kEpiAffine);
+    const bool two_planes = I::kOut2 && p.out_planes == 2;
     uint32_t stage = 0, phase = 0;
     uint32_t ablock = 0;              // auxiliary stages seen so far
     uint32_t sbuf = 0;                // staging buffer of the next store block
     int aff_n_blk = -1;               // N block whose scale / shift sit in shared memory
-    Acc acc[kFrag];
+    Acc acc[1][kFrag];
 #pragma unroll
-    for (int i = 0; i < kFrag; ++i) acc[i] = 0.0f;
+    for (int i = 0; i < kFrag; ++i) acc[0][i] = 0.0f;
 
     for (int w = blockIdx.x; w < total_tiles; w += gridDim.x) {
       int n_blk, sample, row0;
       tile_coords(p, w, n_blk, sample, row0);
       const int m_blk = w / p.n_tiles;  // row-tile index: 4 slabs of 32 rows each
 
-      // ---- main loop: wgmma over this warpgroup's 64 rows, one k-block per pipeline stage
-      uint32_t prev_stage = 0;
-      for (int it = 0; it < k_iters; ++it) {
-        mbar_wait(full_bar + stage * 8, phase);
-#ifdef VP3D_TIMELINE
-        if (warp == 4 && lane == 0 && w == (int)blockIdx.x && it == 0) TL(4);
-#endif
-        // this warpgroup's 64 rows of the A tile start 8 KiB in (a whole number of swizzle atoms)
-        const uint64_t da = make_gmma_desc_sw128(smem_a + stage * Cfg::kABytes + wg * 64 * 128, 16, 1024);
-        const uint64_t db = make_gmma_desc_sw128(smem_b + stage * Cfg::kBBytes, 16, 1024);
-        wgmma_fence_operands(acc);
-        wgmma_fence();
-        if constexpr (I8) wgmma_kblock_i8<BLOCK_N>(acc, da, db, it == 0);
-        else if constexpr (LEAN) wgmma_kblock<BLOCK_N, F16>(acc, da, db, it == 0);
-        else if (f16) wgmma_kblock<BLOCK_N, true>(acc, da, db, it == 0);
-        else wgmma_kblock<BLOCK_N, false>(acc, da, db, it == 0);
-        wgmma_commit();
-        wgmma_fence_operands(acc);
-        if (it > 0) {
-          // the previous k-block's MMAs have retired: its stage may be refilled
-          wgmma_wait<1>();
-          wgmma_fence_operands(acc);
-          if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
-        }
-        prev_stage = stage;
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_operands(acc);
-      if (k_iters > 0 && lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+      // ---- main loop: wgmma over this warpgroup's 64 rows, one k-block per pipeline stage; its
+      // rows of the A tile start 8 KiB in (a whole number of swizzle atoms)
+      mma_tile<I>(acc, p, f16, smem_a, wg * 64 * 128, smem_b, full_bar, empty_bar, stage, phase,
+                  k_iters, lane, warp == 4 && lane == 0 && w == (int)blockIdx.x, [] {});
 #ifdef VP3D_TIMELINE
       if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(7); TL(8); }
 #endif
@@ -627,9 +644,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       if (do_affine && n_blk != aff_n_blk) {
         named_bar_sync(1, 256);
         const int e = (int)threadIdx.x - 128;
-        if (e < BLOCK_N) {
-          s_affine[e] = __ldg(p.scale + n_blk * BLOCK_N + e);
-          s_affine[BLOCK_N + e] = __ldg(p.shift + n_blk * BLOCK_N + e);
+        if (e < I::kBlockN) {
+          s_affine[e] = __ldg(p.scale + n_blk * I::kBlockN + e);
+          s_affine[I::kBlockN + e] = __ldg(p.shift + n_blk * I::kBlockN + e);
         }
         named_bar_sync(1, 256);
         aff_n_blk = n_blk;
@@ -648,7 +665,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         out_row[h] = (long long)sample * p.out_rows + t_in[h];
         res_row[h] = 0;
         res_ok[h] = valid[h];
-        if (!RES) {
+        if (!I::kRes) {
           int rsmp = sample, rtt = t_in[h];
           if (!p.dilated && p.res_sample_div > 0) {
             rsmp = t_in[h] / p.res_sample_div;
@@ -665,20 +682,20 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
 #pragma unroll
       for (int sb = 0; sb < kBlocksPerTile; ++sb) {
-        const int cb = n_blk * BLOCK_N + sb * 64;  // first column of the store block
+        const int cb = n_blk * I::kBlockN + sb * 64;  // first column of the store block
         const bool res_here = do_res && cb >= p.res_col_begin && cb < p.res_col_begin + p.res_cols;
-        const bool aux_here = RES && (res_here || bnb);
+        const bool aux_here = I::kRes && (res_here || bnb);
         const uint32_t rs = aux_here ? ablock % (uint32_t)res_stages : 0u;
         const uint32_t rphase = aux_here ? (ablock / (uint32_t)res_stages) & 1u : 0u;
         if (aux_here) {
           ++ablock;
           mbar_wait(rfull_bar + rs * 8, rphase);  // tiles have landed
         }
-        const uint32_t aux0 = smem_res + (rs * aux_tiles) * Cfg::kTileBytes;
+        const uint32_t aux0 = smem_res + (rs * aux_tiles) * I::kTileBytes;
         // this warpgroup's staging slice(s): [hi] or [hi, lo], 64 rows x 128 B each
-        const uint32_t my_store = smem_store + (wg * 2 + sbuf) * (OUT2 ? 2 : 1) * Cfg::kHalfBytes;
-        // its u8 slice: 64 rows of 64 bytes (U8 == 2: inside the 16-bit slice)
-        const uint32_t my_u8 = U8 == 2 ? my_store : smem_u8 + (uint32_t)(wg * 2 + sbuf) * (64 * 64);
+        const uint32_t my_store = smem_store + (wg * 2 + sbuf) * (I::kOut2 ? 2 : 1) * I::kHalfBytes;
+        // its u8 slice: 64 rows of 64 bytes (u8 alone: inside the 16-bit slice)
+        const uint32_t my_u8 = I::kU8Alone ? my_store : smem_u8 + (uint32_t)(wg * 2 + sbuf) * (64 * 64);
         if (!do_f32) {
           // The slice must have been read out by the bulk store issued from it two blocks ago.
           if (tid == 0) tma_store_wait_read<1>();
@@ -690,11 +707,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           const int j = sb * 8 + jj;
           const int cl = sb * 64 + jj * 8 + cq;   // column inside the N block
           const int c = cb + jj * 8 + cq;         // output column
-          float v[2][2] = {{static_cast<float>(acc[4 * j]), static_cast<float>(acc[4 * j + 1])},
-                           {static_cast<float>(acc[4 * j + 2]), static_cast<float>(acc[4 * j + 3])}};
+          float v[2][2] = {{static_cast<float>(acc[0][4 * j]), static_cast<float>(acc[0][4 * j + 1])},
+                           {static_cast<float>(acc[0][4 * j + 2]), static_cast<float>(acc[0][4 * j + 3])}};
           if (do_affine) {
             const float2 sc = *reinterpret_cast<const float2*>(s_affine + cl);
-            const float2 sh = *reinterpret_cast<const float2*>(s_affine + BLOCK_N + cl);
+            const float2 sh = *reinterpret_cast<const float2*>(s_affine + I::kBlockN + cl);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               v[h][0] = fmaf(v[h][0], sc.x, sh.x);
@@ -705,14 +722,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
             for (int h = 0; h < 2; ++h) { v[h][0] = fmaxf(v[h][0], 0.0f); v[h][1] = fmaxf(v[h][1], 0.0f); }
           }
-          if (RES) {
+          if (I::kRes) {
             if (res_here) {
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const uint32_t off = sw128_off(64 * wg + rl0 + 8 * h, jj * 8 + cq);
                 add_pair(v[h][0], v[h][1], ld_shared_u32(aux0 + off), f16);
                 for (int pl = 1; pl < p.res_planes; ++pl)   // lo plane of a split-bf16 residual
-                  add_pair(v[h][0], v[h][1], ld_shared_u32(aux0 + pl * Cfg::kTileBytes + off), false);
+                  add_pair(v[h][0], v[h][1], ld_shared_u32(aux0 + pl * I::kTileBytes + off), false);
               }
             }
           } else if (res_here) {
@@ -738,24 +755,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
               if (c + 1 < p.n_valid) op[1] = v[h][1];
             }
           } else {
-            if constexpr (U8 != 0) {
+            if constexpr (I::kU8) {
 #pragma unroll
               for (int h = 0; h < 2; ++h)
                 st_u8_pair(my_u8 + (uint32_t)(rl0 + 8 * h) * 64u + jj * 8 + cq, v[h][0], v[h][1],
                            p.u8_inv_s);
             }
 #pragma unroll
-            for (int h = 0; h < 2 && kStore16; ++h) {
+            for (int h = 0; h < 2 && I::kStore16; ++h) {
               const uint32_t hi = f16 ? pack_f16x2(v[h][0], v[h][1]) : pack_bf16x2(v[h][0], v[h][1]);
               const uint32_t off = sw128_off(rl0 + 8 * h, jj * 8 + cq);
               st_shared_u32(my_store + off, hi);
               if (two_planes_t) {
                 const uint32_t lo = pack_bf16x2(v[h][0] - bf16_lo_to_f(hi), v[h][1] - bf16_hi_to_f(hi));
-                st_shared_u32(my_store + Cfg::kHalfBytes + off, lo);
+                st_shared_u32(my_store + I::kHalfBytes + off, lo);
               }
             }
           }
-          if (RES && bnb) {
+          if (I::kRes && bnb) {
             // dY = G(as stored) * dropmask/(1-p) * [Z*scale+shift > 0]; sums over the slab's rows
             const int ch = c % p.bnb_c;   // channel of the layer below (columns repeat per tap)
             const bool drop = p.bnb_p > 0.0f;
@@ -765,7 +782,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const uint32_t zu =
-                  ld_shared_u32(aux0 + (aux_tiles - 1) * Cfg::kTileBytes + sw128_off(64 * wg + rl0 + 8 * h, jj * 8 + cq));
+                  ld_shared_u32(aux0 + (aux_tiles - 1) * I::kTileBytes + sw128_off(64 * wg + rl0 + 8 * h, jj * 8 + cq));
               const float z2[2] = {bf16_lo_to_f(zu), bf16_hi_to_f(zu)};
               // mask hash of the element pair (c, c + 1), keyed by the 32-column chunk it lies in
               const int c0 = c & ~31;
@@ -801,13 +818,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
             }
           }
         }
-        if (RES && aux_here) mbar_arrive(rempty_bar + rs * 8);  // this thread is done with the stage
-        if (TRAIN && ((RES && bnb) || do_stats)) {
+        if (I::kRes && aux_here) mbar_arrive(rempty_bar + rs * 8);  // this thread is done with the stage
+        if (I::kTrain && ((I::kRes && bnb) || do_stats)) {
           // per-slab (32 rows) partials, summed in a fixed order afterwards (bn_stats_finalize /
           // launch_ordered_col_sums): run-to-run reproducible, unlike atomics
           slab_reduce(ss, sq, s_pair, lane, wq, bar_slab);
           if (!(wq & 1) && lane < 4) {
-            float* sp = ((RES && bnb) ? p.bnb_sums : p.stats) +
+            float* sp = ((I::kRes && bnb) ? p.bnb_sums : p.stats) +
                         ((size_t)(m_blk * 4 + 2 * wg + (wq >> 1)) * 2) * p.n_pad + cb + 2 * lane;
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) {
@@ -826,10 +843,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
             for (int hb = 0; hb < 2; ++hb) {
               const int r = row0 + 64 * wg + 32 * hb;
-              if constexpr (kStore16) tma_store_4d(&tmap_out, my_store + hb * 4096u, cb, r, sample, 0);
+              if constexpr (I::kStore16) tma_store_4d(&tmap_out, my_store + hb * 4096u, cb, r, sample, 0);
               // (u8 instances are lean, never BatchNorm-backward: tmap_z maps the u8 plane)
-              if constexpr (U8 != 0) tma_store_4d(&tmap_z, my_u8 + hb * 2048u, cb, r, sample, 0);
-              if (two_planes_t) tma_store_4d(&tmap_out, my_store + Cfg::kHalfBytes + hb * 4096u, cb, r, sample, 1);
+              if constexpr (I::kU8) tma_store_4d(&tmap_z, my_u8 + hb * 2048u, cb, r, sample, 0);
+              if (two_planes_t) tma_store_4d(&tmap_out, my_store + I::kHalfBytes + hb * 4096u, cb, r, sample, 1);
             }
             tma_store_commit();
           }
@@ -867,14 +884,12 @@ static int conv_tiles(const ConvGemmArgs& a) {
   return m_tiles * a.n_tiles;
 }
 
-template <int BLOCK_N, bool RES, bool OUT2, bool TRAIN, bool LEAN = false, bool F16 = false,
-          bool PP = false, bool I8 = false, int U8 = 0>
+template <class I>
 static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                                const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                                const CUtensorMap& tmap_z, const ConvGemmArgs& args, int num_sms,
                                cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, RES, OUT2, TRAIN, LEAN, PP, U8>;
-  auto kernel = conv_gemm_kernel<BLOCK_N, RES, OUT2, TRAIN, LEAN, F16, PP, I8, U8>;
+  auto kernel = conv_gemm_kernel<I>;
   // the dynamic shared memory opt-in is a per-device attribute
   static bool attr_set[kMaxDevices] = {};
   int dev = 0;
@@ -882,7 +897,7 @@ static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tma
   if (e != cudaSuccess) return e;
   if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
   if (!attr_set[dev]) {
-    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, I::kSmemBytes);
     if (e != cudaSuccess) return e;
     attr_set[dev] = true;
   }
@@ -893,7 +908,7 @@ static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tma
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(workers, 1, 1);
   cfg.blockDim = dim3(384, 1, 1);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.dynamicSmemBytes = I::kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   int n_attr = 0;
@@ -924,69 +939,71 @@ static bool lean_ok(const ConvGemmArgs& a, bool res) {
          a.res_col_begin == 0 && a.res_cols >= a.n_pad;
 }
 
-template <int BLOCK_N, bool RES, bool OUT2>
-static cudaError_t launch_train(const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
-                                const CUtensorMap& r, const CUtensorMap& z, const ConvGemmArgs& args,
-                                int num_sms, cudaStream_t stream) {
-  if ((args.flags & kEpiStats) || args.bnb)
-    return launch_impl<BLOCK_N, RES, OUT2, true>(a, w, o, r, z, args, num_sms, stream);
-  if constexpr (!OUT2) {
-    if (lean_ok(args, RES)) {
-      // Ping-pong pays only where a CTA gets a second tile whose MMAs can run under the first
-      // tile's epilogue; with one tile per CTA both warpgroups share it (cooperative).
-      if (conv_tiles(args) > num_sms)
-        return args.f16 ? launch_impl<BLOCK_N, RES, false, false, true, true, true>(a, w, o, r, z, args, num_sms, stream)
-                        : launch_impl<BLOCK_N, RES, false, false, true, false, true>(a, w, o, r, z, args, num_sms, stream);
-      return args.f16 ? launch_impl<BLOCK_N, RES, false, false, true, true>(a, w, o, r, z, args, num_sms, stream)
-                      : launch_impl<BLOCK_N, RES, false, false, true, false>(a, w, o, r, z, args, num_sms, stream);
-    }
+// The instance a launch runs.  run_conv has checked the int8 / u8 combinations already.
+static InstKey select_instance(const ConvGemmArgs& a, int block_n, bool multi_tile) {
+  InstKey k = {block_n, Epi::kGeneral, Fmt::kRuntime, Sched::kCooperative, a.res_tma || a.bnb,
+               a.out_planes == 2 && !(a.flags & kEpiOutF32), U8Out::kNone};
+  if ((a.flags & kEpiStats) || a.bnb) {
+    k.epi = Epi::kTrain;
+    return k;
   }
-  return launch_impl<BLOCK_N, RES, OUT2, false>(a, w, o, r, z, args, num_sms, stream);
+  // the int8 and u8-output launches have no general counterpart: always lean
+  const bool quant = a.i8 || a.out_u8;
+  if (!quant && (k.out2 || !lean_ok(a, k.res))) return k;
+  k.epi = Epi::kLean;
+  k.fmt = a.i8 ? Fmt::kI8 : a.f16 ? Fmt::kF16 : Fmt::kBf16;
+  if (a.out_u8) k.u8 = a.out ? U8Out::kBeside : U8Out::kAlone;
+  // Ping-pong pays only where a CTA gets a second tile whose MMAs can run under the first tile's
+  // epilogue; with one tile per CTA both warpgroups share it (cooperative).
+  if (multi_tile) k.sched = Sched::kPingPong;
+  return k;
 }
 
-// The int8 eval instances and the fp16 ones with a u8 second output: always the lean epilogue (they
-// have no general counterpart), ping-pong by the same rule as the 16-bit lean launches.
-template <int BLOCK_N, bool RES, bool I8, int U8>
-static cudaError_t launch_quant(const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
-                                const CUtensorMap& r, const CUtensorMap& z, const ConvGemmArgs& args,
-                                int num_sms, cudaStream_t stream) {
-  if (conv_tiles(args) > num_sms)
-    return launch_impl<BLOCK_N, RES, false, false, true, true, true, I8, U8>(a, w, o, r, z, args, num_sms, stream);
-  return launch_impl<BLOCK_N, RES, false, false, true, true, false, I8, U8>(a, w, o, r, z, args, num_sms, stream);
-}
+template <class... Is>
+struct InstList {};
 
-template <int BLOCK_N>
-static cudaError_t launch_quant_variants(const CUtensorMap& a, const CUtensorMap& w,
-                                         const CUtensorMap& o, const CUtensorMap& r,
-                                         const CUtensorMap& z, const ConvGemmArgs& args,
-                                         int num_sms, cudaStream_t stream) {
-  const bool res = args.res_tma != 0;
-  const bool u8 = args.out_u8 != nullptr;
-  // what the int8 chain runs: H (u8 only), X_i (fp16 [+ u8]), and the fp16 expand with Q_0
-  if (!args.f16 || args.bnb || args.out_planes != 1 ||
-      args.flags != (kEpiAffine | kEpiRelu | (res ? kEpiResidual : 0)) ||
-      (res && (args.res_planes != 1 || args.res_col_begin != 0 || args.res_cols < args.n_pad)))
-    return cudaErrorInvalidValue;
-  if (args.i8) {
-    if (res) {
-      if (!args.out) return cudaErrorInvalidValue;
-      return u8 ? launch_quant<BLOCK_N, true, true, 1>(a, w, o, r, z, args, num_sms, stream)
-                : launch_quant<BLOCK_N, true, true, 0>(a, w, o, r, z, args, num_sms, stream);
-    }
-    if (args.out || !u8) return cudaErrorInvalidValue;
-    return launch_quant<BLOCK_N, false, true, 2>(a, w, o, r, z, args, num_sms, stream);
-  }
-  if (res || !u8 || !args.out) return cudaErrorInvalidValue;
-  return launch_quant<BLOCK_N, false, false, 1>(a, w, o, r, z, args, num_sms, stream);
-}
+// Every compiled instance, for BN = 128 and 64.
+template <int BN>
+using Instances = InstList<
+    // training forward and data-gradient GEMMs: [residual / BatchNorm-backward Z] x [two planes]
+    Inst<BN, Epi::kTrain, Fmt::kRuntime, Sched::kCooperative, false, false>,
+    Inst<BN, Epi::kTrain, Fmt::kRuntime, Sched::kCooperative, false, true>,
+    Inst<BN, Epi::kTrain, Fmt::kRuntime, Sched::kCooperative, true, false>,
+    Inst<BN, Epi::kTrain, Fmt::kRuntime, Sched::kCooperative, true, true>,
+    // every other eval launch: the shrink (fp32), split-bf16, register-path residuals, VP3D_LEAN=0
+    Inst<BN, Epi::kGeneral, Fmt::kRuntime, Sched::kCooperative, false, false>,
+    Inst<BN, Epi::kGeneral, Fmt::kRuntime, Sched::kCooperative, false, true>,
+    Inst<BN, Epi::kGeneral, Fmt::kRuntime, Sched::kCooperative, true, false>,
+    Inst<BN, Epi::kGeneral, Fmt::kRuntime, Sched::kCooperative, true, true>,
+    // lean 16-bit inference layers: format x schedule x [residual]
+    Inst<BN, Epi::kLean, Fmt::kBf16, Sched::kCooperative, false>,
+    Inst<BN, Epi::kLean, Fmt::kBf16, Sched::kCooperative, true>,
+    Inst<BN, Epi::kLean, Fmt::kBf16, Sched::kPingPong, false>,
+    Inst<BN, Epi::kLean, Fmt::kBf16, Sched::kPingPong, true>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kCooperative, false>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kCooperative, true>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kPingPong, false>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kPingPong, true>,
+    // the int8 chain, per schedule: H (u8 alone), X_i (fp16 [+ u8]), the fp16 expand with Q_0
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kCooperative, false, false, U8Out::kAlone>,
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kCooperative, true, false, U8Out::kNone>,
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kCooperative, true, false, U8Out::kBeside>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kCooperative, false, false, U8Out::kBeside>,
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kPingPong, false, false, U8Out::kAlone>,
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kPingPong, true, false, U8Out::kNone>,
+    Inst<BN, Epi::kLean, Fmt::kI8, Sched::kPingPong, true, false, U8Out::kBeside>,
+    Inst<BN, Epi::kLean, Fmt::kF16, Sched::kPingPong, false, false, U8Out::kBeside>>;
 
-template <int BLOCK_N, bool RES>
-static cudaError_t launch_planes(const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
-                                 const CUtensorMap& r, const CUtensorMap& z, const ConvGemmArgs& args,
-                                 int num_sms, cudaStream_t stream) {
-  if (args.out_planes == 2 && !(args.flags & kEpiOutF32))
-    return launch_train<BLOCK_N, RES, true>(a, w, o, r, z, args, num_sms, stream);
-  return launch_train<BLOCK_N, RES, false>(a, w, o, r, z, args, num_sms, stream);
+// launch_impl of the listed instance whose key is k (cudaErrorInvalidValue if none is)
+template <class... Is>
+static cudaError_t launch_listed(InstList<Is...>, const InstKey& k, const CUtensorMap& a,
+                                 const CUtensorMap& w, const CUtensorMap& o, const CUtensorMap& r,
+                                 const CUtensorMap& z, const ConvGemmArgs& args, int num_sms,
+                                 cudaStream_t stream) {
+  cudaError_t e = cudaErrorInvalidValue;
+  (void)((k == Is::kKey && ((e = launch_impl<Is>(a, w, o, r, z, args, num_sms, stream)), true)) ||
+         ...);
+  return e;
 }
 
 #ifdef VP3D_TIMELINE
@@ -1010,22 +1027,10 @@ cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_
 #else
   const ConvGemmArgs& args = args_in;
 #endif
-  if (args.i8 || args.out_u8) {
-    if (block_n == 128) return launch_quant_variants<128>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
-    if (block_n == 64) return launch_quant_variants<64>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
-    return cudaErrorInvalidValue;
-  }
-  const bool res = args.res_tma != 0 || args.bnb != 0;
-  switch (block_n) {
-    case 128:
-      return res ? launch_planes<128, true>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream)
-                 : launch_planes<128, false>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
-    case 64:
-      return res ? launch_planes<64, true>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream)
-                 : launch_planes<64, false>(tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
-    default:
-      return cudaErrorInvalidValue;
-  }
+  const InstKey k = select_instance(args, block_n, conv_tiles(args) > num_sms);
+  if (block_n == 128)
+    return launch_listed(Instances<128>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
+  return launch_listed(Instances<64>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
 }
 
 }  // namespace vp3d

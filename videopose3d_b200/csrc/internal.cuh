@@ -31,9 +31,11 @@ int fail(int code, const char* fmt, ...);
 
 // 4-D bf16 map (k, row, sample, plane), box (64, box_rows, 1, 1), 128-byte swizzle; with
 // elem_bytes = 1 a byte map (u8 / s8 operands) whose box is 128 elements wide (the same 128 bytes).
+// box_bytes and swizzle set another box width (in bytes) and swizzle.
 int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint64_t row_stride,
                 uint64_t samples, uint64_t sample_stride, uint64_t planes, uint64_t plane_stride,
-                uint32_t box_rows, int elem_bytes = 2);
+                uint32_t box_rows, int elem_bytes = 2, uint32_t box_bytes = 128,
+                CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 // 2-D bf16 map (k, row), box (64, box_rows), 128-byte swizzle; elem_bytes as above.
 int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint32_t box_rows,
                 int elem_bytes = 2);
