@@ -699,6 +699,43 @@ int vp3d_stream_push_ex(vp3d_plan* plan, void* state, const float* x, int k,
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 int vp3d_stream_release(vp3d_plan* plan, void* state);
 
+/* ---- offline inference on a list of clips (run.py:186-193, 663-721 over a known set of clips) ----
+ * Replaces the per-clip loop of run.py's evaluate() -- UnchunkedGenerator(common/generators.py:
+ * 213-240) padding each clip, model(batch) (common/model.py:63-77, 126-138), the flip average of
+ * run.py:674-680 -- with ONE GEMM chain over many clips.  Each clip is edge-padded as the generator
+ * pads it (pad + causal_shift copies of its first frame in front, pad - causal_shift of its last
+ * behind, pad = (RF - 1) / 2), the padded clips are concatenated, and the dilated eval chain of
+ * vp3d_forward_eval runs over them as one sample of `rows` frames.  Output row t of the chain
+ * depends on rows [t, t + RF - 1] only, so a clip's T outputs are exactly its own forward: per clip
+ * bit-identical to vp3d_forward_eval on the padded clip whenever that takes the dilated schedule
+ * (T >= 2 or a dense model; a 1-frame clip pads to RF frames, where vp3d_forward_eval takes the
+ * strided schedule and sums in another order -- the chain then gives a streaming session's bits).
+ *
+ * Clip i of T_i frames takes copies * (T_i + RF - 1) packed rows (copies = 2 with
+ * VP3D_CLIPS_AUGMENT: the plain copy, then the mirrored one of common/generators.py:223-237).
+ * vp3d_clips_workspace_bytes: device bytes of one chain's workspace (0 for a plan or size the chain
+ * does not cover).
+ * vp3d_forward_clips: one chain.  x: the flat fp32 store (rows, J_in, F) the clips are read from;
+ * clip_first (int64), clip_len (int32) and y_first (int64): DEVICE arrays of `clips` entries, frame f
+ * of clip i is store row clip_first[i] + f, its output frame t goes to row y_first[i] + t of the flat
+ * fp32 output y (rows, J_out, 3).  rows must equal copies * sum_i (clip_len[i] + RF - 1); the host
+ * checks what it can see without reading the device table (at least copies * RF rows per clip, a
+ * multiple of copies), and the kernels touch no chain row outside [0, rows) whatever the table holds
+ * (lengths below 1 read as 1).  kps_src / joints_src: HOST int32 mirror maps of J_in / J_out entries
+ * as for vp3d_stream_init_ex (kps_src required with VP3D_CLIPS_AUGMENT, joints_src NULL = negate x
+ * only, the trajectory model; up to 256 joints), checked and passed to the kernels by value: the
+ * call makes no copy.  With augment y receives the flip average, (plain + mirror(mirrored)) * 0.5.
+ * TemporalModel (VP3D_VARIANT_DILATED, dense or not) in bf16, bf16x3, fp16 and int8 (folded scales);
+ * `mixed` is refused (its per-layer split depends on the geometry).  Launches 1 + (2B + 2) + 1
+ * kernels (vp3d_last_launch_count), asynchronous on `stream`, no host synchronisation. */
+#define VP3D_CLIPS_AUGMENT 1
+size_t vp3d_clips_workspace_bytes(const vp3d_plan* plan, int64_t rows, int flags);
+int vp3d_forward_clips(vp3d_plan* plan, const float* x, const int64_t* clip_first,
+                       const int32_t* clip_len, int clips, int64_t rows, int flags,
+                       const int32_t* kps_src, const int32_t* joints_src, float* y,
+                       const int64_t* y_first, void* workspace, size_t workspace_bytes,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,6 +28,7 @@ VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
 VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_LOSS_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
+VP3D_CLIPS_AUGMENT = 1
 
 _LIB_NAME = "libvp3d_b200.so"
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_lib", _LIB_NAME)
@@ -319,6 +320,10 @@ SIGNATURES = {
     "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_clips_workspace_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int]),
+    "vp3d_forward_clips": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_int64,
+                                                                  ctypes.c_int]
+                           + [ctypes.c_void_p] * 5 + [ctypes.c_size_t, ctypes.c_void_p]),
 }
 
 _lib = None

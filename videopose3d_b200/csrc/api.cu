@@ -655,11 +655,13 @@ extern "C" __attribute__((visibility("default"))) int vp3d_output_frames(const v
 }
 
 struct WsLayout {
-  size_t a0 = 0, x0 = 0, x1 = 0, h = 0, q = 0, total = 0;
+  size_t a0 = 0, x0 = 0, x1 = 0, h = 0, q = 0, yf = 0, total = 0;
   size_t a0_plane = 0, x_plane = 0, h_plane = 0;  // elements per plane
 };
 
-static WsLayout ws_layout(const vp3d_plan* p, int N, int T, bool strided, const int* L) {
+// y_rows > 0 (vp3d_forward_clips only): an fp32 buffer of y_rows shrink rows at the end
+static WsLayout ws_layout(const vp3d_plan* p, int N, int T, bool strided, const int* L,
+                          size_t y_rows = 0) {
   WsLayout w;
   const size_t a0_rows = strided ? (size_t)N * L[0] : (size_t)N * T;
   const size_t a0_ld = strided ? p->k0_pad : p->c_in_pad;
@@ -674,6 +676,7 @@ static WsLayout ws_layout(const vp3d_plan* p, int N, int T, bool strided, const 
   // int8: H is stored as u8 only (in the fp16 H buffer), and one u8 buffer holds Q_i: block i + 1's
   // first conv reads it before its 1x1 conv writes Q_{i+1} (the next kernel of the stream)
   if (p->int8) { w.q = off; off = align_up(off + w.x_plane, 1024); }
+  if (y_rows) { w.yf = off; off = align_up(off + y_rows * p->c_out_raw * sizeof(float), 1024); }
   w.total = off + 1024;
   return w;
 }
@@ -827,39 +830,30 @@ static void dilated_chain(const vp3d_plan* p, int N, int T, const int* L, InferC
   }
 }
 
-// The offline eval forward (y != null) or, with `amax`, the calibration pass of vp3d_calibrate_int8
-// (the chain without shrink, every quantised activation's maximum folded into amax).
-static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
-                        size_t ws_bytes, cudaStream_t stream, unsigned* amax) {
-  if (N < 1) return fail(VP3D_ERR_INVALID, "forward_eval: batch must be >= 1");
+// What every offline chain needs of the plan: packed weights and, in int8, folded scales.
+static int eval_ready(const vp3d_plan* p, const char* what) {
   if (!p->conv_packed || !p->bn_packed)
-    return fail(VP3D_ERR_STATE, "forward_eval: vp3d_set_weights has not been called");
+    return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
   if (p->int8 && !p->int8_folded)
-    return fail(VP3D_ERR_STATE, "forward_eval: int8 plan without activation scales (call "
-                "vp3d_set_int8_scales, then vp3d_set_weights)");
-  const bool strided = use_strided(p, T);
-  int L[VP3D_MAX_WIDTHS];
-  if (!layer_rows(p, T, strided, L))
-    return fail(VP3D_ERR_INVALID, "forward_eval: sequence of %d frames is shorter than the "
-                "receptive field (%d)", T, vp3d_receptive_field(p));
-  if (strided) VP3D_TRY(strided_trim(p, L));   // trailing frames the strided convs ignore
-  const WsLayout wl = ws_layout(p, N, T, strided, L);
-  if (!ws || ws_bytes < wl.total) return fail(VP3D_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-                                              ws_bytes, wl.total);
-  uint8_t* base = ws_base(ws);
+    return fail(VP3D_ERR_STATE, "%s: int8 plan without activation scales (call "
+                "vp3d_set_int8_scales, then vp3d_set_weights)", what);
+  return VP3D_OK;
+}
+
+// The offline chain in workspace layout wl over N samples with L[i] rows out of stage i: X_i
+// alternates between the workspace's two X buffers, its planes and H's packed to the rows of stage
+// i; and the per-layer operand precision.  The caller adds the geometry (strided_chain /
+// dilated_chain), the shrink output and the measurement hooks.
+static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, int N, const int* L,
+                       InferChain* out) {
   const int* fw = p->cfg.filter_widths;
   const int C = p->C;
   auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
-  // the chain's buffers: X_i alternates between the workspace's two X buffers, its planes and H's
-  // packed to the rows of stage i
-  InferChain c;
+  InferChain& c = *out;
   memset(&c, 0, sizeof(c));
   c.stages = p->nb + 1;
   c.in_plane = (long long)wl.a0_plane;
   c.h = bf(wl.h);
-  c.y = y;
-  c.profile = true;
-  c.amax = amax;
   if (p->int8) c.hq = base + wl.h;
   for (int i = 0; i <= p->nb; ++i) {
     ChainStage& s = c.st[i];
@@ -892,6 +886,31 @@ static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, vo
                                                                          : p->cfg.precision;
     }
   }
+}
+
+// The offline eval forward (y != null) or, with `amax`, the calibration pass of vp3d_calibrate_int8
+// (the chain without shrink, every quantised activation's maximum folded into amax).
+static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
+                        size_t ws_bytes, cudaStream_t stream, unsigned* amax) {
+  if (N < 1) return fail(VP3D_ERR_INVALID, "forward_eval: batch must be >= 1");
+  VP3D_TRY(eval_ready(p, "forward_eval"));
+  const bool strided = use_strided(p, T);
+  int L[VP3D_MAX_WIDTHS];
+  if (!layer_rows(p, T, strided, L))
+    return fail(VP3D_ERR_INVALID, "forward_eval: sequence of %d frames is shorter than the "
+                "receptive field (%d)", T, vp3d_receptive_field(p));
+  if (strided) VP3D_TRY(strided_trim(p, L));   // trailing frames the strided convs ignore
+  const WsLayout wl = ws_layout(p, N, T, strided, L);
+  if (!ws || ws_bytes < wl.total) return fail(VP3D_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+                                              ws_bytes, wl.total);
+  uint8_t* base = ws_base(ws);
+  const int* fw = p->cfg.filter_widths;
+  auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(base + off); };
+  InferChain c;
+  eval_chain(p, wl, base, N, L, &c);
+  c.y = y;
+  c.profile = true;
+  c.amax = amax;
 
   // ---- input packing (model.py:127 / :188), then the chain
   int launches = 0;
@@ -933,6 +952,108 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval(vp3d_pla
                                  size_t ws_bytes, void* stream_) {
   if (!p || !x || !y) return fail(VP3D_ERR_INVALID, "forward_eval: null argument");
   return eval_forward(p, x, y, N, T, ws, ws_bytes, static_cast<cudaStream_t>(stream_), nullptr);
+}
+
+// ------------------------------------------------------------------ clips (vp3d_forward_clips)
+// The checks of a clip chain's flags and row count that need no plan.
+static int clips_args(long long rows, int flags, const char* what) {
+  if (flags & ~VP3D_CLIPS_AUGMENT)
+    return fail(VP3D_ERR_INVALID, "%s: unknown flags 0x%x", what, (unsigned)flags);
+  const int copies = flags & VP3D_CLIPS_AUGMENT ? 2 : 1;
+  if (rows < 1 || rows % copies)
+    return fail(VP3D_ERR_INVALID, "%s: rows (%lld) must be a positive multiple of %d", what, rows,
+                copies);
+  // the GEMMs index rows (and round them up to whole 128-row tiles) in int32
+  if (rows > 0x7fffffffLL - kBlockM)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: %lld rows overflow the chain's int32 row indices", what,
+                rows);
+  return VP3D_OK;
+}
+
+// Geometry of a clip chain of `rows` packed rows: the offline dilated chain as one sample of `rows`
+// frames.  Fails for plans and sizes the clip chain does not cover.
+static int clips_geometry(const vp3d_plan* p, long long rows, int flags, const char* what, int* L) {
+  VP3D_TRY(clips_args(rows, flags, what));
+  if (p->cfg.variant != VP3D_VARIANT_DILATED)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: clip chains need the TemporalModel (dilated) variant; a "
+                "TemporalModelOptimized1f state_dict loads into TemporalModel unchanged", what);
+  if (p->cfg.precision == VP3D_PRECISION_MIXED)
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'mixed' is not supported: its per-layer split "
+                "depends on the geometry", what);
+  const int rf = vp3d_receptive_field(p);
+  if (rows < rf || !layer_rows(p, (int)rows, false, L))
+    return fail(VP3D_ERR_INVALID, "%s: %lld rows are fewer than one clip takes (%d)", what, rows, rf);
+  return VP3D_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) size_t vp3d_clips_workspace_bytes(
+    const vp3d_plan* p, int64_t rows, int flags) {
+  int L[VP3D_MAX_WIDTHS];
+  if (!p || clips_geometry(p, rows, flags, "clips_workspace_bytes", L) != VP3D_OK) return 0;
+  return ws_layout(p, 1, (int)rows, false, L, (size_t)L[p->nb]).total;
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_forward_clips(
+    vp3d_plan* p, const float* x, const int64_t* clip_first, const int32_t* clip_len, int clips,
+    int64_t rows, int flags, const int32_t* kps_src, const int32_t* joints_src, float* y,
+    const int64_t* y_first, void* ws, size_t ws_bytes, void* stream_) {
+  const char* what = "forward_clips";
+  if (!x || !clip_first || !clip_len || !y || !y_first)
+    return fail(VP3D_ERR_INVALID, "%s: null x, clip table or y", what);
+  if (clips < 1) return fail(VP3D_ERR_INVALID, "%s: clips must be >= 1 (got %d)", what, clips);
+  const bool aug = flags & VP3D_CLIPS_AUGMENT;
+  if (!aug && (kps_src || joints_src))
+    return fail(VP3D_ERR_INVALID, "%s: mirror maps given without VP3D_CLIPS_AUGMENT", what);
+  if (aug && !kps_src) return fail(VP3D_ERR_INVALID, "%s: VP3D_CLIPS_AUGMENT needs kps_src", what);
+  VP3D_TRY(clips_args(rows, flags, what));
+  const int copies = aug ? 2 : 1;
+  if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
+  int L[VP3D_MAX_WIDTHS];
+  VP3D_TRY(clips_geometry(p, rows, flags, what, L));
+  const int rf = vp3d_receptive_field(p);
+  if (rows < (long long)copies * clips * rf)
+    return fail(VP3D_ERR_INVALID, "%s: %lld rows cannot hold %d clips (each takes at least %d x "
+                "%d rows)", what, (long long)rows, clips, copies, rf);
+  const int j_in = p->cfg.num_joints_in, j_out = p->cfg.num_joints_out;
+  if (aug) {
+    if (j_in > kClipMaxJoints || j_out > kClipMaxJoints)
+      return fail(VP3D_ERR_UNSUPPORTED, "%s: augment supports up to %d joints", what,
+                  kClipMaxJoints);
+    VP3D_TRY(check_mirror_map(kps_src, j_in, what, "kps_src"));
+    if (joints_src) VP3D_TRY(check_mirror_map(joints_src, j_out, what, "joints_src"));
+  }
+  VP3D_TRY(eval_ready(p, what));
+  const int T = (int)rows;
+  const WsLayout wl = ws_layout(p, 1, T, false, L, (size_t)L[p->nb]);
+  if (!ws || ws_bytes < wl.total)
+    return fail(VP3D_ERR_WORKSPACE, "%s: workspace too small: %zu < %zu", what, ws_bytes, wl.total);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  uint8_t* base = ws_base(ws);
+  InferChain c;
+  eval_chain(p, wl, base, 1, L, &c);
+  float* ybuf = reinterpret_cast<float*>(base + wl.yf);
+  c.y = ybuf;
+  dilated_chain(p, 1, T, L, &c);
+
+  ClipChain t;
+  t.first = reinterpret_cast<const long long*>(clip_first);
+  t.len = clip_len;
+  t.y_first = reinterpret_cast<const long long*>(y_first);
+  t.clips = clips;
+  t.copies = copies;
+  t.rf = rf;
+  t.front = (rf - 1) / 2 + (p->cfg.causal ? (rf - 1) / 2 : 0);   // run.py:186-193
+  t.rows = rows;
+  // ---- the clips' padded copies (generators.py:216-238), the chain, each clip's rows
+  CUDA_TRY(launch_clip_pack(t, x, p->c_in_raw, p->cfg.in_features, aug ? kps_src : nullptr,
+                            reinterpret_cast<__nv_bfloat16*>(base + wl.a0), p->c_in_pad, p->planes,
+                            (long long)wl.a0_plane, p->f16, stream));
+  int launches = 1;
+  VP3D_TRY(run_infer_chain(p, c, stream, &launches));
+  CUDA_TRY(launch_clip_output(t, ybuf, L[p->nb], p->c_out_raw, aug ? joints_src : nullptr, y,
+                              stream));
+  p->last_launches = launches + 1;
+  return VP3D_OK;
 }
 
 extern "C" __attribute__((visibility("default"))) int vp3d_calibrate_int8(

@@ -238,6 +238,27 @@ struct InferChain {
 };
 // runs the chain on `stream` and adds its launches to *launches
 int run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream, int* launches);
+
+// clips.cu: the clip table of one vp3d_forward_clips chain (device arrays) and its geometry
+constexpr int kClipMaxJoints = 256;   // joints a mirror map (kernel parameter) can hold
+struct ClipChain {
+  const long long* first;    // [clips] store row of each clip's frame 0
+  const int* len;            // [clips] frames (values below 1 read as 1)
+  const long long* y_first;  // [clips] output row of each clip's frame 0
+  int clips, copies, rf, front;   // front = pad + causal shift: edge copies ahead of frame 0
+  long long rows;            // packed rows of the chain
+};
+// the chain's 16-bit input [planes][rows][ld] from the fp32 store x; kps: the host mirror map of
+// the J_in = c_raw / feat input joints (augment, copies == 2) or null
+cudaError_t launch_clip_pack(const ClipChain& t, const float* x, int c_raw, int feat, const int* kps,
+                             __nv_bfloat16* a0, int ld, int planes, long long plane, int f16,
+                             cudaStream_t stream);
+// each clip's valid rows of the shrink output ybuf [out_rows][c_out] into y (flip-averaged with two
+// copies; jsrc: host map of the c_out / 3 output joints, or null)
+cudaError_t launch_clip_output(const ClipChain& t, const float* ybuf, long long out_rows, int c_out,
+                               const int* jsrc, float* y, cudaStream_t stream);
+// stream.cu: every entry of a host mirror map lies in [0, n)
+int check_mirror_map(const int32_t* map, int n, const char* what, const char* name);
 void train_state_destroy(TrainState* t);
 int train_pack_transposed(vp3d_plan* p, const vp3d_weights* w, cudaStream_t stream,
                           bool also_forward);

@@ -562,7 +562,7 @@ VP3D_EXPORT size_t vp3d_stream_state_bytes(const vp3d_plan* p, int S, int K) {
   return vp3d_stream_state_bytes_ex(p, S, K, 0);
 }
 
-static int check_mirror_map(const int32_t* map, int n, const char* what, const char* name) {
+int vp3d::check_mirror_map(const int32_t* map, int n, const char* what, const char* name) {
   for (int j = 0; j < n; ++j)
     if (map[j] < 0 || map[j] >= n)
       return fail(VP3D_ERR_INVALID, "%s: %s[%d] = %d is not a joint index in [0, %d)", what, name, j,

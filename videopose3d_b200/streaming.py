@@ -202,14 +202,15 @@ def predict_schedule(lengths, streams, max_frames, lookahead):
 def _check_sequence(x, joints, features, device):
     if not isinstance(x, torch.Tensor):
         raise TypeError("predict expects a list of torch tensors")
-    if not x.is_cuda:
-        raise RuntimeError("videopose3d_b200 streaming runs on CUDA (sm_90a) tensors only; "
-                           "there is no CPU fallback")
-    if x.dtype != torch.float32:
-        raise TypeError(f"expected float32 sequences, got {x.dtype}")
+    # (shape and dtype first: they are checked the same way whatever device the tensor is on)
     if x.dim() != 3 or x.shape[1] != joints or x.shape[2] != features or x.shape[0] < 1:
         raise ValueError(f"expected sequences of shape (T >= 1, {joints}, {features}), "
                          f"got {tuple(x.shape)}")
+    if x.dtype != torch.float32:
+        raise TypeError(f"expected float32 sequences, got {x.dtype}")
+    if not x.is_cuda:
+        raise RuntimeError("videopose3d_b200 runs on CUDA (sm_90a) tensors only; there is no CPU "
+                           "fallback")
     if x.device != device:
         raise RuntimeError("input and parameters are on different devices")
 

@@ -151,6 +151,7 @@ class TemporalModelBase(nn.Module):
         self._grad_reducer = None  # data_parallel.GradientReducer, set by its attach()
         # int8 calibration: (amax CPU float tensor [2B], parameter versions it belongs to), or None
         self._int8 = None
+        self.last_predict_launches = 0   # kernels the last predict() launched
 
     def _build_layers(self, strided):
         """Create the parameter containers with the reference's names, shapes and default init.
@@ -679,6 +680,20 @@ class TemporalModelBase(nn.Module):
         return StreamingSession(self, streams, max_frames, augment=augment, kps_left=kps_left,
                                 kps_right=kps_right, joints_left=joints_left,
                                 joints_right=joints_right)
+
+    def predict(self, sequences, augment=False, kps_left=None, kps_right=None, joints_left=None,
+                joints_right=None, max_rows=None):
+        """Offline inference on a list of whole clips (videopose3d_b200.clips): CUDA fp32
+        (T_i, J_in, F) tensors, T_i >= 1, in; their (T_i, J_out, 3) outputs (views into one
+        buffer) out, in input order.  Each clip's output is the eval forward on the clip
+        edge-padded as UnchunkedGenerator pads it, bit for bit (with `augment=True` and its left /
+        right lists: run.py's flip average, run.py:674-680), computed by a few GEMM chains over
+        the concatenated padded clips of at most `max_rows` packed rows each.  TemporalModel in
+        eval() mode, any precision but 'mixed'; inference only (run it under torch.no_grad()).
+        Not in the reference."""
+        from .clips import predict
+        return predict(self, sequences, augment=augment, kps_left=kps_left, kps_right=kps_right,
+                       joints_left=joints_left, joints_right=joints_right, max_rows=max_rows)
 
 
 def _train_forward(module, plan, x, stream, momenta=None, p_drop=0.0, seed=0, flags=0):
