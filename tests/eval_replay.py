@@ -19,15 +19,26 @@ Both schedules: the strided one (tap-major row order, ``use_strided``) and the d
 (per-sample tiles).  Per-layer precision as ``vp3d_forward_eval`` picks it, including the FLOP rule
 of ``mixed``.  Buffers that the kernel writes are prefilled with NaN, so a lo plane outside its lo
 range (or any row nobody wrote) poisons whatever reads it.
+
+``"int8"`` (``replay(..., "int8", gemm, amax=...)``) restates ``run_infer_chain`` for an int8 plan:
+the expand in fp16, also writing the u8 codes Q_0; per block a u8 x s8 conv Q_{i-1} -> H (u8
+alone) and a u8 x s8 1x1 conv H -> X_i (fp16, residual X_{i-1}) [+ Q_i]; the shrink in fp16.  Its
+int8 GEMMs have exact int32 sums and a fixed fp32 epilogue, so ``fake_conv`` restates them bit for
+bit.  It is not in PRECISIONS: its output is not the float64 forward's (int8_oracle restates it).
 """
 from fractions import Fraction
 
+import numpy as np
 import torch
+import torch.nn.functional as F
 
+import int8_oracle as io
 from gpu_utils import conv_gemm, expected_conv
 
 PRECISIONS = ("fp16", "bf16", "mixed", "bf16x3")
-K_BF16, K_BF16X3, K_FP16 = 0, 1, 3       # VP3D_PRECISION_* of a conv descriptor
+INT8 = "int8"
+K_BF16, K_BF16X3, K_FP16, K_INT8 = 0, 1, 3, 4   # VP3D_PRECISION_* of a conv descriptor
+BLOCK_K8 = 128                           # K per k-block of the int8 GEMM (k_per_tap padded to it)
 FP16_MAX = 65504.0
 BLOCK_M = 128                            # rows per output tile of the conv GEMM
 EPS = 1e-5                               # nn.BatchNorm1d default (model.py:32)
@@ -49,7 +60,7 @@ class Plan:
     fw, C, causal=False, dense=False) -- the keys of the golden fixtures' meta."""
 
     def __init__(self, cfg, precision, N, T):
-        if precision not in PRECISIONS:
+        if precision not in PRECISIONS + (INT8,):
             raise ValueError(f"unknown precision {precision!r}")
         fw = [int(w) for w in cfg["fw"]]
         causal, dense = bool(cfg.get("causal", False)), bool(cfg.get("dense", False))
@@ -62,8 +73,10 @@ class Plan:
         self.c_in_pad = round_up(self.c_in_raw, 64)
         self.k0_pad = round_up(self.c_in_raw * fw[0], 64)
         self.c_out_pad = round_up(self.c_out_raw, 64)
-        self.f16 = precision == "fp16"
+        self.int8 = precision == INT8
+        self.f16 = precision in ("fp16", INT8)     # (int8: fp16 expand, residual stream, shrink)
         self.planes = 2 if precision in ("mixed", "bf16x3") else 1
+        self.k_conv = round_up(self.C, BLOCK_K8) if self.int8 else self.C   # K per tap, block convs
         # api.cu plan_create: pad / causal shifts / dilation / taps per stage
         self.pad, self.shift_dil, self.shift_str = [fw[0] // 2], [0], [0]
         self.shift_dil[0] = self.shift_str[0] = fw[0] // 2 if causal else 0
@@ -239,8 +252,9 @@ def pack_weights(sd, p, st):
           "expand_dil": pack(ew, p.C, p.c_in_pad, False),
           "expand_aff": bn("expand_bn", p.C)}
     for j in range(2 * p.nb):
-        pk[f"conv{j}"] = pack(w_of(f"layers_conv.{j}.weight"), p.C, p.C, False)
         pk[f"aff{j}"] = bn(f"layers_bn.{j}", p.C)
+        if not p.int8:   # (int8: the s8 packs of pack_int8)
+            pk[f"conv{j}"] = pack(w_of(f"layers_conv.{j}.weight"), p.C, p.C, False)
     pk["shrink"] = pack(w_of("shrink.weight"), p.c_out_pad, p.C, False)
     dt = torch.float64 if st.exact else torch.float32
     scale = torch.zeros(p.c_out_pad, dtype=dt, device=dev)
@@ -251,24 +265,62 @@ def pack_weights(sd, p, st):
     return pk
 
 
+def pack_int8(sd, p, amax, pk, device):
+    """The int8 plan's block-conv operands, into pk: per layer j the s8 pack [taps][C][k_conv]
+    (int8_oracle.quant_weight, zero past c_real and in the K padding) and the folded affine
+    scale' = fp32(bn_s * fp32(s_w * s_in)) (int8_oracle.int8_affine) with the kernel's fp32 fmaf
+    BatchNorm shift (bn_fold, not int8_oracle's float64 one); pk["inv_s"]: the fp32 reciprocals
+    of the activation scales of the 2B calibration maxima amax."""
+    s_act, inv = io.act_scales(np.asarray(amax, np.float32))
+    cr = p.c_real
+    sdn = {k: v.detach().cpu().numpy() for k, v in sd.items()}
+    for j in range(2 * p.nb):
+        sc, _, wq = io.int8_affine(sdn, j, s_act[j])
+        w8 = torch.zeros(wq.shape[2], p.C, p.k_conv, dtype=torch.int8)
+        w8[:, :cr, :cr] = torch.from_numpy(wq.transpose(2, 0, 1).astype(np.int8))
+        scale = torch.zeros(p.C, dtype=torch.float32)
+        scale[:cr] = torch.from_numpy(sc)
+        pk[f"conv{j}"] = w8.to(device)
+        pk[f"aff{j}"] = (scale.to(device), pk[f"aff{j}"][1])
+    pk["inv_s"] = [float(v) for v in inv]
+
+
 # ---------------------------------------------------------------------------- launches
 class Launch:
-    """One conv GEMM: descriptor fields + operand tensors (16-bit planes [planes][rows][ld])."""
+    """One conv GEMM: descriptor fields + operand tensors (16-bit planes [planes][rows][ld]; an
+    int8 launch: u8 A [1][rows][ld] and s8 W).  out_u8 [1][rows][C]: the u8 codes of the stored
+    values times inv_s (an fp32 value), beside `out` or alone."""
 
-    def __init__(self, name, desc, a, w, scale, shift, res=None, out=None, out_f32=None):
+    def __init__(self, name, desc, a, w, scale, shift, res=None, out=None, out_f32=None,
+                 out_u8=None, inv_s=None):
         self.name, self.desc = name, desc
         self.a, self.w, self.scale, self.shift = a, w, scale, shift
         self.res, self.out, self.out_f32 = res, out, out_f32
+        self.out_u8, self.inv_s = out_u8, inv_s
+
+    def _m_tiles(self):
+        d = self.desc
+        return d["samples"] * -(-d["out_rows"] // BLOCK_M) if d["per_sample_tiles"] \
+            else -(-d["out_rows"] // BLOCK_M)
 
     @property
     def block_n(self):
         """The N tile width run_conv picks for this launch."""
         d = self.desc
-        m_tiles = d["samples"] * -(-d["out_rows"] // BLOCK_M) if d["per_sample_tiles"] \
-            else -(-d["out_rows"] // BLOCK_M)
-        sms = torch.cuda.get_device_properties(0).multi_processor_count \
-            if torch.cuda.is_available() else 132
-        return 128 if d["n_pad"] % 128 == 0 and m_tiles * (d["n_pad"] // 128) * 2 >= sms else 64
+        return 128 if d["n_pad"] % 128 == 0 and self._m_tiles() * (d["n_pad"] // 128) * 2 >= \
+            num_sms() else 64
+
+    @property
+    def tiles(self):
+        """Output tiles of the launch (m tiles x n_pad / block_n)."""
+        return self._m_tiles() * (self.desc["n_pad"] // self.block_n)
+
+    @property
+    def pingpong(self):
+        """Whether select_instance gives an int8 / u8-output launch (always a lean instance) the
+        ping-pong schedule: when some CTA gets a second tile."""
+        assert self.desc["precision"] == K_INT8 or self.out_u8 is not None, self.name
+        return self.tiles > num_sms()
 
     def total_rows(self):
         d = self.desc
@@ -295,6 +347,11 @@ class Launch:
         return t * d["res_row_step"] + d["res_row_off"]
 
 
+def num_sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count \
+        if torch.cuda.is_available() else 132
+
+
 def new_desc(**kw):
     d = dict.fromkeys(DESC_FIELDS, 0)
     for k, v in kw.items():
@@ -311,11 +368,15 @@ def fake_conv(lc, with_err=False):
     The first term is the order-of-summation error; the second is the tensor cores' own: each of
     the `steps` k16 wgmma steps (pairs * taps * k_per_tap / 16) adds into the fp32 accumulator
     truncating, not rounding to nearest -- a bias toward zero of up to one ulp of the partial sum
-    per step, which dominates the split-bf16 layers' error."""
+    per step, which dominates the split-bf16 layers' error.
+    An int8 launch is restated exactly (int8_epilogue); its err is zero."""
     d = lc.desc
     geo = dict(samples=d["samples"], a_rows=d["a_rows"], taps=d["taps"], k_per_tap=d["k_per_tap"],
                per_sample_tiles=bool(d["per_sample_tiles"]), tap_row_step=d["tap_row_step"],
                tap_col_step=d["tap_col_step"], out_rows=d["out_rows"])
+    if d["precision"] == K_INT8:
+        v = int8_epilogue(lc, geo)
+        return v, (torch.zeros_like(v) if with_err else None)
     a = lc.a[:d["a_planes"]].double()
     w = lc.w.double()
     if d["precision"] == K_BF16X3:   # hi*hi + lo*hi + hi*lo (pairs 0, 1, 2 of the kernel)
@@ -340,13 +401,45 @@ def fake_conv(lc, with_err=False):
     return v, err
 
 
+def int8_epilogue(lc, geo):
+    """The value an int8 launch stores, before its output rounding: fp32 values (as float64).
+    The sums of u8 x s8 products are integers below 2^53, so float64 adds them exactly in any
+    order: they are the kernel's int32 sums.  Then the kernel's fp32 chain, operation by operation:
+        fmaxf(fmaf(fp32(acc), scale', shift), 0)   [+ residual, an fp32 add of the fp16 value].
+    A reads as zero past its row (a_ld) up to the K padding k_per_tap: TMA fills it so."""
+    d = lc.desc
+    assert lc.a.dtype == torch.uint8 and lc.w.dtype == torch.int8 and d["a_planes"] == 1
+    a = lc.a[0].double()
+    a = F.pad(a, (0, d["k_per_tap"] - a.shape[-1]))
+    acc = expected_conv(a, lc.w.double(), **geo)
+    assert float(acc.abs().max()) < 2.0 ** 31, f"{lc.name}: int32 sums overflow"
+    n = acc.shape[1]
+    v = fma_f32(acc.float(), lc.scale.float().expand(acc.shape[0], n),
+                lc.shift.float().expand(acc.shape[0], n)).view(acc.shape).to(acc.device)
+    v = v.clamp_min(0.0)
+    if lc.res is not None:
+        assert d["res_planes"] == 1 and lc.res.dtype == torch.float16
+        v = v + lc.res[0].float()[lc.residual_rows().to(v.device)]
+    return v.double()
+
+
+def quant_u8(v32, inv_s):
+    """cvt.rni.sat.u8.f32(v * inv_s): the fp32 product, rounded half to even, clamped to [0, 255]."""
+    q = (v32 * torch.tensor(inv_s, dtype=torch.float32, device=v32.device)).round()
+    return q.clamp(0, 255).to(torch.uint8)
+
+
 def store(lc, v):
     """Write the epilogue value v (float64) into the launch's output as the kernel stores it."""
     d = lc.desc
+    if lc.out_u8 is not None:
+        lc.out_u8[0] = quant_u8(v.float(), lc.inv_s)
     if lc.out_f32 is not None:
         lc.out_f32.copy_(v[:, :d["n_valid"]].to(lc.out_f32.dtype))
         return
     out = lc.out
+    if out is None:
+        return
     out.fill_(float("nan"))
     lo = lc.lo_mask().to(v.device)
     if out.dtype == torch.float64:          # exact mode: the value, a zero lo plane
@@ -373,26 +466,29 @@ def fake_gemm(lc):
 def gpu_gemm(lc):
     """One launch through ``vp3d_conv_gemm`` with the replay's own buffers."""
     d = lc.desc
-    res = {}
+    kw = {}
     if lc.res is not None:
         assert lc.res.shape[0] == d["res_planes"]
-        res = dict(res=lc.res, res_rows_per_sample=d["res_rows_per_sample"],
-                   res_row_step=d["res_row_step"], res_row_off=d["res_row_off"],
-                   res_sample_div=d["res_sample_div"])
+        kw = dict(res=lc.res, res_rows_per_sample=d["res_rows_per_sample"],
+                  res_row_step=d["res_row_step"], res_row_off=d["res_row_off"],
+                  res_sample_div=d["res_sample_div"])
     assert lc.a.shape[0] == d["a_planes"]
+    if lc.out_u8 is not None:
+        kw.update(out_u8=lc.out_u8, out_u8_inv_scale=lc.inv_s)
     conv_gemm(lc.a, d["samples"], d["a_rows"], d["a_ld"], lc.w, d["taps"], d["k_per_tap"],
               d["n_pad"], per_sample_tiles=d["per_sample_tiles"], tap_row_step=d["tap_row_step"],
               tap_col_step=d["tap_col_step"], out_rows=d["out_rows"], precision=d["precision"],
               scale=lc.scale, shift=lc.shift, relu=bool(d["relu"]), out=lc.out,
               out_f32=lc.out_f32, out_f32_cols=d["n_valid"] if lc.out_f32 is not None else None,
               out_plane_stride=d["out_plane_stride"], a_plane_stride=d["a_plane_stride"],
-              lo_row_begin=d["lo_row_begin"], lo_row_end=d["lo_row_end"], **res)
+              lo_row_begin=d["lo_row_begin"], lo_row_end=d["lo_row_end"], **kw)
 
 
 class Replay:
     """Result of ``replay``: y (N, L_out, J_out, 3), the launches in order (``launch_count``
     counts the input pack too, like ``vp3d_last_launch_count``), the plan and the activations
-    [(name, level, buffer)] in forward_numpy's collect order: X_0, H_1, X_1, H_2, X_2, ..."""
+    [(name, level, buffer)] in forward_numpy's collect order: X_0, H_1, X_1, H_2, X_2, ...
+    (int8: X_0, Q_0, H_1, X_1, Q_1, ..., H_B, X_B, the Q and H buffers u8 codes)."""
 
     def __init__(self, plan, y, launches, acts):
         self.plan, self.y, self.launches, self.acts = plan, y, launches, acts
@@ -413,15 +509,21 @@ def stored_value(buf):
     return v
 
 
-def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None):
+def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None, amax=None):
     """Run the eval forward's schedule for input x (N, T, J, F) with `gemm` executing every conv
     GEMM (``gpu_gemm`` or ``fake_gemm``).  exact: float64 operands and activations (use with
     ``fake_gemm``).  collect: a list that receives the de-permuted activations (numpy float64,
-    forward_numpy's collect order)."""
+    forward_numpy's collect order; int8: int8_oracle.forward_int8's, without the last block's
+    absent Q).  amax: the 2B calibration maxima of precision "int8" (``int8_calibration()``)."""
     N, T = int(x.shape[0]), int(x.shape[1])
     p = Plan(cfg, precision, N, T)
+    i8 = p.int8
+    if i8 and (exact or amax is None):
+        raise ValueError("the int8 replay needs amax and runs in the kernels' formats (exact=False)")
     st = Storage(p, exact, x.device)
     pk = pack_weights(sd, p, st)
+    if i8:
+        pack_int8(sd, p, amax, pk, x.device)
     fw, C, L, R, nb, planes = p.fw, p.C, p.L, p.R, p.nb, p.planes
     xs = x.reshape(N, T, p.c_in_raw).to(torch.float64 if exact else torch.float32)
     launches, acts = [], []
@@ -429,11 +531,16 @@ def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None):
     def prec(layer_x3):
         return K_FP16 if p.f16 else (K_BF16X3 if layer_x3 else K_BF16)
 
-    def run(name, desc, a, w, aff, res=None, out=None, out_f32=None):
-        lc = Launch(name, desc, a, w, aff[0], aff[1], res=res, out=out, out_f32=out_f32)
+    def run(name, desc, a, w, aff, res=None, out=None, out_f32=None, out_u8=None, inv_s=None):
+        lc = Launch(name, desc, a, w, aff[0], aff[1], res=res, out=out, out_f32=out_f32,
+                    out_u8=out_u8, inv_s=inv_s)
         gemm(lc)
         launches.append(lc)
         return lc
+
+    def empty_u8(rows):
+        # (u8 has no NaN: rows nobody writes keep 0xFF; the GPU test reruns each launch on 0x00)
+        return torch.full((1, rows, C), 255, dtype=torch.uint8, device=x.device)
 
     # ---- input pack + expand
     if p.strided:
@@ -457,15 +564,20 @@ def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None):
                 relu=1, n_pad=C, out_ld=C, out_plane_stride=R[0] * C,
                 lo_row_begin=lo_b, lo_row_end=lo_e)
     xcur = st.empty(planes, R[0], C)
-    run("expand", desc, a0, w0, pk["expand_aff"], out=xcur)
+    # int8: the fp16 expand also writes Q_0, the u8 input of block 1
+    qcur = empty_u8(R[0]) if i8 and nb > 0 else None
+    run("expand", desc, a0, w0, pk["expand_aff"], out=xcur, out_u8=qcur,
+        inv_s=pk["inv_s"][0] if qcur is not None else None)
     acts.append(("X0", 0, xcur))
+    if qcur is not None:
+        acts.append(("Q0", 0, qcur))
 
     # ---- residual blocks
     for i in range(1, nb + 1):
         x3 = p.x3[i]
         Lin, Lout = L[i - 1], L[i]
         h_planes = 2 if x3 else 1      # H only needs a lo plane when its consumer is split-bf16
-        h = st.empty(h_planes, N * Lout, C)
+        h = empty_u8(N * Lout) if i8 else st.empty(h_planes, N * Lout, C)
         desc = new_desc(a_planes=planes, precision=prec(x3), out_planes=h_planes,
                         res_planes=planes, taps=p.taps[i], k_per_tap=C, n_pad=C, relu=1,
                         out_plane_stride=N * Lout * C, out_ld=C, a_ld=C)
@@ -475,8 +587,13 @@ def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None):
         else:
             desc.update(samples=N, a_rows=Lin, per_sample_tiles=1, tap_row_step=p.dilation[i],
                         out_rows=Lout)
-        run(f"block {i} conv 1", desc, xcur, pk[f"conv{2 * (i - 1)}"], pk[f"aff{2 * (i - 1)}"],
-            out=h)
+        if i8:   # Q_{i-1} x s8 -> H, u8 alone (the K per tap padded to 128 past the row of C)
+            desc.update(precision=K_INT8, k_per_tap=p.k_conv, out_plane_stride=0)
+            run(f"block {i} conv 1", desc, qcur, pk[f"conv{2 * (i - 1)}"],
+                pk[f"aff{2 * (i - 1)}"], out_u8=h, inv_s=pk["inv_s"][2 * (i - 1) + 1])
+        else:
+            run(f"block {i} conv 1", desc, xcur, pk[f"conv{2 * (i - 1)}"],
+                pk[f"aff{2 * (i - 1)}"], out=h)
         acts.append((f"H{i}", i, h))
 
         xnext = st.empty(planes, N * Lout, C)
@@ -492,10 +609,17 @@ def replay(sd, cfg, x, precision, gemm, *, exact=False, collect=None):
             desc.update(samples=N, a_rows=Lout, per_sample_tiles=1, out_rows=Lout,
                         res_rows_per_sample=Lin, res_row_step=1,
                         res_row_off=p.pad[i] + p.shift_dil[i])
+        qnext = None
+        if i8:   # H x s8 + X_{i-1} -> X_i in fp16, and Q_i for the next block
+            desc.update(precision=K_INT8, k_per_tap=p.k_conv)
+            qnext = empty_u8(N * Lout) if i < nb else None
         run(f"block {i} conv 2", desc, h, pk[f"conv{2 * (i - 1) + 1}"],
-            pk[f"aff{2 * (i - 1) + 1}"], res=xcur, out=xnext)
+            pk[f"aff{2 * (i - 1) + 1}"], res=xcur, out=xnext, out_u8=qnext,
+            inv_s=pk["inv_s"][2 * i] if qnext is not None else None)
         acts.append((f"X{i}", i, xnext))
-        xcur = xnext
+        if qnext is not None:
+            acts.append((f"Q{i}", i, qnext))
+        xcur, qcur = xnext, qnext
 
     # ---- shrink into fp32 (N, L_out, J_out, 3)
     y = torch.full((R[nb], p.c_out_raw), float("nan"),

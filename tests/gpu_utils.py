@@ -36,14 +36,18 @@ def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_
               out_f32_cols=None, stats=None, bnb_z=None, bnb_scale=None, bnb_shift=None,
               bnb_mean=None, bnb_invstd=None, bnb_sums=None, bnb_c=0, bnb_p=0.0, bnb_seed=0,
               bnb_layer=0, out=None, out_f32=None, out_plane_stride=0, a_plane_stride=0,
-              lo_row_begin=0, lo_row_end=0):
+              lo_row_begin=0, lo_row_end=0, out_u8=None, out_u8_ld=None, out_u8_inv_scale=None):
     """Launch vp3d_conv_gemm; returns (out_bf16_planes or None, out_f32 or None).
     bnb_*: the fused BatchNorm-backward reductions (see vp3d_conv_desc); bnb_z is a bf16 tensor
     with the output's [rows][n_pad] view, the vectors fp32 [bnb_c], bnb_sums fp32 [slabs][2][n_pad].
     out / out_f32: caller-owned outputs ([planes][rows][ld] 16-bit, or [rows][ld] fp32, ld = the
     row pitch); they are filled with NaN before the launch, like the ones allocated here, so that
     whatever the kernel leaves unwritten (a lo plane outside [lo_row_begin, lo_row_end)) reads NaN.
-    out_plane_stride / a_plane_stride: 0 = the planes are contiguous."""
+    out_plane_stride / a_plane_stride: 0 = the planes are contiguous.
+    precision VP3D_PRECISION_INT8 (4): A is u8 [1][rows][a_ld] and W s8 [taps][n_pad][k_per_tap].
+    out_u8: a caller-owned u8 output [.., rows, out_u8_ld] (default ld: its last dimension) of the
+    codes of every stored value times out_u8_inv_scale; u8 has no NaN, so it is left as the caller
+    filled it.  With out_u8 and no `out`, the launch writes u8 alone (int8 without a residual)."""
     lib = _capi.load()
     dev = a_planes_t.device
     total_rows = samples * out_rows if per_sample_tiles else out_rows
@@ -80,14 +84,18 @@ def conv_gemm(a_planes_t, samples, a_rows, a_ld, w_planes_t, taps, k_per_tap, n_
         out32.fill_(float("nan"))
         d.out_f32 = out32.data_ptr(); d.out_f32_ld = out32.shape[-1]
         d.n_valid = out_f32_cols or out32.shape[-1]
-    elif out_f32_cols is None:
+    elif out_f32_cols is None and out_u8 is None:
         out = torch.full((out_planes, total_rows, n_pad), float("nan"),
-                         dtype=torch.float16 if precision == 3 else torch.bfloat16, device=dev)
+                         dtype=torch.float16 if precision in (3, 4) else torch.bfloat16, device=dev)
         d.out = out.data_ptr(); d.out_planes = out_planes; d.out_plane_stride = out[0].numel()
         d.out_ld = n_pad
-    else:
+    elif out_f32_cols is not None:
         out32 = torch.full((total_rows, out_f32_cols), float("nan"), dtype=torch.float32, device=dev)
         d.out_f32 = out32.data_ptr(); d.out_f32_ld = out_f32_cols; d.n_valid = out_f32_cols
+    if out_u8 is not None:
+        assert out_u8.dtype == torch.uint8 and out_u8_inv_scale is not None
+        d.out_u8 = out_u8.data_ptr(); d.out_u8_ld = out_u8_ld or out_u8.shape[-1]
+        d.out_u8_inv_scale = float(out_u8_inv_scale)
     if stats is not None:
         d.stats = stats.data_ptr()
     stream = torch.cuda.current_stream().cuda_stream

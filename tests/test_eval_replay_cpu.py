@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import eval_replay as er
+import int8_oracle as io
 from oracle import temporal_model_oracle as orc
 
 TM, OPT = "TemporalModel", "TemporalModelOptimized1f"
@@ -69,6 +70,100 @@ def test_exact_replay_equals_forward_numpy(name, cfg, N, T, precision):
         if lc.out is not None:
             assert (lc.out[0][:, rep.plan.c_real:] == 0).all(), lc.name
     assert rep.launch_count == 3 + 2 * rep.plan.nb
+
+
+@pytest.mark.parametrize("name,cfg,N,T", ARCHS, ids=[a[0] for a in ARCHS])
+def test_int8_replay_equals_forward_int8(name, cfg, N, T):
+    """The int8 schedule with the fake GEMM (exact integer sums, the kernels' fp32 epilogue and
+    quantisation) against int8_oracle's float64 restatement of the same forward: they differ by
+    the fp32 fmaf BatchNorm shift and epilogue versus float64 ones, which move single codes by one
+    and values by an fp16 rounding.  Plus the descriptors of every launch of the chain."""
+    sd = _sd(cfg)
+    x = orc.make_input(N, T, cfg["J"], cfg["F"], seed=1)
+    kw = dict(causal=cfg["causal"], dense=cfg["dense"],
+              strided=er.Plan(cfg, er.INT8, N, T).strided)
+    # the calibration maxima, made distinct (fp16 maxima of two layers can coincide) so that a
+    # launch quantising with another layer's scale shows in its descriptor
+    amax = io.calibrate(sd, x.numpy(), cfg["fw"], **kw)
+    amax = (amax * (1 + np.arange(amax.size) / 64)).astype(np.float32)
+    acts = []
+    rep = er.replay(sd, cfg, x, er.INT8, er.fake_gemm, amax=amax, collect=acts)
+    ref_acts = []
+    ref = io.forward_int8(sd, x.numpy(), cfg["fw"], amax, collect=ref_acts, **kw)
+    ref_acts = [a for a in ref_acts if a is not None]   # (the last block writes no Q)
+    y = rep.y.numpy()
+    assert y.shape == ref.shape
+    print(f"\n{name}: int8 replay vs forward_int8 {np.abs(y - ref).max() / np.abs(ref).max():.2e}")
+    assert np.abs(y - ref).max() <= 1e-3 * np.abs(ref).max()
+    names = [a[0] for a in rep.acts]
+    assert len(acts) == len(ref_acts) == 2 + 3 * rep.plan.nb - 1
+    for k, (got, exp) in enumerate(zip(acts, ref_acts)):
+        exp = exp[:, :got.shape[1]]
+        assert got.shape == exp.shape, names[k]
+        if names[k][0] in "QH":   # u8 codes
+            assert np.abs(got - exp).max() <= 1, names[k]
+        else:   # fp16 roundings, and the codes one apart in earlier layers: a few fp16 ulps
+            assert np.abs(got - exp).max() <= 3e-3 * np.abs(exp).max(), names[k]
+
+    # the launches of run_infer_chain in an int8 plan
+    p, ls = rep.plan, rep.launches
+    _, inv = io.act_scales(amax)
+    assert len(set(inv.tolist())) == len(inv)
+    assert rep.launch_count == 3 + 2 * p.nb == 1 + len(ls)
+    expand, shrink = ls[0], ls[-1]
+    assert expand.desc["precision"] == shrink.desc["precision"] == er.K_FP16
+    assert expand.inv_s == float(inv[0]) and expand.out_u8 is not None
+    assert shrink.out_u8 is None and shrink.out_f32 is not None
+    q_prev, x_prev = expand.out_u8, expand.out
+    for i in range(1, p.nb + 1):
+        c1, c2 = ls[2 * i - 1], ls[2 * i]
+        assert (c1.name, c2.name) == (f"block {i} conv 1", f"block {i} conv 2")
+        for lc in (c1, c2):
+            d = lc.desc
+            assert d["precision"] == er.K_INT8 and d["a_planes"] == 1 and d["a_ld"] == p.C
+            assert d["k_per_tap"] == er.round_up(p.C, 128) and lc.w.shape[-1] == d["k_per_tap"]
+            assert lc.a.dtype == torch.uint8 and lc.w.dtype == torch.int8
+        # conv 1: Q_{i-1} -> H, u8 alone
+        assert c1.a is q_prev and c1.out is None and c1.res is None
+        assert c1.inv_s == float(inv[2 * (i - 1) + 1])
+        # conv 2: H -> X_i in fp16 over the residual X_{i-1}, and Q_i except in the last block
+        assert c2.a is c1.out_u8 and c2.res is x_prev and c2.out.dtype == torch.float16
+        if i < p.nb:
+            assert c2.out_u8 is not None and c2.inv_s == float(inv[2 * i])
+        else:
+            assert c2.out_u8 is None and c2.inv_s is None
+        q_prev, x_prev = c2.out_u8, c2.out
+    assert shrink.a is x_prev
+
+
+def test_int8_epilogue_rounding():
+    """The restated int8 epilogue on hand-picked values: fmaf rounds once, codes round half to
+    even and saturate, fp16 saturates to 65504."""
+    desc = er.new_desc(a_planes=1, samples=1, a_rows=4, a_ld=64, taps=1, k_per_tap=128,
+                       n_pad=64, out_rows=4, precision=er.K_INT8, relu=1, res_planes=1,
+                       res_row_step=1)
+    a = torch.zeros(1, 4, 64, dtype=torch.uint8)
+    a[0, :, 0] = torch.tensor([1, 2, 3, 255], dtype=torch.uint8)
+    w = torch.zeros(1, 64, 128, dtype=torch.int8)
+    w[0, 0, 0], w[0, 1, 0], w[0, 2, 0] = 1, -1, 127
+    # col 0: 0.5 acc + 1 + residual; col 1: negative -> ReLU 0; col 2: 127 acc * 1e3 saturates
+    # (K runs to 128 past the row of 64: A reads as zero there)
+    scale = torch.zeros(64)
+    scale[0], scale[1], scale[2] = 0.5, 1.0, 1e3
+    shift = torch.zeros(64)
+    shift[0] = 1.0
+    res = torch.zeros(1, 4, 64, dtype=torch.float16)
+    res[0, :, 0] = torch.tensor([0.25, 0.0, 0.5, 0.0], dtype=torch.float16)
+    lc = er.Launch("t", desc, a, w, scale, shift, res=res,
+                   out=torch.empty(1, 4, 64, dtype=torch.float16),
+                   out_u8=torch.empty(1, 4, 64, dtype=torch.uint8), inv_s=1.0)
+    er.fake_gemm(lc)
+    # col 0: 0.5 a + 1 + res = 1.75, 2.0, 3.0, 128.5  ->  codes 2, 2, 3, 128 (half to even)
+    assert lc.out[0, :, 0].tolist() == [1.75, 2.0, 3.0, 128.5]
+    assert lc.out_u8[0, :, 0].tolist() == [2, 2, 3, 128]
+    assert lc.out[0, :, 1].tolist() == [0.0] * 4 and lc.out_u8[0, :, 1].tolist() == [0] * 4
+    assert lc.out[0, 3, 2].item() == 65504.0 and lc.out_u8[0, 3, 2].item() == 255
+    assert (lc.out[0, :, 3:] == 0).all() and (lc.out_u8[0, :, 3:] == 0).all()
 
 
 def _peel(r, n, perm_regions, perm_widths, last_rows):

@@ -2,9 +2,11 @@
 
 1. GEMM: vp3d_conv_gemm with precision INT8 on random u8 / s8 operands, both geometries, both tile
    widths, both schedules (cooperative / ping-pong), with and without the residual, writing u8 alone
-   or fp16 [+ u8]; and the fp16 GEMM with a u8 second output.  The int32 sums are exact, so against
-   an exact integer product and the fp32 epilogue only the output rounding remains: fp16 within one
-   fp16 rounding, u8 within one code.  The number of elements that are not bit-identical is printed.
+   or fp16 [+ u8]; and the fp16 GEMM with a u8 second output.  The int32 sums are exact and the int8
+   epilogue a fixed chain of fp32 operations (eval_replay.int8_epilogue), so the int8 launches
+   equal its restatement bit for bit; the fp16 GEMM, whose fp32 accumulation order is not
+   restated, stays within one fp16 rounding and one code.  The number of elements that are not
+   bit-identical is printed.
 2. Calibration: amax equals, exactly, the maximum of every fp16 activation the fp16 forward stores
    (the fp16 replay of eval_replay, tied to model(x) bit for bit), and repeats bit for bit.
 3. Model: model(x) in int8 against int8_oracle.forward_int8 (same calibration) and against the
@@ -68,12 +70,9 @@ def _launch(a, samples, a_rows, a_ld, w, taps, k_pad, n_pad, *, per_sample, tap_
     torch.cuda.synchronize()
 
 
-def _epilogue(acc, scale, shift, res):
-    """fp32 epilogue on exact sums: max(fp32(acc) * scale + shift, 0) [+ res] (fma rounded once)."""
-    v = (acc.float().double() * scale.double() + shift.double()).float().clamp_min(0)
-    if res is not None:
-        v = v + res.float()
-    return v
+def _epilogue(acc, scale, shift):
+    """fp32 epilogue of the fp16 GEMM on its float64 sums: max(fp32(acc) * scale + shift, 0)."""
+    return (acc.float().double() * scale.double() + shift.double()).float().clamp_min(0)
 
 
 # (id, per_sample, samples, a_rows, out_rows, taps, step, c_in, n_pad, res, u8, int8)
@@ -102,7 +101,6 @@ def test_int8_gemm(cuda_device, g):
         a[:, c_in:] = 0
         w = torch.randint(-127, 128, (taps, n_pad, k_pad), generator=gen, dtype=torch.int8)
         w[:, :, c_in:] = 0
-        a_val, w_val = a.double(), w.double()[:, :, :a_ld]
         scale = torch.rand(n_pad, generator=gen) * 2e-5
         precision = _capi.VP3D_PRECISION_INT8
     else:
@@ -118,13 +116,20 @@ def test_int8_gemm(cuda_device, g):
         res_rows = out_rows + (2 if per_sample else 0)
         res = (torch.rand(S * res_rows, n_pad, generator=gen) * 2).half().to(dev)
     a, w, scale, shift = a.to(dev), w.to(dev), scale.to(dev).float(), shift.to(dev).float()
-    acc = expected_conv(a_val.to(dev), w_val.to(dev), samples=S, a_rows=a_rows, taps=taps,
-                        k_per_tap=a_ld, per_sample_tiles=per_sample, tap_row_step=step,
-                        tap_col_step=0, out_rows=out_rows)
-    r = None
-    if has_res:
-        r = (res.view(S, -1, n_pad)[:, 1:1 + out_rows] if per_sample else res).reshape(-1, n_pad)
-    v = _epilogue(acc, scale, shift, r)
+    if int8:   # the exact restatement: integer sums, then the kernel's fp32 operations
+        desc = er.new_desc(a_planes=1, samples=S, a_rows=a_rows, a_ld=a_ld, taps=taps,
+                           k_per_tap=k_pad, n_pad=n_pad, per_sample_tiles=int(per_sample),
+                           tap_row_step=step, out_rows=out_rows, precision=er.K_INT8, relu=1,
+                           res_planes=1, res_rows_per_sample=out_rows + 2 if per_sample else 0,
+                           res_row_step=1, res_row_off=1 if per_sample else 0)
+        lc = er.Launch(name, desc, a.unsqueeze(0), w, scale, shift,
+                       res=res.unsqueeze(0) if has_res else None)
+        v = er.fake_conv(lc)[0].float()
+    else:
+        acc = expected_conv(a_val.to(dev), w_val.to(dev), samples=S, a_rows=a_rows, taps=taps,
+                            k_per_tap=a_ld, per_sample_tiles=per_sample, tap_row_step=step,
+                            tap_col_step=0, out_rows=out_rows)
+        v = _epilogue(acc, scale, shift)
     inv_s = float(np.float32(255.0) / np.float32(float(v.max()) * 0.9))
     out = torch.full((rows_out, n_pad), float("nan"), dtype=torch.float16, device=dev) \
         if (has_res or not int8) else None
@@ -134,17 +139,30 @@ def test_int8_gemm(cuda_device, g):
             res_rows_per_sample=out_rows + 2 if per_sample else 0,
             res_row_off=1 if per_sample else 0, out=out, out_u8=q, inv_s=inv_s)
     report = [name]
+    if int8:
+        exact = []
+        if out is not None:
+            exp = v.clamp(-er.FP16_MAX, er.FP16_MAX).half()
+            exact.append(("fp16", out.view(torch.int16), exp.view(torch.int16)))
+        if q is not None:
+            exact.append(("u8", q, er.quant_u8(v, np.float32(inv_s))))
+        for fmt, got, exp in exact:
+            report.append(f"{fmt} {int((got != exp).sum())}/{got.numel()} not bit-identical")
+        print("\n" + ", ".join(report))
+        for fmt, got, exp in exact:
+            assert torch.equal(got, exp), \
+                f"{name}: {fmt} output differs from the exact int8 epilogue in {int((got != exp).sum())}"
+        return
     if out is not None:
         exp = v.half()
         # one fp16 rounding (of a value the kernel may round differently in its last fp32 bit);
         # the fp16 GEMM also accumulates in fp32: up to K * 2^-24 of sum |a| |w|, scaled
         bound = 2.0 ** -11 * (v.abs().double() + exp.abs().double()) + 2.0 ** -24
-        if not int8:
-            acc_abs = expected_conv(a_val.abs().to(dev), w_val.abs().to(dev), samples=S,
-                                    a_rows=a_rows, taps=taps, k_per_tap=a_ld,
-                                    per_sample_tiles=per_sample, tap_row_step=step,
-                                    tap_col_step=0, out_rows=out_rows)
-            bound = bound + taps * a_ld * 2.0 ** -24 * acc_abs * scale.double()
+        acc_abs = expected_conv(a_val.abs().to(dev), w_val.abs().to(dev), samples=S,
+                                a_rows=a_rows, taps=taps, k_per_tap=a_ld,
+                                per_sample_tiles=per_sample, tap_row_step=step,
+                                tap_col_step=0, out_rows=out_rows)
+        bound = bound + taps * a_ld * 2.0 ** -24 * acc_abs * scale.double()
         diff = (out.double() - exp.double()).abs()
         assert not torch.isnan(out).any(), f"{name}: rows left unwritten"
         assert bool((diff <= bound).all()), \
