@@ -124,9 +124,13 @@ def _stats_inputs(dev, c, c_real, dilated, out_rows, N, seed, offset_heavy=False
 
 
 def _stats_ref(z, gamma, beta, rm, rv, c_real, momentum):
-    n = z.shape[0]
     mean = z.mean(0)
-    var = ((z - mean) ** 2).mean(0)
+    return _stats_ref_moments(mean, ((z - mean) ** 2).mean(0), z.shape[0], gamma, beta, rm, rv,
+                              c_real, momentum)
+
+
+def _stats_ref_moments(mean, var, n, gamma, beta, rm, rv, c_real, momentum):
+    """The float64 finalize of a batch of n rows with per-channel mean and (biased) var."""
     inv = 1.0 / torch.sqrt(var + float(torch.tensor(EPS, dtype=torch.float32)))
     sc = gamma[:c_real].double() * inv
     unb = var * n / (n - 1) if n > 1 else var
@@ -355,21 +359,15 @@ def test_bn_apply_matches_fp64(cuda_device, c, planes, p, res_kind):
         torch.cuda.synchronize()
         assert st == 0, _lib().vp3d_last_error()
         zv = _val(zp)
-        act = torch.relu(zv * sc.double() + sh.double())
         mask = _mask(LAYER, rows, c, p).to(dev) if p > 0 else 1.0
-        r = torch.arange(rows, device=dev)
+        rmap = (div, rps, step, off)
 
         def ref_of(mask_, shift_rows=0):
-            v = act * mask_
-            if rp is not None:
-                rr = (r // div) * rps + (r % div) * step + off if div else r * step + off
-                v = v + _val(rp)[(rr + shift_rows).clamp(0, res_rows - 1)]
-            return v
+            return _apply_ref(zv, sc, sh, mask_, _val(rp) if rp is not None else None, rmap,
+                              shift_rows)
         ref = ref_of(mask)
-        resmag = _val(rp).abs().max() if rp is not None else 0.0
-        fp32 = 8 * U * ((zv * sc.double()).abs() + sh.double().abs() + resmag) * (1 / (1 - p))
         got = _val(x)
-        tol = (2.0 ** -8 if planes == 1 else 2.0 ** -16) * ref.abs() + fp32
+        tol = _apply_tol(ref, zv, sc, sh, _val(rp) if rp is not None else None, p, planes)
         assert not torch.isnan(got).any()
         assert bool(((got - ref).abs() <= tol).all()), (rows, float((got - ref).abs().max()))
         if planes == 2:
@@ -382,9 +380,56 @@ def test_bn_apply_matches_fp64(cuda_device, c, planes, p, res_kind):
             assert not bool(((got - ref_of(mask, 1)).abs() <= tol).all())
 
 
+def _apply_ref(zv, sc, sh, mask, res=None, rmap=(0, 0, 1, 0), shift_rows=0):
+    """float64 bn_apply: relu(z * scale + shift) * mask [+ res at the RowMap rows (div,
+    rows_per_sample, step, off): (r / div) * rows_per_sample + (r % div) * step + off, or
+    r * step + off without div; shift_rows reads them that many rows off]."""
+    v = torch.relu(zv * sc.double() + sh.double()) * mask
+    if res is not None:
+        div, rps, step, off = rmap
+        r = torch.arange(zv.shape[0], device=zv.device)
+        rr = (r // div) * rps + (r % div) * step + off if div else r * step + off
+        v = v + res[(rr + shift_rows).clamp(0, res.shape[0] - 1)]
+    return v
+
+
+def _apply_tol(ref, zv, sc, sh, res, p, planes):
+    """bn_apply's gate: one rounding to the output planes plus 8 u of the fp32 terms."""
+    resmag = res.abs().max() if res is not None else 0.0
+    fp32 = 8 * U * ((zv * sc.double()).abs() + sh.double().abs() + resmag) * (1 / (1 - p))
+    return (2.0 ** -8 if planes == 1 else 2.0 ** -16) * ref.abs() + fp32
+
+
 # ---------------------------------------------------------------------------------------------
 # backward: reduce + apply
 # ---------------------------------------------------------------------------------------------
+def _bwd_sums_ref(gv, zv, sc, sh, mean, inv, mask):
+    """float64 sums of the BatchNorm backward: dY = G * mask * [z * scale + shift > 0],
+    s1 = sum dY, s2 = sum dY (z - mean) * invstd, and their gates 32 u sum|terms| (+ 2 u |s2| for
+    the product by invstd).  Returns (dY, s1, s2, tol1, tol2)."""
+    live = (zv * sc.double() + sh.double()) > 0
+    dy = gv * mask * live
+    zc = zv - mean.double()
+    s2 = (dy * zc).sum(0) * inv.double()
+    k = 32
+    return (dy, dy.sum(0), s2, k * U * dy.abs().sum(0),
+            k * U * (dy * zc).abs().sum(0) * inv.double() + 2 * U * s2.abs())
+
+
+def _bwd_apply_ref(dy, zv, sc, mean, inv, sums, n, frozen):
+    """float64 dZ of bn_bwd_apply from the kernel's sums over n rows (frozen: scale * dY), and the
+    fp32 term of its gate (8 u of the terms of scale dY + B z + D)."""
+    scd = sc.double()
+    c = scd.shape[0]
+    s1, s2 = sums[:c].double(), sums[c:].double()
+    if frozen:
+        return scd * dy, 8 * U * scd * dy.abs()
+    xh = (zv - mean.double()) * inv.double()
+    B = (scd * inv.double() * s2 / n).abs()
+    fp32 = 8 * U * (scd * dy.abs() + scd * s1.abs() / n + B * (zv.abs() + mean.double().abs()))
+    return scd * (dy - s1 / n - xh * s2 / n), fp32
+
+
 @pytest.mark.parametrize("frozen", [False, True])
 @pytest.mark.parametrize("p", [0.0, 0.25])
 @pytest.mark.parametrize("planes", [1, 2])
@@ -415,14 +460,9 @@ def test_bn_backward_matches_fp64(cuda_device, c, c_real, rows, planes, p, froze
     assert st == 0, _lib().vp3d_last_error()
     assert torch.count_nonzero(counter) == 0
     zv, gv = _val(zp), _val(gp)
-    live = (zv * sc.double() + sh.double()) > 0
     mask = _mask(LAYER, rows, c, p).to(dev) if p > 0 else 1.0
-    dy = gv * mask * live
-    xh = (zv - mean.double()) * inv.double()
-    s1, s2 = dy.sum(0), dy.mul(zv - mean.double()).sum(0) * inv.double()
-    k = 32
-    tol1 = k * U * dy.abs().sum(0)
-    tol2 = k * U * (dy * (zv - mean.double())).abs().sum(0) * inv.double() + 2 * U * s2.abs()
+    dy, s1, s2, tol1, tol2 = _bwd_sums_ref(gv, zv, sc, sh, mean, inv, mask)
+    live = (zv * sc.double() + sh.double()) > 0
     assert bool(((sums[:c].double() - s1).abs() <= tol1).all())
     assert bool(((sums[c:].double() - s2).abs() <= tol2).all())
     if p > 0:   # rejects the sums of another layer's mask
@@ -442,16 +482,10 @@ def test_bn_backward_matches_fp64(cuda_device, c, c_real, rows, planes, p, froze
     assert torch.equal(dbeta[:c_real], sums[:c_real]) and torch.equal(dgamma[:c_real], sums[c:c + c_real])
     assert torch.isnan(dgamma[c_real:]).all() and torch.isnan(dbeta[c_real:]).all(), \
         "entries past c_real must stay untouched"
-    scd = sc.double()
 
     def ref_dz(n):
-        if frozen:
-            return scd * dy
-        return scd * (dy - sums[:c].double() / n - xh * sums[c:].double() / n)
-    ref = ref_dz(rows)
-    B = (scd * inv.double() * sums[c:].double() / rows).abs()
-    fp32 = 8 * U * (scd * dy.abs() + (0 if frozen else scd * sums[:c].double().abs() / rows
-                                    + B * (zv.abs() + mean.double().abs())))
+        return _bwd_apply_ref(dy, zv, sc, mean, inv, sums, n, frozen)[0]
+    ref, fp32 = _bwd_apply_ref(dy, zv, sc, mean, inv, sums, rows, frozen)
     tol = (2.0 ** -8 if planes == 1 else 2.0 ** -16) * ref.abs() + fp32
     got = _val(dz)
     if planes == 2:
