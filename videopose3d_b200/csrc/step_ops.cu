@@ -36,7 +36,8 @@ __device__ __forceinline__ void adam_update(float& p, float g, float& m, float& 
   v = __fmaf_rn(__fmul_rn(h.one_minus_beta2, g), g, __fmul_rn(v, h.beta2));
   float second = v;
   if (amsgrad) {
-    vmax = fmaxf(vmax, v);
+    // NaN-propagating like torch.maximum (fmaxf would drop a NaN and keep the old maximum)
+    vmax = (vmax >= v || vmax != vmax) ? vmax : v;
     second = vmax;
   }
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(second), h.bc2_sqrt), h.eps);

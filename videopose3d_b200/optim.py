@@ -78,6 +78,7 @@ class FusedAdam(torch.optim.Optimizer):
             with torch.enable_grad():
                 loss = closure()
         lib = _capi.load()
+        self.last_launches = 0   # over every group of this step
         for group in self.param_groups:
             beta1, beta2 = group["betas"]
             by_step = {}  # parameters that share a step count share a launch
@@ -101,7 +102,6 @@ class FusedAdam(torch.optim.Optimizer):
                     self._check(st[key], key)
                 st["step"] += 1
                 by_step.setdefault(int(st["step"].item()), []).append((p, st))
-            self.last_launches = 0
             for step, items in by_step.items():
                 dev = items[0][0].device
                 if any(p.device != dev for p, _ in items):
@@ -145,6 +145,6 @@ class FusedAdam(torch.optim.Optimizer):
                 for p, _ in items:
                     # the kernel wrote through raw pointers: tell autograd / the weight-pack cache
                     torch.autograd.graph.increment_version(p)
-                for m, plan, _ in by_model.values():
-                    m._mark_train_packs_current(plan)   # after the version bumps above
+                for m, plan, rows in by_model.values():   # after the version bumps above
+                    m._mark_train_packs_current(plan, [p for p, _ in rows])
         return loss

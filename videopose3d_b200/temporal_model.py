@@ -485,11 +485,18 @@ class TemporalModelBase(nn.Module):
         plan = self._engine.plans.get((device.index, self._train_precision))
         return plan if plan is not None and plan.train is not None else None
 
-    def _mark_train_packs_current(self, plan):
-        """The fused optimizer step has just re-packed every conv weight of the training plan `plan`:
-        record the parameters' new versions so that the next forward does not pack again.  The step
-        ran on the plan, so it is the one ``last_launch_count`` reports."""
-        plan.train = self._versions()
+    def _mark_train_packs_current(self, plan, repacked):
+        """The fused optimizer step has just re-packed the conv weights in `repacked` (the parameters
+        it updated) on the training plan `plan`: record their new versions so that the next forward
+        does not pack again.  Every other conv weight keeps the version its packs were made from, so
+        a change that did not go through this step (another optimizer, an in-place edit of a frozen
+        weight) still forces the full re-pack.  The step ran on the plan, so it is the one
+        ``last_launch_count`` reports."""
+        ids = {id(t) for t in repacked}
+        conv, _ = self._param_tensors()
+        now = self._versions()
+        plan.train = (tuple(v if id(t) in ids else old
+                            for t, v, old in zip(conv, now[0], plan.train[0])), now[1])
         self._engine.last = plan
 
     def _sync_expand_t(self, plan, stream):
