@@ -115,9 +115,12 @@ __device__ __forceinline__ double unit(const double* e, double* u) {
 // adds scale * d distance-sum / d p (this lane's joint) to g.  *degenerate: the rotation's gap test.
 __device__ __forceinline__ double p_mpjpe_pose(const double* p, const double* t, bool on, int J,
                                                bool grads, double scale, double* g, bool* degenerate) {
+  // The centroids divide by J, as np.mean does: J copies of one fp32 value sum exactly in fp64, so a
+  // pose with every joint at one point centres to exactly 0 and gives NaN (0 / 0) like the
+  // reference.  Multiplying by 1.0 / J instead leaves a spread of round-off and a finite answer.
   const double inv_j = 1.0 / J;
-  const double mx0 = warp_sum(t[0]) * inv_j, mx1 = warp_sum(t[1]) * inv_j, mx2 = warp_sum(t[2]) * inv_j;
-  const double my0 = warp_sum(p[0]) * inv_j, my1 = warp_sum(p[1]) * inv_j, my2 = warp_sum(p[2]) * inv_j;
+  const double mx0 = warp_sum(t[0]) / J, mx1 = warp_sum(t[1]) / J, mx2 = warp_sum(t[2]) / J;
+  const double my0 = warp_sum(p[0]) / J, my1 = warp_sum(p[1]) / J, my2 = warp_sum(p[2]) / J;
   double x0[3] = {on ? t[0] - mx0 : 0.0, on ? t[1] - mx1 : 0.0, on ? t[2] - mx2 : 0.0};
   double y0[3] = {on ? p[0] - my0 : 0.0, on ? p[1] - my1 : 0.0, on ? p[2] - my2 : 0.0};
   const double nx = sqrt(warp_sum(x0[0] * x0[0] + x0[1] * x0[1] + x0[2] * x0[2]));
