@@ -145,6 +145,34 @@ int vp3d_forward_eval(vp3d_plan* plan, const float* x, float* y, int N, int T, v
  * reproducible.  Calls accumulate (zero amax before the first batch). */
 int vp3d_calibrate_int8(vp3d_plan* fp16_plan, const float* x, int N, int T, void* workspace,
                         size_t workspace_bytes, float* amax, void* stream);
+/* Activation histograms for the int8 calibration, so that a threshold below the maximum can be
+ * chosen (vp3d_int8_thresholds; not in the reference).  hist is a DEVICE array of
+ * vp3d_int8_hist_bytes(plan) bytes (0 for a plan without residual blocks): u64 counts hist[l][b],
+ * l < 2B as amax above and b < 31744 one bin per fp16 bit pattern 0x0000 .. 0x7BFF (values with the
+ * sign bit count as 0, which they quantise to), then 2B counts of invalid values (inf / NaN; a
+ * non-finite value of x counts for layer 0).  Only the model's `channels` real channels count.
+ * vp3d_calibrate_int8_hist has vp3d_calibrate_int8's preconditions and ADDS one batch to hist:
+ * calls accumulate (zero hist once), and integer counts make the result independent of order. */
+size_t vp3d_int8_hist_bytes(const vp3d_plan* fp16_plan);
+int vp3d_calibrate_int8_hist(vp3d_plan* fp16_plan, const float* x, int N, int T, void* workspace,
+                             size_t workspace_bytes, uint64_t* hist, void* stream);
+/* Clipping thresholds from such histograms, one per layer (not in the reference): amax_out[l]
+ * (DEVICE fp32) is the value of one fp16 bin, ready for vp3d_set_int8_scales.
+ *   AMAX:       the largest non-empty bin; equals what vp3d_calibrate_int8 gives, bit for bit.
+ *   PERCENTILE: param = p in (0, 100]: the smallest bin whose cumulative count reaches
+ *               c = ceil(p / 100 * n) (fp64, n the layer's count, zeros included); p = 100 is AMAX.
+ *   MSE:        the fp16 value t in [amax / 256, amax] with the smallest quantisation error
+ *               E(t) = sum_b n_b (x_b - s q_b)^2 (fp64; s = fp32(t / 255), q_b = min(255,
+ *               rint(fp32(x_b * fp32(1 / s)))) as the int8 forward quantises); the larger t on a tie.
+ * An all-zero layer gives 0; a layer with invalid values gives NaN, which vp3d_set_int8_scales
+ * refuses.  Integer counts and fixed-order fp64 sums: the same histogram gives the same bits on every
+ * run.  scratch: DEVICE memory of vp3d_int8_thresholds_scratch_bytes(layers) bytes. */
+#define VP3D_INT8_CALIB_AMAX 0
+#define VP3D_INT8_CALIB_PERCENTILE 1
+#define VP3D_INT8_CALIB_MSE 2
+size_t vp3d_int8_thresholds_scratch_bytes(int layers);
+int vp3d_int8_thresholds(const uint64_t* hist, int layers, int method, double param,
+                         float* amax_out, void* scratch, size_t scratch_bytes, void* stream);
 /* Stores the activation scales of an int8 plan from n = 2B HOST amax values (as above): s = amax /
  * 255 in fp32 (1 when amax is 0), 1 / s in fp32.  The next vp3d_set_weights that leaves both the
  * conv and the BatchNorm packs current folds them into the int8 affine; until then vp3d_forward_eval

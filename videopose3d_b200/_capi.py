@@ -29,6 +29,7 @@ VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2
 VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_LOSS_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
 VP3D_CLIPS_AUGMENT = 1
+VP3D_INT8_CALIB_AMAX, VP3D_INT8_CALIB_PERCENTILE, VP3D_INT8_CALIB_MSE = 0, 1, 2
 
 _LIB_NAME = "libvp3d_b200.so"
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_lib", _LIB_NAME)
@@ -214,6 +215,14 @@ SIGNATURES = {
     "vp3d_calibrate_int8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                            ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_int8_hist_bytes": (ctypes.c_size_t, [ctypes.c_void_p]),
+    "vp3d_calibrate_int8_hist": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                                ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                                ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_int8_thresholds_scratch_bytes": (ctypes.c_size_t, [ctypes.c_int]),
+    "vp3d_int8_thresholds": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                            ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p,
+                                            ctypes.c_size_t, ctypes.c_void_p]),
     "vp3d_set_int8_scales": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
                                             ctypes.c_int]),
     "vp3d_int8_packs": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,

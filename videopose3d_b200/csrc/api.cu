@@ -726,9 +726,13 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
     ++*launches;
     return VP3D_OK;
   };
-  // calibration: fold the maximum of a stored fp16 plane into amax[l]
+  // calibration: fold the maximum of a stored fp16 plane into amax[l], or add its real channels
+  // to the histogram of layer l
   auto amax = [&](int l, const __nv_bfloat16* x, long long n) -> int {
     if (c.amax) CUDA_TRY(launch_amax_f16(x, n, c.amax + l, stream));
+    if (c.hist)
+      CUDA_TRY(launch_hist_f16(x, n / C, C, p->c_real, c.hist + (size_t)l * kHistBins,
+                               c.hist + (size_t)2 * p->nb * kHistBins + l, num_sms(), stream));
     return VP3D_OK;
   };
   for (int i = 0; i < c.stages; ++i) {
@@ -888,10 +892,12 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
   }
 }
 
-// The offline eval forward (y != null) or, with `amax`, the calibration pass of vp3d_calibrate_int8
-// (the chain without shrink, every quantised activation's maximum folded into amax).
+// The offline eval forward (y != null) or, with `amax` or `hist`, the calibration pass of
+// vp3d_calibrate_int8 / vp3d_calibrate_int8_hist (the chain without shrink, every quantised
+// activation's maximum folded into amax or its values counted into hist).
 static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, void* ws,
-                        size_t ws_bytes, cudaStream_t stream, unsigned* amax) {
+                        size_t ws_bytes, cudaStream_t stream, unsigned* amax,
+                        unsigned long long* hist = nullptr) {
   if (N < 1) return fail(VP3D_ERR_INVALID, "forward_eval: batch must be >= 1");
   VP3D_TRY(eval_ready(p, "forward_eval"));
   const bool strided = use_strided(p, T);
@@ -911,6 +917,7 @@ static int eval_forward(vp3d_plan* p, const float* x, float* y, int N, int T, vo
   c.y = y;
   c.profile = true;
   c.amax = amax;
+  c.hist = hist;
 
   // ---- input packing (model.py:127 / :188), then the chain
   int launches = 0;
@@ -1068,6 +1075,32 @@ extern "C" __attribute__((visibility("default"))) int vp3d_calibrate_int8(
   // (fp32 values >= 0: their bit patterns order like the values)
   return eval_forward(p, x, nullptr, N, T, ws, ws_bytes, static_cast<cudaStream_t>(stream_),
                       reinterpret_cast<unsigned*>(amax));
+}
+
+extern "C" __attribute__((visibility("default"))) size_t vp3d_int8_hist_bytes(const vp3d_plan* p) {
+  if (!p || p->nb < 1) return 0;
+  return (size_t)2 * p->nb * (kHistBins + 1) * sizeof(uint64_t);
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_calibrate_int8_hist(
+    vp3d_plan* p, const float* x, int N, int T, void* ws, size_t ws_bytes, uint64_t* hist,
+    void* stream_) {
+  if (!p || !x || !hist) return fail(VP3D_ERR_INVALID, "calibrate_int8_hist: null argument");
+  if (p->cfg.precision != VP3D_PRECISION_FP16)
+    return fail(VP3D_ERR_INVALID, "calibrate_int8_hist: needs an fp16 plan (the activations it "
+                "measures are the fp16 forward's)");
+  if (p->nb < 1) return fail(VP3D_ERR_INVALID, "calibrate_int8_hist: the model has no residual block");
+  if (reinterpret_cast<uintptr_t>(hist) % 8)
+    return fail(VP3D_ERR_INVALID, "calibrate_int8_hist: hist not 8-byte aligned");
+  if (N < 1) return fail(VP3D_ERR_INVALID, "calibrate_int8_hist: batch must be >= 1");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  unsigned long long* h = reinterpret_cast<unsigned long long*>(hist);
+  VP3D_TRY(eval_forward(p, x, nullptr, N, T, ws, ws_bytes, stream, nullptr, h));
+  // the input pack saturates inf and NaN to finite fp16, so no histogram would show them: they
+  // count as invalid values of X_0
+  CUDA_TRY(launch_count_nonfinite(x, (long long)N * T * p->c_in_raw, h + (size_t)2 * p->nb * kHistBins,
+                                  num_sms(), stream));
+  return VP3D_OK;
 }
 
 extern "C" __attribute__((visibility("default"))) int vp3d_int8_packs(

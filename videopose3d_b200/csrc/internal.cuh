@@ -235,6 +235,9 @@ struct InferChain {
   // calibration (vp3d_calibrate_int8): fp32 bits of amax[2B], folded after every GEMM whose output
   // an int8 plan quantises; null otherwise
   unsigned* amax;
+  // calibration (vp3d_calibrate_int8_hist): the histograms of the same planes, [2B][kHistBins]
+  // counts followed by the 2B invalid counts; null otherwise
+  unsigned long long* hist;
 };
 // runs the chain on `stream` and adds its launches to *launches
 int run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream, int* launches);

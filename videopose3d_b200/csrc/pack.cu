@@ -1,5 +1,7 @@
 #include "pack.cuh"
 
+#include "conv_gemm.cuh"   // kMaxDevices
+
 #include <string.h>
 
 #include <stdint.h>
@@ -248,6 +250,103 @@ cudaError_t launch_amax_f16(const void* x, long long n, unsigned* amax_bits, cud
   long long blocks = (n8 + 255) / 256;
   if (blocks > 132 * 8) blocks = 132 * 8;
   amax_f16_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), n8, amax_bits);
+  return cudaGetLastError();
+}
+
+// Every block counts its share of the plane into a private u32 histogram in shared memory and adds
+// the non-empty bins to the u64 one.  Zeros (half or more of post-ReLU activations) would serialise
+// on one shared bin: they are counted in registers and added once per warp, like the invalid ones.
+// Vector i holds channels 8 * (i mod c8) .. + 7 of its row; the column is stepped, not divided.
+constexpr int kHistThreads = 1024;
+constexpr int kHistMinVecs = 8 * kHistThreads;   // vectors per block below which fewer blocks run
+
+__global__ void __launch_bounds__(kHistThreads)
+hist_f16_kernel(const uint4* __restrict__ x, long long n8, int c8, int c_real,
+                unsigned long long* __restrict__ hist, unsigned long long* __restrict__ invalid) {
+  extern __shared__ unsigned s_hist[];
+  for (int b = threadIdx.x; b < kHistBins; b += blockDim.x) s_hist[b] = 0;
+  __syncthreads();
+  unsigned zeros = 0, bad = 0;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  int col = (int)(i % c8);
+  const int col_step = (int)(stride % c8);
+  for (; i < n8; i += stride) {
+    const int valid = c_real - 8 * col;   // real channels in this vector (<= 0: all padding)
+    if (valid > 0) {
+      const uint4 v = __ldg(x + i);
+      const unsigned u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        if (k < valid) {
+          const unsigned h = (u[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
+          if (h == 0u || (h & 0x8000u)) ++zeros;   // what cvt.rni.sat.u8 makes 0
+          else if (h >= (unsigned)kHistBins) ++bad;   // inf, NaN
+          else atomicAdd(&s_hist[h], 1u);
+        }
+      }
+    }
+    col += col_step;
+    if (col >= c8) col -= c8;
+  }
+  zeros = __reduce_add_sync(0xffffffffu, zeros);
+  bad = __reduce_add_sync(0xffffffffu, bad);
+  if ((threadIdx.x & 31) == 0) {
+    if (zeros) atomicAdd(&s_hist[0], zeros);
+    if (bad) atomicAdd(invalid, (unsigned long long)bad);
+  }
+  __syncthreads();
+  for (int b = threadIdx.x; b < kHistBins; b += blockDim.x)
+    if (s_hist[b]) atomicAdd(hist + b, (unsigned long long)s_hist[b]);
+}
+
+cudaError_t launch_hist_f16(const void* x, long long rows, int ld, int c_real, unsigned long long* hist,
+                            unsigned long long* invalid, int num_sms, cudaStream_t stream) {
+  if (ld % 8 || c_real < 1 || c_real > ld || rows < 0 || reinterpret_cast<uintptr_t>(x) % 16)
+    return cudaErrorInvalidValue;
+  const long long n8 = rows * (ld / 8);
+  if (n8 == 0) return cudaSuccess;
+  // A block counts at most 8 * kHistThreads * ceil(n8 / (blocks * kHistThreads)) < 8 * n8 / blocks
+  // + 8 * kHistThreads elements per launch; with blocks >= 8 * n8 / 2^31 that is below 2^31 + 2^13,
+  // so no u32 shared bin (nor a thread's or a warp's register count) can wrap.
+  long long blocks = (n8 + kHistMinVecs - 1) / kHistMinVecs;
+  if (blocks > num_sms) blocks = num_sms;
+  const long long floor_blocks = (8 * n8 + (1LL << 31) - 1) >> 31;
+  if (blocks < floor_blocks) blocks = floor_blocks;
+  if (blocks > 0x7fffffffLL) return cudaErrorInvalidValue;
+  const size_t smem = kHistBins * sizeof(unsigned);
+  // the dynamic shared memory opt-in is a per-device attribute
+  static bool attr_set[kMaxDevices] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
+  if (!attr_set[dev]) {
+    e = cudaFuncSetAttribute(hist_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    attr_set[dev] = true;
+  }
+  hist_f16_kernel<<<(int)blocks, kHistThreads, smem, stream>>>(reinterpret_cast<const uint4*>(x), n8,
+                                                               ld / 8, c_real, hist, invalid);
+  return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256)
+count_nonfinite_kernel(const float* __restrict__ x, long long n, unsigned long long* __restrict__ count) {
+  unsigned c = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x)
+    c += (__float_as_uint(__ldg(x + i)) & 0x7f800000u) == 0x7f800000u;
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, (unsigned long long)c);
+}
+
+cudaError_t launch_count_nonfinite(const float* x, long long n, unsigned long long* count,
+                                   int num_sms, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  long long blocks = (n + 255) / 256;
+  if (blocks > 8LL * num_sms) blocks = 8LL * num_sms;
+  count_nonfinite_kernel<<<(int)blocks, 256, 0, stream>>>(x, n, count);
   return cudaGetLastError();
 }
 

@@ -81,6 +81,15 @@ cudaError_t launch_int8_fold(const float* bn_scale, const float* w_scale, float 
 // amax_bits = max(amax_bits, fp32 bits of max(x)) over n fp16 values >= 0 (n % 8 == 0, x 16-byte
 // aligned; -0 counts as 0), one integer atomicMax per block.
 cudaError_t launch_amax_f16(const void* x, long long n, unsigned* amax_bits, cudaStream_t stream);
+// Calibration histogram of one stored fp16 plane [rows][ld] (x 16-byte aligned, ld % 8 == 0): of
+// every row's first c_real channels, bit patterns with the sign bit set add to hist[0], patterns
+// 0x0001 .. 0x7BFF to hist[pattern], inf and NaN to *invalid.  u64 counts, so calls accumulate.
+constexpr int kHistBins = 0x7C00;   // 31 744: every finite fp16 value >= 0
+cudaError_t launch_hist_f16(const void* x, long long rows, int ld, int c_real, unsigned long long* hist,
+                            unsigned long long* invalid, int num_sms, cudaStream_t stream);
+// *count += the number of inf / NaN values among x[0, n)
+cudaError_t launch_count_nonfinite(const float* x, long long n, unsigned long long* count,
+                                   int num_sms, cudaStream_t stream);
 
 // Eval-mode BatchNorm1d (model.py:32,117,119; eps = 1e-5) as y = x*scale + shift.
 // gamma/beta/mean/var: [c]; scale/shift: [c_pad] (padding: scale 0, shift 0).  mean_out /

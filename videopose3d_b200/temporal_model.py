@@ -21,6 +21,8 @@ from . import _capi
 _PRECISIONS = {"bf16": _capi.VP3D_PRECISION_BF16, "bf16x3": _capi.VP3D_PRECISION_BF16X3,
                "mixed": _capi.VP3D_PRECISION_MIXED, "fp16": _capi.VP3D_PRECISION_FP16,
                "int8": _capi.VP3D_PRECISION_INT8}
+_CALIB_METHODS = {"amax": _capi.VP3D_INT8_CALIB_AMAX,
+                  "percentile": _capi.VP3D_INT8_CALIB_PERCENTILE, "mse": _capi.VP3D_INT8_CALIB_MSE}
 
 
 # id(parameter) -> weakref(owning model): lets optim.FusedAdam find the model whose packed bf16
@@ -257,13 +259,27 @@ class TemporalModelBase(nn.Module):
         return self
 
     # ------------------------------------------------------------------ int8 calibration
-    def calibrate_int8(self, inputs):
+    def calibrate_int8(self, inputs, method="amax", percentile=99.99):
         """Measure the activation ranges of the 'int8' eval mode: runs the fp16 eval forward
         (without shrink) on `inputs` -- one CUDA float32 (N, T, J, F) tensor, a list of them, or an
         ``UnchunkedGenerator`` on the device (every batch of one epoch) -- and keeps, for every
-        residual-block conv, the maximum of its input over all of them.  Recorded with the current
-        parameter versions: after any parameter change an int8 forward raises until the model is
-        recalibrated or a calibration is loaded.  Not in the reference."""
+        residual-block conv, a clipping threshold of its input over all of them (the int8 scale is
+        threshold / 255; larger values saturate at 255).  `method`:
+
+        - "amax": the maximum;
+        - "percentile": the smallest value at or above `percentile` percent (in (0, 100]) of the
+          values, zeros included, from an exact histogram with one bin per fp16 value;
+        - "mse": the fp16 value between max / 256 and max that minimises the squared quantisation
+          error over that histogram.
+
+        The last two keep one outlier (a glitch frame of a 2-D detector, a long-tailed activation)
+        from coarsening the scale of every ordinary value.  Recorded with the current parameter
+        versions: after any parameter change an int8 forward raises until the model is recalibrated
+        or a calibration is loaded.  Not in the reference."""
+        if method not in _CALIB_METHODS:
+            raise ValueError(f"method must be one of {sorted(_CALIB_METHODS)} (got {method!r})")
+        if method == "percentile" and not 0.0 < float(percentile) <= 100.0:
+            raise ValueError(f"percentile must be in (0, 100] (got {percentile})")
         if hasattr(inputs, "next_epoch"):
             inputs = [batch[-1] for batch in inputs.next_epoch()]
         elif torch.is_tensor(inputs):
@@ -275,11 +291,17 @@ class TemporalModelBase(nn.Module):
         device = self.expand_conv.weight.device
         if device.type != "cuda":
             raise RuntimeError("module parameters must be on a CUDA device")
-        amax = torch.zeros(len(self.layers_conv), dtype=torch.float32, device=device)
+        layers = len(self.layers_conv)
+        hist = None   # "amax" (and a model without residual blocks): the maxima alone
         with torch.cuda.device(device):
             plan = self._get_plan(device, "fp16")
             stream = torch.cuda.current_stream(device).cuda_stream
             self._sync_weights(plan, stream)
+            if method == "amax" or layers == 0:
+                amax = torch.zeros(layers, dtype=torch.float32, device=device)
+            else:
+                hist = torch.zeros(lib.vp3d_int8_hist_bytes(plan) // 8, dtype=torch.int64,
+                                   device=device)
             for x in inputs:
                 if not (torch.is_tensor(x) and x.is_cuda and x.device == device
                         and x.dtype == torch.float32 and x.dim() == 4
@@ -293,10 +315,28 @@ class TemporalModelBase(nn.Module):
                     raise ValueError(f"input of {T} frames is shorter than the receptive field "
                                      f"({self.receptive_field()})")
                 ws = self._get_workspace(nbytes, device)
-                _capi.check(lib.vp3d_calibrate_int8(plan, x.data_ptr(), N, T, ws.data_ptr(),
-                                                    ws.numel(), amax.data_ptr(), stream),
-                            "vp3d_calibrate_int8")
-        self._int8 = (amax.cpu(), self._versions())
+                if hist is None:
+                    _capi.check(lib.vp3d_calibrate_int8(plan, x.data_ptr(), N, T, ws.data_ptr(),
+                                                        ws.numel(), amax.data_ptr(), stream),
+                                "vp3d_calibrate_int8")
+                else:
+                    _capi.check(lib.vp3d_calibrate_int8_hist(plan, x.data_ptr(), N, T,
+                                                             ws.data_ptr(), ws.numel(),
+                                                             hist.data_ptr(), stream),
+                                "vp3d_calibrate_int8_hist")
+            if hist is not None:
+                scratch = torch.empty(lib.vp3d_int8_thresholds_scratch_bytes(layers),
+                                      dtype=torch.uint8, device=device)
+                amax = torch.empty(layers, dtype=torch.float32, device=device)
+                _capi.check(lib.vp3d_int8_thresholds(hist.data_ptr(), layers, _CALIB_METHODS[method],
+                                                     float(percentile), amax.data_ptr(),
+                                                     scratch.data_ptr(), scratch.numel(), stream),
+                            "vp3d_int8_thresholds")
+        amax = amax.cpu()
+        if hist is not None and not bool(torch.isfinite(amax).all()):   # (NaN: invalid values)
+            raise ValueError("calibrate_int8: inf or NaN values in the calibration inputs or their "
+                             "activations")
+        self._int8 = (amax, self._versions())
         return self
 
     def int8_calibration(self):
