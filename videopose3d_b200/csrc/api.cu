@@ -508,19 +508,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
 extern "C" __attribute__((visibility("default"))) void vp3d_plan_destroy(vp3d_plan* p) {
   if (!p) return;
   for (void* q : p->allocs) cudaFree(q);
-  if (p->d_x) cudaFree(p->d_x);
-  if (p->d_y) cudaFree(p->d_y);
-  if (p->d_ws) cudaFree(p->d_ws);
-  if (p->stream) cudaStreamDestroy(p->stream);
-  for (auto& s : p->slots) {
-    if (s.d_x) cudaFree(s.d_x);
-    if (s.d_y) cudaFree(s.d_y);
-    if (s.copied) cudaEventDestroy(s.copied);
-    if (s.done) cudaEventDestroy(s.done);
-  }
-  if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
-  for (cudaEvent_t e : p->copy_events) cudaEventDestroy(e);
-  for (cudaEvent_t e : p->prof_events) cudaEventDestroy(e);
+  for (cudaEvent_t e : p->prof_events) if (e) cudaEventDestroy(e);
   if (p->train) train_state_destroy(p->train);
   delete p;
 }
@@ -668,16 +656,16 @@ static WsLayout ws_layout(const vp3d_plan* p, int N, int T, bool strided, const 
   w.a0_plane = a0_rows * a0_ld;
   w.x_plane = (size_t)N * L[0] * p->C;
   w.h_plane = p->nb > 0 ? (size_t)N * L[1] * p->C : 0;
-  size_t off = 0;
-  w.a0 = off; off = align_up(off + w.a0_plane * p->planes * 2, 1024);
-  w.x0 = off; off = align_up(off + w.x_plane * p->planes * 2, 1024);
-  w.x1 = off; off = align_up(off + w.h_plane * p->planes * 2, 1024);  // block outputs are <= L[1] rows
-  w.h = off;  off = align_up(off + w.h_plane * p->planes * 2, 1024);
+  Arena a{1024};
+  w.a0 = a.take(w.a0_plane * p->planes * 2);
+  w.x0 = a.take(w.x_plane * p->planes * 2);
+  w.x1 = a.take(w.h_plane * p->planes * 2);  // block outputs are <= L[1] rows
+  w.h = a.take(w.h_plane * p->planes * 2);
   // int8: H is stored as u8 only (in the fp16 H buffer), and one u8 buffer holds Q_i: block i + 1's
   // first conv reads it before its 1x1 conv writes Q_{i+1} (the next kernel of the stream)
-  if (p->int8) { w.q = off; off = align_up(off + w.x_plane, 1024); }
-  if (y_rows) { w.yf = off; off = align_up(off + y_rows * p->c_out_raw * sizeof(float), 1024); }
-  w.total = off + 1024;
+  if (p->int8) w.q = a.take(w.x_plane);
+  if (y_rows) w.yf = a.take(y_rows * p->c_out_raw * sizeof(float));
+  w.total = a.total();
   return w;
 }
 
@@ -690,15 +678,33 @@ extern "C" __attribute__((visibility("default"))) size_t vp3d_workspace_bytes(co
   return ws_layout(p, N, T, strided, L).total;
 }
 
+// ------------------------------------------------------------------ host-buffer staging
+HostStaging::~HostStaging() {
+  if (stream) cudaStreamDestroy(stream);
+  if (copy_stream) cudaStreamDestroy(copy_stream);
+  for (cudaEvent_t e : copy_events) if (e) cudaEventDestroy(e);
+  for (Slot& s : slots) {
+    if (s.copied) cudaEventDestroy(s.copied);
+    if (s.done) cudaEventDestroy(s.done);
+  }
+}
+
+// create *s (non-blocking) / *e on first use
+static int lazy_stream(cudaStream_t* s) {
+  if (!*s) CUDA_TRY(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
+  return VP3D_OK;
+}
+static int lazy_event(cudaEvent_t* e, unsigned flags = cudaEventDisableTiming) {
+  if (!*e) CUDA_TRY(cudaEventCreateWithFlags(e, flags));
+  return VP3D_OK;
+}
+
 // measurement hook: record an event pair around launch number p->prof_launch
 static int prof_event(vp3d_plan* p, int launch, bool begin, cudaStream_t stream) {
   if (p->prof_launch < 0 || launch != p->prof_launch) return VP3D_OK;
   const size_t idx = p->prof_used + (begin ? 0 : 1);
-  while (p->prof_events.size() <= idx) {
-    cudaEvent_t e;
-    CUDA_TRY(cudaEventCreate(&e));
-    p->prof_events.push_back(e);
-  }
+  if (p->prof_events.size() <= idx) p->prof_events.resize(idx + 1, nullptr);
+  VP3D_TRY(lazy_event(&p->prof_events[idx], cudaEventDefault));
   CUDA_TRY(cudaEventRecord(p->prof_events[idx], stream));
   if (!begin) p->prof_used += 2;
   return VP3D_OK;
@@ -1146,69 +1152,50 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval_host(vp3
   if (!p || !x_host || !y_host) return fail(VP3D_ERR_INVALID, "forward_eval_host: null argument");
   const int t_out = vp3d_output_frames(p, T);
   if (t_out < 1 || N < 1) return fail(VP3D_ERR_INVALID, "forward_eval_host: bad shape");
-  if (!p->stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+  HostStaging& h = p->host;
+  VP3D_TRY(lazy_stream(&h.stream));
   const size_t xb = (size_t)N * T * p->c_in_raw * sizeof(float);
   const size_t yb = (size_t)N * t_out * p->c_out_raw * sizeof(float);
-  const size_t wb = vp3d_workspace_bytes(p, N, T);
-  if (xb > p->d_x_bytes) {
-    if (p->d_x) cudaFree(p->d_x);
-    p->d_x = nullptr; p->d_x_bytes = 0;
-    CUDA_TRY(cudaMalloc(&p->d_x, xb));
-    p->d_x_bytes = xb;
-  }
-  if (yb > p->d_y_bytes) {
-    if (p->d_y) cudaFree(p->d_y);
-    p->d_y = nullptr; p->d_y_bytes = 0;
-    CUDA_TRY(cudaMalloc(&p->d_y, yb));
-    p->d_y_bytes = yb;
-  }
-  if (wb > p->d_ws_bytes) {
-    if (p->d_ws) cudaFree(p->d_ws);
-    p->d_ws = nullptr; p->d_ws_bytes = 0;
-    CUDA_TRY(cudaMalloc(&p->d_ws, wb));
-    p->d_ws_bytes = wb;
-  }
+  VP3D_TRY(h.x.grow(xb));
+  VP3D_TRY(h.y.grow(yb));
+  VP3D_TRY(h.ws.grow(vp3d_workspace_bytes(p, N, T)));
   // Batch rows are independent in eval mode: split the batch into chunks so that the host->device
   // copy of chunk i+1 (copy stream) overlaps the kernels of chunk i (compute stream).  PCIe moves
   // 33.8 MB per 1024 x 243 batch, which is longer than the whole forward.
   int chunks = N >= 512 ? 2 : 1;
   if (const char* env = getenv("VP3D_HOST_CHUNKS")) {  // measurement knob
     const int c = atoi(env);
-    if (c >= 1 && c <= 16 && c <= N) chunks = c;
+    if (c >= 1 && c <= kMaxHostChunks && c <= N) chunks = c;
   }
   if (chunks == 1) {
-    CUDA_TRY(cudaMemcpyAsync(p->d_x, x_host, xb, cudaMemcpyHostToDevice, p->stream));
-    VP3D_TRY(vp3d_forward_eval(p, p->d_x, p->d_y, N, T, p->d_ws, p->d_ws_bytes, p->stream));
+    CUDA_TRY(cudaMemcpyAsync(h.x.ptr, x_host, xb, cudaMemcpyHostToDevice, h.stream));
+    VP3D_TRY(vp3d_forward_eval(p, h.x.ptr, h.y.ptr, N, T, h.ws.ptr, h.ws.bytes, h.stream));
   } else {
-    if (!p->copy_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->copy_stream, cudaStreamNonBlocking));
-    while ((int)p->copy_events.size() < chunks) {
-      cudaEvent_t e;
-      CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      p->copy_events.push_back(e);
-    }
+    VP3D_TRY(lazy_stream(&h.copy_stream));
+    for (int c = 0; c < chunks; ++c) VP3D_TRY(lazy_event(&h.copy_events[c]));
     const size_t x_row = (size_t)T * p->c_in_raw, y_row = (size_t)t_out * p->c_out_raw;
     int launches = 0;
-    // the previous call's kernels may still read d_x: order the copies behind them
-    CUDA_TRY(cudaEventRecord(p->copy_events[0], p->stream));
-    CUDA_TRY(cudaStreamWaitEvent(p->copy_stream, p->copy_events[0], 0));
+    // the previous call's kernels may still read h.x: order the copies behind them
+    CUDA_TRY(cudaEventRecord(h.copy_events[0], h.stream));
+    CUDA_TRY(cudaStreamWaitEvent(h.copy_stream, h.copy_events[0], 0));
     for (int c = 0; c < chunks; ++c) {
       const int n0 = (int)((long long)N * c / chunks), n1 = (int)((long long)N * (c + 1) / chunks);
-      CUDA_TRY(cudaMemcpyAsync(p->d_x + n0 * x_row, x_host + n0 * x_row,
+      CUDA_TRY(cudaMemcpyAsync(h.x.ptr + n0 * x_row, x_host + n0 * x_row,
                                (size_t)(n1 - n0) * x_row * sizeof(float), cudaMemcpyHostToDevice,
-                               p->copy_stream));
-      CUDA_TRY(cudaEventRecord(p->copy_events[c], p->copy_stream));
+                               h.copy_stream));
+      CUDA_TRY(cudaEventRecord(h.copy_events[c], h.copy_stream));
     }
     for (int c = 0; c < chunks; ++c) {
       const int n0 = (int)((long long)N * c / chunks), n1 = (int)((long long)N * (c + 1) / chunks);
-      CUDA_TRY(cudaStreamWaitEvent(p->stream, p->copy_events[c], 0));
-      VP3D_TRY(vp3d_forward_eval(p, p->d_x + n0 * x_row, p->d_y + n0 * y_row, n1 - n0, T, p->d_ws,
-                                 p->d_ws_bytes, p->stream));
+      CUDA_TRY(cudaStreamWaitEvent(h.stream, h.copy_events[c], 0));
+      VP3D_TRY(vp3d_forward_eval(p, h.x.ptr + n0 * x_row, h.y.ptr + n0 * y_row, n1 - n0, T,
+                                 h.ws.ptr, h.ws.bytes, h.stream));
       launches += p->last_launches;
     }
     p->last_launches = launches;
   }
-  CUDA_TRY(cudaMemcpyAsync(y_host, p->d_y, yb, cudaMemcpyDeviceToHost, p->stream));
-  CUDA_TRY(cudaStreamSynchronize(p->stream));
+  CUDA_TRY(cudaMemcpyAsync(y_host, h.y.ptr, yb, cudaMemcpyDeviceToHost, h.stream));
+  CUDA_TRY(cudaStreamSynchronize(h.stream));
   return VP3D_OK;
 }
 
@@ -1222,42 +1209,28 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval_host_sub
   if (slot < 0 || slot > 1) return fail(VP3D_ERR_INVALID, "host_submit: slot must be 0 or 1");
   const int t_out = vp3d_output_frames(p, T);
   if (t_out < 1 || N < 1) return fail(VP3D_ERR_INVALID, "host_submit: bad shape");
-  vp3d_plan::HostSlot& s = p->slots[slot];
+  HostStaging& h = p->host;
+  HostStaging::Slot& s = h.slots[slot];
   if (s.busy) return fail(VP3D_ERR_STATE, "host_submit: slot %d still in flight (call wait first)", slot);
-  if (!p->stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-  if (!p->copy_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->copy_stream, cudaStreamNonBlocking));
-  if (!s.copied) {
-    CUDA_TRY(cudaEventCreateWithFlags(&s.copied, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-  }
+  VP3D_TRY(lazy_stream(&h.stream));
+  VP3D_TRY(lazy_stream(&h.copy_stream));
+  VP3D_TRY(lazy_event(&s.copied));
+  VP3D_TRY(lazy_event(&s.done));
   const size_t xb = (size_t)N * T * p->c_in_raw * sizeof(float);
   const size_t yb = (size_t)N * t_out * p->c_out_raw * sizeof(float);
   const size_t wb = vp3d_workspace_bytes(p, N, T);
-  if (xb > s.x_bytes) {
-    if (s.d_x) cudaFree(s.d_x);
-    s.d_x = nullptr; s.x_bytes = 0;
-    CUDA_TRY(cudaMalloc(&s.d_x, xb));
-    s.x_bytes = xb;
+  VP3D_TRY(s.x.grow(xb));
+  VP3D_TRY(s.y.grow(yb));
+  if (wb > h.ws.bytes) {
+    CUDA_TRY(cudaStreamSynchronize(h.stream));  // the other slot may be using the old workspace
+    VP3D_TRY(h.ws.grow(wb));
   }
-  if (yb > s.y_bytes) {
-    if (s.d_y) cudaFree(s.d_y);
-    s.d_y = nullptr; s.y_bytes = 0;
-    CUDA_TRY(cudaMalloc(&s.d_y, yb));
-    s.y_bytes = yb;
-  }
-  if (wb > p->d_ws_bytes) {
-    CUDA_TRY(cudaStreamSynchronize(p->stream));  // the other slot may be using the old workspace
-    if (p->d_ws) cudaFree(p->d_ws);
-    p->d_ws = nullptr; p->d_ws_bytes = 0;
-    CUDA_TRY(cudaMalloc(&p->d_ws, wb));
-    p->d_ws_bytes = wb;
-  }
-  CUDA_TRY(cudaMemcpyAsync(s.d_x, x_host, xb, cudaMemcpyHostToDevice, p->copy_stream));
-  CUDA_TRY(cudaEventRecord(s.copied, p->copy_stream));
-  CUDA_TRY(cudaStreamWaitEvent(p->stream, s.copied, 0));
-  VP3D_TRY(vp3d_forward_eval(p, s.d_x, s.d_y, N, T, p->d_ws, p->d_ws_bytes, p->stream));
-  CUDA_TRY(cudaMemcpyAsync(y_host, s.d_y, yb, cudaMemcpyDeviceToHost, p->stream));
-  CUDA_TRY(cudaEventRecord(s.done, p->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.x.ptr, x_host, xb, cudaMemcpyHostToDevice, h.copy_stream));
+  CUDA_TRY(cudaEventRecord(s.copied, h.copy_stream));
+  CUDA_TRY(cudaStreamWaitEvent(h.stream, s.copied, 0));
+  VP3D_TRY(vp3d_forward_eval(p, s.x.ptr, s.y.ptr, N, T, h.ws.ptr, h.ws.bytes, h.stream));
+  CUDA_TRY(cudaMemcpyAsync(y_host, s.y.ptr, yb, cudaMemcpyDeviceToHost, h.stream));
+  CUDA_TRY(cudaEventRecord(s.done, h.stream));
   s.busy = true;
   return VP3D_OK;
 }
@@ -1265,7 +1238,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval_host_sub
 extern "C" __attribute__((visibility("default"))) int vp3d_forward_eval_host_wait(vp3d_plan* p,
                                                                                  int slot) {
   if (!p || slot < 0 || slot > 1) return fail(VP3D_ERR_INVALID, "host_wait: bad argument");
-  vp3d_plan::HostSlot& s = p->slots[slot];
+  HostStaging::Slot& s = p->host.slots[slot];
   if (!s.busy) return fail(VP3D_ERR_STATE, "host_wait: slot %d has nothing in flight", slot);
   CUDA_TRY(cudaEventSynchronize(s.done));
   s.busy = false;

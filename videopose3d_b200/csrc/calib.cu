@@ -39,20 +39,16 @@ struct Scratch {
   double* err;
 };
 
-size_t scratch_layout(int layers, uint8_t* base, Scratch* s) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    uint8_t* ptr = base ? base + off : nullptr;
-    off = align_up(off + bytes, 256);
-    return ptr;
-  };
+// carves the scratch from address base (0: only its size is wanted); returns its size
+size_t scratch_layout(int layers, uintptr_t base, Scratch* s) {
+  Arena a{256};
   const size_t bins = (size_t)layers * kHistBins;
-  s->stats = reinterpret_cast<LayerStats*>(take(layers * sizeof(LayerStats)));
-  s->val = reinterpret_cast<float*>(take(bins * sizeof(float)));
-  s->cnt = reinterpret_cast<double*>(take(bins * sizeof(double)));
-  s->cum = reinterpret_cast<unsigned long long*>(take(bins * sizeof(unsigned long long)));
-  s->err = reinterpret_cast<double*>(take((size_t)layers * kMaxCands * sizeof(double)));
-  return off + 256;   // room to align the caller's base
+  s->stats = reinterpret_cast<LayerStats*>(base + a.take(layers * sizeof(LayerStats)));
+  s->val = reinterpret_cast<float*>(base + a.take(bins * sizeof(float)));
+  s->cnt = reinterpret_cast<double*>(base + a.take(bins * sizeof(double)));
+  s->cum = reinterpret_cast<unsigned long long*>(base + a.take(bins * sizeof(unsigned long long)));
+  s->err = reinterpret_cast<double*>(base + a.take((size_t)layers * kMaxCands * sizeof(double)));
+  return a.total();
 }
 
 __device__ __forceinline__ float bin_value(int bits) {
@@ -226,7 +222,7 @@ select_kernel(Scratch s, int method, double pct, float* __restrict__ out) {
 extern "C" __attribute__((visibility("default"))) size_t vp3d_int8_thresholds_scratch_bytes(int layers) {
   if (layers < 1 || layers > VP3D_MAX_LAYERS) return 0;
   Scratch s;
-  return scratch_layout(layers, nullptr, &s);
+  return scratch_layout(layers, 0, &s);
 }
 
 extern "C" __attribute__((visibility("default"))) int vp3d_int8_thresholds(
@@ -245,11 +241,10 @@ extern "C" __attribute__((visibility("default"))) int vp3d_int8_thresholds(
   if (reinterpret_cast<uintptr_t>(hist) % 8 || reinterpret_cast<uintptr_t>(amax_out) % 4)
     return fail(VP3D_ERR_INVALID, "%s: hist or amax_out misaligned", what);
   Scratch s;
-  const size_t need = scratch_layout(layers, nullptr, &s);
+  const size_t need = scratch_layout(layers, 0, &s);
   if (!scratch || scratch_bytes < need)
     return fail(VP3D_ERR_WORKSPACE, "%s: scratch too small: %zu < %zu", what, scratch_bytes, need);
-  uint8_t* base = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(scratch), 256));
-  scratch_layout(layers, base, &s);
+  scratch_layout(layers, reinterpret_cast<uintptr_t>(ws_base(scratch, 256)), &s);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const unsigned long long* h = reinterpret_cast<const unsigned long long*>(hist);
   compact_kernel<<<layers, kCompactThreads, 0, stream>>>(h, s, layers);

@@ -43,9 +43,22 @@ int make_map_2d(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, 
 int pick_block_n(int n_pad);
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-// the 1 KiB-aligned base of a caller's workspace or state buffer (their sizes include the slack)
-inline uint8_t* ws_base(void* ws) {
-  return reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), 1024));
+// Carves a caller-sized device buffer (workspace, streaming state, scratch) into buffers that each
+// start on an `align` boundary.  total() adds `align` bytes of slack so that any pointer the caller
+// passes can be rounded up by ws_base: the two halves of one contract.
+struct Arena {
+  size_t align, off = 0;
+  // the offset of the next buffer of `bytes` bytes
+  size_t take(size_t bytes) {
+    const size_t o = off;
+    off = align_up(off + bytes, align);
+    return o;
+  }
+  size_t total() const { return off + align; }
+};
+// the aligned base of a caller's buffer sized by Arena::total with the same alignment
+inline uint8_t* ws_base(void* ws, size_t align = 1024) {
+  return reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(ws), align));
 }
 int num_sms();
 int run_conv(const vp3d_conv_desc* d, cudaStream_t stream);
@@ -112,6 +125,45 @@ int launch_adam_pack(const AdamPackItem* items, int n, int planes, int64_t step,
                      double beta1, double beta2, double eps, double weight_decay,
                      cudaStream_t stream);
 
+// A device allocation that grows to the largest size asked of it and is freed with its owner.
+template <class T>
+struct DeviceBuffer {
+  T* ptr = nullptr;
+  size_t bytes = 0;
+  DeviceBuffer() = default;
+  DeviceBuffer(const DeviceBuffer&) = delete;
+  DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+  ~DeviceBuffer() { if (ptr) cudaFree(ptr); }
+  int grow(size_t n) {
+    if (n <= bytes) return VP3D_OK;
+    if (ptr) cudaFree(ptr);
+    ptr = nullptr; bytes = 0;
+    CUDA_TRY(cudaMalloc(&ptr, n));
+    bytes = n;
+    return VP3D_OK;
+  }
+};
+
+constexpr int kMaxHostChunks = 16;   // H2D chunks of one vp3d_forward_eval_host call
+
+// What the host-buffer entries (vp3d_forward_eval_host, _submit / _wait) create on first use and
+// keep for the plan's lifetime.
+struct HostStaging {
+  DeviceBuffer<float> x, y;
+  DeviceBuffer<void> ws;                     // shared by every host entry and both slots
+  cudaStream_t stream = nullptr;             // compute
+  cudaStream_t copy_stream = nullptr;        // H2D chunks overlap the compute stream
+  cudaEvent_t copy_events[kMaxHostChunks] = {};
+  // pipelined host API: two independent staging slots
+  struct Slot {
+    DeviceBuffer<float> x, y;
+    cudaEvent_t copied = nullptr, done = nullptr;
+    bool busy = false;
+  };
+  Slot slots[2];
+  ~HostStaging();
+};
+
 }  // namespace vp3d
 
 struct vp3d_plan {
@@ -143,24 +195,8 @@ struct vp3d_plan {
   vp3d::PackedConv* conv_t[VP3D_MAX_LAYERS] = {};
   std::vector<void*> allocs;
   bool conv_packed = false, bn_packed = false;
-  // host-API staging (owned)
-  float* d_x = nullptr;
-  float* d_y = nullptr;
-  void* d_ws = nullptr;
-  size_t d_x_bytes = 0, d_y_bytes = 0, d_ws_bytes = 0;
-  cudaStream_t stream = nullptr;
-  cudaStream_t copy_stream = nullptr;     // host API: H2D chunks overlap the compute stream
-  std::vector<cudaEvent_t> copy_events;
+  vp3d::HostStaging host;
   int last_launches = 0;
-  // pipelined host API (vp3d_forward_eval_host_submit / _wait): two independent staging slots
-  struct HostSlot {
-    float* d_x = nullptr;
-    float* d_y = nullptr;
-    size_t x_bytes = 0, y_bytes = 0;
-    cudaEvent_t copied = nullptr, done = nullptr;
-    bool busy = false;
-  };
-  HostSlot slots[2];
   // measurement hook: event pairs around one chosen launch of each forward
   int prof_launch = -1;
   std::vector<cudaEvent_t> prof_events;  // start/stop pairs

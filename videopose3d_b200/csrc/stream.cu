@@ -74,32 +74,28 @@ StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   L.rings = p->nb + 1;
   const int planes = p->planes;
   const int P = physical_rows(S, flags);
-  size_t off = 0;
-  L.count = off; off = align_up(off + (size_t)2 * S * 8, 1024);
-  L.active = off; off = align_up(off + (size_t)2 * S, 1024);
-  L.length = off; off = align_up(off + (size_t)2 * S * 8, 1024);
+  Arena a{1024};
+  L.count = a.take((size_t)2 * S * 8);
+  L.active = a.take((size_t)2 * S);
+  L.length = a.take((size_t)2 * S * 8);
   for (int l = 0; l < L.rings; ++l) {
     L.H[l] = 2 * p->pad[l];
     L.R[l] = L.H[l] + K + 1;
     L.ld[l] = l == 0 ? p->c_in_pad : p->C;
     L.plane[l] = 2LL * L.R[l] * P * L.ld[l];
-    L.ring[l] = off;
-    off = align_up(off + (size_t)L.plane[l] * planes * 2, 1024);
+    L.ring[l] = a.take((size_t)L.plane[l] * planes * 2);
   }
   const size_t act = (size_t)planes * K * P * p->C * 2;
-  L.h = off; off = align_up(off + act, 1024);
-  L.xlast = off; off = align_up(off + act, 1024);
+  L.h = a.take(act);
+  L.xlast = a.take(act);
   L.v[0] = 0;
-  for (int l = 1; l < L.rings; ++l) {
-    L.v[l] = off;
-    off = align_up(off + (size_t)planes * P * p->C * 2, 1024);
-  }
-  L.ybuf = off; off = align_up(off + (size_t)K * P * p->c_out_raw * 4, 1024);
+  for (int l = 1; l < L.rings; ++l) L.v[l] = a.take((size_t)planes * P * p->C * 2);
+  L.ybuf = a.take((size_t)K * P * p->c_out_raw * 4);
   if (flags & VP3D_STREAM_AUGMENT) {
-    L.kps = off; off = align_up(off + (size_t)p->cfg.num_joints_in * 4, 1024);
-    L.jsrc = off; off = align_up(off + (size_t)p->cfg.num_joints_out * 4, 1024);
+    L.kps = a.take((size_t)p->cfg.num_joints_in * 4);
+    L.jsrc = a.take((size_t)p->cfg.num_joints_out * 4);
   }
-  L.total = off + 1024;   // slack for aligning the caller's pointer
+  L.total = a.total();
   return L;
 }
 

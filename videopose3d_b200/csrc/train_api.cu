@@ -159,28 +159,23 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
   const bool strided = p->cfg.variant == VP3D_VARIANT_STRIDED;
   TrainLayout w;
   const size_t C = p->C, pl = p->planes;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t o = off;
-    off = align_up(off + bytes, 1024);
-    return o;
-  };
+  Arena a{1024};
   for (int i = 0; i <= p->nb; ++i) w.rows[i] = (long long)N * L[i];
-  w.a0 = take(strided ? pl * w.rows[0] * p->k0_pad * 2 : pl * (size_t)N * T * p->c_in_pad * 2);
-  w.z[0] = take(pl * w.rows[0] * C * 2);
-  w.x[0] = take(pl * w.rows[0] * C * 2);
+  w.a0 = a.take(strided ? pl * w.rows[0] * p->k0_pad * 2 : pl * (size_t)N * T * p->c_in_pad * 2);
+  w.z[0] = a.take(pl * w.rows[0] * C * 2);
+  w.x[0] = a.take(pl * w.rows[0] * C * 2);
   for (int i = 1; i <= p->nb; ++i) {
     const size_t b = pl * w.rows[i] * C * 2;
-    w.z[2 * i - 1] = take(b);
-    w.h[i] = take(b);
-    w.z[2 * i] = take(b);
-    w.x[i] = take(b);
+    w.z[2 * i - 1] = a.take(b);
+    w.h[i] = a.take(b);
+    w.z[2 * i] = a.take(b);
+    w.x[i] = a.take(b);
   }
   const size_t big = pl * w.rows[0] * C * 2;
-  w.g0 = take(big);
-  w.g1 = take(big);
-  w.dz = take(big);
-  w.dyp = take(pl * w.rows[p->nb] * p->shrink_t->k_pad * 2);   // dY in K layout of shrink_t
+  w.g0 = a.take(big);
+  w.g1 = a.take(big);
+  w.dz = a.take(big);
+  w.dyp = a.take(pl * w.rows[p->nb] * p->shrink_t->k_pad * 2);   // dY in K layout of shrink_t
   // wgrad partials: up to 8 splits x taps x C x max(C, k0_pad) fp32
   int max_taps = 1;
   for (int i = 1; i <= p->nb; ++i) max_taps = p->taps[i] > max_taps ? p->taps[i] : max_taps;
@@ -188,7 +183,7 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
   if ((size_t)p->c_in_pad > n_max) n_max = p->c_in_pad;
   if (!strided && p->cfg.filter_widths[0] > max_taps) max_taps = p->cfg.filter_widths[0];
   w.partial_bytes = (size_t)8 * max_taps * round_up(p->C, 128) * round_up((int)n_max, 64) * 4;
-  w.partial = take(w.partial_bytes);
+  w.partial = a.take(w.partial_bytes);
   // slab partials [4 * row tiles][2][columns]: the widest producer is a GEMM over rows[i] rows with
   // taps*C columns (strided data gradient) or N * tiles(L) row tiles with C columns (dilated)
   {
@@ -203,11 +198,11 @@ TrainLayout train_layout(const vp3d_plan* p, int N, int T, const int* L) {
     const size_t bias_part = (size_t)((w.rows[p->nb] + 63) / 64) * (p->c_out_raw > 64 ? p->c_out_raw : 64);
     need = bias_part > need ? bias_part : need;
     w.slab_floats = need + 1024;
-    w.slab = take(w.slab_floats * sizeof(float));
+    w.slab = a.take(w.slab_floats * sizeof(float));
   }
   if (strided && T != p->cfg.filter_widths[0] * L[0])
-    w.dx_stage = take((size_t)w.rows[0] * p->cfg.filter_widths[0] * p->c_in_raw * sizeof(float));
-  w.total = off + 1024;
+    w.dx_stage = a.take((size_t)w.rows[0] * p->cfg.filter_widths[0] * p->c_in_raw * sizeof(float));
+  w.total = a.total();
   return w;
 }
 
