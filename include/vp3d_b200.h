@@ -51,7 +51,8 @@ typedef enum {
                                 its rounding error: ~4e-4 of fp32 on cfg2, inside north_star's 1e-3.
                                 Stores saturate at +-65504.  Inference only (training runs bf16 /
                                 bf16x3: gradients need the bf16 exponent range) */
-  VP3D_PRECISION_INT8 = 4    /* eval only: the two convs of every residual block multiply u8
+  VP3D_PRECISION_INT8 = 4    /* eval only: the two convs of every residual block (or of those
+                                vp3d_set_int8_blocks selects; the rest run as in FP16) multiply u8
                                 activations by s8 weights into exact int32 sums (one activation scale
                                 s = amax / 255 per quantised tensor from vp3d_calibrate_int8, weight
                                 scale max|W| / 127 per output channel, folded into the BatchNorm
@@ -178,10 +179,20 @@ int vp3d_int8_thresholds(const uint64_t* hist, int layers, int method, double pa
  * conv and the BatchNorm packs current folds them into the int8 affine; until then vp3d_forward_eval
  * returns VP3D_ERR_STATE. */
 int vp3d_set_int8_scales(vp3d_plan* int8_plan, const float* amax_host, int n);
+/* Chooses which residual blocks of an int8 plan run u8 x s8 (not in the reference): bit i - 1 of
+ * mask selects block i (1..B); the default is every block.  The other blocks run exactly as in
+ * VP3D_PRECISION_FP16 (fp16 operands and packs, K per tap = channels rounded up to 64); expand and
+ * shrink stay fp16.  Where an fp16 block i feeds an int8 block, one extra launch quantises the
+ * stored fp16 X_i to Q_i.  The calibration is the same for every mask.  A changed mask marks the
+ * conv packs stale: vp3d_forward_eval returns VP3D_ERR_STATE until the next vp3d_set_weights
+ * (VP3D_PACK_CONV) re-packs and re-folds.  VP3D_ERR_INVALID for a null plan, a plan that is not
+ * int8 or bits at or above B. */
+int vp3d_set_int8_blocks(vp3d_plan* int8_plan, uint32_t mask);
 /* Copies the int8 packs of layers_conv[layer] of an int8 plan (as its last vp3d_set_weights left
  * them) to DEVICE buffers, each may be NULL: w_s8 [taps][n_pad][k_pad] s8 with n_pad = channels
  * rounded up to 64 and k_pad = n_pad rounded up to 128; w_scale and q_scale [n_pad] fp32 (q_scale
- * as last folded; VP3D_ERR_STATE before the first fold).  For checking the packs. */
+ * as last folded; VP3D_ERR_STATE before the first fold).  VP3D_ERR_INVALID for a layer of a block
+ * that vp3d_set_int8_blocks left in fp16.  For checking the packs. */
 int vp3d_int8_packs(const vp3d_plan* int8_plan, int layer, void* w_s8, float* w_scale,
                     float* q_scale, void* stream);
 

@@ -225,6 +225,7 @@ SIGNATURES = {
                                             ctypes.c_size_t, ctypes.c_void_p]),
     "vp3d_set_int8_scales": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
                                             ctypes.c_int]),
+    "vp3d_set_int8_blocks": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint32]),
     "vp3d_int8_packs": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_forward_eval_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,

@@ -312,6 +312,21 @@ int plan_alloc(vp3d_plan* p, void** out, size_t bytes) {
   return VP3D_OK;
 }
 
+// K per tap of layers_conv[l]'s forward pack: C, or in an int8 block C padded to the 128-element
+// k-blocks of the u8 x s8 GEMM (zero weights)
+static int conv_k_pad(const vp3d_plan* p, int l) {
+  return block_is_int8(p, l / 2 + 1) ? round_up(p->C, kBlockK8) : p->C;
+}
+
+// Device bytes allocated for pack k: a block conv of an int8 plan holds either format, whichever
+// vp3d_set_int8_blocks picks for its block; the 16-bit pack (K per tap C, 2 bytes) is the larger.
+static size_t pack_capacity(const vp3d_plan* p, const PackedConv& k) {
+  const size_t b = pack_bytes(p, k);
+  if (!p->int8 || k.transposed || k.src < 0) return b;
+  const size_t b16 = (size_t)k.stored_taps * k.n_pad * p->C * sizeof(__nv_bfloat16);
+  return b > b16 ? b : b16;
+}
+
 // The pack table of a plan whose shape fields are set (internal.cuh, PackedConv).
 static void plan_packs(vp3d_plan* p) {
   auto add = [p](int src, int c_out, int c_in, int taps, bool transposed, bool merged, int n_pad,
@@ -326,10 +341,8 @@ static void plan_packs(vp3d_plan* p) {
   auto layer_taps = [p](int l) { return l % 2 == 0 ? p->taps[l / 2 + 1] : 1; };
   p->expand_dil = add(kSrcExpand, cr, p->c_in_raw, w0, false, false, C, p->c_in_pad);
   p->expand_flat = add(kSrcExpand, cr, p->c_in_raw, w0, false, true, C, p->k0_pad);
-  // (int8 block convs: 128-element k-blocks, the K per tap padded to 128 with zero weights)
-  const int k_conv = p->int8 ? round_up(C, kBlockK8) : C;
   for (int l = 0; l < 2 * p->nb; ++l)
-    p->conv[l] = add(l, cr, cr, layer_taps(l), false, false, C, k_conv);
+    p->conv[l] = add(l, cr, cr, layer_taps(l), false, false, C, conv_k_pad(p, l));
   p->shrink = add(kSrcShrink, p->c_out_raw, cr, 1, false, false, p->c_out_pad, C);
   for (int l = 0; l < 2 * p->nb; ++l) p->conv_t[l] = add(l, cr, cr, layer_taps(l), true, false, C, C);
   // K of the shrink data gradient (dY's columns) padded to 128: also the row pitch of the padded dY
@@ -439,6 +452,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
   p->c_out_pad = round_up(p->c_out_raw, 64);
   p->int8 = cfg->precision == VP3D_PRECISION_INT8 ? 1 : 0;
   p->f16 = (cfg->precision == VP3D_PRECISION_FP16 || p->int8) ? 1 : 0;
+  p->int8_mask = p->int8 ? (1u << p->nb) - 1u : 0u;
   p->planes = (cfg->precision == VP3D_PRECISION_BF16 || p->f16) ? 1 : 2;
   // model.py:31, 107-121 / :172-184
   p->pad[0] = cfg->filter_widths[0] / 2;
@@ -473,7 +487,7 @@ extern "C" __attribute__((visibility("default"))) int vp3d_plan_create(const vp3
   do {
     for (int i = 0; i < p->n_packs && !st; ++i)
       if (!p->packs[i].transposed)
-        st = plan_alloc(p, reinterpret_cast<void**>(&p->packs[i].w), pack_bytes(p, p->packs[i]));
+        st = plan_alloc(p, reinterpret_cast<void**>(&p->packs[i].w), pack_capacity(p, p->packs[i]));
     if (st) break;
     // affine vectors: expand + 2*nb layers (C each) + shrink (c_out_pad)
     float* aff = nullptr;
@@ -568,8 +582,9 @@ extern "C" __attribute__((visibility("default"))) int vp3d_set_weights(vp3d_plan
     p->int8_folded = false;
     if (p->int8_scales && p->conv_packed && p->bn_packed) {
       for (int l = 0; l < 2 * p->nb; ++l)
-        CUDA_TRY(launch_int8_fold(p->conv[l]->scale, p->conv[l]->w_scale, p->act_scale[l],
-                                  p->conv[l]->q_scale, p->C, stream));
+        if (block_is_int8(p, l / 2 + 1))
+          CUDA_TRY(launch_int8_fold(p->conv[l]->scale, p->conv[l]->w_scale, p->act_scale[l],
+                                    p->conv[l]->q_scale, p->C, stream));
       p->int8_folded = true;
     }
   }
@@ -790,8 +805,19 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
     }
     d.out = s.out; d.out_plane_stride = s.out_plane;
     d.lo_row_begin = s.lo_row_begin; d.lo_row_end = s.lo_row_end;
-    if (s.q_out) { d.out_u8 = s.q_out; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[2 * i]; }
+    // Q_i: the expand's epilogue writes Q_0 from its fp32 value; no GEMM writes fp16 + residual +
+    // u8, so after an fp16 block a pass of its own quantises the stored fp16 X_i
+    if (s.q_out && i == 0) {
+      d.out_u8 = s.q_out; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[0];
+    }
     VP3D_TRY(launch(d));
+    if (s.q_out && i > 0) {
+      if (c.profile) VP3D_TRY(prof_event(p, *launches, true, stream));
+      CUDA_TRY(launch_quantize_u8(s.out, s.q_out, (long long)c.samples * s.out_rows, C, p->c_real,
+                                  p->act_inv[2 * i], num_sms(), stream));
+      if (c.profile) VP3D_TRY(prof_event(p, *launches, false, stream));
+      ++*launches;
+    }
     if (i < p->nb) VP3D_TRY(amax(2 * i, s.out, (long long)c.samples * s.out_rows * C));
   }
   if (!c.y) return VP3D_OK;
@@ -870,7 +896,8 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
     s.in = i == 0 ? bf(wl.a0) : c.st[i - 1].out;
     s.out = bf(i % 2 ? wl.x1 : wl.x0);
     s.out_plane = s.h_plane = (long long)N * L[i] * C;
-    if (p->int8 && i < p->nb) s.q_out = base + wl.q;
+    // Q_i exists where block i + 1 runs u8 x s8
+    if (i < p->nb && block_is_int8(p, i + 1)) s.q_out = base + wl.q;
   }
 
   // Per-layer operand precision.  index 0 = expand, 1..nb = residual blocks, nb+1 = shrink.
@@ -880,7 +907,7 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
   //            split-bf16 (they carry most of the bf16 error, tools/precision_study.py),
   //            residual blocks run plain bf16 on the hi plane unless they hold < 0.5% of the
   //            forward FLOPs (negligible even at the narrow-tile rate of such layers).
-  //   int8   : residual blocks u8 x s8, expand and shrink fp16.
+  //   int8   : the residual blocks of int8_mask u8 x s8; expand, shrink and the other blocks fp16.
   {
     double fl[VP3D_MAX_WIDTHS + 1], total = 0.0;
     fl[0] = (double)N * L[0] * p->c_in_raw * fw[0] * C;
@@ -892,8 +919,9 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
       const bool edge = i == 0 || i == p->nb + 1;
       c.precision[i] = p->cfg.precision == VP3D_PRECISION_MIXED
                            ? (x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16)
-                       : p->cfg.precision == VP3D_PRECISION_INT8 && edge ? VP3D_PRECISION_FP16
-                                                                         : p->cfg.precision;
+                       : p->int8 ? (!edge && block_is_int8(p, i) ? VP3D_PRECISION_INT8
+                                                                  : VP3D_PRECISION_FP16)
+                                 : p->cfg.precision;
     }
   }
 }
@@ -1113,6 +1141,9 @@ extern "C" __attribute__((visibility("default"))) int vp3d_int8_packs(
     const vp3d_plan* p, int layer, void* w_s8, float* w_scale, float* q_scale, void* stream_) {
   if (!p || !p->int8) return fail(VP3D_ERR_INVALID, "int8_packs: not an int8 plan");
   if (layer < 0 || layer >= 2 * p->nb) return fail(VP3D_ERR_INVALID, "int8_packs: no layer %d", layer);
+  if (!block_is_int8(p, layer / 2 + 1))
+    return fail(VP3D_ERR_INVALID, "int8_packs: layer %d is in block %d, which runs fp16 "
+                "(vp3d_set_int8_blocks)", layer, layer / 2 + 1);
   if (!p->conv_packed) return fail(VP3D_ERR_STATE, "int8_packs: weights not packed yet");
   if (q_scale && !p->int8_folded) return fail(VP3D_ERR_STATE, "int8_packs: scales not folded yet");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -1143,6 +1174,23 @@ extern "C" __attribute__((visibility("default"))) int vp3d_set_int8_scales(vp3d_
     p->act_inv[l] = 1.0f / s;
   }
   p->int8_scales = true;
+  p->int8_folded = false;
+  return VP3D_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int vp3d_set_int8_blocks(vp3d_plan* p,
+                                                                          uint32_t mask) {
+  if (!p) return fail(VP3D_ERR_INVALID, "set_int8_blocks: null plan");
+  if (!p->int8) return fail(VP3D_ERR_INVALID, "set_int8_blocks: not an int8 plan");
+  const uint32_t all = (1u << p->nb) - 1u;
+  if (mask & ~all)
+    return fail(VP3D_ERR_INVALID, "set_int8_blocks: mask 0x%x selects blocks beyond the plan's %d",
+                (unsigned)mask, p->nb);
+  if (mask == p->int8_mask) return VP3D_OK;
+  p->int8_mask = mask;
+  for (int l = 0; l < 2 * p->nb; ++l) p->conv[l]->k_pad = conv_k_pad(p, l);
+  // the packs of the blocks that changed format are stale until the next vp3d_set_weights
+  p->conv_packed = false;
   p->int8_folded = false;
   return VP3D_OK;
 }

@@ -80,9 +80,10 @@ struct PackedConv {
   __nv_bfloat16* w = nullptr;  // transposed packs: allocated with the training state
   float* scale = nullptr;      // forward packs: eval affine of the conv's output [n_pad]
   float* shift = nullptr;
-  // int8 plans, residual-block convs: w holds s8 [taps][n_pad][k_pad] (k_pad a multiple of 128),
-  // w_scale its per-channel weight scales and q_scale the affine scale with both dequantisation
-  // factors folded in (launch_int8_fold), both [n_pad]
+  // int8 plans, the convs of the blocks in int8_mask: w holds s8 [taps][n_pad][k_pad] (k_pad a
+  // multiple of 128), w_scale its per-channel weight scales and q_scale the affine scale with both
+  // dequantisation factors folded in (launch_int8_fold), both [n_pad]; the other blocks' convs
+  // hold the fp16 pack of an FP16 plan (k_pad = C)
   float* w_scale = nullptr;
   float* q_scale = nullptr;
 };
@@ -175,6 +176,8 @@ struct vp3d_plan {
   int planes = 1;
   int f16 = 0;  // VP3D_PRECISION_FP16 (and INT8): 16-bit stores hold IEEE fp16
   int int8 = 0; // VP3D_PRECISION_INT8: the residual blocks' convs run u8 x s8
+  // int8: bit i - 1 set = block i runs u8 x s8, the others as in FP16 (vp3d_set_int8_blocks)
+  uint32_t int8_mask = 0;
   // int8: activation scale s and 1 / s of every block conv's input (vp3d_set_int8_scales), and
   // whether the packs' q_scale vectors have been folded from the current scales
   bool int8_scales = false, int8_folded = false;
@@ -213,9 +216,13 @@ bool use_strided(const vp3d_plan* p, int T);
 // rows per sample after each stage: L[0] = rows out of expand, L[i] = rows out of block i
 int layer_rows(const vp3d_plan* p, int T, bool strided, int* L);
 int strided_trim(const vp3d_plan* p, int* L);
-// int8 plans keep the residual-block convs' forward packs in s8
+// whether residual block i (1..nb) runs u8 x s8
+inline bool block_is_int8(const vp3d_plan* p, int i) {
+  return p->int8 && ((p->int8_mask >> (i - 1)) & 1u);
+}
+// int8 plans keep the forward packs of their int8 blocks' convs in s8
 inline bool pack_is_s8(const vp3d_plan* p, const PackedConv& k) {
-  return p->int8 && !k.transposed && k.src >= 0;
+  return !k.transposed && k.src >= 0 && block_is_int8(p, k.src / 2 + 1);
 }
 inline size_t pack_bytes(const vp3d_plan* p, const PackedConv& k) {
   return (size_t)p->planes * k.stored_taps * k.n_pad * k.k_pad *

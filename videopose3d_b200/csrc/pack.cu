@@ -1,6 +1,7 @@
 #include "pack.cuh"
 
 #include "conv_gemm.cuh"   // kMaxDevices
+#include "ptx.cuh"         // quant_u8
 
 #include <string.h>
 
@@ -347,6 +348,48 @@ cudaError_t launch_count_nonfinite(const float* x, long long n, unsigned long lo
   long long blocks = (n + 255) / 256;
   if (blocks > 8LL * num_sms) blocks = 8LL * num_sms;
   count_nonfinite_kernel<<<(int)blocks, 256, 0, stream>>>(x, n, count);
+  return cudaGetLastError();
+}
+
+// One 16-byte vector (8 fp16 values of one row) per thread and step; vector i holds channels
+// 8 * (i mod c8) .. + 7, the column stepped as in hist_f16_kernel.
+__global__ void __launch_bounds__(256)
+quantize_u8_kernel(const uint4* __restrict__ x, uint2* __restrict__ q, long long n8, int c8,
+                   int c_real, float inv_s) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  int col = (int)(i % c8);
+  const int col_step = (int)(stride % c8);
+  for (; i < n8; i += stride) {
+    const int valid = c_real - 8 * col;   // real channels in this vector
+    uint32_t b[2] = {0u, 0u};
+    if (valid > 0) {
+      const uint4 v = __ldg(x + i);
+      const unsigned u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float f = __half2float(__ushort_as_half((unsigned short)(u[k >> 1] >> (16 * (k & 1)))));
+        if (k < valid) b[k >> 2] |= quant_u8(f, inv_s) << (8 * (k & 3));
+      }
+    }
+    q[i] = make_uint2(b[0], b[1]);
+    col += col_step;
+    if (col >= c8) col -= c8;
+  }
+}
+
+cudaError_t launch_quantize_u8(const void* x, uint8_t* q, long long rows, int ld, int c_real,
+                               float inv_s, int num_sms, cudaStream_t stream) {
+  if (ld % 8 || c_real < 1 || c_real > ld || rows < 0 || reinterpret_cast<uintptr_t>(x) % 16 ||
+      reinterpret_cast<uintptr_t>(q) % 8)
+    return cudaErrorInvalidValue;
+  const long long n8 = rows * (ld / 8);
+  if (n8 == 0) return cudaSuccess;
+  long long blocks = (n8 + 255) / 256;
+  if (blocks > 8LL * num_sms) blocks = 8LL * num_sms;
+  quantize_u8_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const uint4*>(x),
+                                                      reinterpret_cast<uint2*>(q), n8, ld / 8,
+                                                      c_real, inv_s);
   return cudaGetLastError();
 }
 

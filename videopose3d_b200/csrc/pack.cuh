@@ -87,6 +87,11 @@ cudaError_t launch_amax_f16(const void* x, long long n, unsigned* amax_bits, cud
 constexpr int kHistBins = 0x7C00;   // 31 744: every finite fp16 value >= 0
 cudaError_t launch_hist_f16(const void* x, long long rows, int ld, int c_real, unsigned long long* hist,
                             unsigned long long* invalid, int num_sms, cudaStream_t stream);
+// u8 codes of one stored fp16 plane [rows][ld] (x 16-byte, q 8-byte aligned, ld % 8 == 0) into q
+// [rows][ld]: q = cvt.rni.sat.u8.f32(fp32(x) * inv_s) on every row's first c_real channels, 0 on
+// the rest.  Makes Q_i of an int8 block whose input an fp16 block wrote.
+cudaError_t launch_quantize_u8(const void* x, uint8_t* q, long long rows, int ld, int c_real,
+                               float inv_s, int num_sms, cudaStream_t stream);
 // *count += the number of inf / NaN values among x[0, n)
 cudaError_t launch_count_nonfinite(const float* x, long long n, unsigned long long* count,
                                    int num_sms, cudaStream_t stream);

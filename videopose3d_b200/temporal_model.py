@@ -47,9 +47,11 @@ class _Plan:
     (VP3D_PACK_EXPAND_T, the expand conv weight's entry only).  ``bn_sync`` is (reducer, ctypes
     exchange callback) while the plan's synchronized BatchNorm is on (vp3d_set_bn_sync): the plan
     holds the callback as long as it may call it.  ``int8`` is the calibration (the module's
-    ``_int8`` tuple) whose scales an int8 plan holds, None before any."""
+    ``_int8`` tuple) whose scales an int8 plan holds, None before any; ``int8_mask`` the block
+    mask (vp3d_set_int8_blocks) it was last given, None before any."""
 
-    __slots__ = ("handle", "precision", "eval", "train", "expand_t", "bn_sync", "int8")
+    __slots__ = ("handle", "precision", "eval", "train", "expand_t", "bn_sync", "int8",
+                 "int8_mask")
 
     def __init__(self, handle, precision):
         self.handle = handle
@@ -57,6 +59,7 @@ class _Plan:
         self.eval = self.train = self.expand_t = None
         self.bn_sync = None
         self.int8 = None
+        self.int8_mask = None
 
     @property
     def _as_parameter_(self):
@@ -153,6 +156,8 @@ class TemporalModelBase(nn.Module):
         self._grad_reducer = None  # data_parallel.GradientReducer, set by its attach()
         # int8 calibration: (amax CPU float tensor [2B], parameter versions it belongs to), or None
         self._int8 = None
+        # blocks (1..B) the 'int8' precision runs u8 x s8, None = all (set_int8_blocks)
+        self._int8_blocks = None
         self.last_predict_launches = 0   # kernels the last predict() launched
 
     def _build_layers(self, strided):
@@ -236,8 +241,8 @@ class TemporalModelBase(nn.Module):
         'int8': the residual blocks' convs on u8 activations times s8 weights (exact int32 sums),
         the rest as 'fp16' -- about 0.73x the fp16 forward time on the bench model (H100), at
         ~5e-3 of fp32 on a random-init model (ten times fp16's error; trained checkpoints not
-        measured).  Needs ``calibrate_int8`` or ``load_int8_calibration`` first.  Not in the
-        reference."""
+        measured).  Needs ``calibrate_int8`` or ``load_int8_calibration`` first;
+        ``set_int8_blocks`` keeps chosen blocks in fp16.  Not in the reference."""
         if precision not in _PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(_PRECISIONS)}")
         self._precision = precision
@@ -357,9 +362,42 @@ class TemporalModelBase(nn.Module):
         self._int8 = (amax.clone(), self._versions())
         return self
 
+    def set_int8_blocks(self, blocks=None):
+        """Which residual blocks (numbered 1..B) the 'int8' precision runs on u8 x s8: an iterable
+        of block numbers, ``[]`` for none, or None (the default) for all.  Every other block runs
+        exactly as in 'fp16'; expand and shrink are fp16 either way.  Keeping the blocks whose
+        quantisation costs the most accuracy in fp16 trades some of int8's speed for accuracy;
+        measure each block's error as in the README.  One calibration serves every set.  Kept out
+        of the state_dict, like the calibration; copies and pickles carry it.  Returns self.  Not in
+        the reference."""
+        nb = len(self.filter_widths) - 1
+        if blocks is not None:
+            blocks = list(blocks)
+            for b in blocks:
+                if isinstance(b, bool) or not isinstance(b, int):
+                    raise ValueError(f"int8 blocks are ints in 1..{nb} (got {b!r})")
+                if not 1 <= b <= nb:
+                    raise ValueError(f"int8 block {b} is outside 1..{nb}")
+            blocks = tuple(sorted(set(blocks)))
+        self._int8_blocks = blocks
+        return self
+
+    @property
+    def int8_blocks(self):
+        """The blocks (1..B) the 'int8' precision runs on u8 x s8, as a sorted tuple."""
+        if self._int8_blocks is None:
+            return tuple(range(1, len(self.filter_widths)))
+        return self._int8_blocks
+
     def _sync_int8(self, plan):
-        """Give an int8 plan the scales of the current calibration (its next weight sync folds
-        them); raises when there is none or the parameters changed since it was taken."""
+        """Give an int8 plan the block set and the scales of the current calibration (its next
+        weight sync re-packs and folds them); raises when there is no calibration or the parameters
+        changed since it was taken."""
+        mask = sum(1 << (b - 1) for b in self.int8_blocks)
+        if plan.int8_mask != mask:
+            _capi.check(_capi.load().vp3d_set_int8_blocks(plan, mask), "vp3d_set_int8_blocks")
+            plan.int8_mask = mask
+            plan.eval = None   # the next sync re-packs in the new formats
         if self._int8 is None:
             raise RuntimeError("precision 'int8' needs calibrate_int8(inputs) or "
                                "load_int8_calibration(amax) first")
