@@ -86,6 +86,31 @@ CASES = {
                                 N=2, T=250, store_sd=False),
     "opt_33333_c1024": dict(cls="TemporalModelOptimized1f", J=17, F=2, Jout=17, fw=[3, 3, 3, 3, 3],
                             C=1024, N=8, T=243, store_sd=False),
+    # filter widths other than 3 and 5: run.py's documented examples 3,3,7 (RF 63) and 3,5,5, an
+    # expand of width 7, 1-tap layers (no history), and the 32-joint skeleton with 3-D inputs
+    "tm_337_c256_rf": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 3, 7], C=256, N=3, T=63,
+                           store_sd=False),
+    "tm_337_c256_t90": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 3, 7], C=256, N=2, T=90,
+                            store_sd=False),
+    "opt_337_c128": dict(cls="TemporalModelOptimized1f", J=17, F=2, Jout=17, fw=[3, 3, 7], C=128, N=4,
+                         T=63, store_sd=False),
+    "tm_355_c100_t90_causal": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 5, 5], C=100, N=2,
+                                   T=90, causal=True),
+    "tm_733_c128_t80": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[7, 3, 3], C=128, N=2, T=80,
+                            store_sd=False),
+    "tm_313_c64_t20": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 1, 3], C=64, N=3, T=20),
+    "tm_133_c64_t20": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[1, 3, 3], C=64, N=3, T=20),
+    "tm_333_c128_j32_f3": dict(cls="TemporalModel", J=32, F=3, Jout=32, fw=[3, 3, 3], C=128, N=2, T=40,
+                               store_sd=False),
+    "tm_337_c64_t80_dense": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 3, 7], C=64, N=2, T=80,
+                                 dense=True, store_sd=False),
+    "opt_337_c64_train": dict(cls="TemporalModelOptimized1f", J=17, F=2, Jout=17, fw=[3, 3, 7], C=64,
+                              N=6, T=63, train=True, momentum=0.1),
+    "opt_733_c64_train": dict(cls="TemporalModelOptimized1f", J=17, F=2, Jout=17, fw=[7, 3, 3], C=64,
+                              N=6, T=63, train=True, momentum=0.1),
+    # dilated training on run.py --stride 140 chunks: 140 output frames per sample, two 128-row tiles
+    "tm_337_c64_t202_train": dict(cls="TemporalModel", J=17, F=2, Jout=17, fw=[3, 3, 7], C=64, N=2,
+                                  T=202, train=True, momentum=0.1, store_sd=False),
 }
 
 

@@ -45,6 +45,9 @@ CASES = {
     "tm_333_c100_j15": dict(cls=_TM, J=15, F=2, Jout=15, fw=[3, 3, 3], C=100, N=2, T=30),
     "opt_333_c64_rf": dict(cls=_OPT, J=17, F=2, Jout=17, fw=[3, 3, 3], C=64, N=4, T=27),
     "opt_333_c64_t30": dict(cls=_OPT, J=17, F=2, Jout=17, fw=[3, 3, 3], C=64, N=3, T=30),
+    # expand width 7: the tap-merged transposed expand and the strided tail (68 = 7 * 9 + 5);
+    # 16 channels keep every gradient whole and the fixture small
+    "opt_733_c16_t68": dict(cls=_OPT, J=17, F=2, Jout=17, fw=[7, 3, 3], C=16, N=3, T=68),
     # train mode, dropout 0 (BatchNorm batch statistics)
     "train_opt_333_c64": dict(cls=_OPT, J=17, F=2, Jout=17, fw=[3, 3, 3], C=64, N=6, T=27,
                               train=True),

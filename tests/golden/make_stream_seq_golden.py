@@ -29,11 +29,14 @@ OUT = os.path.join(HERE, "stream_seq")
 # Human3.6M's 17-joint skeleton (the reference's kps_left/right and joints_left/right, run.py:67-69)
 LEFT, RIGHT = [4, 5, 6, 11, 12, 13], [1, 2, 3, 14, 15, 16]
 
-# name -> (filter widths, causal, dense, channels, J_out, augment, lengths, seed); RF 27 and 45
+# name -> (filter widths, causal, dense, channels, J_out, augment, lengths, seed); RF 27, 45, 63
+# (3,3,7: run.py's documented example) and 9 (3,1,3: a 1-tap block, whose ring keeps no history)
 CASES = {
     "seq_333_c64_tta": ([3, 3, 3], False, False, 64, 17, True, [40, 1, 13, 29, 5, 2], 61),
     "seq_333_c64_causal": ([3, 3, 3], True, False, 64, 17, False, [33, 7, 1, 26, 50], 62),
     "seq_353_c128_traj_tta": ([3, 5, 3], False, False, 128, 1, True, [1, 60, 44, 3, 17], 63),
+    "seq_337_c64_tta": ([3, 3, 7], False, False, 64, 17, True, [70, 1, 20, 63, 2, 64], 64),
+    "seq_313_c64_causal": ([3, 1, 3], True, False, 64, 17, False, [15, 1, 9, 30, 4, 8], 65),
 }
 
 

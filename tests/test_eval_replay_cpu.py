@@ -36,6 +36,21 @@ ARCHS = [
     ("tm_333_j15_f3", _cfg(TM, [3, 3, 3], 64, J=15, F=3, Jout=15), 3, 27),
     ("tm_353_traj", _cfg(TM, [3, 5, 3], 128, Jout=1), 2, 60),
     ("tm_333333_c64_split", _cfg(TM, [3, 3, 3, 3, 3, 3], 64), 1, 729),
+    # widths other than 3 and 5, and the 32-joint skeleton (tests/test_gpu_architectures.py)
+    ("a337_cone", _cfg(TM, [3, 3, 7], 1024), 2, 63),
+    ("a337_dilated", _cfg(TM, [3, 3, 7], 1024), 1, 90),
+    ("a337_opt", _cfg(OPT, [3, 3, 7], 1024), 2, 63),
+    ("a355c_cone", _cfg(TM, [3, 5, 5], 100, causal=True), 2, 75),
+    ("a355c_dilated", _cfg(TM, [3, 5, 5], 100, causal=True), 1, 100),
+    ("a733_opt", _cfg(OPT, [7, 3, 3], 256), 2, 63),
+    ("a733_dilated", _cfg(TM, [7, 3, 3], 256), 1, 80),
+    ("a313_cone", _cfg(TM, [3, 1, 3], 128), 3, 9),
+    ("a313_dilated", _cfg(TM, [3, 1, 3], 128), 2, 20),
+    ("a133_opt", _cfg(OPT, [1, 3, 3], 128), 3, 9),
+    ("a133_dilated", _cfg(TM, [1, 3, 3], 128), 2, 20),
+    ("j32_cone", _cfg(TM, [3, 3, 3], 256, J=32, F=3, Jout=32), 2, 27),
+    ("j32_dilated", _cfg(TM, [3, 3, 3], 256, J=32, F=3, Jout=32), 1, 40),
+    ("d337_dense", _cfg(TM, [3, 3, 7], 128, dense=True), 1, 80),
 ]
 
 
@@ -176,7 +191,8 @@ def _peel(r, n, perm_regions, perm_widths, last_rows):
     return row + n * last_rows + t
 
 
-@pytest.mark.parametrize("fw,N", [([3, 3, 3, 3, 3], 5), ([3, 5, 3], 4), ([5, 3], 3), ([3, 7], 2)])
+@pytest.mark.parametrize("fw,N", [([3, 3, 3, 3, 3], 5), ([3, 5, 3], 4), ([5, 3], 3), ([3, 7], 2),
+                                  ([3, 3, 7], 2), ([7, 3, 3], 2), ([3, 1, 3], 3), ([1, 3, 3], 3)])
 def test_tap_major_permutation(fw, N):
     cfg = _cfg(OPT, fw, 64)
     p = er.Plan(cfg, "fp16", N, 1 + 2 * sum(orc.arch(fw)["pad"]))

@@ -212,7 +212,10 @@ def _check_ranks_agree(res):
 
 SHARDED = [("opt_35_c128_train_causal", 3),   # N = 70: rows 24 / 23 / 23
            ("tm_333_c128_train", 2),          # N = 3: 2 / 1 sequences, dilated
-           ("opt_333_c128_train", 2)]         # N = 40: equal shards
+           ("opt_333_c128_train", 2),         # N = 40: equal shards
+           ("opt_337_c64_train", 4),          # N = 6: 2 / 2 / 1 / 1, a width-7 block
+           ("opt_733_c64_train", 2),          # N = 6: expand width 7
+           ("tm_337_c64_t202_train", 2)]      # N = 2: one 140-frame sequence each, dilated
 
 
 @pytest.mark.parametrize("name,world", SHARDED)

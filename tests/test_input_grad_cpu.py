@@ -68,7 +68,7 @@ def compare(got, want):
 
 
 def test_fixture_set():
-    assert len(NAMES) == 14
+    assert len(NAMES) == 15
     total = sum(os.path.getsize(os.path.join(GOLDEN, n + ".npz")) for n in NAMES)
     assert total < 2 * 1024 * 1024
 

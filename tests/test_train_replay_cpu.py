@@ -37,6 +37,16 @@ ARCHS = [
     ("tm_333_dilated", _cfg(TM, [3, 3, 3], 64), 2, 40),
     ("tm_35_causal", _cfg(TM, [3, 5], 64, causal=True), 2, 30),
     ("tm_33_dense", _cfg(TM, [3, 3], 64, dense=True), 2, 20),
+    # widths other than 3 and 5, and the 32-joint skeleton (tests/test_gpu_architectures.py)
+    ("opt_337", _cfg(OPT, [3, 3, 7], 128), 2, 63),
+    ("opt_355_causal", _cfg(OPT, [3, 5, 5], 100, causal=True), 2, 75),
+    ("opt_733_t68", _cfg(OPT, [7, 3, 3], 64), 2, 68),
+    ("opt_313", _cfg(OPT, [3, 1, 3], 64), 3, 9),
+    ("opt_133", _cfg(OPT, [1, 3, 3], 64), 3, 9),
+    ("opt_j32_f3", _cfg(OPT, [3, 3, 3], 64, J=32, F=3, Jout=32), 3, 27),
+    ("tm_337_dilated", _cfg(TM, [3, 3, 7], 64), 1, 70),
+    ("tm_313_dilated", _cfg(TM, [3, 1, 3], 64), 2, 20),
+    ("tm_337_dense", _cfg(TM, [3, 3, 7], 64, dense=True), 1, 70),
 ]
 
 
@@ -129,7 +139,10 @@ def _launches(p, dx):
 
 @pytest.mark.parametrize("precision", ["bf16", "bf16x3"])
 @pytest.mark.parametrize("name,cfg,N,T", [("opt_333_t29", _cfg(OPT, [3, 3, 3], 64), 3, 29),
-                                          ("tm_35_causal", _cfg(TM, [3, 5], 64, causal=True), 2, 30)])
+                                          ("tm_35_causal", _cfg(TM, [3, 5], 64, causal=True), 2, 30),
+                                          ("opt_733_t68", _cfg(OPT, [7, 3, 3], 64), 2, 68),
+                                          ("opt_133", _cfg(OPT, [1, 3, 3], 64), 2, 9),
+                                          ("tm_337_dilated", _cfg(TM, [3, 3, 7], 64), 1, 70)])
 def test_float64_replay_input_gradient(name, cfg, N, T, precision):
     """dx: the strided tail (T != w0 * L0: the trailing frames get zero) and the dilated transposed
     expand conv, against float64 autograd; also the launch counts."""
@@ -139,7 +152,7 @@ def test_float64_replay_input_gradient(name, cfg, N, T, precision):
     bad = {k: v for k, v in d.items() if not v <= TOL}
     assert not bad, bad
     if cfg["cls"] == OPT:
-        assert torch.all(rep.dx[:, 27:] == 0)
+        assert torch.all(rep.dx[:, rep.plan.fw[0] * rep.plan.L[0]:] == 0)
     assert (rep.fwd_launches, rep.bwd_launches) == _launches(rep.plan, True)
 
 
@@ -179,6 +192,7 @@ MUTATIONS = [
     ("tap_sign", ("tm_333_dilated", _cfg(TM, [3, 3, 3], 64), 2, 40)),
     ("pingpong", ("opt_333_c64", _cfg(OPT, [3, 3, 3], 64), 4, 27)),
     ("pingpong", ("tm_35_causal", _cfg(TM, [3, 5], 64, causal=True), 2, 30)),
+    ("tap_sign", ("tm_337_dilated", _cfg(TM, [3, 3, 7], 64), 1, 70)),
 ]
 
 
