@@ -393,6 +393,19 @@ typedef struct {
 } vp3d_conv_desc;
 
 int vp3d_conv_gemm(const vp3d_conv_desc* d, void* stream);
+/* The kernel instance vp3d_conv_gemm(d) would run on the current device, under the SM limit of
+ * vp3d_set_sm_limit: validates d and builds the launch exactly as vp3d_conv_gemm does, then writes
+ * key[0..6] instead of launching:
+ *   block_n (64 | 128), epilogue (0 training, 1 general, 2 lean),
+ *   operand format (0 bf16 / fp16 read from the launch, 1 bf16, 2 fp16, 3 int8),
+ *   schedule (0 cooperative, 1 ping-pong), auxiliary TMA tiles (0 | 1), two output planes (0 | 1),
+ *   u8 output (0 none, 1 beside the 16-bit plane, 2 alone).
+ * VP3D_ERR_UNSUPPORTED if that instance is not compiled (vp3d_conv_gemm then fails too);
+ * VP3D_ERR_INVALID for out_rows == 0 (nothing is launched). */
+int vp3d_conv_gemm_instance(const vp3d_conv_desc* d, int* key);
+/* The keys of every compiled conv GEMM instance, 7 ints each as above, into keys[0 .. 7 * max);
+ * returns how many instances are compiled (possibly more than max). */
+int vp3d_conv_gemm_instances(int* keys, int max);
 
 /* Weight gradient of one temporal convolution, the call vp3d_backward makes for every conv layer
  * (autograd's conv backward-filter):

@@ -130,3 +130,40 @@ def expected_conv(a_val, w_val, *, samples, a_rows, taps, k_per_tap, per_sample_
         c0 = tap * tap_col_step
         acc += flat[r0:r0 + out_rows, c0:c0 + k_per_tap] @ w_val[tap].T
     return acc
+
+
+def expected_residual(res_val, n_pad, *, samples, out_rows, per_sample_tiles, res_rows_per_sample=0,
+                      res_row_step=1, res_row_off=0, res_sample_div=0, res_check_rows=0,
+                      res_col_begin=0, res_cols=0):
+    """fp64 value the epilogue adds to every output element, [total_rows, n_pad] (zero where
+    nothing is added).  res_val: [planes, rows, res_ld] fp64, the planes summed.
+    Output row t of sample s (flat tiles: s = 0, t = the row; with res_sample_div, s = t // div and
+    t = t % div) reads residual row s * res_rows_per_sample + t * res_row_step + res_row_off; with
+    res_check_rows a row whose in-sample index t * step + off falls outside [0, res_rows_per_sample)
+    adds nothing (a per-sample TMA map zero-fills those rows the same way).  Output column c reads
+    residual column c - res_col_begin when its 64-column store block [c0, c0 + 64) starts inside
+    [res_col_begin, res_col_begin + res_cols) (res_cols 0: n_pad)."""
+    dev = res_val.device
+    total = samples * out_rows if per_sample_tiles else out_rows
+    r = torch.arange(total, device=dev)
+    if per_sample_tiles:
+        smp, t = r // out_rows, r % out_rows
+    elif res_sample_div > 0:
+        smp, t = r // res_sample_div, r % res_sample_div
+    else:
+        smp, t = torch.zeros_like(r), r
+    in_sample = t * res_row_step + res_row_off
+    ok = torch.ones_like(r, dtype=torch.bool)
+    if res_check_rows:
+        ok = (in_sample >= 0) & (in_sample < res_rows_per_sample)
+    src = smp * res_rows_per_sample + in_sample
+    cols = res_cols if res_cols > 0 else n_pad
+    c = torch.arange(n_pad, device=dev)
+    cb = c // 64 * 64
+    col_ok = (cb >= res_col_begin) & (cb < res_col_begin + cols)
+    val = res_val.sum(0)
+    out = torch.zeros(total, n_pad, dtype=torch.float64, device=dev)
+    rows_ok, cols_ok = torch.nonzero(ok).flatten(), torch.nonzero(col_ok).flatten()
+    out[rows_ok[:, None], cols_ok[None, :]] = \
+        val[src[rows_ok][:, None], (cols_ok - res_col_begin)[None, :]].double()
+    return out

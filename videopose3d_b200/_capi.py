@@ -260,6 +260,9 @@ SIGNATURES = {
     "vp3d_profile_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
                                          ctypes.POINTER(ctypes.c_int)]),
     "vp3d_conv_gemm": (ctypes.c_int, [ctypes.POINTER(ConvDesc), ctypes.c_void_p]),
+    "vp3d_conv_gemm_instance": (ctypes.c_int, [ctypes.POINTER(ConvDesc),
+                                               ctypes.POINTER(ctypes.c_int)]),
+    "vp3d_conv_gemm_instances": (ctypes.c_int, [ctypes.POINTER(ctypes.c_int), ctypes.c_int]),
     "vp3d_wgrad_gemm": (ctypes.c_int, [ctypes.POINTER(WgradDesc), ctypes.c_void_p]),
     "vp3d_bn_stats_finalize": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _F, _F, _P, _P, _P, _P, _I,
                                     _I, _P, _SZ, _P, _I, _P]),

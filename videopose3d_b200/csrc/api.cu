@@ -119,13 +119,25 @@ int num_sms() {
 }
 
 // ------------------------------------------------------------------ operator level
-int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
+// Everything one conv GEMM launch passes to launch_conv_gemm, validated and built from its
+// descriptor by prepare_conv.  run_conv launches it; vp3d_conv_gemm_instance asks which kernel
+// instance that launch would run -- the same preparation either way.
+struct ConvLaunch {
+  CUtensorMap ma, mw, mo, mr, mz;
+  ConvGemmArgs g;
+  int block_n = 64;
+  int sms = 0;
+  bool empty = false;   // no output rows: nothing to launch
+};
+
+static int prepare_conv(const vp3d_conv_desc* d, ConvLaunch* L) {
   if (!d || !d->a || !d->w) return fail(VP3D_ERR_INVALID, "conv_gemm: null operand");
   if (d->a_ld % 64 || d->k_per_tap % 64 || d->n_pad % 64)
     return fail(VP3D_ERR_INVALID, "conv_gemm: a_ld, k_per_tap and n_pad must be multiples of 64");
   if (d->taps < 1 || d->out_rows < 0 || d->samples < 1)
     return fail(VP3D_ERR_INVALID, "conv_gemm: bad geometry");
-  if (d->out_rows == 0) return VP3D_OK;
+  L->empty = d->out_rows == 0;
+  if (L->empty) return VP3D_OK;
   const int a_planes = d->a_planes > 0 ? d->a_planes : 1;
   const int pairs = d->precision == VP3D_PRECISION_BF16X3 ? 3 : 1;
   const int i8 = d->precision == VP3D_PRECISION_INT8 ? 1 : 0;
@@ -152,22 +164,25 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   // 128-wide N tiles (a 128 x 128 tile per CTA: 64 x 128 wgmma per consumer warpgroup) while they
   // still fill half a wave of the SMs; small layers (few row tiles) fall back to 64-wide tiles so
   // that more SMs share the work.
-  int block_n = 64;
+  int& block_n = L->block_n;
+  L->sms = num_sms();
+  block_n = 64;
   {
     const long long m_tiles = d->per_sample_tiles
                                   ? (long long)d->samples * ((d->out_rows + kBlockM - 1) / kBlockM)
                                   : ((long long)d->out_rows + kBlockM - 1) / kBlockM;
-    if (d->n_pad % 128 == 0 && m_tiles * (d->n_pad / 128) * 2 >= num_sms()) block_n = 128;
+    if (d->n_pad % 128 == 0 && m_tiles * (d->n_pad / 128) * 2 >= L->sms) block_n = 128;
   }
 
-  CUtensorMap ma, mw;
+  CUtensorMap& ma = L->ma;
+  CUtensorMap& mw = L->mw;
   const uint64_t a_rows = d->a_rows, a_ld = d->a_ld;
   // (an explicit plane stride when the A rows are a window into a larger buffer, e.g. a history ring)
   const uint64_t plane_stride = d->a_plane_stride > 0 ? (uint64_t)d->a_plane_stride
                                                       : (uint64_t)d->samples * a_rows * a_ld;
   VP3D_TRY(make_map_4d(&ma, d->a, a_ld, a_rows, a_ld, d->samples, a_rows * a_ld, a_planes,
                        plane_stride, kBlockM, i8 ? 1 : 2));
-  ConvGemmArgs g;
+  ConvGemmArgs& g = L->g;
   memset(&g, 0, sizeof(g));
   g.dilated = d->per_sample_tiles ? 1 : 0;
   g.samples = d->samples;
@@ -216,7 +231,8 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   if (!d->out && !d->out_f32 && !d->out_u8) return fail(VP3D_ERR_INVALID, "conv_gemm: no output");
   if (d->out && (d->out_ld % 8)) return fail(VP3D_ERR_INVALID, "conv_gemm: out_ld % 8 != 0");
   if (d->res && (d->res_ld % 8)) return fail(VP3D_ERR_INVALID, "conv_gemm: res_ld % 8 != 0");
-  CUtensorMap mo = ma;
+  CUtensorMap& mo = L->mo;
+  mo = ma;
   if (d->out) {
     const uint64_t o_rows = d->out_rows, o_ld = d->out_ld;
     const uint64_t o_samples = d->per_sample_tiles ? d->samples : 1;
@@ -232,7 +248,8 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   // with the view's rows `step*ld` elements long (strided layout: off < step), or rows shifted by
   // `off` (step == 1).  Other maps (flat tiles split over samples, bounds-checked rows) keep the
   // register path.
-  CUtensorMap mr = ma;
+  CUtensorMap& mr = L->mr;
+  mr = ma;
   g.res_tma = 0;
   // (per-sample maps zero-fill rows outside the sample, which is exactly what res_check_rows asks)
   if (d->res && (!d->res_check_rows || (d->per_sample_tiles && d->res_row_step == 1)) && d->out &&
@@ -267,7 +284,8 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
     }
   }
   // fused BatchNorm-backward reductions: Z rides the auxiliary TMA path with the output's geometry
-  CUtensorMap mz = mo;
+  CUtensorMap& mz = L->mz;
+  mz = mo;
   g.bnb = 0;
   if (d->bnb_z) {
     if (!d->out || g.out_planes != 1 || (d->res && !g.res_tma) || d->bnb_c <= 0 || d->bnb_c % 64)
@@ -299,7 +317,24 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
                 "TMA can load (one box of a strided row view)");
   VP3D_TRY(make_map_2d(&mw, d->w, d->k_per_tap, (uint64_t)w_planes * d->taps * d->n_pad, block_n,
                        i8 ? 1 : 2));
-  CUDA_TRY(launch_conv_gemm(ma, mw, mo, mr, mz, g, block_n, num_sms(), stream));
+  return VP3D_OK;
+}
+
+int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
+  ConvLaunch L;
+  VP3D_TRY(prepare_conv(d, &L));
+  if (L.empty) return VP3D_OK;
+  CUDA_TRY(launch_conv_gemm(L.ma, L.mw, L.mo, L.mr, L.mz, L.g, L.block_n, L.sms, stream));
+  return VP3D_OK;
+}
+
+static int conv_instance(const vp3d_conv_desc* d, int* key) {
+  if (!key) return fail(VP3D_ERR_INVALID, "conv_gemm_instance: null key");
+  ConvLaunch L;
+  VP3D_TRY(prepare_conv(d, &L));
+  if (L.empty) return fail(VP3D_ERR_INVALID, "conv_gemm_instance: no output rows, nothing is launched");
+  if (!conv_gemm_instance(L.g, L.block_n, L.sms, key))
+    return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm_instance: the selected instance is not compiled");
   return VP3D_OK;
 }
 
@@ -1320,4 +1355,12 @@ extern "C" __attribute__((visibility("default"))) int vp3d_profile_read(vp3d_pla
 
 extern "C" __attribute__((visibility("default"))) int vp3d_conv_gemm(const vp3d_conv_desc* d, void* stream) {
   return run_conv(d, static_cast<cudaStream_t>(stream));
+}
+extern "C" __attribute__((visibility("default"))) int vp3d_conv_gemm_instance(const vp3d_conv_desc* d,
+                                                                              int* key) {
+  return conv_instance(d, key);
+}
+extern "C" __attribute__((visibility("default"))) int vp3d_conv_gemm_instances(int* keys, int max) {
+  if (max > 0 && !keys) return fail(VP3D_ERR_INVALID, "conv_gemm_instances: null keys");
+  return vp3d::conv_gemm_instances(keys, max);
 }

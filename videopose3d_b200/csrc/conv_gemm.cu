@@ -1016,6 +1016,48 @@ void conv_gemm_debug_set_timeline(unsigned long long* buf, int max_launches) {
 }
 #endif
 
+// The instance a launch of `args` at tile width block_n on num_sms SMs runs (launch_conv_gemm and
+// conv_gemm_instance both ask here)
+static InstKey launch_key(const ConvGemmArgs& args, int block_n, int num_sms) {
+  return select_instance(args, block_n, conv_tiles(args) > num_sms);
+}
+
+template <class... Is>
+static bool listed(InstList<Is...>, const InstKey& k) {
+  return ((k == Is::kKey) || ...);
+}
+
+static void key_ints(const InstKey& k, int* out) {
+  out[0] = k.block_n;
+  out[1] = (int)k.epi;
+  out[2] = (int)k.fmt;
+  out[3] = (int)k.sched;
+  out[4] = k.res ? 1 : 0;
+  out[5] = k.out2 ? 1 : 0;
+  out[6] = (int)k.u8;
+}
+
+bool conv_gemm_instance(const ConvGemmArgs& args, int block_n, int num_sms, int key[7]) {
+  const InstKey k = launch_key(args, block_n, num_sms);
+  key_ints(k, key);
+  return block_n == 128 ? listed(Instances<128>{}, k) : listed(Instances<64>{}, k);
+}
+
+// the keys of a list's instances into keys[7 i], at most max of them; returns the list's length
+template <class... Is>
+static int list_keys(InstList<Is...>, int* keys, int max) {
+  const InstKey all[] = {Is::kKey...};
+  const int n = (int)sizeof...(Is);
+  for (int i = 0; i < n && i < max; ++i) key_ints(all[i], keys + 7 * i);
+  return n;
+}
+
+int conv_gemm_instances(int* keys, int max) {
+  const int n128 = list_keys(Instances<128>{}, keys, max);
+  const int done = n128 < max ? n128 : max;
+  return n128 + list_keys(Instances<64>{}, keys + 7 * done, max - done);
+}
+
 cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                              const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                              const CUtensorMap& tmap_z, const ConvGemmArgs& args_in, int block_n,
@@ -1027,7 +1069,7 @@ cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_
 #else
   const ConvGemmArgs& args = args_in;
 #endif
-  const InstKey k = select_instance(args, block_n, conv_tiles(args) > num_sms);
+  const InstKey k = launch_key(args, block_n, num_sms);
   if (block_n == 128)
     return launch_listed(Instances<128>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
   return launch_listed(Instances<64>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);

@@ -125,6 +125,13 @@ void conv_gemm_debug_set_timeline(unsigned long long* buf, int max_launches);
 // tmap_w: box rows = block_n.  block_n is 128 or 64.
 void conv_gemm_set_pdl(int on);   // programmatic dependent launch of the GEMM kernels (default on)
 bool conv_gemm_pdl_enabled();     // (also honoured by the small kernels between the GEMMs, launch.cuh)
+// The instance launch_conv_gemm runs for these arguments, as the 7 ints of vp3d_conv_gemm_instance
+// (include/vp3d_b200.h); false if it is not compiled (launch_conv_gemm then returns
+// cudaErrorInvalidValue).
+bool conv_gemm_instance(const ConvGemmArgs& args, int block_n, int num_sms, int key[7]);
+// The keys of every compiled instance (block_n 128, then 64) into keys[7 i], at most max of them;
+// returns how many are compiled.
+int conv_gemm_instances(int* keys, int max);
 cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
                              const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
                              const CUtensorMap& tmap_z, const ConvGemmArgs& args, int block_n,
