@@ -123,7 +123,7 @@ int num_sms() {
 // descriptor by prepare_conv.  run_conv launches it; vp3d_conv_gemm_instance asks which kernel
 // instance that launch would run -- the same preparation either way.
 struct ConvLaunch {
-  CUtensorMap ma, mw, mo, mr, mz;
+  CUtensorMap ma, mw, mw64, mo, mr, mz;   // (mw64: W in 64-row boxes, for the half tiles)
   ConvGemmArgs g;
   int block_n = 64;
   int sms = 0;
@@ -315,8 +315,10 @@ static int prepare_conv(const vp3d_conv_desc* d, ConvLaunch* L) {
   if ((i8 || d->out_u8) && d->res && !g.res_tma)
     return fail(VP3D_ERR_UNSUPPORTED, "conv_gemm: int8 / u8-output launches need a residual that "
                 "TMA can load (one box of a strided row view)");
-  VP3D_TRY(make_map_2d(&mw, d->w, d->k_per_tap, (uint64_t)w_planes * d->taps * d->n_pad, block_n,
-                       i8 ? 1 : 2));
+  const uint64_t w_rows = (uint64_t)w_planes * d->taps * d->n_pad;
+  VP3D_TRY(make_map_2d(&mw, d->w, d->k_per_tap, w_rows, block_n, i8 ? 1 : 2));
+  L->mw64 = mw;
+  if (block_n == 128) VP3D_TRY(make_map_2d(&L->mw64, d->w, d->k_per_tap, w_rows, 64, i8 ? 1 : 2));
   return VP3D_OK;
 }
 
@@ -324,7 +326,7 @@ int run_conv(const vp3d_conv_desc* d, cudaStream_t stream) {
   ConvLaunch L;
   VP3D_TRY(prepare_conv(d, &L));
   if (L.empty) return VP3D_OK;
-  CUDA_TRY(launch_conv_gemm(L.ma, L.mw, L.mo, L.mr, L.mz, L.g, L.block_n, L.sms, stream));
+  CUDA_TRY(launch_conv_gemm(L.ma, L.mw, L.mw64, L.mo, L.mr, L.mz, L.g, L.block_n, L.sms, stream));
   return VP3D_OK;
 }
 

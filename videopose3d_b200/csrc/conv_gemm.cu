@@ -14,7 +14,8 @@
 // while the consumers are in the epilogue of the current one.
 // Lean inference launches with more tiles than CTAs use the ping-pong instances instead: each
 // consumer warpgroup computes all 128 rows of every other tile, so that one warpgroup's epilogue
-// runs under the other's MMAs.
+// runs under the other's MMAs.  At 128 wide, a last wave of at most half the grid runs as twice as
+// many 128 x 64 half tiles (n64 MMAs, one 64-column store block), one per CTA.
 // The int8 eval instances run the same pipeline on u8 A / s8 W tiles of 128 x 128 bytes per
 // k-block (int32 accumulators, k32 MMAs), and may store a u8 copy of their output.
 #include "conv_gemm.cuh"
@@ -134,6 +135,17 @@ __device__ __forceinline__ void tile_coords(const ConvGemmArgs& p, int tile, int
   }
 }
 
+// Work item w of a launch whose tiles [0, full_tiles) run whole and whose remaining tiles run as
+// two 128 x 64 halves each (items full_tiles + 2 i + h: half h of tile full_tiles + i).  Returns
+// whether the item is a half tile; c_off is its first column inside the N block (0 or 64).
+__device__ __forceinline__ bool item_coords(const ConvGemmArgs& p, int full_tiles, int w,
+                                            int& n_blk, int& sample, int& row0, int& c_off) {
+  const bool half = w >= full_tiles;
+  c_off = half ? 64 * ((w - full_tiles) & 1) : 0;
+  tile_coords(p, half ? full_tiles + ((w - full_tiles) >> 1) : w, n_blk, sample, row0);
+  return half;
+}
+
 __device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
@@ -212,26 +224,29 @@ __device__ __forceinline__ void tl_stamp(const ConvGemmArgs& p, int ev) {
 #define TL(ev) ((void)0)
 #endif
 
-// One k-block (one 128-byte swizzle row of K) of m64 x BLOCK_N MMAs into each of the H accumulator
+// One k-block (one 128-byte swizzle row of K) of m64 x N MMAs into each of the H accumulator
 // halves in turn, half h reading the A rows of descriptor da[h]: four k16 steps of 16 elements, or
 // for int8 (u8 x s8) four k32 steps of 32 elements -- 32 B each, +2 in the descriptors' address >> 4.
-template <int BLOCK_N, Fmt FMT, int H, class Acc>
-__device__ __forceinline__ void wgmma_kblock(Acc (&acc)[H][BLOCK_N / 2], const uint64_t (&da)[H],
+// An n64 MMA into a 128-wide accumulator (a half tile) uses its first 32 registers: columns 0-63.
+template <int N, Fmt FMT, int H, int F, class Acc>
+__device__ __forceinline__ void wgmma_kblock(Acc (&acc)[H][F], const uint64_t (&da)[H],
                                              uint64_t db, bool first) {
+  static_assert((N == 64 || N == 128) && N / 2 <= F, "not a wgmma width of this accumulator");
 #pragma unroll
   for (int h = 0; h < H; ++h) {
+    auto& d = reinterpret_cast<Acc(&)[N / 2]>(acc[h]);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
       if constexpr (FMT == Fmt::kI8) {
-        if constexpr (BLOCK_N == 128) wgmma_m64n128k32_u8s8(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
-        else wgmma_m64n64k32_u8s8(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
-      } else if constexpr (BLOCK_N == 128) {
-        if constexpr (FMT == Fmt::kF16) wgmma_m64n128_f16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
-        else wgmma_m64n128_bf16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+        if constexpr (N == 128) wgmma_m64n128k32_u8s8(d, da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n64k32_u8s8(d, da[h] + 2 * k, db + 2 * k, accumulate);
+      } else if constexpr (N == 128) {
+        if constexpr (FMT == Fmt::kF16) wgmma_m64n128_f16(d, da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n128_bf16(d, da[h] + 2 * k, db + 2 * k, accumulate);
       } else {
-        if constexpr (FMT == Fmt::kF16) wgmma_m64n64_f16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
-        else wgmma_m64n64_bf16(acc[h], da[h] + 2 * k, db + 2 * k, accumulate);
+        if constexpr (FMT == Fmt::kF16) wgmma_m64n64_f16(d, da[h] + 2 * k, db + 2 * k, accumulate);
+        else wgmma_m64n64_bf16(d, da[h] + 2 * k, db + 2 * k, accumulate);
       }
     }
   }
@@ -243,8 +258,9 @@ __device__ __forceinline__ void wgmma_kblock(Acc (&acc)[H][BLOCK_N / 2], const u
 // Each k-block is one wgmma group; a stage is released once wait_group 1 shows the group reading it
 // has retired.  `issued()` runs after the last group is issued, before the wait for it.
 // The runtime format test of the general instances stays outside the k16 steps: a branch inside a
-// group makes ptxas close it with an extra null HGMMA (DESIGN.md section 4).
-template <class I, int H, class Issued>
+// group makes ptxas close it with an extra null HGMMA (DESIGN.md section 4).  N: the MMA width,
+// I::kBlockN, or 64 for a half tile of a 128-wide instance (its W stage holds the first 64 rows).
+template <class I, int N = I::kBlockN, int H, class Issued>
 __device__ __forceinline__ void mma_tile(typename I::Acc (&acc)[H][I::kBlockN / 2],
                                          const ConvGemmArgs& p, bool f16, uint32_t smem_a,
                                          uint32_t a_off, uint32_t smem_b, uint32_t full_bar,
@@ -265,9 +281,9 @@ __device__ __forceinline__ void mma_tile(typename I::Acc (&acc)[H][I::kBlockN / 
 #pragma unroll
     for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
     wgmma_fence();
-    if constexpr (I::kFmt != Fmt::kRuntime) wgmma_kblock<I::kBlockN, I::kFmt>(acc, da, db, it == 0);
-    else if (f16) wgmma_kblock<I::kBlockN, Fmt::kF16>(acc, da, db, it == 0);
-    else wgmma_kblock<I::kBlockN, Fmt::kBf16>(acc, da, db, it == 0);
+    if constexpr (I::kFmt != Fmt::kRuntime) wgmma_kblock<N, I::kFmt>(acc, da, db, it == 0);
+    else if (f16) wgmma_kblock<N, Fmt::kF16>(acc, da, db, it == 0);
+    else wgmma_kblock<N, Fmt::kBf16>(acc, da, db, it == 0);
     wgmma_commit();
 #pragma unroll
     for (int h = 0; h < H; ++h) wgmma_fence_operands(acc[h]);
@@ -293,6 +309,7 @@ template <class I>
 __global__ void __launch_bounds__(384, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
                  const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ CUtensorMap tmap_w64,
                  const __grid_constant__ CUtensorMap tmap_out,
                  const __grid_constant__ CUtensorMap tmap_res,
                  const __grid_constant__ CUtensorMap tmap_z, const ConvGemmArgs p) {
@@ -327,6 +344,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
   const int m_tiles = p.dilated ? p.samples * p.tiles_per_sample : p.tiles_per_sample;
   const int total_tiles = m_tiles * p.n_tiles;
+  // work items: whole tiles, then (128-wide ping-pong instances, planned by launch_impl) the last
+  // half_items / 2 tiles as half_items 128 x 64 halves, at most one per CTA
+  constexpr bool kHalves = I::kPP && I::kBlockN == 128;
+  const int half_items = kHalves ? p.half_items : 0;
+  const int full_tiles = total_tiles - half_items / 2;
+  const int n_items = full_tiles + half_items;
   const int k_iters = p.pairs * p.taps * p.kblocks_per_tap;
   // auxiliary tiles per 64-column store block: the residual plane(s) and, for the fused
   // BatchNorm-backward reductions, the Z tile.  kResSlots / tiles stages are in flight.
@@ -339,6 +362,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w);
+    if (kHalves && half_items > 0) tma_prefetch_desc(&tmap_w64);
     tma_prefetch_desc(&tmap_out);
     if (I::kRes) tma_prefetch_desc(&tmap_res);
     if (I::kRes && bnb) tma_prefetch_desc(&tmap_z);
@@ -391,8 +415,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int n_pre = kEarlyW ? (k_iters < I::kStages ? k_iters : I::kStages) : 0;
       int mode = n_pre > 0 ? 0 : 2;
       if (kEarlyW && mode == 2) mbar_wait(dep_bar, 0);
+      // whole tiles first: w < full_tiles (a CTA's first item is always a whole tile)
       int w = blockIdx.x;
-      if (w < total_tiles) {
+      if (w < full_tiles) {
         int n_blk, sample, row0;
         tile_coords(p, w, n_blk, sample, row0);
         uint32_t stage = 0, phase = 0;
@@ -431,9 +456,34 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
           }
           if (it == k_iters) {
             w += gridDim.x;
-            if (w >= total_tiles) break;
+            if (w >= full_tiles) break;
             tile_coords(p, w, n_blk, sample, row0);
             it = 0; pair = 0; tap = 0; kb = 0;
+          }
+        }
+        if constexpr (kHalves) {
+          // then the CTA's half tile, if it has one (its last item, see item_coords): the whole A
+          // tile and the 64 W rows of its columns (box of tmap_w64) into the first half of the
+          // stage's W slot.  (Kept out of the loop above, which stays the whole-tile loop.)
+          if (w < n_items) {
+            int c_off;
+            item_coords(p, full_tiles, w, n_blk, sample, row0, c_off);
+            for (int h_it = 0, h_pair = 0, h_tap = 0, h_kb = 0; h_it < k_iters; ++h_it) {
+              const uint32_t fb = full_bar + stage * 8;
+              mbar_wait(empty_bar + stage * 8, phase ^ 1);
+              mbar_expect_tx(fb, I::kABytes + I::kBBytes / 2);
+              const int w_row = ((h_pair == 2 ? 1 : 0) * p.taps + h_tap) * p.n_pad +
+                                n_blk * I::kBlockN + c_off;
+              tma_load_2d(&tmap_w64, fb, smem_b + stage * I::kBBytes, h_kb * kBK, w_row);
+              tma_load_4d(&tmap_a, fb, smem_a + stage * I::kABytes,
+                          h_tap * p.tap_col_step + h_kb * kBK, row0 + h_tap * p.tap_row_step,
+                          sample, h_pair == 1 ? 1 : 0);
+              if (++stage == I::kStages) { stage = 0; phase ^= 1; }
+              if (++h_kb == p.kblocks_per_tap) {
+                h_kb = 0;
+                if (++h_tap == p.taps) { h_tap = 0; ++h_pair; }
+              }
+            }
           }
         }
       }
@@ -444,17 +494,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       // ping-pong: the residual tiles in tile order; tile j goes to warpgroup j & 1, whose two
       // landing slots (2 g, 2 g + 1) form a ring of their own
       uint32_t filled[2] = {0u, 0u};   // residual tiles sent to warpgroup 0 / 1 so far
-      for (int j = 0, w = blockIdx.x; w < total_tiles; ++j, w += gridDim.x) {
-        int n_blk, sample, row0;
-        tile_coords(p, w, n_blk, sample, row0);
+      for (int j = 0, w = blockIdx.x; w < n_items; ++j, w += gridDim.x) {
+        int n_blk, sample, row0, c_off;
+        const bool half = item_coords(p, full_tiles, w, n_blk, sample, row0, c_off);
         const int g = j & 1;
-        for (int sb = 0; sb < kBlocksPerTile; ++sb) {
+        for (int sb = 0; sb < (half ? 1 : kBlocksPerTile); ++sb) {
           const uint32_t n = g ? filled[1] : filled[0];
           const uint32_t slot = 2u * g + (n & 1u);
           mbar_wait(rempty_bar + slot * 8, ((n >> 1) & 1u) ^ 1u);
           mbar_expect_tx(rfull_bar + slot * 8, I::kTileBytes);
           tma_load_4d(&tmap_res, rfull_bar + slot * 8, smem_res + slot * I::kTileBytes,
-                      n_blk * I::kBlockN + sb * 64 + p.res_tma_col_off, row0 + p.res_tma_row_off,
+                      n_blk * I::kBlockN + c_off + sb * 64 + p.res_tma_col_off,
+                      row0 + p.res_tma_row_off,
                       sample, 0);
           if (g) ++filled[1];
           else ++filled[0];
@@ -505,28 +556,36 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
     for (int i = 0; i < kFrag; ++i) acc[0][i] = acc[1][i] = 0.0f;
 
-    for (int j = wg, w = blockIdx.x + wg * gridDim.x; w < total_tiles; j += 2, w += 2 * gridDim.x) {
-      int n_blk, sample, row0;
-      tile_coords(p, w, n_blk, sample, row0);
+    // Item j = w's k-loop and epilogue; kHalf: a half tile (one 64-column store block, n64 MMAs
+    // into the first 64 columns of acc).  The loop below runs the whole tiles; a half tile is
+    // always a CTA's last item (launch_impl gives at most one to a CTA), so it runs after the loop
+    // from a copy of its own, and the loop keeps the registers of the whole-tile path alone.
+    const auto run_item = [&](int j, int w, auto half_tag) {
+      constexpr bool kHalf = decltype(half_tag)::value;
+      constexpr int kSb = kHalf ? 1 : kBlocksPerTile;   // 64-column store blocks
+      int n_blk, sample, row0, c_off = 0;
+      if constexpr (kHalf) item_coords(p, full_tiles, w, n_blk, sample, row0, c_off);
+      else tile_coords(p, w, n_blk, sample, row0);
 
-      // ---- main loop: k-block it of tile j sits in the producer's (j k_iters + it)-th fill
+      // ---- main loop: k-block it of item j sits in the producer's (j k_iters + it)-th fill
       const uint32_t fill = (uint32_t)j * (uint32_t)k_iters;
       uint32_t stage = fill % I::kStages, phase = (fill / I::kStages) & 1u;
-      if (j > 0) named_bar_sync(bar_mine, 256);   // tile j - 1's k-loop has been issued
-      mma_tile<I>(acc, p, I::kF16, smem_a, 0u, smem_b, full_bar, empty_bar, stage, phase, k_iters,
-                  lane, warp == 4 && lane == 0 && w == (int)blockIdx.x, [&] {
-                    // tile j + 1 may issue
-                    if (w + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);
-                  });
+      if (j > 0) named_bar_sync(bar_mine, 256);   // item j - 1's k-loop has been issued
+      mma_tile<I, kHalf ? 64 : I::kBlockN>(
+          acc, p, I::kF16, smem_a, 0u, smem_b, full_bar, empty_bar, stage, phase, k_iters, lane,
+          warp == 4 && lane == 0 && w == (int)blockIdx.x, [&] {
+            // item j + 1 may issue
+            if (w + (int)gridDim.x < n_items) named_bar_arrive(bar_other, 256);
+          });
 #ifdef VP3D_TIMELINE
       if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(7); TL(8); }
 #endif
 
-      const float* scale = p.scale + n_blk * I::kBlockN;
-      const float* shift = p.shift + n_blk * I::kBlockN;
+      const float* scale = p.scale + n_blk * I::kBlockN + c_off;
+      const float* shift = p.shift + n_blk * I::kBlockN + c_off;
 #pragma unroll
-      for (int sb = 0; sb < kBlocksPerTile; ++sb) {
-        const int cb = n_blk * I::kBlockN + sb * 64;   // first column of the store block
+      for (int sb = 0; sb < kSb; ++sb) {
+        const int cb = n_blk * I::kBlockN + c_off + sb * 64;   // first column of the store block
         uint32_t tile_smem;
         if constexpr (I::kRes) {
           // in place: every thread overwrites the residual elements it adds with its results
@@ -588,12 +647,17 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         // the landing tiles go back to the auxiliary producer once the stores have read them
         tma_store_wait_read<0>();
 #pragma unroll
-        for (int sb = 0; sb < kBlocksPerTile; ++sb)
-          mbar_arrive(rempty_bar + (2u * wg + ((res_seen - kBlocksPerTile + sb) & 1u)) * 8);
+        for (int sb = 0; sb < kSb; ++sb)
+          mbar_arrive(rempty_bar + (2u * wg + ((res_seen - kSb + sb) & 1u)) * 8);
       }
 #ifdef VP3D_TIMELINE
       if (warp == 4 && lane == 0) { if (w == (int)blockIdx.x) TL(9); TL(10); }
 #endif
+    };
+    int j = wg, w = blockIdx.x + wg * gridDim.x;
+    for (; w < full_tiles; j += 2, w += 2 * gridDim.x) run_item(j, w, std::false_type{});
+    if constexpr (kHalves) {
+      if (w < n_items) run_item(j, w, std::true_type{});
     }
     // the staging tiles must outlive every bulk store that reads them
     if (tid == 0) tma_store_wait_all<0>();
@@ -886,9 +950,9 @@ static int conv_tiles(const ConvGemmArgs& a) {
 
 template <class I>
 static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
-                               const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
-                               const CUtensorMap& tmap_z, const ConvGemmArgs& args, int num_sms,
-                               cudaStream_t stream) {
+                               const CUtensorMap& tmap_w64, const CUtensorMap& tmap_out,
+                               const CUtensorMap& tmap_res, const CUtensorMap& tmap_z,
+                               const ConvGemmArgs& args_in, int num_sms, cudaStream_t stream) {
   auto kernel = conv_gemm_kernel<I>;
   // the dynamic shared memory opt-in is a per-device attribute
   static bool attr_set[kMaxDevices] = {};
@@ -901,9 +965,20 @@ static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tma
     if (e != cudaSuccess) return e;
     attr_set[dev] = true;
   }
-  const int total = conv_tiles(args);
+  const int total = conv_tiles(args_in);
   if (total <= 0) return cudaSuccess;
   const int workers = total < num_sms ? total : num_sms;
+  // The last wave of a 128-wide ping-pong launch: its `left` tiles would keep `left` SMs busy for
+  // a whole tile while the other workers - left wait.  Where they fit twice into the grid they run
+  // as 2 left half tiles of 128 x 64 instead, one per CTA, each about half as long.  The plan
+  // follows from the tile count and the grid alone, and a half tile stores the bits of the whole
+  // one (the same k order and n64 instruction path as the 64-wide instances).
+  ConvGemmArgs args = args_in;
+  args.half_items = 0;
+  if constexpr (I::kPP && I::kBlockN == 128) {
+    const int left = total % workers;
+    if (left > 0 && 2 * left <= workers) args.half_items = 2 * left;
+  }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(workers, 1, 1);
@@ -919,7 +994,8 @@ static cudaError_t launch_impl(const CUtensorMap& tmap_a, const CUtensorMap& tma
   }
   cfg.attrs = attr;
   cfg.numAttrs = n_attr;
-  return cudaLaunchKernelEx(&cfg, kernel, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args);
+  return cudaLaunchKernelEx(&cfg, kernel, tmap_a, tmap_w, tmap_w64, tmap_out, tmap_res, tmap_z,
+                            args);
 }
 
 // Lean inference epilogue (VP3D_LEAN=0 falls back to the general one): exactly affine + ReLU
@@ -997,11 +1073,13 @@ using Instances = InstList<
 // launch_impl of the listed instance whose key is k (cudaErrorInvalidValue if none is)
 template <class... Is>
 static cudaError_t launch_listed(InstList<Is...>, const InstKey& k, const CUtensorMap& a,
-                                 const CUtensorMap& w, const CUtensorMap& o, const CUtensorMap& r,
+                                 const CUtensorMap& w, const CUtensorMap& w64,
+                                 const CUtensorMap& o, const CUtensorMap& r,
                                  const CUtensorMap& z, const ConvGemmArgs& args, int num_sms,
                                  cudaStream_t stream) {
   cudaError_t e = cudaErrorInvalidValue;
-  (void)((k == Is::kKey && ((e = launch_impl<Is>(a, w, o, r, z, args, num_sms, stream)), true)) ||
+  (void)((k == Is::kKey &&
+          ((e = launch_impl<Is>(a, w, w64, o, r, z, args, num_sms, stream)), true)) ||
          ...);
   return e;
 }
@@ -1059,9 +1137,10 @@ int conv_gemm_instances(int* keys, int max) {
 }
 
 cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
-                             const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
-                             const CUtensorMap& tmap_z, const ConvGemmArgs& args_in, int block_n,
-                             int num_sms, cudaStream_t stream) {
+                             const CUtensorMap& tmap_w64, const CUtensorMap& tmap_out,
+                             const CUtensorMap& tmap_res, const CUtensorMap& tmap_z,
+                             const ConvGemmArgs& args_in, int block_n, int num_sms,
+                             cudaStream_t stream) {
 #ifdef VP3D_TIMELINE
   ConvGemmArgs args = args_in;
   args.timeline = (g_timeline && g_timeline_next < g_timeline_max)
@@ -1071,8 +1150,10 @@ cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_
 #endif
   const InstKey k = launch_key(args, block_n, num_sms);
   if (block_n == 128)
-    return launch_listed(Instances<128>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
-  return launch_listed(Instances<64>{}, k, tmap_a, tmap_w, tmap_out, tmap_res, tmap_z, args, num_sms, stream);
+    return launch_listed(Instances<128>{}, k, tmap_a, tmap_w, tmap_w64, tmap_out, tmap_res, tmap_z,
+                         args, num_sms, stream);
+  return launch_listed(Instances<64>{}, k, tmap_a, tmap_w, tmap_w64, tmap_out, tmap_res, tmap_z,
+                       args, num_sms, stream);
 }
 
 }  // namespace vp3d

@@ -105,6 +105,9 @@ struct ConvGemmArgs {
   // 16-bit plane, or alone when `out` is null.  out_u8 (non-null) selects the u8 instances.
   uint8_t* out_u8;
   float u8_inv_s;
+  // ---- work items (set by the launcher, not the caller): the last half_items / 2 tiles run as
+  // half_items 128 x 64 half tiles (128-wide ping-pong instances; 0 = whole tiles only)
+  int half_items;
 #ifdef VP3D_TIMELINE
   // debug build (`make dbg`): per-launch time stamps of the first and the last CTA
   unsigned long long* timeline;   // [2 CTAs][32 events][globaltimer ns, clock64] or null
@@ -122,7 +125,8 @@ void conv_gemm_debug_set_timeline(unsigned long long* buf, int max_launches);
 // tmap_z: same geometry as tmap_out over the Z tensor of the layer below; used only when args.bnb.
 // With args.out_u8 it maps the u8 output instead: 4-D (channel, row, sample, 1) bytes, box
 // (64, 32, 1, 1), no swizzle.
-// tmap_w: box rows = block_n.  block_n is 128 or 64.
+// tmap_w: box rows = block_n.  block_n is 128 or 64.  tmap_w64: the same weights with box rows 64
+// (the half tiles of a 128-wide launch; at block_n 64 pass tmap_w again).
 void conv_gemm_set_pdl(int on);   // programmatic dependent launch of the GEMM kernels (default on)
 bool conv_gemm_pdl_enabled();     // (also honoured by the small kernels between the GEMMs, launch.cuh)
 // The instance launch_conv_gemm runs for these arguments, as the 7 ints of vp3d_conv_gemm_instance
@@ -133,8 +137,9 @@ bool conv_gemm_instance(const ConvGemmArgs& args, int block_n, int num_sms, int 
 // returns how many are compiled.
 int conv_gemm_instances(int* keys, int max);
 cudaError_t launch_conv_gemm(const CUtensorMap& tmap_a, const CUtensorMap& tmap_w,
-                             const CUtensorMap& tmap_out, const CUtensorMap& tmap_res,
-                             const CUtensorMap& tmap_z, const ConvGemmArgs& args, int block_n,
-                             int num_sms, cudaStream_t stream);
+                             const CUtensorMap& tmap_w64, const CUtensorMap& tmap_out,
+                             const CUtensorMap& tmap_res, const CUtensorMap& tmap_z,
+                             const ConvGemmArgs& args, int block_n, int num_sms,
+                             cudaStream_t stream);
 
 }  // namespace vp3d
