@@ -717,6 +717,21 @@ int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frame
  *     slot s (frame >= 0) is written to row y_rows[s] + t, rows of frame -1 are not written.  frame
  *     (S, k) is still written and is required.  The output kernel then always runs (one launch
  *     more where a push would shrink straight into y).
+ * vp3d_stream_push_counts: vp3d_stream_push_ex plus one optional DEVICE array (push_ex is
+ * push_counts with count = NULL: the same bits and launches):
+ *   count (S int32, or NULL = k for every slot): slot s has count[s] real frames in this push, 0 to
+ *     k, so streams that skip or drop frames share one session.  They are x[s, :count[s]] (rows
+ *     x_rows[s] + f in row-addressed mode); x[s, f >= count[s]] is never read.  count is read only
+ *     for a slot that holds an open sequence (active, or starting in this push) and does not end in
+ *     this push: an ending slot's real frames are its first end[s], draining and idle slots advance
+ *     as without counts.  Output row f of a counted slot is frame (frames pushed before) + f -
+ *     lookahead for f < count[s] (under the warm-up rule), -1 for f >= count[s]; the slot's frame
+ *     counter advances by count[s], and its later outputs stay those of the offline forward on its
+ *     own padded sequence.  Values outside [0, k], and 0 on a slot that starts in this push (a start
+ *     needs its first frame), are read as k.  With count != NULL two realign launches follow the
+ *     last GEMM (the host cannot see the values): they move the history of every slot with
+ *     count[s] < k forward by k - count[s] frames, 4 * sum_l H_l * ld_l * planes * 2 bytes per
+ *     physical row moved (about 2 MB at arc 3,3,3,3,3, C = 1024, fp16), nothing for the others.
  * vp3d_stream_finish: emits the last `lookahead` frames of every slot by repeating each slot's
  * newest frame (the generator's end padding) into y (S, lookahead, J_out, 3) / frame (S,
  * lookahead), then marks every slot idle.  A slot whose sequence ended in an earlier push returns
@@ -748,6 +763,10 @@ int vp3d_stream_push(vp3d_plan* plan, void* state, const float* x, int k, const 
 int vp3d_stream_push_ex(vp3d_plan* plan, void* state, const float* x, int k,
                         const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
                         const int64_t* y_rows, float* y, int64_t* frame, void* stream);
+int vp3d_stream_push_counts(vp3d_plan* plan, void* state, const float* x, int k,
+                            const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
+                            const int64_t* y_rows, float* y, int64_t* frame, const int32_t* count,
+                            void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 int vp3d_stream_release(vp3d_plan* plan, void* state);
 

@@ -38,6 +38,24 @@
 // active, length) is double-buffered by push parity: the input kernel reads buffer `parity` and
 // writes buffer `parity ^ 1`, so the pack, which depends on the bookkeeping of its slot, reads only
 // values no block of the same launch writes, whatever order the blocks run in.
+//
+// Per-slot frame counts (vp3d_stream_push_counts's `count`).  Every push works from one invariant:
+// at its start, positions [q - H_l, q) of ring l hold the slot's last H_l ring-l inputs.  A slot
+// with n < k real frames still runs all k GEMM rows: rows f < n read only history and earlier real
+// rows, so they are exact; rows f >= n are scratch.  The realign kernel then restores the invariant
+// for the next push by moving the slot's last H_l positions forward by k - n in every ring: window
+// positions [w0 + n, w0 + n + H) go to [w0 + k, w0 + k + H), so the newest real frame sits at the
+// window end as after k real frames.  Source and destination overlap; the mirrored rings order the
+// copy without scratch memory, because a window of H + k < R positions never holds a position
+// together with its mirror (p +- R):
+//   phase 1 reads the sources (window positions only) and writes them to the MIRROR copies of the
+//     destination, none of which lies in the window: no block reads what another block writes.  It
+//     also overwrites the mirror copies of history positions [w0 + k, w0 + H), which is safe because
+//     phase 1 never reads a mirror position and phase 2 rewrites their window copies to match;
+//   phase 2 (the next launch, after phase 1 has completed) copies those mirror copies back onto the
+//     destination window positions, reading only mirror positions.  Both copies then agree, as the
+//     next push's input kernel and its mirror pass expect.
+// Both phases cover ring 0 and rings 1..nb, every plane and both physical rows of an AUGMENT slot.
 #include "internal.cuh"
 #include "launch.cuh"
 
@@ -113,6 +131,7 @@ struct StepArgs {
   const int* kps;          // AUGMENT: [J_in] mirror source of every input joint; null: no rows >= S
   const uint8_t* start;    // (S,) or null
   const int* end;          // (S,) or null: the sequence ends after frame end[s] - 1 of this push
+  const int* count;        // (S,) or null: real frames of an open sequence in this push (slot_count)
   // per slot, the buffer of this push's parity (read) and of the next one (written):
   const long long* count_in;    // frames of the current sequence pushed so far
   const uint8_t* active_in;     // 1 while the slot holds a sequence (also while it drains)
@@ -141,17 +160,31 @@ __device__ __forceinline__ int slot_end(const StepArgs& a, int s) {
   return e < -1 || e > a.k ? -1 : e;
 }
 
-// Frames of this push that row r packs from x: k for an open sequence, end[s] for one that ends in
-// this push, 0 once it has ended or in finish mode (the newest packed frame is repeated instead).
-// An idle slot packs its dense x as it always has; row-addressed x is not read for it.  Only
-// pre-push values are read: the bookkeeping loop of the same launch writes the other buffer.
+// Frames slot s advances by in this push: count[s] for a slot that holds an open sequence (active,
+// or starting in this push) that does not end in it, k for every other slot (an ending slot's real
+// frames are its first end[s]; draining and idle slots advance as without counts).  Values outside
+// [0, k], and 0 on a starting slot (a start needs its first frame), read as k.  The input kernel
+// and the realign kernel both decide through this function, from pre-push values only.
+__device__ __forceinline__ int slot_count(const StepArgs& a, int s) {
+  if (!a.count) return a.k;
+  const bool st = a.start && a.start[s];
+  if (!st && (!a.active_in[s] || a.length_in[s] >= 0)) return a.k;
+  if (slot_end(a, s) >= 0) return a.k;
+  const int n = a.count[s];
+  return n < (st ? 1 : 0) || n > a.k ? a.k : n;
+}
+
+// Frames of this push that row r packs from x: slot_count for an open sequence, end[s] for one that
+// ends in this push, 0 once it has ended or in finish mode (the newest packed frame is repeated
+// instead).  An idle slot packs its dense x as it always has; row-addressed x is not read for it.
+// Only pre-push values are read: the bookkeeping loop of the same launch writes the other buffer.
 __device__ __forceinline__ int packed_frames(const StepArgs& a, int s) {
   if (!a.x) return 0;
   const bool st = a.start && a.start[s];
   if (!st && !a.active_in[s]) return a.x_rows ? 0 : a.k;
   if (!st && a.length_in[s] >= 0) return 0;
   const int e = slot_end(a, s);
-  return e >= 0 ? e : a.k;
+  return e >= 0 ? e : slot_count(a, s);
 }
 
 // One launch at the head of every push:
@@ -174,13 +207,14 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
     uint8_t act = a.active_in[s];
     if (a.start && a.start[s]) { c = 0; act = 1; len = -1; }
     const int e = slot_end(a, (int)s);
+    const int n = slot_count(a, (int)s);   // rows f >= n are no frame (a counted slot's scratch)
     if (act && len < 0 && e >= 0) len = c + e;
     for (int f = 0; f < a.k; ++f) {
       const long long idx = c + f - a.lookahead;
       a.frame[s * a.frame_ld + a.frame_off + f] =
-          (act && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
+          (act && f < n && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
     }
-    c += a.k;
+    c += n;
     // idle once frame length - 1 is out (at once for a sequence without frames: start with end 0)
     if (act && len >= 0 && (c - a.lookahead >= len || len == 0)) act = 0;
     a.count_out[s] = c;
@@ -253,6 +287,87 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
                                             (long long)mirror_pos(pos, r.R) * a.P * r.ld) + e;
       *dst = *src;
     }
+  }
+}
+
+// One phase of the realign of a counted push (header comment): every physical row whose slot got
+// n = slot_count < k real frames moves its last H positions of every ring forward by k - n.
+// phase = 0 (the header comment's phase 1) copies window positions w0 + n + j to the mirror copies
+// of w0 + k + j, phase = 1 (phase 2) those mirror copies back onto w0 + k + j (j < H).
+// The rows are taken kRealignTile at a time: every block lists the tile's realigned rows in shared
+// memory, in row order (a ballot prefix sum, so every block holds the same list: the grid splits
+// one flat index over it), then the grid strides over their row_vecs 16-byte vectors each, so a
+// few realigned rows still spread over every block and a push without any costs one scan of the
+// counts.  Each thread loads four vectors before it stores any.  Launched with 256 threads.
+constexpr int kRealignTile = 1024;
+
+__global__ void __launch_bounds__(256) stream_realign_kernel(const StepArgs a, int phase,
+                                                             int row_vecs) {
+  pdl_entry();
+  constexpr int kBatch = 4, kWarps = 8;
+  __shared__ int rows[kRealignTile], frames[kRealignTile];
+  __shared__ int warp_rows[kWarps];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int r0 = 0; r0 < a.P; r0 += kRealignTile) {
+    int listed = 0;   // the same in every thread
+    for (int c = 0; c < kRealignTile; c += kWarps * 32) {
+      const int r = r0 + c + threadIdx.x;
+      const int n = r < a.P ? slot_count(a, r < a.S ? r : r - a.S) : a.k;
+      const unsigned take = __ballot_sync(0xffffffffu, n < a.k);
+      if (lane == 0) warp_rows[warp] = __popc(take);
+      __syncthreads();
+      int at = listed;
+      for (int w = 0; w < kWarps; ++w) {
+        if (w < warp) at += warp_rows[w];
+        listed += warp_rows[w];
+      }
+      if (n < a.k) {
+        at += __popc(take & ((1u << lane) - 1));
+        rows[at] = r;
+        frames[at] = n;
+      }
+      __syncthreads();
+    }
+    const long long total = (long long)listed * row_vecs;
+    for (long long i0 = (long long)blockIdx.x * blockDim.x * kBatch + threadIdx.x; i0 < total;
+         i0 += (long long)gridDim.x * blockDim.x * kBatch) {
+      uint4 v[kBatch];
+      uint4* dst[kBatch];
+#pragma unroll
+      for (int u = 0; u < kBatch; ++u) {
+        const long long i = i0 + u * blockDim.x;
+        if (i >= total) break;
+        const int at = (int)(i / row_vecs);
+        int rem = (int)(i - (long long)at * row_vecs);
+        const int r = rows[at], n = frames[at];
+#pragma unroll
+        for (int l = 0; l < kMaxRings; ++l) {   // (unrolled: the ring table stays in parameter space)
+          if (l >= a.rings) break;
+          const StreamRing& g = a.ring[l];
+          const int vec = g.ld / 8;
+          const int m = a.planes * g.H * vec;
+          if (rem >= m) {
+            rem -= m;
+            continue;
+          }
+          const int e = rem % vec, q = rem / vec;
+          const int j = q % g.H, pl = q / g.H;
+          const int to = g.w0 + a.k + j;   // a window position, < 2R
+          const int from = phase == 0 ? g.w0 + n + j : mirror_pos(to, g.R);
+          __nv_bfloat16* pb = g.base + pl * g.plane;
+          v[u] = *(reinterpret_cast<const uint4*>(pb + ((long long)from * a.P + r) * g.ld) + e);
+          dst[u] = reinterpret_cast<uint4*>(
+                       pb + ((long long)(phase == 0 ? mirror_pos(to, g.R) : to) * a.P + r) * g.ld) + e;
+          break;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kBatch; ++u) {
+        if (i0 + u * blockDim.x >= total) break;
+        *dst[u] = v[u];
+      }
+    }
+    __syncthreads();   // the lists of the next tile overwrite these
   }
 }
 
@@ -400,7 +515,8 @@ int stream_lookahead(const vp3d_plan* p) {
 // of a flat one; frame the matching (S, y_frames) entries.  The GEMMs run over P physical rows per
 // frame (S, or 2S with AUGMENT).
 static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
-                       const uint8_t* start, const int* end, const long long* x_rows,
+                       const uint8_t* start, const int* end, const int* count,
+                       const long long* x_rows,
                        const long long* y_rows, float* y, int y_frames, int f_off, long long* frame,
                        cudaStream_t stream) {
   const int S = h.S, K = h.K, C = p->C, planes = p->planes;
@@ -437,6 +553,7 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.kps = aug ? reinterpret_cast<const int*>(base + L.kps) : nullptr;
   a.start = start;
   a.end = end;
+  a.count = count;
   {
     const int in = h.parity, out = h.parity ^ 1;
     long long* count = reinterpret_cast<long long*>(base + L.count);
@@ -505,6 +622,21 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
 
   // ---- the push: expand (model.py:127), residual blocks (:129-135), shrink (:137)
   VP3D_TRY(run_infer_chain(p, push, stream, &launches));
+  if (count) {
+    // the slots with fewer real frames than k: both realign phases, after the last GEMM read the
+    // rings (the host cannot see the counts, so they always run)
+    int row_vecs = 0;   // 16-byte vectors a realigned row moves per phase
+    for (int l = 0; l < L.rings; ++l) row_vecs += planes * ring[l].H * ring[l].ld / 8;
+    // four vectors per thread over one full tile, at most four blocks per SM: enough loads in
+    // flight for HBM bandwidth, and few blocks to scan the counts when no row realigns
+    int grid = grid_for((long long)row_vecs * (P < kRealignTile ? P : kRealignTile) / 4);
+    if (grid > 132 * 4) grid = 132 * 4;
+    for (int phase = 0; phase < 2; ++phase) {
+      CUDA_TRY(launch_pdl(stream_realign_kernel, dim3(grid), dim3(256), 0, stream, a, phase,
+                          row_vecs));
+      ++launches;
+    }
+  }
   if (!direct) {
     CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
                         dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
@@ -638,8 +770,9 @@ static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost
 }
 
 static int stream_push(const char* what, vp3d_plan* p, void* state, const float* x, int k,
-                       const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
-                       const int64_t* y_rows, float* y, int64_t* frame, void* stream) {
+                       const uint8_t* start_mask, const int32_t* end, const int32_t* count,
+                       const int64_t* x_rows, const int64_t* y_rows, float* y, int64_t* frame,
+                       void* stream) {
   if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
   if (k < 1) return fail(VP3D_ERR_INVALID, "%s: k must be >= 1 (got %d)", what, k);
   if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
@@ -653,25 +786,33 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
     return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
   if (!p->conv_packed || !p->bn_packed)
     return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
-  return stream_step(p, ws_base(state), *h, x, k, start_mask, end,
+  return stream_step(p, ws_base(state), *h, x, k, start_mask, end, count,
                      reinterpret_cast<const long long*>(x_rows),
                      reinterpret_cast<const long long*>(y_rows), y, k, 0,
                      reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
+}
+
+VP3D_EXPORT int vp3d_stream_push_counts(vp3d_plan* p, void* state, const float* x, int k,
+                                        const uint8_t* start_mask, const int32_t* end,
+                                        const int64_t* x_rows, const int64_t* y_rows, float* y,
+                                        int64_t* frame, const int32_t* count, void* stream) {
+  return stream_push("stream_push_counts", p, state, x, k, start_mask, end, count, x_rows, y_rows,
+                     y, frame, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, int k,
                                     const uint8_t* start_mask, const int32_t* end,
                                     const int64_t* x_rows, const int64_t* y_rows, float* y,
                                     int64_t* frame, void* stream) {
-  return stream_push("stream_push_ex", p, state, x, k, start_mask, end, x_rows, y_rows, y, frame,
-                     stream);
+  return stream_push("stream_push_ex", p, state, x, k, start_mask, end, nullptr, x_rows, y_rows, y,
+                     frame, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push(vp3d_plan* p, void* state, const float* x, int k,
                                  const uint8_t* start_mask, float* y, int64_t* frame,
                                  void* stream) {
-  return stream_push("stream_push", p, state, x, k, start_mask, nullptr, nullptr, nullptr, y, frame,
-                     stream);
+  return stream_push("stream_push", p, state, x, k, start_mask, nullptr, nullptr, nullptr, nullptr,
+                     y, frame, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t* frame,
@@ -689,7 +830,8 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
   int launches = 0;
   for (int off = 0; off < la; off += h->K) {
     const int k = la - off < h->K ? la - off : h->K;
-    VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, nullptr, nullptr, nullptr, y, la, off,
+    VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, nullptr, nullptr, nullptr, nullptr, y,
+                         la, off,
                          reinterpret_cast<long long*>(frame), s));
     launches += p->last_launches;
   }

@@ -6,7 +6,8 @@ output frame.  A session keeps every conv layer's past activations in device rin
 the new frames' share (``include/vp3d_b200.h``, vp3d_stream_*):
 
     sess = model.streaming(streams=S, max_frames=K)   # TemporalModel in eval()
-    y, frame = sess.push(x, start=None, end=None)   # x: (S, k, J_in, F) CUDA fp32, 1 <= k <= K
+    y, frame = sess.push(x, start=None, end=None, count=None)   # x: (S, k, J_in, F) CUDA fp32,
+                                                               # 1 <= k <= K
     y, frame = sess.finish()              # the look-ahead tail of every slot; slots become idle
     sess.reset()                          # drop all history
     ys = sess.predict([x0, x1, ...])      # whole (T_i, J_in, F) sequences, scheduled over the slots
@@ -23,6 +24,10 @@ slot is fed its last frame repeated (the generator's end padding), its last `loo
 out over the following pushes while the other slots go on, and the slot is idle once the last one is
 out.  ``predict`` uses this to run a list of sequences of any lengths through the slots, longest
 first, each slot taking the next sequence once the previous one has drained.
+
+``count[s] = n`` (0 <= n <= k) gives slot s only the n real frames x[s, :n] in this push, so
+cameras that drop frames, deliver late or run at different rates share one session: each slot's
+outputs stay those of the offline forward on its own padded sequence, and rows f >= n get frame -1.
 
 Test-time flip augmentation, run.py's default (common/arguments.py:43):
 
@@ -122,21 +127,31 @@ class FrameBook:
         self.length = np.full(streams, -1, np.int64)
         self.lookahead = lookahead
 
-    def push(self, k, start=None, end=None):
-        if start is not None:
-            start = np.asarray(start, bool)
-            self.count[start] = 0
-            self.active[start] = True
-            self.length[start] = -1
-        if end is not None:
-            end = np.asarray(end, np.int64)
-            end = np.where((end < -1) | (end > k), -1, end)   # as the device reads it
-            ends = self.active & (self.length < 0) & (end >= 0)
-            self.length[ends] = self.count[ends] + end[ends]
-        idx = self.count[:, None] + np.arange(k)[None, :] - self.lookahead
+    def push(self, k, start=None, end=None, count=None):
+        S = len(self.count)
+        start = np.zeros(S, bool) if start is None else np.asarray(start, bool)
+        self.count[start] = 0
+        self.active[start] = True
+        self.length[start] = -1
+        end = np.full(S, -1, np.int64) if end is None else np.asarray(end, np.int64)
+        end = np.where((end < -1) | (end > k), -1, end)   # as the device reads it
+        is_open = self.active & (self.length < 0)
+        ends = is_open & (end >= 0)
+        self.length[ends] = self.count[ends] + end[ends]
+        # frames each slot advances by: count[s] for an open sequence that does not end here, read
+        # as the device reads it (outside [0, k], or 0 on a starting slot: k), k for every other slot
+        n = np.full(S, k, np.int64)
+        if count is not None:
+            c = np.asarray(count, np.int64)
+            c = np.where((c < 0) | (c > k) | (start & (c == 0)), k, c)
+            counted = is_open & (end < 0)
+            n[counted] = c[counted]
+        f = np.arange(k)[None, :]
+        idx = self.count[:, None] + f - self.lookahead
         length = self.length[:, None]
-        frame = np.where(self.active[:, None] & (idx >= 0) & ((length < 0) | (idx < length)), idx, -1)
-        self.count += k
+        frame = np.where(self.active[:, None] & (f < n[:, None]) & (idx >= 0)
+                         & ((length < 0) | (idx < length)), idx, -1)
+        self.count += n
         # idle once frame length - 1 is out (at once for a sequence without frames)
         done = self.active & (self.length >= 0) & ((self.count - self.lookahead >= self.length)
                                                    | (self.length == 0))
@@ -347,6 +362,25 @@ class StreamingSession:
                 raise ValueError(f"slot {s} starts and ends with end = 0: a sequence without frames")
         return end
 
+    def _count_list(self, count, k, start):
+        """None, a device tensor, or the validated host list of ints in [0, k]."""
+        if count is None:
+            return None
+        if isinstance(count, torch.Tensor):
+            self._slot_tensor(count, "count")
+            if count.dtype != torch.int32:
+                raise TypeError(f"count must be an int32 tensor, got {count.dtype}")
+            return count
+        count = [int(v) for v in count]
+        if len(count) != self.streams:
+            raise ValueError(f"count must list {self.streams} slots")
+        for s, n in enumerate(count):
+            if not 0 <= n <= k:
+                raise ValueError(f"count[{s}] = {n} is outside [0, k = {k}]")
+            if n == 0 and isinstance(start, list) and start[s]:
+                raise ValueError(f"slot {s} starts with count = 0: a start needs its first frame")
+        return count
+
     def _start_mask(self, start):
         start = self._start_list(start)
         if start is None:
@@ -357,34 +391,45 @@ class StreamingSession:
             return None
         return torch.tensor(start, dtype=torch.uint8).to(self.device)
 
-    def push(self, x, start=None, end=None):
-        """Push k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64).
+    def push(self, x, start=None, end=None, count=None):
+        """Push up to k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64).
 
         start: S bools (list or device tensor), slots that begin a new sequence with x[s, 0].
         end: S ints in [-1, k] (list or CUDA int32 tensor), end[s] = n >= 0 ends slot s's sequence
         after frame n - 1 of this push (x[s, n:] is not read), -1 = it continues.  Values of a
-        device tensor outside [-1, k] count as -1."""
+        device tensor outside [-1, k] count as -1.
+        count: S ints in [0, k] (list or CUDA int32 tensor), the real frames x[s, :count[s]] slot s
+        has in this push (x[s, count[s]:] is not read, its rows get frame -1), for streams that skip
+        or drop frames; None = k for every slot.  Read for open sequences that do not end in this
+        push; at least 1 on a starting slot.  Values of a device tensor outside [0, k] (and 0 on a
+        starting slot) count as k.  Counts below k add two launches."""
         k = check_push_input(x, self.streams, self.max_frames, self.model.num_joints_in,
                              self.model.in_features)
         if x.device != self.device:
             raise RuntimeError("input and parameters are on different devices")
         start = self._start_list(start)
         end = self._end_list(end, k, start)   # host lists are checked before any device work
+        count = self._count_list(count, k, start)
         x = x.contiguous()
         mask = self._start_mask(start)
         if isinstance(end, list):
             end = torch.tensor(end, dtype=torch.int32).to(self.device) if max(end) >= 0 else None
         elif end is not None:
             end = end.contiguous()
+        if isinstance(count, list):   # every slot full: the plain push's launches
+            count = torch.tensor(count, dtype=torch.int32).to(self.device) if min(count) < k else None
+        elif count is not None:
+            count = count.contiguous()
         y = torch.empty((self.streams, k, self.model.num_joints_out, 3), dtype=torch.float32,
                         device=self.device)
         frame = torch.empty((self.streams, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
             stream = self._prepare()
-            _capi.check(_capi.load().vp3d_stream_push_ex(
+            _capi.check(_capi.load().vp3d_stream_push_counts(
                 self._plan, self._state.data_ptr(), x.data_ptr(), k,
                 None if mask is None else mask.data_ptr(), None if end is None else end.data_ptr(),
-                None, None, y.data_ptr(), frame.data_ptr(), stream), "vp3d_stream_push_ex")
+                None, None, y.data_ptr(), frame.data_ptr(),
+                None if count is None else count.data_ptr(), stream), "vp3d_stream_push_counts")
         return y, frame
 
     def predict(self, sequences):
