@@ -750,8 +750,25 @@ int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frame
  * run.py:678).  init_ex checks every entry is in [0, J) and copies the maps into the state, so a push
  * still makes no host-to-device copy.  Unknown flag bits, and maps without AUGMENT, are errors.
  * vp3d_stream_state_bytes / vp3d_stream_init are the _ex calls with flags = 0 and no maps; push,
- * finish and release take either kind of session, with x, start_mask, y and frame shaped by S. */
+ * finish and release take either kind of session, with x, start_mask, y and frame shaped by S.
+ *
+ * Provisional outputs (VP3D_STREAM_PROVISIONAL, flags of the _ex calls, combinable with AUGMENT):
+ * the session may also be pushed with vp3d_stream_push_provisional, which is
+ * vp3d_stream_push_counts with dense x / y (x_rows = y_rows = NULL) that in addition writes what
+ * vp3d_stream_finish would return if it were called right after this push, without ending anything:
+ *   y_prov (S, lookahead, J_out, 3) fp32, frame_prov (S, lookahead) int64 (both DEVICE, required):
+ *     per slot the frames [c - lookahead, c) of its sequence that are not final yet (c = frames
+ *     pushed so far), computed with the generator's end padding as if the sequence ended now; -1
+ *     below frame 0, past an ended sequence's length and for idle slots; flip-averaged with AUGMENT.
+ *     The same bits as that finish, and the push's own y / frame and every later push are what
+ *     they would be without the request.  The push's GEMMs run over k + lookahead frame rows
+ *     (the look-ahead tail rides in the same launches); the output kernel always runs.
+ * The flag sizes every ring for K + lookahead new rows (vp3d_stream_state_bytes_ex grows) and is
+ * VP3D_ERR_INVALID on a causal plan (lookahead 0; state_bytes_ex returns 0).  A push_provisional on a
+ * session initialised without it is VP3D_ERR_STATE.  Plain pushes and finish of a flagged session
+ * keep their bits and launches. */
 #define VP3D_STREAM_AUGMENT 1
+#define VP3D_STREAM_PROVISIONAL 4
 int vp3d_stream_lookahead(const vp3d_plan* plan);
 size_t vp3d_stream_state_bytes(const vp3d_plan* plan, int S, int K);
 int vp3d_stream_init(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, void* stream);
@@ -767,6 +784,10 @@ int vp3d_stream_push_counts(vp3d_plan* plan, void* state, const float* x, int k,
                             const uint8_t* start_mask, const int32_t* end, const int64_t* x_rows,
                             const int64_t* y_rows, float* y, int64_t* frame, const int32_t* count,
                             void* stream);
+int vp3d_stream_push_provisional(vp3d_plan* plan, void* state, const float* x, int k,
+                                 const uint8_t* start_mask, const int32_t* end,
+                                 const int32_t* count, float* y, int64_t* frame, float* y_prov,
+                                 int64_t* frame_prov, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 int vp3d_stream_release(vp3d_plan* plan, void* state);
 

@@ -28,6 +28,7 @@ VP3D_SEMI_POS, VP3D_SEMI_TRAJ, VP3D_SEMI_PROJ, VP3D_SEMI_BONE = 1, 2, 4, 8
 VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2, 4, 8
 VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_LOSS_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
+VP3D_STREAM_PROVISIONAL = 4
 VP3D_CLIPS_AUGMENT = 1
 VP3D_INT8_CALIB_AMAX, VP3D_INT8_CALIB_PERCENTILE, VP3D_INT8_CALIB_MSE = 0, 1, 2
 
@@ -332,6 +333,9 @@ SIGNATURES = {
                                            ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_push_counts": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                                ctypes.c_int] + [ctypes.c_void_p] * 8),
+    "vp3d_stream_push_provisional": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p,
+                                                    ctypes.c_void_p, ctypes.c_int]
+                                     + [ctypes.c_void_p] * 8),
     "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),

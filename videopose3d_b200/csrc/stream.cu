@@ -56,14 +56,37 @@
 //     destination window positions, reading only mirror positions.  Both copies then agree, as the
 //     next push's input kernel and its mirror pass expect.
 // Both phases cover ring 0 and rings 1..nb, every plane and both physical rows of an AUGMENT slot.
+//
+// Provisional outputs (VP3D_STREAM_PROVISIONAL, vp3d_stream_push_provisional).  A push of k frames
+// also returns what vp3d_stream_finish would return right after it, for the la = lookahead frames
+// that are not final yet, without changing the session.  The chain of the push runs over k + la
+// frame rows instead of k: rows [k, k + la) (the tail) are fed the end padding, the slot's last real
+// frame repeated, exactly as the rows f >= n of a counted or ending slot already are, so row n + j
+// (n = slot_count) is the j-th row finish would compute, with the same operands in the same k-order.
+// The flag sizes every ring with R_l = H_l + K + la + 1 positions, so the window of such a push,
+// [w0, w0 + H + k + la), still never holds a position together with its mirror.  The tail lands in
+// positions [w0 + H + k, w0 + H + k + la) (ring 0: both copies); modulo R these are residues
+// w0 + H + k + j, which lie outside the residues [w0, w0 + H + k) of this push's history and new
+// rows because H + k + la < R.  So speculative writes never touch history, and never a row whose
+// mirror copy is pending: the next push copies only rows [w0 + H, w0 + H + k) (prev_k = k), and its
+// history [w0 + k, w0 + k + H) is H residues that again exclude the tail's (H + la < R).  A later
+// push reads a tail residue as history only after writing it as one of its new rows.  The
+// realign of a counted push moves only window positions [w0, w0 + H + k) and writes their mirror
+// copies, none of which lies in the tail's window copies.  The bookkeeping is double-buffered by
+// parity as for every push, q / prev_q / prev_k / parity advance as for k frames, and the output
+// kernel reads n from the two bookkeeping buffers (count after - count before), so nothing of the
+// tail persists.
 #include "internal.cuh"
 #include "launch.cuh"
 
 namespace vp3d {
 
+int stream_lookahead(const vp3d_plan* p);
+
 namespace {
 
 constexpr int kMaxRings = VP3D_MAX_WIDTHS;   // ring 0 = network input, ring i = block i input
+constexpr int kStreamFlags = VP3D_STREAM_AUGMENT | VP3D_STREAM_PROVISIONAL;
 
 struct StreamRing {
   __nv_bfloat16* base;   // plane 0, position 0
@@ -75,6 +98,7 @@ struct StreamRing {
 
 struct StreamLayout {
   int rings = 0;
+  int tail = 0;                 // PROVISIONAL: the look-ahead rows a push may append (else 0)
   int H[kMaxRings], R[kMaxRings], ld[kMaxRings];
   long long plane[kMaxRings];   // elements per ring plane
   size_t ring[kMaxRings];       // byte offsets
@@ -90,25 +114,27 @@ inline int physical_rows(int S, int flags) { return flags & VP3D_STREAM_AUGMENT 
 StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   StreamLayout L;
   L.rings = p->nb + 1;
+  L.tail = flags & VP3D_STREAM_PROVISIONAL ? stream_lookahead(p) : 0;
   const int planes = p->planes;
   const int P = physical_rows(S, flags);
+  const int rows = K + L.tail;   // frame rows a push computes at most
   Arena a{1024};
   L.count = a.take((size_t)2 * S * 8);
   L.active = a.take((size_t)2 * S);
   L.length = a.take((size_t)2 * S * 8);
   for (int l = 0; l < L.rings; ++l) {
     L.H[l] = 2 * p->pad[l];
-    L.R[l] = L.H[l] + K + 1;
+    L.R[l] = L.H[l] + rows + 1;
     L.ld[l] = l == 0 ? p->c_in_pad : p->C;
     L.plane[l] = 2LL * L.R[l] * P * L.ld[l];
     L.ring[l] = a.take((size_t)L.plane[l] * planes * 2);
   }
-  const size_t act = (size_t)planes * K * P * p->C * 2;
+  const size_t act = (size_t)planes * rows * P * p->C * 2;
   L.h = a.take(act);
   L.xlast = a.take(act);
   L.v[0] = 0;
   for (int l = 1; l < L.rings; ++l) L.v[l] = a.take((size_t)planes * P * p->C * 2);
-  L.ybuf = a.take((size_t)K * P * p->c_out_raw * 4);
+  L.ybuf = a.take((size_t)rows * P * p->c_out_raw * 4);
   if (flags & VP3D_STREAM_AUGMENT) {
     L.kps = a.take((size_t)p->cfg.num_joints_in * 4);
     L.jsrc = a.take((size_t)p->cfg.num_joints_out * 4);
@@ -141,6 +167,8 @@ struct StepArgs {
   long long* length_out;
   long long* frame;        // (S, frame_ld) int64
   int frame_ld, frame_off, lookahead;
+  int tail;                // provisional push: lookahead end-padding rows after the k (else 0)
+  long long* frame_prov;   // (S, tail) int64, the frames of those rows (tail > 0)
 };
 
 // Channel c of the mirrored input frame (generators.py:235-237) is source channel *src, negated when
@@ -198,7 +226,10 @@ __device__ __forceinline__ int packed_frames(const StepArgs& a, int s) {
 //     finish mode, and for the frames of a slot after its sequence's end, each physical row's last
 //     real frame is repeated instead (the generator's end padding, generators.py:216-238): packed
 //     from x[s, end - 1] in the push that ends it, the newest ring-0 position after that;
-//   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb.
+//   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb;
+//   * a provisional push (tail > 0): rows [k, k + tail) packed as the end padding of rows f >= n,
+//     and frame_prov[s, j] = count after the push - lookahead + j under the rules of `frame`, with
+//     the bookkeeping after the push: the frames vp3d_stream_finish would number right after it.
 __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) {
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nthr = (long long)gridDim.x * blockDim.x;
@@ -220,11 +251,16 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
     a.count_out[s] = c;
     a.active_out[s] = act;
     a.length_out[s] = len;
+    for (int j = 0; j < a.tail; ++j) {
+      const long long idx = c - a.lookahead + j;
+      a.frame_prov[s * a.tail + j] = (act && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
+    }
   }
 
   const StreamRing& r0 = a.ring[0];
   const int pairs = r0.ld >> 1;
-  const long long n_pack = (long long)a.k * a.P * pairs;
+  // rows f >= k (the tail) take the f >= n branch below: x[s, n - 1], or the newest ring-0 position
+  const long long n_pack = (long long)(a.k + a.tail) * a.P * pairs;
   const int src_pos = pos_mod_dev(r0.w0 + r0.H - 1, r0.R);
   for (long long i = tid; i < n_pack; i += nthr) {
     const int cp = (int)(i % pairs);
@@ -412,23 +448,43 @@ __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a
 // augment: rows f * 2S + s (plain) and f * 2S + S + s (mirrored) are flip-averaged (run.py:674-680),
 // output joint j of the mirrored row read from joint_src[j] (null: no joint swap, the trajectory
 // model).
+// Provisional push (prov.tail > 0): prov.y (S, tail, c_out) receives row j of slot s from frame row
+// n + j, n = the frames the slot advanced by (prov.count_out[s] minus prov.count_in[s], or minus 0
+// for a starting slot: the input kernel's bookkeeping of this push).
+struct ProvOut {
+  float* y;
+  const long long* count_in;
+  const long long* count_out;
+  const uint8_t* start;
+  int tail;
+};
+
 __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, float* y, int S, int k,
                                                             int c_out, int y_frames, int f_off,
                                                             int augment, const int* joint_src,
                                                             const long long* frame,
-                                                            const long long* y_rows) {
+                                                            const long long* y_rows,
+                                                            const ProvOut prov) {
   pdl_entry();
-  const long long n = (long long)k * S * c_out;
+  const long long n = (long long)(k + prov.tail) * S * c_out;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % c_out);
     const long long r = i / c_out;
-    const int s = (int)(r % S), f = (int)(r / S);
-    long long dst = ((long long)s * y_frames + f_off + f) * c_out + c;
-    if (y_rows) {
-      const long long t = frame[(long long)s * y_frames + f_off + f];
-      if (t < 0) continue;
-      dst = (__ldg(y_rows + s) + t) * c_out + c;
+    const int s = (int)(r % S);
+    int f = (int)(r / S);   // the frame row of ybuf
+    float* out;
+    if (f < k) {
+      out = y + ((long long)s * y_frames + f_off + f) * c_out + c;
+      if (y_rows) {
+        const long long t = frame[(long long)s * y_frames + f_off + f];
+        if (t < 0) continue;
+        out = y + (__ldg(y_rows + s) + t) * c_out + c;
+      }
+    } else {
+      const int j = f - k;
+      out = prov.y + ((long long)s * prov.tail + j) * c_out + c;
+      f = (int)(prov.count_out[s] - (prov.start && prov.start[s] ? 0 : prov.count_in[s])) + j;
     }
     float v;
     if (augment) {
@@ -437,9 +493,9 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
       const float* row0 = ybuf + ((long long)f * 2 * S + s) * c_out;
       v = flip_average(row0[c], row0[(long long)S * c_out + js * 3 + e], e);
     } else {
-      v = ybuf[i];
+      v = ybuf[((long long)f * S + s) * c_out + c];
     }
-    y[dst] = v;
+    *out = v;
   }
 }
 
@@ -458,9 +514,10 @@ inline __nv_bfloat16* ring_rows(const StreamRing& r, int pos, int P) {
 // The push of k frames as a flat chain over ring windows.  The window of ring i is its frame
 // positions [w0, w0 + H + k): tap j of the k * P new rows lies dilation * P rows after tap j - 1, the
 // residual (the centre tap, causal: the newest; model.py:130-132) a row offset into the same window.
-// Stage i writes the new rows of ring i + 1, the last stage the buffer shrink reads.
+// Stage i writes the new rows of ring i + 1, the last stage the buffer shrink reads.  A provisional
+// push appends its `tail` rows to the k: the same chain over k + tail frame rows.
 void push_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const StreamRing* ring,
-                int P, int K, int k, float* y, InferChain* c) {
+                int P, int K, int k, int tail, float* y, InferChain* c) {
   memset(c, 0, sizeof(*c));
   c->stages = p->nb + 1;
   c->samples = 1;
@@ -472,13 +529,13 @@ void push_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const 
   for (int i = 0; i <= p->nb; ++i) {
     ChainStage& s = c->st[i];
     s.in = ring_rows(ring[i], ring[i].w0, P);
-    s.in_rows = (ring[i].H + k) * P;
+    s.in_rows = (ring[i].H + k + tail) * P;
     const StreamRing* next = i < p->nb ? &ring[i + 1] : nullptr;
     s.out = next ? ring_rows(*next, next->w0 + next->H, P)
                  : reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
-    s.h_plane = (long long)K * P * p->C;
+    s.h_plane = (long long)(K + L.tail) * P * p->C;
     s.out_plane = next ? next->plane : s.h_plane;
-    s.out_rows = k * P;
+    s.out_rows = (k + tail) * P;
     s.tap_row_step = p->dilation[i] * P;
     s.res_row_off = (p->pad[i] + p->shift_dil[i]) * P;
   }
@@ -513,16 +570,18 @@ int stream_lookahead(const vp3d_plan* p) {
 // One push of k frames (x null: k copies of every slot's newest frame).  y receives rows
 // [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, or with y_rows the rows y_rows[s] + frame
 // of a flat one; frame the matching (S, y_frames) entries.  The GEMMs run over P physical rows per
-// frame (S, or 2S with AUGMENT).
+// frame (S, or 2S with AUGMENT).  y_prov non-null (a PROVISIONAL session): the push also computes the
+// lookahead end-padding rows and writes y_prov (S, lookahead, c_out) / frame_prov (S, lookahead).
 static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
                        const uint8_t* start, const int* end, const int* count,
                        const long long* x_rows,
                        const long long* y_rows, float* y, int y_frames, int f_off, long long* frame,
-                       cudaStream_t stream) {
+                       float* y_prov, long long* frame_prov, cudaStream_t stream) {
   const int S = h.S, K = h.K, C = p->C, planes = p->planes;
   const bool aug = h.flags & VP3D_STREAM_AUGMENT;
   const int P = physical_rows(S, h.flags);
   const StreamLayout L = stream_layout(p, S, K, h.flags);
+  const int tail = y_prov ? L.tail : 0;
   int launches = 0;
 
   StepArgs a;
@@ -569,8 +628,10 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.frame_ld = y_frames;
   a.frame_off = f_off;
   a.lookahead = stream_lookahead(p);
+  a.tail = tail;
+  a.frame_prov = frame_prov;
   {
-    long long work = (long long)k * P * (p->c_in_pad / 2);
+    long long work = (long long)(k + tail) * P * (p->c_in_pad / 2);
     for (int l = 1; l < L.rings; ++l) work += (long long)planes * h.prev_k * P * C / 8;
     if (work < S) work = S;
     // a plain launch: the first kernel of a push may follow a weight re-pack, which the GEMMs'
@@ -583,11 +644,13 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   const long long v_plane = (long long)P * C;
   auto vbuf = [&](int l) { return reinterpret_cast<__nv_bfloat16*>(base + L.v[l]); };
   // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
-  // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs)
-  const bool direct = !aug && !y_rows && (y_frames == 1 || S == 1);
+  // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs and
+  // provisional pushes)
+  const bool direct = !aug && !y_rows && !tail && (y_frames == 1 || S == 1);
   float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
   InferChain push;
-  push_chain(p, L, base, ring, P, K, k, direct ? y + (long long)f_off * p->c_out_raw : ybuf, &push);
+  push_chain(p, L, base, ring, P, K, k, tail,
+             direct ? y + (long long)f_off * p->c_out_raw : ybuf, &push);
 
   if (start && p->nb >= 1) {
     // ---- v-pass: v_1 = expand(x0), v_{i+1} = block_i(v_i)
@@ -638,11 +701,20 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     }
   }
   if (!direct) {
-    CUDA_TRY(launch_pdl(stream_output_kernel, dim3(grid_for((long long)k * S * p->c_out_raw)),
-                        dim3(256), 0, stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames,
-                        f_off, (int)aug,
+    ProvOut prov;
+    memset(&prov, 0, sizeof(prov));
+    if (tail) {
+      prov.y = y_prov;
+      prov.count_in = a.count_in;
+      prov.count_out = a.count_out;
+      prov.start = start;
+      prov.tail = tail;
+    }
+    CUDA_TRY(launch_pdl(stream_output_kernel,
+                        dim3(grid_for((long long)(k + tail) * S * p->c_out_raw)), dim3(256), 0,
+                        stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames, f_off, (int)aug,
                         h.joint_src ? (const int*)(base + L.jsrc) : (const int*)nullptr,
-                        (const long long*)frame, y_rows));
+                        (const long long*)frame, y_rows, prov));
     ++launches;
   }
   h.parity ^= 1;
@@ -666,7 +738,9 @@ static int stream_supported(const vp3d_plan* p, const char* what) {
 
 // every row index of a session's rings and buffers fits an int
 static bool stream_fits(const vp3d_plan* p, int S, int K, int flags) {
-  return (long long)physical_rows(S, flags) * (K + 2LL * vp3d_receptive_field(p)) <= 0x7fffffffLL;
+  const int tail = flags & VP3D_STREAM_PROVISIONAL ? stream_lookahead(p) : 0;
+  return (long long)physical_rows(S, flags) * (K + tail + 2LL * vp3d_receptive_field(p)) <=
+         0x7fffffffLL;
 }
 
 }  // namespace vp3d
@@ -681,8 +755,9 @@ VP3D_EXPORT int vp3d_stream_lookahead(const vp3d_plan* p) {
 }
 
 VP3D_EXPORT size_t vp3d_stream_state_bytes_ex(const vp3d_plan* p, int S, int K, int flags) {
-  if (!p || S < 1 || K < 1 || (flags & ~VP3D_STREAM_AUGMENT) || !stream_fits(p, S, K, flags))
+  if (!p || S < 1 || K < 1 || (flags & ~kStreamFlags) || !stream_fits(p, S, K, flags))
     return 0;
+  if ((flags & VP3D_STREAM_PROVISIONAL) && stream_lookahead(p) == 0) return 0;
   return stream_layout(p, S, K, flags).total;
 }
 
@@ -703,7 +778,7 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
                        void* stream) {
   if (S < 1 || K < 1)
     return fail(VP3D_ERR_INVALID, "%s: streams (%d) and max_frames (%d) must be >= 1", what, S, K);
-  if (flags & ~VP3D_STREAM_AUGMENT)
+  if (flags & ~kStreamFlags)
     return fail(VP3D_ERR_INVALID, "%s: unknown flags 0x%x", what, (unsigned)flags);
   const bool aug = flags & VP3D_STREAM_AUGMENT;
   if (!aug && (kps_src || joints_src))
@@ -713,6 +788,10 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
   if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
   if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
   VP3D_TRY(stream_supported(p, what));
+  if ((flags & VP3D_STREAM_PROVISIONAL) && stream_lookahead(p) == 0)
+    return fail(VP3D_ERR_INVALID,
+                "%s: VP3D_STREAM_PROVISIONAL on a causal model (lookahead 0: every output is final)",
+                what);
   const int j_in = p->cfg.num_joints_in, j_out = p->cfg.num_joints_out;
   if (aug) {
     VP3D_TRY(check_mirror_map(kps_src, j_in, what, "kps_src"));
@@ -772,7 +851,7 @@ static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost
 static int stream_push(const char* what, vp3d_plan* p, void* state, const float* x, int k,
                        const uint8_t* start_mask, const int32_t* end, const int32_t* count,
                        const int64_t* x_rows, const int64_t* y_rows, float* y, int64_t* frame,
-                       void* stream) {
+                       float* y_prov, int64_t* frame_prov, void* stream) {
   if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
   if (k < 1) return fail(VP3D_ERR_INVALID, "%s: k must be >= 1 (got %d)", what, k);
   if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
@@ -782,6 +861,9 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
   if (!x || !y || !frame) return fail(VP3D_ERR_INVALID, "%s: null x, y or frame", what);
   StreamHost* h = nullptr;
   VP3D_TRY(stream_lookup(p, state, what, &h));
+  if (y_prov && !(h->flags & VP3D_STREAM_PROVISIONAL))
+    return fail(VP3D_ERR_STATE, "%s: the session was not initialised with VP3D_STREAM_PROVISIONAL",
+                what);
   if (k > h->K)
     return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
   if (!p->conv_packed || !p->bn_packed)
@@ -789,7 +871,8 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
   return stream_step(p, ws_base(state), *h, x, k, start_mask, end, count,
                      reinterpret_cast<const long long*>(x_rows),
                      reinterpret_cast<const long long*>(y_rows), y, k, 0,
-                     reinterpret_cast<long long*>(frame), static_cast<cudaStream_t>(stream));
+                     reinterpret_cast<long long*>(frame), y_prov,
+                     reinterpret_cast<long long*>(frame_prov), static_cast<cudaStream_t>(stream));
 }
 
 VP3D_EXPORT int vp3d_stream_push_counts(vp3d_plan* p, void* state, const float* x, int k,
@@ -797,7 +880,17 @@ VP3D_EXPORT int vp3d_stream_push_counts(vp3d_plan* p, void* state, const float* 
                                         const int64_t* x_rows, const int64_t* y_rows, float* y,
                                         int64_t* frame, const int32_t* count, void* stream) {
   return stream_push("stream_push_counts", p, state, x, k, start_mask, end, count, x_rows, y_rows,
-                     y, frame, stream);
+                     y, frame, nullptr, nullptr, stream);
+}
+
+VP3D_EXPORT int vp3d_stream_push_provisional(vp3d_plan* p, void* state, const float* x, int k,
+                                             const uint8_t* start_mask, const int32_t* end,
+                                             const int32_t* count, float* y, int64_t* frame,
+                                             float* y_prov, int64_t* frame_prov, void* stream) {
+  if (!y_prov || !frame_prov)
+    return fail(VP3D_ERR_INVALID, "stream_push_provisional: null y_prov or frame_prov");
+  return stream_push("stream_push_provisional", p, state, x, k, start_mask, end, count, nullptr,
+                     nullptr, y, frame, y_prov, frame_prov, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, int k,
@@ -805,14 +898,14 @@ VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, i
                                     const int64_t* x_rows, const int64_t* y_rows, float* y,
                                     int64_t* frame, void* stream) {
   return stream_push("stream_push_ex", p, state, x, k, start_mask, end, nullptr, x_rows, y_rows, y,
-                     frame, stream);
+                     frame, nullptr, nullptr, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push(vp3d_plan* p, void* state, const float* x, int k,
                                  const uint8_t* start_mask, float* y, int64_t* frame,
                                  void* stream) {
   return stream_push("stream_push", p, state, x, k, start_mask, nullptr, nullptr, nullptr, nullptr,
-                     y, frame, stream);
+                     y, frame, nullptr, nullptr, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t* frame,
@@ -831,8 +924,7 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
   for (int off = 0; off < la; off += h->K) {
     const int k = la - off < h->K ? la - off : h->K;
     VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, nullptr, nullptr, nullptr, nullptr, y,
-                         la, off,
-                         reinterpret_cast<long long*>(frame), s));
+                         la, off, reinterpret_cast<long long*>(frame), nullptr, nullptr, s));
     launches += p->last_launches;
   }
   // every slot idle in the buffer the next push reads

@@ -39,6 +39,23 @@ mirrors it (common/generators.py:223-237), and returns the flip average of run.p
 bit-identical to ``metrics.flip_average(model(b), jl, jr)[0]`` with ``b`` the generator's (2, T +
 2 pad, J, F) batch.  The trajectory model (num_joints_out = 1) takes no joints lists (negate x only,
 run.py:678).
+
+Provisional poses for the frames still inside the look-ahead (non-causal models):
+
+    sess = model.streaming(streams=S, max_frames=K, provisional=True)
+    y, frame, y_prov, frame_prov = sess.push(x, start, end, count, provisional=True)
+
+``y_prov`` (S, lookahead, J_out, 3) / ``frame_prov`` (S, lookahead) are what ``finish()`` would
+return if it were called right after this push, bit for bit and with the same frame numbers, but
+nothing ends: the push's own ``y, frame`` and every later push are what they would be without the
+request.  Per slot they cover the frames [c - lookahead, c) of its sequence (c = frames pushed so
+far) that are not final yet, -1 below frame 0, past an ended sequence and for idle slots; each is
+the offline forward on the sequence as pushed so far, edge-padded.  Frame t thus gets a provisional
+pose as soon as its input arrives and its final one `lookahead` frames later, from one session.  The
+look-ahead tail rides in the push's own launches (its GEMMs run over k + lookahead frame rows), and
+the flag makes every ring hold `lookahead` positions more (``ring_bytes_per_stream(...,
+provisional=True)``).  A published checkpoint (arc 3,3,3,3,3, not causal) has a look-ahead of 121
+frames, 2.4 s at 50 fps, which this removes from the latency of a first estimate.
 """
 import weakref
 
@@ -68,15 +85,23 @@ def ring_history(filter_widths, dense=False):
     return hist
 
 
-def ring_bytes_per_stream(model, max_frames, planes=1, augment=False):
+def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisional=False):
     """Device bytes of history one stream slot occupies (both mirror halves, every plane; twice that
-    with augment: the slot's mirrored copy has rings of its own)."""
+    with augment: the slot's mirrored copy has rings of its own).  provisional: every ring also
+    holds the `lookahead` positions of the tail a provisional push appends (not for causal
+    models, whose look-ahead is 0)."""
     fw = model.filter_widths
     c_in = -(-model.num_joints_in * model.in_features // 64) * 64
     c = -(-model._channels // 64) * 64
+    tail = 0
+    if provisional:
+        tail = lookahead(model)
+        if tail == 0:
+            raise ValueError("provisional outputs need a non-causal model (a causal one has no "
+                             "look-ahead: every output is final)")
     total = 0
     for i, h in enumerate(ring_history(fw)):
-        total += 2 * (h + max_frames + 1) * (c_in if i == 0 else c) * 2 * planes
+        total += 2 * (h + max_frames + tail + 1) * (c_in if i == 0 else c) * 2 * planes
     return 2 * total if augment else total
 
 
@@ -127,7 +152,9 @@ class FrameBook:
         self.length = np.full(streams, -1, np.int64)
         self.lookahead = lookahead
 
-    def push(self, k, start=None, end=None, count=None):
+    def push(self, k, start=None, end=None, count=None, provisional=False):
+        """The (S, k) frame numbers of a push; provisional=True also returns the (S, lookahead)
+        numbers of its provisional rows, those finish() would give right after it."""
         S = len(self.count)
         start = np.zeros(S, bool) if start is None else np.asarray(start, bool)
         self.count[start] = 0
@@ -156,7 +183,12 @@ class FrameBook:
         done = self.active & (self.length >= 0) & ((self.count - self.lookahead >= self.length)
                                                    | (self.length == 0))
         self.active[done] = False
-        return frame
+        if not provisional:
+            return frame
+        idx = self.count[:, None] + np.arange(self.lookahead)[None, :] - self.lookahead
+        length = self.length[:, None]
+        prov = np.where(self.active[:, None] & (idx >= 0) & ((length < 0) | (idx < length)), idx, -1)
+        return frame, prov
 
     def finish(self):
         frame = self.push(self.lookahead) if self.lookahead else \
@@ -254,7 +286,7 @@ class StreamingSession:
     UnchunkedGenerator returns the test-time flip average instead."""
 
     def __init__(self, model, streams, max_frames, augment=False, kps_left=None, kps_right=None,
-                 joints_left=None, joints_right=None):
+                 joints_left=None, joints_right=None, provisional=False):
         from .temporal_model import TemporalModel
         if type(model)._variant != TemporalModel._variant:
             raise NotImplementedError(
@@ -277,7 +309,12 @@ class StreamingSession:
         self._kps_src, self._joints_src = augment_maps(model, augment, kps_left, kps_right,
                                                        joints_left, joints_right)
         self.augment = bool(augment)
-        self._flags = _capi.VP3D_STREAM_AUGMENT if self.augment else 0
+        self.provisional = bool(provisional)
+        if self.provisional and lookahead(model) == 0:
+            raise ValueError("provisional=True needs a non-causal model: a causal model has no "
+                             "look-ahead, every output of a push is already final")
+        self._flags = (_capi.VP3D_STREAM_AUGMENT if self.augment else 0) | \
+            (_capi.VP3D_STREAM_PROVISIONAL if self.provisional else 0)
         device = model.expand_conv.weight.device
         if device.type != "cuda":
             raise RuntimeError("streaming needs the model on a CUDA device; there is no CPU fallback")
@@ -391,7 +428,7 @@ class StreamingSession:
             return None
         return torch.tensor(start, dtype=torch.uint8).to(self.device)
 
-    def push(self, x, start=None, end=None, count=None):
+    def push(self, x, start=None, end=None, count=None, provisional=False):
         """Push up to k new frames per slot; returns (y (S, k, J_out, 3), frame (S, k) int64).
 
         start: S bools (list or device tensor), slots that begin a new sequence with x[s, 0].
@@ -402,7 +439,13 @@ class StreamingSession:
         has in this push (x[s, count[s]:] is not read, its rows get frame -1), for streams that skip
         or drop frames; None = k for every slot.  Read for open sequences that do not end in this
         push; at least 1 on a starting slot.  Values of a device tensor outside [0, k] (and 0 on a
-        starting slot) count as k.  Counts below k add two launches."""
+        starting slot) count as k.  Counts below k add two launches.
+        provisional: also return y_prov (S, lookahead, J_out, 3) and frame_prov (S, lookahead)
+        int64, what finish() would return right after this push (module docstring); needs a
+        session made with provisional=True."""
+        if provisional and not self.provisional:
+            raise RuntimeError("push(provisional=True) needs a session made with "
+                               "model.streaming(..., provisional=True)")
         k = check_push_input(x, self.streams, self.max_frames, self.model.num_joints_in,
                              self.model.in_features)
         if x.device != self.device:
@@ -423,6 +466,19 @@ class StreamingSession:
         y = torch.empty((self.streams, k, self.model.num_joints_out, 3), dtype=torch.float32,
                         device=self.device)
         frame = torch.empty((self.streams, k), dtype=torch.int64, device=self.device)
+        if provisional:
+            la = self.lookahead
+            y_prov = torch.empty((self.streams, la, self.model.num_joints_out, 3),
+                                 dtype=torch.float32, device=self.device)
+            frame_prov = torch.empty((self.streams, la), dtype=torch.int64, device=self.device)
+            ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+            with torch.cuda.device(self.device):
+                stream = self._prepare()
+                _capi.check(_capi.load().vp3d_stream_push_provisional(
+                    self._plan, self._state.data_ptr(), x.data_ptr(), k, ptr(mask), ptr(end),
+                    ptr(count), y.data_ptr(), frame.data_ptr(), y_prov.data_ptr(),
+                    frame_prov.data_ptr(), stream), "vp3d_stream_push_provisional")
+            return y, frame, y_prov, frame_prov
         with torch.cuda.device(self.device):
             stream = self._prepare()
             _capi.check(_capi.load().vp3d_stream_push_counts(
