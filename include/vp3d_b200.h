@@ -687,7 +687,8 @@ int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frame
  * causal_shift copies of the first frame in front, pad - causal_shift copies of the last behind.
  * Every conv layer keeps its input history in a time-major device ring inside the caller's state
  * buffer; a push costs the new frames' share of the FLOPs.  TemporalModel (VP3D_VARIANT_DILATED,
- * dense or not) in any precision but MIXED; the plan's packed eval weights are read at every push.
+ * dense or not) in any precision but MIXED (INT8 with VP3D_STREAM_INT8, below); the plan's packed
+ * eval weights are read at every push.
  *
  * vp3d_stream_lookahead: output frame t of a slot is returned by the push that delivers its input
  * frame t + lookahead (lookahead = pad - causal_shift: 0 for a causal model).
@@ -766,9 +767,26 @@ int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frame
  * The flag sizes every ring for K + lookahead new rows (vp3d_stream_state_bytes_ex grows) and is
  * VP3D_ERR_INVALID on a causal plan (lookahead 0; state_bytes_ex returns 0).  A push_provisional on a
  * session initialised without it is VP3D_ERR_STATE.  Plain pushes and finish of a flagged session
- * keep their bits and launches. */
+ * keep their bits and launches.
+ *
+ * int8 sessions (VP3D_STREAM_INT8, flags of the _ex calls, combinable with AUGMENT and
+ * PROVISIONAL): an INT8 plan streams only with this flag (init / init_ex without it stay
+ * VP3D_ERR_UNSUPPORTED, and state_bytes_ex without it keeps its size), and the flag needs an INT8
+ * plan (state_bytes_ex returns 0, init_ex VP3D_ERR_INVALID).  Every push and finish returns, per
+ * slot, the bits of the offline int8 forward (vp3d_forward_eval) on the padded sequence: the blocks
+ * of the plan's int8 mask run u8 x s8, the rest fp16, in the push's own launches.  Each ring of a
+ * residual block keeps a u8 copy of its history next to the 16-bit one (sized for every block,
+ * whatever the mask: about 1.5x the 16-bit ring bytes in all).  Launches: those of the same fp16
+ * session when every block runs int8, plus one quantise launch per fp16 -> int8 block transition in
+ * the push and one in the start pass where it contains that transition.  A push or finish needs
+ * folded scales (vp3d_set_int8_scales, then vp3d_set_weights), VP3D_ERR_STATE otherwise.  The
+ * history depends on the block mask and the activation scales: the session records both at its
+ * first push (or finish) after init, and a later push or finish that finds either changed
+ * (vp3d_set_int8_blocks, vp3d_set_int8_scales) is VP3D_ERR_STATE until the session is initialised
+ * again, so old and new quantisations never mix.  Flag bits 2 and 8 stay unknown. */
 #define VP3D_STREAM_AUGMENT 1
 #define VP3D_STREAM_PROVISIONAL 4
+#define VP3D_STREAM_INT8 16
 int vp3d_stream_lookahead(const vp3d_plan* plan);
 size_t vp3d_stream_state_bytes(const vp3d_plan* plan, int S, int K);
 int vp3d_stream_init(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, void* stream);

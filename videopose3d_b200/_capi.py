@@ -29,6 +29,7 @@ VP3D_EVAL_MPJPE, VP3D_EVAL_P_MPJPE, VP3D_EVAL_N_MPJPE, VP3D_EVAL_VELOCITY = 1, 2
 VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_LOSS_VELOCITY = 1, 2, 4, 8
 VP3D_STREAM_AUGMENT = 1
 VP3D_STREAM_PROVISIONAL = 4
+VP3D_STREAM_INT8 = 16
 VP3D_CLIPS_AUGMENT = 1
 VP3D_INT8_CALIB_AMAX, VP3D_INT8_CALIB_PERCENTILE, VP3D_INT8_CALIB_MSE = 0, 1, 2
 

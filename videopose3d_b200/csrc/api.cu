@@ -804,9 +804,11 @@ int vp3d::run_infer_chain(vp3d_plan* p, const InferChain& c, cudaStream_t stream
       // u8 x s8 block: Q_{i-1} -> H (u8 only) -> X_i (fp16, residual X_{i-1}) [+ Q_i]
       const PackedConv& k1 = *p->conv[2 * (i - 1)];
       const PackedConv& k2 = *p->conv[2 * (i - 1) + 1];
-      if (!c.st[i - 1].q_out || !c.hq) return fail(VP3D_ERR_STATE, "internal: int8 block %d has no u8 input", i);
+      if (!s.q_in || !c.hq) return fail(VP3D_ERR_STATE, "internal: int8 block %d has no u8 input", i);
+      if (s.q_in_bytes < (long long)c.samples * s.in_rows * C)
+        return fail(VP3D_ERR_STATE, "internal: u8 activation plane mismatch in block %d", i);
       vp3d_conv_desc d = conv(i, k1, nullptr, 0, s.in_rows, C);
-      d.a = c.st[i - 1].q_out;
+      d.a = s.q_in;
       d.tap_row_step = s.tap_row_step;
       d.scale = k1.q_scale;
       d.out_u8 = c.hq; d.out_u8_ld = C; d.out_u8_inv_scale = p->act_inv[2 * (i - 1) + 1];
@@ -935,6 +937,10 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
     s.out_plane = s.h_plane = (long long)N * L[i] * C;
     // Q_i exists where block i + 1 runs u8 x s8
     if (i < p->nb && block_is_int8(p, i + 1)) s.q_out = base + wl.q;
+    if (i > 0) {
+      s.q_in = c.st[i - 1].q_out;
+      s.q_in_bytes = (long long)wl.x_plane;
+    }
   }
 
   // Per-layer operand precision.  index 0 = expand, 1..nb = residual blocks, nb+1 = shrink.
@@ -944,7 +950,8 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
   //            split-bf16 (they carry most of the bf16 error, tools/precision_study.py),
   //            residual blocks run plain bf16 on the hi plane unless they hold < 0.5% of the
   //            forward FLOPs (negligible even at the narrow-tile rate of such layers).
-  //   int8   : the residual blocks of int8_mask u8 x s8; expand, shrink and the other blocks fp16.
+  //   int8   : layer_precision: the residual blocks of int8_mask u8 x s8; expand, shrink and the
+  //            other blocks fp16.
   {
     double fl[VP3D_MAX_WIDTHS + 1], total = 0.0;
     fl[0] = (double)N * L[0] * p->c_in_raw * fw[0] * C;
@@ -953,12 +960,9 @@ static void eval_chain(const vp3d_plan* p, const WsLayout& wl, uint8_t* base, in
     for (int i = 0; i <= p->nb + 1; ++i) total += fl[i];
     for (int i = 0; i <= p->nb + 1; ++i) {
       const bool x3 = i == 0 || i == p->nb + 1 || fl[i] < 0.005 * total;
-      const bool edge = i == 0 || i == p->nb + 1;
       c.precision[i] = p->cfg.precision == VP3D_PRECISION_MIXED
                            ? (x3 ? VP3D_PRECISION_BF16X3 : VP3D_PRECISION_BF16)
-                       : p->int8 ? (!edge && block_is_int8(p, i) ? VP3D_PRECISION_INT8
-                                                                  : VP3D_PRECISION_FP16)
-                                 : p->cfg.precision;
+                           : layer_precision(p, i);
     }
   }
 }

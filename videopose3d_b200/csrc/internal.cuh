@@ -114,6 +114,11 @@ struct StreamHost {
   long long prev_q = 0;   // q before the last push
   int prev_k = 0;         // frames of the last push (their ring rows still need their mirror copy)
   int parity = 0;         // bookkeeping buffer the next push reads (the pushes alternate the two)
+  // VP3D_STREAM_INT8: the plan's block mask and activation scales at the first push or finish after
+  // init; the history holds their quantisation, so a later push with other values is an error
+  bool int8_snap = false;
+  uint32_t int8_mask = 0;
+  float act_scale[VP3D_MAX_LAYERS] = {};
 };
 
 // step_ops.cu: Adam / AMSGrad update of conv weights that also refreshes their bf16 packs
@@ -220,6 +225,13 @@ int strided_trim(const vp3d_plan* p, int* L);
 inline bool block_is_int8(const vp3d_plan* p, int i) {
   return p->int8 && ((p->int8_mask >> (i - 1)) & 1u);
 }
+// operands of chain layer i (0 = expand, 1..nb = residual blocks, nb + 1 = shrink) in every
+// precision but `mixed` (whose split depends on the rows, eval_chain): int8 runs the blocks of
+// int8_mask u8 x s8 and expand, shrink and the other blocks fp16
+inline int layer_precision(const vp3d_plan* p, int i) {
+  if (!p->int8) return p->cfg.precision;
+  return i >= 1 && i <= p->nb && block_is_int8(p, i) ? VP3D_PRECISION_INT8 : VP3D_PRECISION_FP16;
+}
 // int8 plans keep the forward packs of their int8 blocks' convs in s8
 inline bool pack_is_s8(const vp3d_plan* p, const PackedConv& k) {
   return !k.transposed && k.src >= 0 && block_is_int8(p, k.src / 2 + 1);
@@ -259,6 +271,11 @@ struct ChainStage {
   int out_rows;              // per sample (per-sample tiles) or in all (flat)
   int tap_row_step, res_row_off;
   int lo_row_begin, lo_row_end;   // as in vp3d_conv_desc, of the GEMM that writes X_i
+  // int8 block i: its u8 A operand Q_{i-1}, [samples][in_rows][C] (the rows of `in`), and the bytes
+  // of the buffer it lies in; the offline chains read what stage i - 1's q_out wrote, a streaming
+  // push a window of ring i's u8 plane
+  const uint8_t* q_in;
+  long long q_in_bytes;
   uint8_t* q_out;            // int8 chain: the u8 copy Q_i of X_i that block i + 1 reads, or null
 };
 // The geometry of one run of the chain: what the offline forward (strided, dilated), the streaming

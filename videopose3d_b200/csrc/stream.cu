@@ -76,6 +76,17 @@
 // parity as for every push, q / prev_q / prev_k / parity advance as for k frames, and the output
 // kernel reads n from the two bookkeeping buffers (count after - count before), so nothing of the
 // tail persists.
+//
+// int8 sessions (VP3D_STREAM_INT8).  Ring i >= 1 of a block in the plan's int8 mask also holds a u8
+// plane Q_{i-1} with the positions of its 16-bit planes (frame t at t mod R and t mod R + R): block
+// i's k-tap conv reads the window [w0, w0 + H + k) of it, while stage i - 1 writes the new rows at
+// w0 + H into both planes (the expand's and an int8 block's epilogue; after an fp16 block a quantise
+// pass over the stored 16-bit rows, as in the offline int8 chain).  The start pass makes the u8
+// v_l(x0) the same way and the broadcast writes it next to the 16-bit one; the input kernel mirrors,
+// and the realign kernel moves, the u8 rows with the 16-bit ones.  Every ordering argument above
+// (mirror halves, tail residues, the two realign phases) is about positions, not planes, so it
+// holds for each plane: the u8 plane is written and read at exactly the positions of the 16-bit
+// planes, by the same kernels in the same order.  H is stored as u8 in `h`, as offline.
 #include "internal.cuh"
 #include "launch.cuh"
 
@@ -86,11 +97,14 @@ int stream_lookahead(const vp3d_plan* p);
 namespace {
 
 constexpr int kMaxRings = VP3D_MAX_WIDTHS;   // ring 0 = network input, ring i = block i input
-constexpr int kStreamFlags = VP3D_STREAM_AUGMENT | VP3D_STREAM_PROVISIONAL;
+constexpr int kStreamFlags = VP3D_STREAM_AUGMENT | VP3D_STREAM_PROVISIONAL | VP3D_STREAM_INT8;
 
 struct StreamRing {
   __nv_bfloat16* base;   // plane 0, position 0
   long long plane;       // elements per plane (2R * P * ld, P physical rows per position)
+  // VP3D_STREAM_INT8, ring i >= 1 of a block in the plan's int8_mask: the u8 plane Q_{i-1} block i
+  // reads, 2R * P * ld bytes with the positions of the 16-bit planes; null otherwise
+  uint8_t* q;
   int ld, H, R;
   int w0;                // first window position of the current push
   int prev_w0, prev_k;   // window start and new frames of the previous push (prev_k = 0: none)
@@ -106,6 +120,10 @@ struct StreamLayout {
   size_t h = 0, xlast = 0, ybuf = 0, total = 0;
   size_t v[kMaxRings];          // v_l(x0) of rings 1..nb: [plane][P][C]
   size_t kps = 0, jsrc = 0;     // AUGMENT: int32 mirror maps [J_in], [J_out]
+  // INT8, rings 1..nb whatever the block mask (the size depends on plan, S, K and flags only): the
+  // u8 plane [2R][P][C] and the u8 v_l(x0) [P][C]; H is stored as u8 in `h`.  After every other
+  // buffer, so that a layout without the flag is the one it always was.
+  size_t q[kMaxRings], vq[kMaxRings];
 };
 
 // rows every ring, activation and output buffer holds per frame position
@@ -138,6 +156,13 @@ StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   if (flags & VP3D_STREAM_AUGMENT) {
     L.kps = a.take((size_t)p->cfg.num_joints_in * 4);
     L.jsrc = a.take((size_t)p->cfg.num_joints_out * 4);
+  }
+  L.q[0] = L.vq[0] = 0;
+  for (int l = 1; l < L.rings; ++l) {
+    L.q[l] = L.vq[l] = 0;
+    if (!(flags & VP3D_STREAM_INT8)) continue;
+    L.q[l] = a.take((size_t)L.plane[l]);
+    L.vq[l] = a.take((size_t)P * p->C);
   }
   L.total = a.total();
   return L;
@@ -323,6 +348,17 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
                                             (long long)mirror_pos(pos, r.R) * a.P * r.ld) + e;
       *dst = *src;
     }
+    if (!r.q) continue;
+    // the u8 plane of the same rows (INT8 sessions, rings of int8 blocks)
+    const long long per_frame_q = (long long)a.P * r.ld / 16;
+    const long long nq = r.prev_k * per_frame_q;
+    for (long long i = tid; i < nq; i += nthr) {
+      const long long e = i % per_frame_q;
+      const int pos = r.prev_w0 + r.H + (int)(i / per_frame_q);
+      const uint4* src = reinterpret_cast<const uint4*>(r.q + (long long)pos * a.P * r.ld) + e;
+      uint4* dst = reinterpret_cast<uint4*>(r.q + (long long)mirror_pos(pos, r.R) * a.P * r.ld) + e;
+      *dst = *src;
+    }
   }
 }
 
@@ -380,20 +416,27 @@ __global__ void __launch_bounds__(256) stream_realign_kernel(const StepArgs a, i
         for (int l = 0; l < kMaxRings; ++l) {   // (unrolled: the ring table stays in parameter space)
           if (l >= a.rings) break;
           const StreamRing& g = a.ring[l];
+          // the ring's 16-bit planes (ld / 8 vectors per row), then its u8 plane (ld / 16)
           const int vec = g.ld / 8;
           const int m = a.planes * g.H * vec;
-          if (rem >= m) {
-            rem -= m;
+          const int m_all = m + (g.q ? g.H * (g.ld / 16) : 0);
+          if (rem >= m_all) {
+            rem -= m_all;
             continue;
           }
-          const int e = rem % vec, q = rem / vec;
+          const bool u8 = rem >= m;
+          const int vr = u8 ? g.ld / 16 : vec;
+          if (u8) rem -= m;
+          const int e = rem % vr, q = rem / vr;
           const int j = q % g.H, pl = q / g.H;
           const int to = g.w0 + a.k + j;   // a window position, < 2R
           const int from = phase == 0 ? g.w0 + n + j : mirror_pos(to, g.R);
-          __nv_bfloat16* pb = g.base + pl * g.plane;
-          v[u] = *(reinterpret_cast<const uint4*>(pb + ((long long)from * a.P + r) * g.ld) + e);
+          const int row_bytes = u8 ? g.ld : 2 * g.ld;
+          uint8_t* pb = u8 ? g.q : reinterpret_cast<uint8_t*>(g.base + pl * g.plane);
+          v[u] = *(reinterpret_cast<const uint4*>(pb + ((long long)from * a.P + r) * row_bytes) + e);
           dst[u] = reinterpret_cast<uint4*>(
-                       pb + ((long long)(phase == 0 ? mirror_pos(to, g.R) : to) * a.P + r) * g.ld) + e;
+                       pb + ((long long)(phase == 0 ? mirror_pos(to, g.R) : to) * a.P + r) *
+                                row_bytes) + e;
           break;
         }
       }
@@ -410,6 +453,7 @@ __global__ void __launch_bounds__(256) stream_realign_kernel(const StepArgs a, i
 struct BcastArgs {
   StreamRing ring[kMaxRings];
   const __nv_bfloat16* src[kMaxRings];   // [plane][S][ld] rows v_l(x0)
+  const uint8_t* src_q[kMaxRings];       // rings with a u8 plane: [P][ld] u8 rows v_l(x0)
   long long src_plane[kMaxRings];
   int rings, planes, S, P;
   const uint8_t* start;
@@ -438,6 +482,19 @@ __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a
       __nv_bfloat16* pbase = r.base + pl * r.plane;
       *(reinterpret_cast<uint4*>(pbase + ((long long)pos * a.P + row) * r.ld) + e) = v;
       *(reinterpret_cast<uint4*>(pbase + ((long long)mirror_pos(pos, r.R) * a.P + row) * r.ld) + e) = v;
+    }
+    if (!r.q) continue;
+    const int vq = r.ld / 16;
+    const long long nq = (long long)r.H * a.P * vq;
+    for (long long i = tid; i < nq; i += nthr) {
+      const int e = (int)(i % vq);
+      const long long q = i / vq;
+      const int row = (int)(q % a.P), j = (int)(q / a.P);
+      if (!a.start[row < a.S ? row : row - a.S]) continue;
+      const uint4 v = *(reinterpret_cast<const uint4*>(a.src_q[l] + (long long)row * r.ld) + e);
+      const int pos = r.w0 + j;
+      *(reinterpret_cast<uint4*>(r.q + ((long long)pos * a.P + row) * r.ld) + e) = v;
+      *(reinterpret_cast<uint4*>(r.q + ((long long)mirror_pos(pos, r.R) * a.P + row) * r.ld) + e) = v;
     }
   }
 }
@@ -510,12 +567,18 @@ inline int grid_for(long long work) {
 inline __nv_bfloat16* ring_rows(const StreamRing& r, int pos, int P) {
   return r.base + (long long)pos * P * r.ld;
 }
+// the same rows of its u8 plane (null without one)
+inline uint8_t* ring_rows_q(const StreamRing& r, int pos, int P) {
+  return r.q ? r.q + (long long)pos * P * r.ld : nullptr;
+}
 
 // The push of k frames as a flat chain over ring windows.  The window of ring i is its frame
 // positions [w0, w0 + H + k): tap j of the k * P new rows lies dilation * P rows after tap j - 1, the
 // residual (the centre tap, causal: the newest; model.py:130-132) a row offset into the same window.
 // Stage i writes the new rows of ring i + 1, the last stage the buffer shrink reads.  A provisional
-// push appends its `tail` rows to the k: the same chain over k + tail frame rows.
+// push appends its `tail` rows to the k: the same chain over k + tail frame rows.  An int8 block i
+// reads the same window of ring i's u8 plane, which stage i - 1 fills at w0 + H as it writes the
+// 16-bit rows (the expand's and int8 blocks' epilogues, or a quantise pass after an fp16 block).
 void push_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const StreamRing* ring,
                 int P, int K, int k, int tail, float* y, InferChain* c) {
   memset(c, 0, sizeof(*c));
@@ -524,13 +587,19 @@ void push_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const 
   c->in_plane = ring[0].plane;
   c->expand = p->expand_dil;
   c->h = reinterpret_cast<__nv_bfloat16*>(base + L.h);
+  if (p->int8) c->hq = base + L.h;
   c->y = y;
-  for (int i = 0; i <= p->nb + 1; ++i) c->precision[i] = p->cfg.precision;   // (never `mixed`)
+  for (int i = 0; i <= p->nb + 1; ++i) c->precision[i] = layer_precision(p, i);   // (never `mixed`)
   for (int i = 0; i <= p->nb; ++i) {
     ChainStage& s = c->st[i];
     s.in = ring_rows(ring[i], ring[i].w0, P);
     s.in_rows = (ring[i].H + k + tail) * P;
+    if (i > 0) {
+      s.q_in = ring_rows_q(ring[i], ring[i].w0, P);
+      s.q_in_bytes = (long long)(2 * ring[i].R - ring[i].w0) * P * ring[i].ld;
+    }
     const StreamRing* next = i < p->nb ? &ring[i + 1] : nullptr;
+    s.q_out = next ? ring_rows_q(*next, next->w0 + next->H, P) : nullptr;
     s.out = next ? ring_rows(*next, next->w0 + next->H, P)
                  : reinterpret_cast<__nv_bfloat16*>(base + L.xlast);
     s.h_plane = (long long)(K + L.tail) * P * p->C;
@@ -556,6 +625,10 @@ void vpass_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const
     s.out = reinterpret_cast<__nv_bfloat16*>(base + L.v[i + 1]);
     s.out_plane = v_plane;
     s.tap_row_step = s.res_row_off = 0;
+    // the u8 v_l(x0) of the rings of int8 blocks, made and read as the push's u8 rows are
+    s.q_in = i == 0 ? nullptr : c->st[i - 1].q_out;
+    s.q_in_bytes = (long long)P * p->C;
+    s.q_out = ring[i + 1].q ? base + L.vq[i + 1] : nullptr;
   }
 }
 
@@ -591,6 +664,7 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     StreamRing& r = ring[l];
     r.base = reinterpret_cast<__nv_bfloat16*>(base + L.ring[l]);
     r.plane = L.plane[l];
+    r.q = (h.flags & VP3D_STREAM_INT8) && l > 0 && block_is_int8(p, l) ? base + L.q[l] : nullptr;
     r.ld = L.ld[l];
     r.H = L.H[l];
     r.R = L.R[l];
@@ -632,7 +706,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.frame_prov = frame_prov;
   {
     long long work = (long long)(k + tail) * P * (p->c_in_pad / 2);
-    for (int l = 1; l < L.rings; ++l) work += (long long)planes * h.prev_k * P * C / 8;
+    for (int l = 1; l < L.rings; ++l)
+      work += (long long)planes * h.prev_k * P * C / 8 + (ring[l].q ? (long long)h.prev_k * P * C / 16 : 0);
     if (work < S) work = S;
     // a plain launch: the first kernel of a push may follow a weight re-pack, which the GEMMs'
     // early weight loads must not overlap
@@ -671,8 +746,10 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
       } else {
         b.src[l] = vbuf(l);
         b.src_plane[l] = v_plane;
+        b.src_q[l] = ring[l].q ? base + L.vq[l] : nullptr;
       }
-      work += (long long)planes * ring[l].H * P * ring[l].ld / 8;
+      work += (long long)planes * ring[l].H * P * ring[l].ld / 8 +
+              (ring[l].q ? (long long)ring[l].H * P * ring[l].ld / 16 : 0);
     }
     b.rings = L.rings;
     b.planes = planes;
@@ -689,7 +766,8 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     // the slots with fewer real frames than k: both realign phases, after the last GEMM read the
     // rings (the host cannot see the counts, so they always run)
     int row_vecs = 0;   // 16-byte vectors a realigned row moves per phase
-    for (int l = 0; l < L.rings; ++l) row_vecs += planes * ring[l].H * ring[l].ld / 8;
+    for (int l = 0; l < L.rings; ++l)
+      row_vecs += planes * ring[l].H * ring[l].ld / 8 + (ring[l].q ? ring[l].H * ring[l].ld / 16 : 0);
     // four vectors per thread over one full tile, at most four blocks per SM: enough loads in
     // flight for HBM bandwidth, and few blocks to scan the counts when no row realigns
     int grid = grid_for((long long)row_vecs * (P < kRealignTile ? P : kRealignTile) / 4);
@@ -725,14 +803,38 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   return VP3D_OK;
 }
 
-static int stream_supported(const vp3d_plan* p, const char* what) {
+static int stream_supported(const vp3d_plan* p, int flags, const char* what) {
   if (p->cfg.variant != VP3D_VARIANT_DILATED)
     return fail(VP3D_ERR_UNSUPPORTED, "%s: streaming needs the TemporalModel (dilated) variant",
                 what);
   if (p->cfg.precision == VP3D_PRECISION_MIXED)
     return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'mixed' is not supported for streaming", what);
-  if (p->cfg.precision == VP3D_PRECISION_INT8)
-    return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'int8' is not supported for streaming", what);
+  if (p->int8 && !(flags & VP3D_STREAM_INT8))
+    return fail(VP3D_ERR_UNSUPPORTED, "%s: precision 'int8' streams only in a session initialised "
+                "with VP3D_STREAM_INT8", what);
+  if (!p->int8 && (flags & VP3D_STREAM_INT8))
+    return fail(VP3D_ERR_INVALID, "%s: VP3D_STREAM_INT8 needs an int8 plan", what);
+  return VP3D_OK;
+}
+
+// An INT8 session's history holds the quantisation of the plan's block mask and activation scales
+// at its first push after init: later pushes need the same ones (and, as every int8 chain, folded
+// scales).
+static int stream_int8_ready(const vp3d_plan* p, StreamHost& h, const char* what) {
+  if (!(h.flags & VP3D_STREAM_INT8)) return VP3D_OK;
+  if (!p->int8_folded)
+    return fail(VP3D_ERR_STATE, "%s: int8 plan without folded activation scales (call "
+                "vp3d_set_int8_scales, then vp3d_set_weights)", what);
+  const size_t scale_bytes = sizeof(float) * 2 * p->nb;
+  if (!h.int8_snap) {
+    h.int8_snap = true;
+    h.int8_mask = p->int8_mask;
+    memcpy(h.act_scale, p->act_scale, scale_bytes);
+    return VP3D_OK;
+  }
+  if (h.int8_mask != p->int8_mask || memcmp(h.act_scale, p->act_scale, scale_bytes) != 0)
+    return fail(VP3D_ERR_STATE, "%s: the plan's int8 blocks or activation scales changed since the "
+                "session's first push; initialise the session again", what);
   return VP3D_OK;
 }
 
@@ -758,6 +860,7 @@ VP3D_EXPORT size_t vp3d_stream_state_bytes_ex(const vp3d_plan* p, int S, int K, 
   if (!p || S < 1 || K < 1 || (flags & ~kStreamFlags) || !stream_fits(p, S, K, flags))
     return 0;
   if ((flags & VP3D_STREAM_PROVISIONAL) && stream_lookahead(p) == 0) return 0;
+  if ((flags & VP3D_STREAM_INT8) && !p->int8) return 0;
   return stream_layout(p, S, K, flags).total;
 }
 
@@ -787,7 +890,7 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
     return fail(VP3D_ERR_INVALID, "%s: VP3D_STREAM_AUGMENT needs kps_src", what);
   if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
   if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
-  VP3D_TRY(stream_supported(p, what));
+  VP3D_TRY(stream_supported(p, flags, what));
   if ((flags & VP3D_STREAM_PROVISIONAL) && stream_lookahead(p) == 0)
     return fail(VP3D_ERR_INVALID,
                 "%s: VP3D_STREAM_PROVISIONAL on a causal model (lookahead 0: every output is final)",
@@ -868,6 +971,7 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
     return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
   if (!p->conv_packed || !p->bn_packed)
     return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
+  VP3D_TRY(stream_int8_ready(p, *h, what));
   return stream_step(p, ws_base(state), *h, x, k, start_mask, end, count,
                      reinterpret_cast<const long long*>(x_rows),
                      reinterpret_cast<const long long*>(y_rows), y, k, 0,
@@ -918,6 +1022,7 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
     return fail(VP3D_ERR_STATE, "stream_finish: vp3d_set_weights has not been called");
   const int la = stream_lookahead(p);
   if (la > 0 && (!y || !frame)) return fail(VP3D_ERR_INVALID, "stream_finish: null y or frame");
+  VP3D_TRY(stream_int8_ready(p, *h, "stream_finish"));
   uint8_t* base = ws_base(state);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int launches = 0;

@@ -56,6 +56,18 @@ look-ahead tail rides in the push's own launches (its GEMMs run over k + lookahe
 the flag makes every ring hold `lookahead` positions more (``ring_bytes_per_stream(...,
 provisional=True)``).  A published checkpoint (arc 3,3,3,3,3, not causal) has a look-ahead of 121
 frames, 2.4 s at 50 fps, which this removes from the latency of a first estimate.
+
+int8 sessions, for a model calibrated for ``set_precision('int8')``:
+
+    sess = model.streaming(streams=S, max_frames=K, int8=True)   # with augment / provisional too
+
+Every output is bit for bit the offline int8 forward ``model(xp)`` on the padded sequence: the
+blocks of ``model.int8_blocks`` run u8 x s8, the rest fp16, in the push's own launches (one quantise
+launch more per fp16 -> int8 block transition).  The rings of the residual blocks keep a u8 copy of
+their history (``ring_bytes_per_stream(..., int8=True)``, about 1.5x the 16-bit bytes).  The history
+holds one calibration's quantisation: ``calibrate_int8``, ``load_int8_calibration`` or
+``set_int8_blocks`` under a session with history make its next push raise until ``reset()``, as a
+parameter change does.  An int8 model without ``int8=True`` cannot stream.
 """
 import weakref
 
@@ -85,11 +97,13 @@ def ring_history(filter_widths, dense=False):
     return hist
 
 
-def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisional=False):
+def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisional=False,
+                          int8=False):
     """Device bytes of history one stream slot occupies (both mirror halves, every plane; twice that
     with augment: the slot's mirrored copy has rings of its own).  provisional: every ring also
     holds the `lookahead` positions of the tail a provisional push appends (not for causal
-    models, whose look-ahead is 0)."""
+    models, whose look-ahead is 0).  int8: the rings of the residual blocks also hold a u8 plane
+    with the same positions (one byte per channel, every block whatever the int8 block set)."""
     fw = model.filter_widths
     c_in = -(-model.num_joints_in * model.in_features // 64) * 64
     c = -(-model._channels // 64) * 64
@@ -101,7 +115,10 @@ def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisiona
                              "look-ahead: every output is final)")
     total = 0
     for i, h in enumerate(ring_history(fw)):
-        total += 2 * (h + max_frames + tail + 1) * (c_in if i == 0 else c) * 2 * planes
+        positions = 2 * (h + max_frames + tail + 1)
+        total += positions * (c_in if i == 0 else c) * 2 * planes
+        if int8 and i > 0:
+            total += positions * c
     return 2 * total if augment else total
 
 
@@ -286,7 +303,7 @@ class StreamingSession:
     UnchunkedGenerator returns the test-time flip average instead."""
 
     def __init__(self, model, streams, max_frames, augment=False, kps_left=None, kps_right=None,
-                 joints_left=None, joints_right=None, provisional=False):
+                 joints_left=None, joints_right=None, provisional=False, int8=False):
         from .temporal_model import TemporalModel
         if type(model)._variant != TemporalModel._variant:
             raise NotImplementedError(
@@ -296,10 +313,15 @@ class StreamingSession:
             raise NotImplementedError(
                 "precision 'mixed' cannot stream: its per-layer split choice depends on the "
                 "sequence length; use 'fp16', 'bf16' or 'bf16x3'")
-        if model.precision == "int8":
+        self.int8 = bool(int8)
+        if self.int8 and model.precision != "int8":
+            raise ValueError(f"int8=True streams a model in precision 'int8' (this one is "
+                             f"{model.precision!r}: call set_precision('int8') first)")
+        if model.precision == "int8" and not self.int8:
             raise NotImplementedError(
-                "precision 'int8' cannot stream (the offline eval forward only); use 'fp16', "
-                "'bf16' or 'bf16x3'")
+                "precision 'int8' streams only in an int8 session: model.streaming(..., "
+                "int8=True), whose rings also keep the u8 history; or use 'fp16', 'bf16' or "
+                "'bf16x3'")
         if model.training:
             raise RuntimeError("streaming is an eval-mode computation: call model.eval() first")
         streams, max_frames = int(streams), int(max_frames)
@@ -314,7 +336,8 @@ class StreamingSession:
             raise ValueError("provisional=True needs a non-causal model: a causal model has no "
                              "look-ahead, every output of a push is already final")
         self._flags = (_capi.VP3D_STREAM_AUGMENT if self.augment else 0) | \
-            (_capi.VP3D_STREAM_PROVISIONAL if self.provisional else 0)
+            (_capi.VP3D_STREAM_PROVISIONAL if self.provisional else 0) | \
+            (_capi.VP3D_STREAM_INT8 if self.int8 else 0)
         device = model.expand_conv.weight.device
         if device.type != "cuda":
             raise RuntimeError("streaming needs the model on a CUDA device; there is no CPU fallback")
@@ -346,7 +369,7 @@ class StreamingSession:
                 self._plan, self._state.data_ptr(), self._state.numel(), self.streams,
                 self.max_frames, self._flags, host_ptr(self._kps_src), host_ptr(self._joints_src),
                 stream), "vp3d_stream_init_ex")
-        self._versions = None
+        self._versions = self._quant = None
         return self
 
     def _prepare(self):
@@ -357,9 +380,19 @@ class StreamingSession:
         if self._versions is not None and current != self._versions:
             raise RuntimeError("the model's parameters changed since this session started; call "
                                "reset() before pushing again (old and new weights never mix)")
+        # an int8 history is also made from the calibration (the `_int8` tuple itself: every
+        # calibrate_int8 / load_int8_calibration makes a new one) and the int8 block set
+        quant = (m._int8, m.int8_blocks) if self.int8 else None
+        if self._versions is not None and self.int8 and (
+                quant[0] is not self._quant[0] or quant[1] != self._quant[1]):
+            raise RuntimeError("the model's int8 calibration or int8 blocks changed since this "
+                               "session started; call reset() before pushing again (old and new "
+                               "quantisations never mix)")
         stream = torch.cuda.current_stream(self.device).cuda_stream
+        # (an int8 plan also takes the model's block set and calibration here: _sync_int8)
         m._sync_weights(self._plan, stream)
         self._versions = current
+        self._quant = quant
         return stream
 
     def _slot_tensor(self, v, name):

@@ -756,17 +756,19 @@ class TemporalModelBase(nn.Module):
         return 0 if self._plan is None else _capi.load().vp3d_last_launch_count(self._plan)
 
     def streaming(self, streams, max_frames=1, augment=False, kps_left=None, kps_right=None,
-                  joints_left=None, joints_right=None, provisional=False):
+                  joints_left=None, joints_right=None, provisional=False, int8=False):
         """A StreamingSession (videopose3d_b200.streaming) of `streams` slots that takes up to
         `max_frames` new frames per slot and push, and returns each output frame as soon as its
         input has arrived.  `augment=True` with UnchunkedGenerator's left / right lists returns
         run.py's test-time flip average (run.py:674-680).  `provisional=True` (non-causal models
         only, ValueError otherwise) lets push(..., provisional=True) also return provisional
-        poses for the frames still inside the look-ahead.  Not in the reference."""
+        poses for the frames still inside the look-ahead.  `int8=True` streams a model in
+        precision 'int8' (ValueError in any other precision; an int8 model needs it), bit for bit
+        its offline int8 forward.  Not in the reference."""
         from .streaming import StreamingSession
         return StreamingSession(self, streams, max_frames, augment=augment, kps_left=kps_left,
                                 kps_right=kps_right, joints_left=joints_left,
-                                joints_right=joints_right, provisional=provisional)
+                                joints_right=joints_right, provisional=provisional, int8=int8)
 
     def predict(self, sequences, augment=False, kps_left=None, kps_right=None, joints_left=None,
                 joints_right=None, max_rows=None):
