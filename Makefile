@@ -6,7 +6,7 @@ NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisi
 CSRC      := videopose3d_b200/csrc
 LIBDIR    := videopose3d_b200/_lib
 LIB       := $(LIBDIR)/libvp3d_b200.so
-SRCS      := $(CSRC)/conv_gemm.cu $(CSRC)/wgrad_gemm.cu $(CSRC)/pack.cu $(CSRC)/train_ops.cu $(CSRC)/api.cu $(CSRC)/train_api.cu $(CSRC)/gather.cu $(CSRC)/step_ops.cu $(CSRC)/semi_loss.cu $(CSRC)/pose_loss.cu $(CSRC)/stream.cu $(CSRC)/clips.cu $(CSRC)/calib.cu
+SRCS      := $(CSRC)/conv_gemm.cu $(CSRC)/wgrad_gemm.cu $(CSRC)/pack.cu $(CSRC)/train_ops.cu $(CSRC)/api.cu $(CSRC)/train_api.cu $(CSRC)/gather.cu $(CSRC)/step_ops.cu $(CSRC)/semi_loss.cu $(CSRC)/pose_loss.cu $(CSRC)/stream.cu $(CSRC)/clips.cu $(CSRC)/calib.cu $(CSRC)/detections.cu
 OBJS      := $(SRCS:$(CSRC)/%.cu=$(LIBDIR)/%.o)
 HDRS      := $(wildcard $(CSRC)/*.cuh) include/vp3d_b200.h
 

@@ -807,6 +807,28 @@ int vp3d_stream_push_provisional(vp3d_plan* plan, void* state, const float* x, i
                                  const int32_t* count, float* y, int64_t* frame, float* y_prov,
                                  int64_t* frame_prov, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
+
+/* Detector input (streaming.StreamingSession.push_detections): the input rows of the pushes one
+ * call makes, from a 2-D detector's pixel keypoints, as the reference's in-the-wild pipeline
+ * prepares them.  It replaces, per released frame, joint and coordinate:
+ *   data/prepare_data_2d_custom.py:39-49  np.interp(indices, indices[mask], kp[mask, i, j]) over
+ *     the frames without a detection (float64, stored as float32): slope = (r - l) / (ib - ia),
+ *     then slope * (t - ia) + l; a detected frame is its own value;
+ *   run.py:93-97, common/camera.py:14-18  X / w * 2 - [1, h / w]: float32 X / w and * 2, a float64
+ *     subtraction of 1 (x) or h / w (y), stored as float32.
+ * Each operation is rounded on its own (no FMA contraction), so the rows are numpy's bits.
+ * kps_px: DEVICE (S, k, J, 2) fp32 pixel keypoints of this call.  last: DEVICE (2, S, J, 2) fp32,
+ * the last detection of every slot, double-buffered: half `parity` is read, half 1 - parity
+ * written.  table: DEVICE int32, S triples (w, h, keep) then `rows` records (slot, left, right,
+ * num, den); keep = the row of kps_px[s] with the slot's newest detection (written to the new
+ * half), -1 = copy the old half.  Record r makes out row r (J x 2 fp32): left = row of kps_px[slot]
+ * with the left value, -1 = the slot's stored last detection, -2 = no frame (zeros); right = row of
+ * the right value of an interpolation with num = t - ia and den = ib - ia, -1 = a copy of the left
+ * value.  Records whose indices fall outside kps_px, or a slot with w or h <= 0, give zeros.  out:
+ * DEVICE (rows, J, 2) fp32.  One launch; argument errors (sizes, parity, null or not 8-byte aligned
+ * pointers) are returned before any device work. */
+int vp3d_stream_pack_detections(const float* kps_px, int S, int k, int J, const int32_t* table,
+                                int64_t rows, float* last, int parity, float* out, void* stream);
 int vp3d_stream_release(vp3d_plan* plan, void* state);
 
 /* ---- offline inference on a list of clips (run.py:186-193, 663-721 over a known set of clips) ----

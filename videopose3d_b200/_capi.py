@@ -340,6 +340,10 @@ SIGNATURES = {
     "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_stream_pack_detections": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                   ctypes.c_int, ctypes.c_void_p, ctypes.c_int64,
+                                                   ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                                   ctypes.c_void_p]),
     "vp3d_clips_workspace_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int]),
     "vp3d_forward_clips": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_int64,
                                                                   ctypes.c_int]

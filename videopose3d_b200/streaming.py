@@ -214,6 +214,237 @@ class FrameBook:
         return frame
 
 
+class DetectionCall:
+    """What one push_detections (or finish) call sends to the device, as DetectionBook plans it.
+
+    pushes: the internal pushes, each a dict of k (<= max_frames) and the per-slot arrays start
+    (bool), end (int32, -1 = none) and count (int32, frames released into this push), plus
+    `counted`: whether the push needs its count array (some open slot releases fewer than k).
+    records: (rows, 5) int32, one per input row of the pushes in order (push, slot, row) -- slot,
+    left, right, num, den as vp3d_stream_pack_detections reads them.  slots: (S, 3) int32 --
+    w, h and the row of this call's newest detection (-1 = keep the stored one).  frames: per slot
+    the video frame indices released, in order.  realigned: (slot, push) pairs that take the
+    realign path (an open slot with fewer frames than the push)."""
+
+    def __init__(self, pushes, records, slots, frames, realigned):
+        self.pushes, self.records, self.slots = pushes, records, slots
+        self.frames, self.realigned = frames, realigned
+
+    @property
+    def rows(self):
+        return len(self.records)
+
+    def table(self):
+        """The bytes copied to the device once per call, and the offsets (from its start) of each
+        push's end / count (int32, S each) and start (uint8, S) arrays: slots and records (int32,
+        vp3d_stream_pack_detections' table) | per push end, count | per push start."""
+        S, n = len(self.slots), len(self.pushes)
+        tab = np.concatenate([self.slots.reshape(-1), self.records.reshape(-1)]).astype(np.int32)
+        head = -(-tab.nbytes // 8) * 8
+        host = np.zeros(head + 8 * S * n + -(-S * n // 8) * 8, np.uint8)
+        host[:tab.nbytes] = tab.view(np.uint8)
+        offsets = []
+        for i, p in enumerate(self.pushes):
+            e, c, st = head + 8 * S * i, head + 8 * S * i + 4 * S, head + 8 * S * n + S * i
+            host[e:e + 4 * S] = p["end"].view(np.uint8)
+            host[c:c + 4 * S] = p["count"].view(np.uint8)
+            host[st:st + S] = p["start"]
+            offsets.append((e, c, st))
+        return host, offsets
+
+
+class DetectionBook:
+    """Host bookkeeping of a session fed by a 2-D detector (StreamingSession.push_detections):
+    which video frames each call releases to the network, and what each is made from, under the
+    rules of the reference's decode (data/prepare_data_2d_custom.py:39-49, np.interp over the
+    frames without a detection).  Per slot: the open video's frames seen so far, its newest
+    detection, the frames released so far (the run between them is pending), the video's
+    resolution, and whether the device slot holds the video yet (from its first released frame,
+    which is always video frame 0, so the device's frame numbers are the video's).
+
+    Release rules: a detection releases the pending frames before it (interpolated from the
+    previous detection, or equal to it before the first one: np.interp's left value) and itself;
+    frames after the last detection are released held (np.interp's right value) by the video's end
+    or finish(); with max_gap = G, a (G + 1)-th pending frame after a detection releases the oldest
+    one held.  A video without detections releases nothing.  Pure host code: the CPU tests drive
+    it, and the session turns each DetectionCall into one table copy, one pack launch and its
+    pushes."""
+
+    def __init__(self, streams, max_frames, max_gap=None, lookahead=0):
+        self.streams, self.max_frames = int(streams), int(max_frames)
+        if max_gap is not None and (isinstance(max_gap, bool) or int(max_gap) != max_gap
+                                    or int(max_gap) < 0):
+            raise ValueError(f"max_gap must be None or an int >= 0 (got {max_gap!r})")
+        self.max_gap = None if max_gap is None else int(max_gap)
+        S = self.streams
+        self.open = np.zeros(S, bool)               # a video is open: started, not ended
+        self.seen = np.zeros(S, np.int64)           # its frames seen so far
+        self.last = np.full(S, -1, np.int64)        # its newest detection, -1 before the first
+        self.released = np.zeros(S, np.int64)       # its frames released so far
+        self.on_device = np.zeros(S, bool)          # the device slot holds it as an open sequence
+        self.resolution = np.zeros((S, 2), np.int64)
+        self.device = FrameBook(S, lookahead)       # the device's bookkeeping under the pushes
+
+    def check(self, detected, start=None, end=None, resolution=None):
+        """The validated (detected (S, k) bool, start (S,) bool, end (S,) int64, resolution (S, 2))
+        of a call; raises ValueError / TypeError before anything changes."""
+        S = self.streams
+        if isinstance(detected, torch.Tensor) and detected.is_cuda:
+            raise TypeError("detected must be a host array: how many frames a slot releases depends "
+                            "on it, and reading it back from the device would synchronise")
+        detected = np.asarray(detected)
+        if detected.dtype != np.bool_:
+            raise TypeError(f"detected must be a bool array, got {detected.dtype}")
+        if detected.ndim != 2 or detected.shape[0] != S or not 1 <= detected.shape[1] <= \
+                self.max_frames:
+            raise ValueError(f"detected must have shape ({S}, k) with 1 <= k <= max_frames = "
+                             f"{self.max_frames}, got {detected.shape}")
+        k = detected.shape[1]
+        if isinstance(start, torch.Tensor) or isinstance(end, torch.Tensor):
+            raise TypeError("push_detections takes start and end as host lists (the host plans "
+                            "the releases from them)")
+        start = np.zeros(S, bool) if start is None else np.array([bool(v) for v in start])
+        if start.shape != (S,):
+            raise ValueError(f"start must list {S} slots")
+        end = np.full(S, -1, np.int64) if end is None else np.array([int(v) for v in end],
+                                                                    np.int64).reshape(-1)
+        if end.shape != (S,):
+            raise ValueError(f"end must list {S} slots")
+        for s in range(S):
+            if not -1 <= end[s] <= k:
+                raise ValueError(f"end[{s}] = {end[s]} is outside [-1, k = {k}]")
+            if end[s] == 0 and start[s]:
+                raise ValueError(f"slot {s} starts and ends with end = 0: a video without frames")
+        res = self.resolution.copy()
+        if resolution is not None:
+            resolution = list(resolution)
+            if len(resolution) != S:
+                raise ValueError(f"resolution must list {S} slots (a (w, h) pair or None each)")
+        for s in np.nonzero(start)[0]:
+            r = None if resolution is None else resolution[s]
+            if r is None:
+                raise ValueError(f"slot {s} starts without a resolution: give resolution[{s}] = "
+                                 "(w, h), the camera's frame size in pixels")
+            w, h = (int(v) for v in r)
+            if w <= 0 or h <= 0:
+                raise ValueError(f"resolution[{s}] = ({w}, {h}): width and height must be > 0")
+            res[s] = (w, h)
+        return detected, start, end, res
+
+    def push(self, detected, start=None, end=None, resolution=None):
+        """Plan one push_detections call (k = detected.shape[1] video frames per slot)."""
+        detected, start, end, res = self.check(detected, start, end, resolution)
+        S, k = detected.shape
+        rel = [[] for _ in range(S)]       # per slot: (t, left, right, num, den)
+        keep = np.full(S, -1, np.int64)
+        drop = np.zeros(S, bool)           # started: without a frame yet, start + end 0 on an active
+                                           # device slot
+        ending = np.zeros(S, bool)         # the device ends the slot's sequence in this call
+        for s in range(S):
+            if start[s]:
+                # (a start that releases nothing yet still ends what the device slot held, a
+                # draining tail included, as a start does in push)
+                drop[s] = True
+                self.open[s], self.on_device[s] = True, False
+                self.seen[s], self.last[s], self.released[s] = 0, -1, 0
+                self.resolution[s] = res[s]
+            if not self.open[s]:
+                continue
+            last_row = -1                  # row of the newest detection in this call, -1 = stored
+            for f in range(k if end[s] < 0 else int(end[s])):
+                t = int(self.seen[s])
+                self.seen[s] += 1
+                if detected[s, f]:
+                    a = int(self.last[s])
+                    for u in range(int(self.released[s]), t):
+                        rel[s].append((u, f, -1, 0, 0) if a < 0 else (u, last_row, f, u - a, t - a))
+                    rel[s].append((t, f, -1, 0, 0))
+                    self.last[s], self.released[s] = t, t + 1
+                    last_row = keep[s] = f
+                elif self.last[s] >= 0 and self.max_gap is not None and \
+                        self.seen[s] - self.released[s] > self.max_gap:
+                    rel[s].append((int(self.released[s]), last_row, -1, 0, 0))
+                    self.released[s] += 1
+            if end[s] >= 0:
+                if self.last[s] >= 0:
+                    for u in range(int(self.released[s]), int(self.seen[s])):
+                        rel[s].append((u, last_row, -1, 0, 0))
+                    self.released[s] = self.seen[s]
+                self.open[s] = False
+                ending[s] = True
+        return self._plan(k, rel, keep, drop, ending)
+
+    def finish(self):
+        """Plan the pushes finish() makes before the device finish: every open video's pending
+        frames released held; every slot then idle."""
+        S = self.streams
+        rel = [[] for _ in range(S)]
+        for s in np.nonzero(self.open & (self.last >= 0))[0]:
+            rel[s] = [(u, -1, -1, 0, 0) for u in range(int(self.released[s]), int(self.seen[s]))]
+            self.released[s] = self.seen[s]
+        none = np.zeros(S, bool)
+        call = self._plan(0, rel, np.full(S, -1, np.int64), none, none)
+        self.open[:] = False
+        self.on_device[:] = False
+        self.device.finish()
+        return call
+
+    def _plan(self, k, rel, keep, drop, ending):
+        """Split the released frames into pushes of at most max_frames, k rows in all at least."""
+        S, K = self.streams, self.max_frames
+        n = np.array([len(r) for r in rel], np.int64)
+        total = max(k, int(n.max()))
+        ks = [min(K, total - o) for o in range(0, total, K)]
+        offs = np.concatenate([[0], np.cumsum(ks)]).astype(np.int64)
+        pushes = [dict(k=kk, start=np.zeros(S, bool), end=np.full(S, -1, np.int32),
+                       count=np.zeros(S, np.int32)) for kk in ks]
+        for i, p in enumerate(pushes):
+            p["count"][:] = np.clip(n - offs[i], 0, ks[i])
+        # the push in which the device's sequence of each slot ends (len(pushes) = it goes on)
+        end_push = np.full(S, len(pushes), np.int64)
+        open_dev = np.zeros(S, bool)   # the device slot holds an open sequence from push 0 on
+        for s in range(S):
+            first = n[s] > 0 and not self.on_device[s]
+            if first:
+                assert rel[s][0][0] == 0, "a video's first released frame is its frame 0"
+                pushes[0]["start"][s] = True
+                self.on_device[s] = True
+            elif drop[s] and self.device.active[s]:
+                pushes[0]["start"][s] = True
+                pushes[0]["end"][s] = 0
+                end_push[s] = 0
+            open_dev[s] = self.on_device[s]
+            if ending[s] and self.on_device[s]:
+                i = int(np.searchsorted(offs, n[s] - 1, side="right")) - 1 if n[s] > 0 else 0
+                pushes[i]["end"][s] = pushes[i]["count"][s]
+                end_push[s] = i
+                self.on_device[s] = False
+        realigned = []
+        for i, p in enumerate(pushes):
+            # count is read for a slot whose open sequence does not end in this push
+            held = [s for s in range(S) if open_dev[s] and i < end_push[s]
+                    and p["count"][s] < p["k"]]
+            p["counted"] = bool(held)
+            realigned += [(s, i) for s in held]
+            self.device.push(p["k"], p["start"], p["end"], p["count"] if held else None)
+        records = np.zeros((int(offs[-1]) * S, 5), np.int32)
+        r = 0
+        for i, kk in enumerate(ks):
+            for s in range(S):
+                chunk = rel[s][offs[i]:offs[i] + kk]
+                for f in range(kk):
+                    if f < len(chunk):
+                        records[r] = (s,) + chunk[f][1:]
+                    else:
+                        records[r] = (s, -2, -1, 0, 0)
+                    r += 1
+        slots = np.zeros((S, 3), np.int32)
+        slots[:, :2] = self.resolution
+        slots[:, 2] = keep
+        frames = [[u[0] for u in r] for r in rel]
+        return DetectionCall(pushes, records, slots, frames, realigned)
+
+
 def predict_schedule(lengths, streams, max_frames, lookahead):
     """The pushes StreamingSession.predict makes for sequences of `lengths` frames: a list of dicts
     with k and the per-slot arrays start (bool), end (int32), x_rows and y_rows (int64), rows
@@ -302,8 +533,11 @@ class StreamingSession:
     with ``model.streaming(streams, max_frames)``; ``augment=True`` with the left / right lists of
     UnchunkedGenerator returns the test-time flip average instead."""
 
+    detections = False   # fed by push_detections (model.streaming(..., detections=True))
+
     def __init__(self, model, streams, max_frames, augment=False, kps_left=None, kps_right=None,
-                 joints_left=None, joints_right=None, provisional=False, int8=False):
+                 joints_left=None, joints_right=None, provisional=False, int8=False,
+                 detections=False, max_gap=None):
         from .temporal_model import TemporalModel
         if type(model)._variant != TemporalModel._variant:
             raise NotImplementedError(
@@ -327,6 +561,17 @@ class StreamingSession:
         streams, max_frames = int(streams), int(max_frames)
         if streams < 1 or max_frames < 1:
             raise ValueError("streams and max_frames must be >= 1")
+        self.detections = bool(detections)
+        if self.detections:
+            if model.in_features != 2:
+                raise ValueError(f"detections=True takes 2-D keypoints (in_features == 2); this "
+                                 f"model has in_features = {model.in_features}")
+            if provisional:
+                raise NotImplementedError("provisional=True with detections=True is not supported")
+            DetectionBook(streams, max_frames, max_gap)   # (checks max_gap)
+        elif max_gap is not None:
+            raise ValueError("max_gap is only used with detections=True")
+        self.max_gap = max_gap
         # host-side int32 maps; vp3d_stream_init_ex copies them into the session state
         self._kps_src, self._joints_src = augment_maps(model, augment, kps_left, kps_right,
                                                        joints_left, joints_right)
@@ -356,6 +601,10 @@ class StreamingSession:
             if nbytes == 0:
                 raise ValueError(f"{streams} streams x {max_frames} frames is too large a session")
             self._state = torch.empty(nbytes, dtype=torch.uint8, device=device)
+            if self.detections:
+                # the last detection of every slot, double-buffered (vp3d_stream_pack_detections)
+                self._last = torch.zeros((2, streams, model.num_joints_in, 2), dtype=torch.float32,
+                                         device=device)
         self._finalizer = weakref.finalize(self, _release, self._plan, self._state.data_ptr(),
                                            model._engine)
         self.reset()
@@ -370,6 +619,12 @@ class StreamingSession:
                 self.max_frames, self._flags, host_ptr(self._kps_src), host_ptr(self._joints_src),
                 stream), "vp3d_stream_init_ex")
         self._versions = self._quant = None
+        if self.detections:
+            self._book = DetectionBook(self.streams, self.max_frames, self.max_gap, self.lookahead)
+            self._parity = 0
+        self.last_call_pushes = 0        # internal pushes of the last push_detections / finish
+        self.last_call_launches = 0      # kernels it launched
+        self.last_call_realigned = 0     # (slot, push) pairs of it that took the realign path
         return self
 
     def _prepare(self):
@@ -476,6 +731,8 @@ class StreamingSession:
         provisional: also return y_prov (S, lookahead, J_out, 3) and frame_prov (S, lookahead)
         int64, what finish() would return right after this push (module docstring); needs a
         session made with provisional=True."""
+        if self.detections:
+            raise RuntimeError("a session made with detections=True is fed by push_detections")
         if provisional and not self.provisional:
             raise RuntimeError("push(provisional=True) needs a session made with "
                                "model.streaming(..., provisional=True)")
@@ -530,6 +787,8 @@ class StreamingSession:
         The schedule (predict_schedule) follows from the lengths alone, so nothing is read back from
         the device: one host-to-device copy of the whole schedule, then one push per step, each
         reading its frames from and writing its outputs to rows of the two flat buffers."""
+        if self.detections:
+            raise RuntimeError("a session made with detections=True is fed by push_detections")
         seqs = list(sequences)
         J, F = self.model.num_joints_in, self.model.in_features
         for x in seqs:
@@ -569,10 +828,101 @@ class StreamingSession:
         offset = np.concatenate([[0], np.cumsum(lengths)])
         return [y[int(offset[i]):int(offset[i + 1])] for i in range(len(seqs))]
 
+    def push_detections(self, kps_px, detected, start=None, end=None, resolution=None):
+        """Push k video frames per slot straight from a 2-D detector (a session made with
+        detections=True); returns (y (S, n, J_out, 3), frame (S, n) int64), n >= k.
+
+        kps_px: (S, k, J_in, 2) CUDA fp32 pixel keypoints, 1 <= k <= max_frames.
+        detected: HOST bool array (S, k), False = no person in that frame (its kps_px values are
+        never read and may be NaN).  It is a host array on purpose: how many frames a slot releases
+        depends on it, and the host sizes the pushes from it without reading anything back from
+        the device.
+        start / end: host lists as for push, counted in video frames (this call's k rows, detected
+        or not).  resolution: per slot None or the camera's (w, h) in pixels, read for the slots
+        that start in this call (required there, both > 0) and kept until the slot's next start.
+
+        Per slot the network receives the video's frames in order, each once, as the reference's
+        in-the-wild pipeline prepares them (decode's np.interp over the missed frames, then
+        run.py's normalize_screen_coordinates): a detection releases itself and the missed frames
+        before it; missed frames after the last detection are released held by `end` or finish();
+        with max_gap = G at most G missed frames wait for the next detection (DetectionBook).
+        A video without any detection releases nothing.  `frame` numbers the video's frames from
+        its start, -1 for rows that are no frame.  A call that releases more than max_frames
+        frames for a slot runs several pushes and returns their rows concatenated."""
+        if not self.detections:
+            raise RuntimeError("push_detections needs a session made with "
+                               "model.streaming(..., detections=True)")
+        J = self.model.num_joints_in
+        k = check_push_input(kps_px, self.streams, self.max_frames, J, 2)
+        if kps_px.device != self.device:
+            raise RuntimeError("input and parameters are on different devices")
+        det = self._book.check(detected, start, end, resolution)[0]   # before anything changes
+        if det.shape != (self.streams, k):
+            raise ValueError(f"detected must have shape ({self.streams}, {k}) like kps_px's first "
+                             f"two dimensions, got {det.shape}")
+        call = self._book.push(det, start, end, resolution)
+        return self._run_detections(call, kps_px.contiguous(), k)
+
+    def _run_detections(self, call, kps, k):
+        """One table copy, one pack launch and the pushes of a DetectionCall."""
+        S, J = self.streams, self.model.num_joints_in
+        pushes = call.pushes
+        self.last_call_pushes = len(pushes)
+        self.last_call_realigned = len(call.realigned)
+        self.last_call_launches = 0
+        outs = []
+        if not pushes:
+            return None
+        host, offsets = call.table()
+        lib = _capi.load()
+        with torch.cuda.device(self.device):
+            stream = self._prepare()
+            buf = torch.from_numpy(host).pin_memory().to(self.device, non_blocking=True)
+            base = buf.data_ptr()
+            xs = torch.empty((call.rows, J, 2), dtype=torch.float32, device=self.device)
+            if kps is None:   # finish: every record reads the stored detection
+                kps, k = self._last, 1
+            _capi.check(lib.vp3d_stream_pack_detections(
+                kps.data_ptr(), S, k, J, base, call.rows, self._last.data_ptr(), self._parity,
+                xs.data_ptr(), stream), "vp3d_stream_pack_detections")
+            self._parity ^= 1
+            self.last_call_launches = 1
+            row = 0
+            for i, p in enumerate(pushes):
+                kk = p["k"]
+                y = torch.empty((S, kk, self.model.num_joints_out, 3), dtype=torch.float32,
+                                device=self.device)
+                frame = torch.empty((S, kk), dtype=torch.int64, device=self.device)
+                e, c, st = (base + o for o in offsets[i])
+                _capi.check(lib.vp3d_stream_push_counts(
+                    self._plan, self._state.data_ptr(), xs[row:row + S * kk].data_ptr(), kk,
+                    st if p["start"].any() else None, e if (p["end"] >= 0).any() else None, None,
+                    None, y.data_ptr(), frame.data_ptr(), c if p["counted"] else None, stream),
+                    "vp3d_stream_push_counts")
+                self.last_call_launches += lib.vp3d_last_launch_count(self._plan)
+                outs.append((y, frame))
+                row += S * kk
+        if len(outs) == 1:
+            return outs[0]
+        return torch.cat([o[0] for o in outs], 1), torch.cat([o[1] for o in outs], 1)
+
     def finish(self):
         """Emit the last `lookahead` frames of every slot (its last frame repeated, as the
         generator's end padding does), then mark every slot idle.  A slot whose sequence ended
-        earlier returns what is left of its tail, -1 after that."""
+        earlier returns what is left of its tail, -1 after that.  A detections session first
+        releases every open video's missed frames after its last detection (held, np.interp's
+        right value) in pushes of its own; their rows come first."""
+        if self.detections:
+            outs = self._run_detections(self._book.finish(), None, 0)
+            launches = self.last_call_launches
+            y, frame = self._finish()
+            self.last_call_launches = launches + self.last_launch_count()
+            if outs is None:
+                return y, frame
+            return torch.cat([outs[0], y], 1), torch.cat([outs[1], frame], 1)
+        return self._finish()
+
+    def _finish(self):
         la = self.lookahead
         y = torch.empty((self.streams, la, self.model.num_joints_out, 3), dtype=torch.float32,
                         device=self.device)

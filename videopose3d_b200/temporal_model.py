@@ -756,7 +756,8 @@ class TemporalModelBase(nn.Module):
         return 0 if self._plan is None else _capi.load().vp3d_last_launch_count(self._plan)
 
     def streaming(self, streams, max_frames=1, augment=False, kps_left=None, kps_right=None,
-                  joints_left=None, joints_right=None, provisional=False, int8=False):
+                  joints_left=None, joints_right=None, provisional=False, int8=False,
+                  detections=False, max_gap=None):
         """A StreamingSession (videopose3d_b200.streaming) of `streams` slots that takes up to
         `max_frames` new frames per slot and push, and returns each output frame as soon as its
         input has arrived.  `augment=True` with UnchunkedGenerator's left / right lists returns
@@ -764,11 +765,16 @@ class TemporalModelBase(nn.Module):
         only, ValueError otherwise) lets push(..., provisional=True) also return provisional
         poses for the frames still inside the look-ahead.  `int8=True` streams a model in
         precision 'int8' (ValueError in any other precision; an int8 model needs it), bit for bit
-        its offline int8 forward.  Not in the reference."""
+        its offline int8 forward.  `detections=True` (in_features == 2) makes a session fed by
+        push_detections: a 2-D detector's pixel keypoints, a host per-frame detection flag and
+        the camera resolution, with missed frames interpolated and screen-normalised on the device
+        as the reference's in-the-wild pipeline does; `max_gap` bounds how many missed frames wait
+        for the next detection.  Not in the reference."""
         from .streaming import StreamingSession
         return StreamingSession(self, streams, max_frames, augment=augment, kps_left=kps_left,
                                 kps_right=kps_right, joints_left=joints_left,
-                                joints_right=joints_right, provisional=provisional, int8=int8)
+                                joints_right=joints_right, provisional=provisional, int8=int8,
+                                detections=detections, max_gap=max_gap)
 
     def predict(self, sequences, augment=False, kps_left=None, kps_right=None, joints_left=None,
                 joints_right=None, max_rows=None):
