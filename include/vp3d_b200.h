@@ -783,10 +783,32 @@ int vp3d_pose_loss_fwd_bwd(const float* pred, const float* target, int32_t frame
  * history depends on the block mask and the activation scales: the session records both at its
  * first push (or finish) after init, and a later push or finish that finds either changed
  * (vp3d_set_int8_blocks, vp3d_set_int8_scales) is VP3D_ERR_STATE until the session is initialised
- * again, so old and new quantisations never mix.  Flag bits 2 and 8 stay unknown. */
+ * again, so old and new quantisations never mix.
+ *
+ * Held provisional outputs (VP3D_STREAM_HELD, flags of the _ex calls, combinable with AUGMENT and
+ * INT8, valid on causal plans; together with PROVISIONAL it is VP3D_ERR_INVALID and state_bytes_ex
+ * returns 0, because push_held with max_held = 0 already is the provisional push): the provisional
+ * outputs of a detector-fed session (streaming.StreamingSession.push_detections), whose slots may
+ * hold pending frames after their last detection that vp3d_stream_finish would first receive as
+ * that detection repeated.  The flag sizes every ring for K + RF - 1 new rows (RF =
+ * vp3d_receptive_field): past RF - 1 end-padding rows every tail row is a bit copy of the last one
+ * computed, so no push computes more.  Flag bits 2, 8 and 32 stay unknown.
+ * vp3d_stream_push_held is vp3d_stream_push_provisional with, per slot, the pending frames of its
+ * open sequence:
+ *   held: DEVICE (S,) int32, read for open sequences only; values outside [0, max_held] read as 0.
+ *   max_held >= 0 and rows >= lookahead + max_held: y_prov (S, rows, J_out, 3) fp32 and frame_prov
+ *     (S, rows) int64 (DEVICE, required).  frame_prov[s, j] = c - lookahead + j for j < lookahead +
+ *     held[s] under the rules of `frame` (c = frames pushed so far), -1 otherwise; y_prov row j with
+ *     a frame >= 0 is, bit for bit, the row vp3d_stream_finish would return for that frame right
+ *     after pushing the held frames as the slot's last frame repeated.  Other rows are unspecified.
+ *   The chain runs over k + T frame rows, T = min(lookahead + max_held, RF - 1); T = 0 (a causal
+ *     plan, max_held = 0) computes no tail and leaves y_prov unwritten.  Launches: those of
+ *     vp3d_stream_push_counts, plus the output kernel where that shrinks straight into y.  Nothing
+ *     of the request persists.  VP3D_ERR_STATE on a session initialised without the flag. */
 #define VP3D_STREAM_AUGMENT 1
 #define VP3D_STREAM_PROVISIONAL 4
 #define VP3D_STREAM_INT8 16
+#define VP3D_STREAM_HELD 64
 int vp3d_stream_lookahead(const vp3d_plan* plan);
 size_t vp3d_stream_state_bytes(const vp3d_plan* plan, int S, int K);
 int vp3d_stream_init(vp3d_plan* plan, void* state, size_t state_bytes, int S, int K, void* stream);
@@ -806,6 +828,10 @@ int vp3d_stream_push_provisional(vp3d_plan* plan, void* state, const float* x, i
                                  const uint8_t* start_mask, const int32_t* end,
                                  const int32_t* count, float* y, int64_t* frame, float* y_prov,
                                  int64_t* frame_prov, void* stream);
+int vp3d_stream_push_held(vp3d_plan* plan, void* state, const float* x, int k,
+                          const uint8_t* start_mask, const int32_t* end, const int32_t* count,
+                          const int32_t* held, int max_held, int rows, float* y, int64_t* frame,
+                          float* y_prov, int64_t* frame_prov, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 
 /* Detector input (streaming.StreamingSession.push_detections): the input rows of the pushes one

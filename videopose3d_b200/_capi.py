@@ -30,6 +30,7 @@ VP3D_POSE_LOSS_MPJPE, VP3D_POSE_LOSS_N_MPJPE, VP3D_POSE_LOSS_P_MPJPE, VP3D_POSE_
 VP3D_STREAM_AUGMENT = 1
 VP3D_STREAM_PROVISIONAL = 4
 VP3D_STREAM_INT8 = 16
+VP3D_STREAM_HELD = 64
 VP3D_CLIPS_AUGMENT = 1
 VP3D_INT8_CALIB_AMAX, VP3D_INT8_CALIB_PERCENTILE, VP3D_INT8_CALIB_MSE = 0, 1, 2
 
@@ -337,6 +338,9 @@ SIGNATURES = {
     "vp3d_stream_push_provisional": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p,
                                                     ctypes.c_void_p, ctypes.c_int]
                                      + [ctypes.c_void_p] * 8),
+    "vp3d_stream_push_held": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_int] + [ctypes.c_void_p] * 4
+                              + [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 5),
     "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),

@@ -59,23 +59,35 @@
 //
 // Provisional outputs (VP3D_STREAM_PROVISIONAL, vp3d_stream_push_provisional).  A push of k frames
 // also returns what vp3d_stream_finish would return right after it, for the la = lookahead frames
-// that are not final yet, without changing the session.  The chain of the push runs over k + la
-// frame rows instead of k: rows [k, k + la) (the tail) are fed the end padding, the slot's last real
-// frame repeated, exactly as the rows f >= n of a counted or ending slot already are, so row n + j
-// (n = slot_count) is the j-th row finish would compute, with the same operands in the same k-order.
-// The flag sizes every ring with R_l = H_l + K + la + 1 positions, so the window of such a push,
-// [w0, w0 + H + k + la), still never holds a position together with its mirror.  The tail lands in
-// positions [w0 + H + k, w0 + H + k + la) (ring 0: both copies); modulo R these are residues
-// w0 + H + k + j, which lie outside the residues [w0, w0 + H + k) of this push's history and new
-// rows because H + k + la < R.  So speculative writes never touch history, and never a row whose
-// mirror copy is pending: the next push copies only rows [w0 + H, w0 + H + k) (prev_k = k), and its
-// history [w0 + k, w0 + k + H) is H residues that again exclude the tail's (H + la < R).  A later
-// push reads a tail residue as history only after writing it as one of its new rows.  The
+// that are not final yet, without changing the session.  The chain of the push runs over k + T
+// frame rows instead of k (T = la here): rows [k, k + T) (the tail) are fed the end padding, the
+// slot's last real frame repeated, exactly as the rows f >= n of a counted or ending slot already
+// are, so row n + j (n = slot_count) is the j-th row finish would compute, with the same operands in
+// the same k-order.  The flag sizes every ring with R_l = H_l + K + tail + 1 positions (tail = la),
+// so the window of such a push, [w0, w0 + H + k + T), still never holds a position together with its
+// mirror.  The tail lands in positions [w0 + H + k, w0 + H + k + T) (ring 0: both copies); modulo R
+// these are residues w0 + H + k + j, which lie outside the residues [w0, w0 + H + k) of this push's
+// history and new rows because H + k + T < R.  So speculative writes never touch history, and never
+// a row whose mirror copy is pending: the next push copies only rows [w0 + H, w0 + H + k) (prev_k =
+// k), and its history [w0 + k, w0 + k + H) is H residues that again exclude the tail's (H + T < R).
+// A later push reads a tail residue as history only after writing it as one of its new rows.  The
 // realign of a counted push moves only window positions [w0, w0 + H + k) and writes their mirror
 // copies, none of which lies in the tail's window copies.  The bookkeeping is double-buffered by
 // parity as for every push, q / prev_q / prev_k / parity advance as for k frames, and the output
 // kernel reads n from the two bookkeeping buffers (count after - count before), so nothing of the
 // tail persists.
+//
+// Held frames (VP3D_STREAM_HELD, vp3d_stream_push_held).  A detector-fed slot may hold P pending
+// frames after its last detection, which finish would first push as that detection repeated, then
+// end-pad: to the network, la + P more copies of the slot's last real frame, the same end padding
+// the tail packs.  So the provisional rows of such a slot are tail rows j < la + P.  Tail row j is
+// frame c - la + j, whose input cone [c - la + j - pad - shift, c - la + j + pad - shift] lies in
+// the constant end padding once j >= RF - 2 (= 2 pad - 1, causal or not); inside a constant cone
+// every layer's rows have the same operands, hence the same bits (the v-pass argument above), so
+// rows j >= RF - 2 are copies of row RF - 2 and a push computes T = min(la + max P, RF - 1) tail
+// rows, whatever the gap.  The flag sizes the rings for tail = RF - 1 >= T: every argument of the
+// previous paragraph holds with H + k + T <= H + K + tail < R.  T = 0 (a causal plan, nothing
+// pending) computes no tail.
 //
 // int8 sessions (VP3D_STREAM_INT8).  Ring i >= 1 of a block in the plan's int8 mask also holds a u8
 // plane Q_{i-1} with the positions of its 16-bit planes (frame t at t mod R and t mod R + R): block
@@ -97,7 +109,8 @@ int stream_lookahead(const vp3d_plan* p);
 namespace {
 
 constexpr int kMaxRings = VP3D_MAX_WIDTHS;   // ring 0 = network input, ring i = block i input
-constexpr int kStreamFlags = VP3D_STREAM_AUGMENT | VP3D_STREAM_PROVISIONAL | VP3D_STREAM_INT8;
+constexpr int kStreamFlags =
+    VP3D_STREAM_AUGMENT | VP3D_STREAM_PROVISIONAL | VP3D_STREAM_INT8 | VP3D_STREAM_HELD;
 
 struct StreamRing {
   __nv_bfloat16* base;   // plane 0, position 0
@@ -112,7 +125,7 @@ struct StreamRing {
 
 struct StreamLayout {
   int rings = 0;
-  int tail = 0;                 // PROVISIONAL: the look-ahead rows a push may append (else 0)
+  int tail = 0;                 // the end-padding rows a push may append (stream_tail)
   int H[kMaxRings], R[kMaxRings], ld[kMaxRings];
   long long plane[kMaxRings];   // elements per ring plane
   size_t ring[kMaxRings];       // byte offsets
@@ -129,10 +142,17 @@ struct StreamLayout {
 // rows every ring, activation and output buffer holds per frame position
 inline int physical_rows(int S, int flags) { return flags & VP3D_STREAM_AUGMENT ? 2 * S : S; }
 
+// end-padding rows a push may append to its k: PROVISIONAL the look-ahead, HELD the RF - 1 rows past
+// which every tail row is a copy (header comment), else 0
+inline int stream_tail(const vp3d_plan* p, int flags) {
+  if (flags & VP3D_STREAM_HELD) return vp3d_receptive_field(p) - 1;
+  return flags & VP3D_STREAM_PROVISIONAL ? stream_lookahead(p) : 0;
+}
+
 StreamLayout stream_layout(const vp3d_plan* p, int S, int K, int flags) {
   StreamLayout L;
   L.rings = p->nb + 1;
-  L.tail = flags & VP3D_STREAM_PROVISIONAL ? stream_lookahead(p) : 0;
+  L.tail = stream_tail(p, flags);
   const int planes = p->planes;
   const int P = physical_rows(S, flags);
   const int rows = K + L.tail;   // frame rows a push computes at most
@@ -192,8 +212,11 @@ struct StepArgs {
   long long* length_out;
   long long* frame;        // (S, frame_ld) int64
   int frame_ld, frame_off, lookahead;
-  int tail;                // provisional push: lookahead end-padding rows after the k (else 0)
-  long long* frame_prov;   // (S, tail) int64, the frames of those rows (tail > 0)
+  int tail;                // provisional push: the T end-padding rows after the k (else 0)
+  int prov_rows;           // rows of frame_prov per slot (0: no provisional request)
+  long long* frame_prov;   // (S, prov_rows) int64, the frames of the provisional rows
+  const int* held;         // (S,) or null: pending held frames of an open sequence (HELD push)
+  int max_held;            // held values outside [0, max_held] read as 0
 };
 
 // Channel c of the mirrored input frame (generators.py:235-237) is source channel *src, negated when
@@ -252,9 +275,11 @@ __device__ __forceinline__ int packed_frames(const StepArgs& a, int s) {
 //     real frame is repeated instead (the generator's end padding, generators.py:216-238): packed
 //     from x[s, end - 1] in the push that ends it, the newest ring-0 position after that;
 //   * the mirror copy of the rows the previous push's GEMMs wrote into rings 1..nb;
-//   * a provisional push (tail > 0): rows [k, k + tail) packed as the end padding of rows f >= n,
-//     and frame_prov[s, j] = count after the push - lookahead + j under the rules of `frame`, with
-//     the bookkeeping after the push: the frames vp3d_stream_finish would number right after it.
+//   * a provisional push: rows [k, k + tail) packed as the end padding of rows f >= n, and
+//     frame_prov[s, j] = count after the push - lookahead + j for j < lookahead + held[s] (held
+//     read for an open sequence only) under the rules of `frame`, with the bookkeeping after the
+//     push: the frames vp3d_stream_finish would number right after it (after a detector-fed slot's
+//     held frames).
 __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) {
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nthr = (long long)gridDim.x * blockDim.x;
@@ -276,9 +301,12 @@ __global__ void __launch_bounds__(256, 1) stream_input_kernel(const StepArgs a) 
     a.count_out[s] = c;
     a.active_out[s] = act;
     a.length_out[s] = len;
-    for (int j = 0; j < a.tail; ++j) {
+    int held = act && len < 0 && a.held ? a.held[s] : 0;
+    if (held < 0 || held > a.max_held) held = 0;
+    for (int j = 0; j < a.prov_rows; ++j) {
       const long long idx = c - a.lookahead + j;
-      a.frame_prov[s * a.tail + j] = (act && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
+      a.frame_prov[s * a.prov_rows + j] =
+          (act && j < a.lookahead + held && idx >= 0 && (len < 0 || idx < len)) ? idx : -1;
     }
   }
 
@@ -505,15 +533,16 @@ __global__ void __launch_bounds__(256) stream_broadcast_kernel(const BcastArgs a
 // augment: rows f * 2S + s (plain) and f * 2S + S + s (mirrored) are flip-averaged (run.py:674-680),
 // output joint j of the mirrored row read from joint_src[j] (null: no joint swap, the trajectory
 // model).
-// Provisional push (prov.tail > 0): prov.y (S, tail, c_out) receives row j of slot s from frame row
-// n + j, n = the frames the slot advanced by (prov.count_out[s] minus prov.count_in[s], or minus 0
-// for a starting slot: the input kernel's bookkeeping of this push).
+// Provisional push (prov.tail > 0): prov.y (S, rows, c_out) receives row j of slot s from frame row
+// n + min(j, tail - 1), n = the frames the slot advanced by (prov.count_out[s] minus
+// prov.count_in[s], or minus 0 for a starting slot: the input kernel's bookkeeping of this push);
+// tail rows past the last computed one are its copies (header comment, held frames).
 struct ProvOut {
   float* y;
   const long long* count_in;
   const long long* count_out;
   const uint8_t* start;
-  int tail;
+  int tail, rows;
 };
 
 __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, float* y, int S, int k,
@@ -523,7 +552,7 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
                                                             const long long* y_rows,
                                                             const ProvOut prov) {
   pdl_entry();
-  const long long n = (long long)(k + prov.tail) * S * c_out;
+  const long long n = (long long)(k + (prov.tail ? prov.rows : 0)) * S * c_out;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % c_out);
@@ -540,8 +569,9 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
       }
     } else {
       const int j = f - k;
-      out = prov.y + ((long long)s * prov.tail + j) * c_out + c;
-      f = (int)(prov.count_out[s] - (prov.start && prov.start[s] ? 0 : prov.count_in[s])) + j;
+      out = prov.y + ((long long)s * prov.rows + j) * c_out + c;
+      f = (int)(prov.count_out[s] - (prov.start && prov.start[s] ? 0 : prov.count_in[s])) +
+          min(j, prov.tail - 1);
     }
     float v;
     if (augment) {
@@ -632,6 +662,16 @@ void vpass_chain(const vp3d_plan* p, const StreamLayout& L, uint8_t* base, const
   }
 }
 
+// A push's provisional request (y null: none): y_prov (S, rows, c_out) / frame_prov (S, rows), the
+// chain's tail rows (y_prov row j is tail row min(j, tail - 1)), and the pending held frames of
+// every slot (null: none; values outside [0, max_held] read as 0).
+struct ProvRequest {
+  float* y = nullptr;
+  long long* frame = nullptr;
+  const int* held = nullptr;
+  int max_held = 0, rows = 0, tail = 0;
+};
+
 }  // namespace
 
 // run.py:186-193 pads pad + causal_shift frames in front and pad - causal_shift behind, with
@@ -643,18 +683,18 @@ int stream_lookahead(const vp3d_plan* p) {
 // One push of k frames (x null: k copies of every slot's newest frame).  y receives rows
 // [f_off, f_off + k) of a (S, y_frames, J_out, 3) tensor, or with y_rows the rows y_rows[s] + frame
 // of a flat one; frame the matching (S, y_frames) entries.  The GEMMs run over P physical rows per
-// frame (S, or 2S with AUGMENT).  y_prov non-null (a PROVISIONAL session): the push also computes the
-// lookahead end-padding rows and writes y_prov (S, lookahead, c_out) / frame_prov (S, lookahead).
+// frame (S, or 2S with AUGMENT).  A provisional request (pr.y non-null) also computes pr.tail
+// end-padding rows and writes y_prov / frame_prov (ProvRequest).
 static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* x, int k,
                        const uint8_t* start, const int* end, const int* count,
                        const long long* x_rows,
                        const long long* y_rows, float* y, int y_frames, int f_off, long long* frame,
-                       float* y_prov, long long* frame_prov, cudaStream_t stream) {
+                       const ProvRequest& pr, cudaStream_t stream) {
   const int S = h.S, K = h.K, C = p->C, planes = p->planes;
   const bool aug = h.flags & VP3D_STREAM_AUGMENT;
   const int P = physical_rows(S, h.flags);
   const StreamLayout L = stream_layout(p, S, K, h.flags);
-  const int tail = y_prov ? L.tail : 0;
+  const int tail = pr.y ? pr.tail : 0;
   int launches = 0;
 
   StepArgs a;
@@ -703,7 +743,10 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   a.frame_off = f_off;
   a.lookahead = stream_lookahead(p);
   a.tail = tail;
-  a.frame_prov = frame_prov;
+  a.prov_rows = pr.y ? pr.rows : 0;
+  a.frame_prov = pr.frame;
+  a.held = pr.held;
+  a.max_held = pr.max_held;
   {
     long long work = (long long)(k + tail) * P * (p->c_in_pad / 2);
     for (int l = 1; l < L.rings; ++l)
@@ -721,7 +764,7 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
   // shrink straight into y when the time-major rows already are y's rows (k == 1 or S == 1, no
   // AUGMENT: the flip average always takes the output kernel, and so do row-addressed outputs and
   // provisional pushes)
-  const bool direct = !aug && !y_rows && !tail && (y_frames == 1 || S == 1);
+  const bool direct = !aug && !y_rows && !pr.y && (y_frames == 1 || S == 1);
   float* ybuf = reinterpret_cast<float*>(base + L.ybuf);
   InferChain push;
   push_chain(p, L, base, ring, P, K, k, tail,
@@ -782,14 +825,16 @@ static int stream_step(vp3d_plan* p, uint8_t* base, StreamHost& h, const float* 
     ProvOut prov;
     memset(&prov, 0, sizeof(prov));
     if (tail) {
-      prov.y = y_prov;
+      prov.y = pr.y;
       prov.count_in = a.count_in;
       prov.count_out = a.count_out;
       prov.start = start;
       prov.tail = tail;
+      prov.rows = pr.rows;
     }
     CUDA_TRY(launch_pdl(stream_output_kernel,
-                        dim3(grid_for((long long)(k + tail) * S * p->c_out_raw)), dim3(256), 0,
+                        dim3(grid_for((long long)(k + (tail ? pr.rows : 0)) * S * p->c_out_raw)),
+                        dim3(256), 0,
                         stream, (const float*)ybuf, y, S, k, p->c_out_raw, y_frames, f_off, (int)aug,
                         h.joint_src ? (const int*)(base + L.jsrc) : (const int*)nullptr,
                         (const long long*)frame, y_rows, prov));
@@ -840,7 +885,7 @@ static int stream_int8_ready(const vp3d_plan* p, StreamHost& h, const char* what
 
 // every row index of a session's rings and buffers fits an int
 static bool stream_fits(const vp3d_plan* p, int S, int K, int flags) {
-  const int tail = flags & VP3D_STREAM_PROVISIONAL ? stream_lookahead(p) : 0;
+  const int tail = stream_tail(p, flags);
   return (long long)physical_rows(S, flags) * (K + tail + 2LL * vp3d_receptive_field(p)) <=
          0x7fffffffLL;
 }
@@ -860,6 +905,7 @@ VP3D_EXPORT size_t vp3d_stream_state_bytes_ex(const vp3d_plan* p, int S, int K, 
   if (!p || S < 1 || K < 1 || (flags & ~kStreamFlags) || !stream_fits(p, S, K, flags))
     return 0;
   if ((flags & VP3D_STREAM_PROVISIONAL) && stream_lookahead(p) == 0) return 0;
+  if ((flags & VP3D_STREAM_PROVISIONAL) && (flags & VP3D_STREAM_HELD)) return 0;
   if ((flags & VP3D_STREAM_INT8) && !p->int8) return 0;
   return stream_layout(p, S, K, flags).total;
 }
@@ -883,6 +929,9 @@ static int stream_init(const char* what, vp3d_plan* p, void* state, size_t state
     return fail(VP3D_ERR_INVALID, "%s: streams (%d) and max_frames (%d) must be >= 1", what, S, K);
   if (flags & ~kStreamFlags)
     return fail(VP3D_ERR_INVALID, "%s: unknown flags 0x%x", what, (unsigned)flags);
+  if ((flags & VP3D_STREAM_PROVISIONAL) && (flags & VP3D_STREAM_HELD))
+    return fail(VP3D_ERR_INVALID, "%s: VP3D_STREAM_HELD and VP3D_STREAM_PROVISIONAL exclude each "
+                "other (a HELD session's push_held with max_held = 0 is the provisional push)", what);
   const bool aug = flags & VP3D_STREAM_AUGMENT;
   if (!aug && (kps_src || joints_src))
     return fail(VP3D_ERR_INVALID, "%s: mirror maps given without VP3D_STREAM_AUGMENT", what);
@@ -954,7 +1003,7 @@ static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost
 static int stream_push(const char* what, vp3d_plan* p, void* state, const float* x, int k,
                        const uint8_t* start_mask, const int32_t* end, const int32_t* count,
                        const int64_t* x_rows, const int64_t* y_rows, float* y, int64_t* frame,
-                       float* y_prov, int64_t* frame_prov, void* stream) {
+                       int prov_flag, ProvRequest pr, void* stream) {
   if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
   if (k < 1) return fail(VP3D_ERR_INVALID, "%s: k must be >= 1 (got %d)", what, k);
   if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
@@ -964,19 +1013,27 @@ static int stream_push(const char* what, vp3d_plan* p, void* state, const float*
   if (!x || !y || !frame) return fail(VP3D_ERR_INVALID, "%s: null x, y or frame", what);
   StreamHost* h = nullptr;
   VP3D_TRY(stream_lookup(p, state, what, &h));
-  if (y_prov && !(h->flags & VP3D_STREAM_PROVISIONAL))
-    return fail(VP3D_ERR_STATE, "%s: the session was not initialised with VP3D_STREAM_PROVISIONAL",
-                what);
+  if (prov_flag && !(h->flags & prov_flag))
+    return fail(VP3D_ERR_STATE, "%s: the session was not initialised with %s", what,
+                prov_flag == VP3D_STREAM_HELD ? "VP3D_STREAM_HELD" : "VP3D_STREAM_PROVISIONAL");
   if (k > h->K)
     return fail(VP3D_ERR_INVALID, "%s: k = %d frames exceeds max_frames = %d", what, k, h->K);
+  const int la = stream_lookahead(p);
+  if (prov_flag == VP3D_STREAM_PROVISIONAL) pr.rows = pr.tail = la;
+  if (prov_flag == VP3D_STREAM_HELD) {
+    if ((long long)pr.rows < (long long)la + pr.max_held)
+      return fail(VP3D_ERR_INVALID, "%s: rows = %d < lookahead %d + max_held %d", what, pr.rows, la,
+                  pr.max_held);
+    const long long t = (long long)la + pr.max_held;
+    pr.tail = (int)(t < vp3d_receptive_field(p) - 1 ? t : vp3d_receptive_field(p) - 1);
+  }
   if (!p->conv_packed || !p->bn_packed)
     return fail(VP3D_ERR_STATE, "%s: vp3d_set_weights has not been called", what);
   VP3D_TRY(stream_int8_ready(p, *h, what));
   return stream_step(p, ws_base(state), *h, x, k, start_mask, end, count,
                      reinterpret_cast<const long long*>(x_rows),
                      reinterpret_cast<const long long*>(y_rows), y, k, 0,
-                     reinterpret_cast<long long*>(frame), y_prov,
-                     reinterpret_cast<long long*>(frame_prov), static_cast<cudaStream_t>(stream));
+                     reinterpret_cast<long long*>(frame), pr, static_cast<cudaStream_t>(stream));
 }
 
 VP3D_EXPORT int vp3d_stream_push_counts(vp3d_plan* p, void* state, const float* x, int k,
@@ -984,7 +1041,7 @@ VP3D_EXPORT int vp3d_stream_push_counts(vp3d_plan* p, void* state, const float* 
                                         const int64_t* x_rows, const int64_t* y_rows, float* y,
                                         int64_t* frame, const int32_t* count, void* stream) {
   return stream_push("stream_push_counts", p, state, x, k, start_mask, end, count, x_rows, y_rows,
-                     y, frame, nullptr, nullptr, stream);
+                     y, frame, 0, ProvRequest(), stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push_provisional(vp3d_plan* p, void* state, const float* x, int k,
@@ -993,8 +1050,30 @@ VP3D_EXPORT int vp3d_stream_push_provisional(vp3d_plan* p, void* state, const fl
                                              float* y_prov, int64_t* frame_prov, void* stream) {
   if (!y_prov || !frame_prov)
     return fail(VP3D_ERR_INVALID, "stream_push_provisional: null y_prov or frame_prov");
+  ProvRequest pr;
+  pr.y = y_prov;
+  pr.frame = reinterpret_cast<long long*>(frame_prov);
   return stream_push("stream_push_provisional", p, state, x, k, start_mask, end, count, nullptr,
-                     nullptr, y, frame, y_prov, frame_prov, stream);
+                     nullptr, y, frame, VP3D_STREAM_PROVISIONAL, pr, stream);
+}
+
+VP3D_EXPORT int vp3d_stream_push_held(vp3d_plan* p, void* state, const float* x, int k,
+                                      const uint8_t* start_mask, const int32_t* end,
+                                      const int32_t* count, const int32_t* held, int max_held,
+                                      int rows, float* y, int64_t* frame, float* y_prov,
+                                      int64_t* frame_prov, void* stream) {
+  if (!y_prov || !frame_prov || !held)
+    return fail(VP3D_ERR_INVALID, "stream_push_held: null y_prov, frame_prov or held");
+  if (max_held < 0)
+    return fail(VP3D_ERR_INVALID, "stream_push_held: max_held must be >= 0 (got %d)", max_held);
+  ProvRequest pr;
+  pr.y = y_prov;
+  pr.frame = reinterpret_cast<long long*>(frame_prov);
+  pr.held = held;
+  pr.max_held = max_held;
+  pr.rows = rows;
+  return stream_push("stream_push_held", p, state, x, k, start_mask, end, count, nullptr, nullptr,
+                     y, frame, VP3D_STREAM_HELD, pr, stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, int k,
@@ -1002,14 +1081,14 @@ VP3D_EXPORT int vp3d_stream_push_ex(vp3d_plan* p, void* state, const float* x, i
                                     const int64_t* x_rows, const int64_t* y_rows, float* y,
                                     int64_t* frame, void* stream) {
   return stream_push("stream_push_ex", p, state, x, k, start_mask, end, nullptr, x_rows, y_rows, y,
-                     frame, nullptr, nullptr, stream);
+                     frame, 0, ProvRequest(), stream);
 }
 
 VP3D_EXPORT int vp3d_stream_push(vp3d_plan* p, void* state, const float* x, int k,
                                  const uint8_t* start_mask, float* y, int64_t* frame,
                                  void* stream) {
   return stream_push("stream_push", p, state, x, k, start_mask, nullptr, nullptr, nullptr, nullptr,
-                     y, frame, nullptr, nullptr, stream);
+                     y, frame, 0, ProvRequest(), stream);
 }
 
 VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t* frame,
@@ -1029,7 +1108,7 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
   for (int off = 0; off < la; off += h->K) {
     const int k = la - off < h->K ? la - off : h->K;
     VP3D_TRY(stream_step(p, base, *h, nullptr, k, nullptr, nullptr, nullptr, nullptr, nullptr, y,
-                         la, off, reinterpret_cast<long long*>(frame), nullptr, nullptr, s));
+                         la, off, reinterpret_cast<long long*>(frame), ProvRequest(), s));
     launches += p->last_launches;
   }
   // every slot idle in the buffer the next push reads

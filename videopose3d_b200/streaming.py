@@ -68,6 +68,22 @@ their history (``ring_bytes_per_stream(..., int8=True)``, about 1.5x the 16-bit 
 holds one calibration's quantisation: ``calibrate_int8``, ``load_int8_calibration`` or
 ``set_int8_blocks`` under a session with history make its next push raise until ``reset()``, as a
 parameter change does.  An int8 model without ``int8=True`` cannot stream.
+
+Sessions fed by a 2-D detector (``detections=True``, ``push_detections``) take pixel keypoints and a
+host "person detected" flag per frame; frames after a slot's last detection are pending until the
+next detection, the video's end, finish() or max_gap.  With ``max_gap=G`` they can also return
+provisional poses, for the look-ahead and for the pending frames:
+
+    sess = model.streaming(streams=S, max_frames=K, detections=True, provisional=True, max_gap=G)
+    y, frame, y_prov, frame_prov = sess.push_detections(kps_px, detected, start, end, resolution,
+                                                        provisional=True)
+
+``y_prov`` (S, lookahead + G, J_out, 3) / ``frame_prov`` (S, lookahead + G) are what finish() would
+return right after the call, bit for bit: the pending frames held (the last detection repeated),
+then the look-ahead tail.  Causal models are accepted with G >= 1 (their provisional rows are the
+pending frames alone).  A push computes at most receptive_field - 1 tail rows however long the gap
+(past that every row is a copy), and the rings hold that many positions more
+(``ring_bytes_per_stream(..., held=True)``).
 """
 import weakref
 
@@ -98,11 +114,13 @@ def ring_history(filter_widths, dense=False):
 
 
 def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisional=False,
-                          int8=False):
+                          int8=False, held=False):
     """Device bytes of history one stream slot occupies (both mirror halves, every plane; twice that
     with augment: the slot's mirrored copy has rings of its own).  provisional: every ring also
     holds the `lookahead` positions of the tail a provisional push appends (not for causal
-    models, whose look-ahead is 0).  int8: the rings of the residual blocks also hold a u8 plane
+    models, whose look-ahead is 0).  held: every ring holds receptive_field - 1 tail positions
+    instead, the most a provisional push of a detector-fed session computes (causal models too;
+    not together with provisional).  int8: the rings of the residual blocks also hold a u8 plane
     with the same positions (one byte per channel, every block whatever the int8 block set)."""
     fw = model.filter_widths
     c_in = -(-model.num_joints_in * model.in_features // 64) * 64
@@ -113,6 +131,11 @@ def ring_bytes_per_stream(model, max_frames, planes=1, augment=False, provisiona
         if tail == 0:
             raise ValueError("provisional outputs need a non-causal model (a causal one has no "
                              "look-ahead: every output is final)")
+    if held:
+        if provisional:
+            raise ValueError("held and provisional exclude each other: held rings already hold "
+                             "the provisional tail")
+        tail = model.receptive_field() - 1
     total = 0
     for i, h in enumerate(ring_history(fw)):
         positions = 2 * (h + max_frames + tail + 1)
@@ -169,9 +192,12 @@ class FrameBook:
         self.length = np.full(streams, -1, np.int64)
         self.lookahead = lookahead
 
-    def push(self, k, start=None, end=None, count=None, provisional=False):
-        """The (S, k) frame numbers of a push; provisional=True also returns the (S, lookahead)
-        numbers of its provisional rows, those finish() would give right after it."""
+    def push(self, k, start=None, end=None, count=None, provisional=False, held=None, rows=None):
+        """The (S, k) frame numbers of a push; provisional=True also returns the (S, rows) numbers
+        of its provisional rows (rows = lookahead by default), those finish() would give right after
+        it.  held: per slot the pending frames finish() would first push held (a detector-fed
+        slot's frames after its last detection, read for open sequences only): row j is a frame
+        for j < lookahead + held[s] (vp3d_stream_push_held)."""
         S = len(self.count)
         start = np.zeros(S, bool) if start is None else np.asarray(start, bool)
         self.count[start] = 0
@@ -202,9 +228,13 @@ class FrameBook:
         self.active[done] = False
         if not provisional:
             return frame
-        idx = self.count[:, None] + np.arange(self.lookahead)[None, :] - self.lookahead
+        j = np.arange(self.lookahead if rows is None else rows)[None, :]
+        h = np.zeros(S, np.int64) if held is None else np.maximum(np.asarray(held, np.int64), 0)
+        h = np.where(self.active & (self.length < 0), h, 0)
+        idx = self.count[:, None] + j - self.lookahead
         length = self.length[:, None]
-        prov = np.where(self.active[:, None] & (idx >= 0) & ((length < 0) | (idx < length)), idx, -1)
+        prov = np.where(self.active[:, None] & (j < self.lookahead + h[:, None]) & (idx >= 0)
+                        & ((length < 0) | (idx < length)), idx, -1)
         return frame, prov
 
     def finish(self):
@@ -224,11 +254,16 @@ class DetectionCall:
     left, right, num, den as vp3d_stream_pack_detections reads them.  slots: (S, 3) int32 --
     w, h and the row of this call's newest detection (-1 = keep the stored one).  frames: per slot
     the video frame indices released, in order.  realigned: (slot, push) pairs that take the
-    realign path (an open slot with fewer frames than the push)."""
+    realign path (an open slot with fewer frames than the push).  out: (S, n) int64, the frame
+    numbers of the rows the call returns (for finish() including the device finish's look-ahead
+    rows).  held: (S,) int32, per slot the pending frames after the call (DetectionBook.push).
+    prov_frames: for a provisional request, (S, lookahead + max_gap) int64, the frame numbers of
+    its rows, those finish() would return right after the call; else None."""
 
-    def __init__(self, pushes, records, slots, frames, realigned):
+    def __init__(self, pushes, records, slots, frames, realigned, out, held, prov_frames=None):
         self.pushes, self.records, self.slots = pushes, records, slots
         self.frames, self.realigned = frames, realigned
+        self.out, self.held, self.prov_frames = out, held, prov_frames
 
     @property
     def rows(self):
@@ -237,11 +272,15 @@ class DetectionCall:
     def table(self):
         """The bytes copied to the device once per call, and the offsets (from its start) of each
         push's end / count (int32, S each) and start (uint8, S) arrays: slots and records (int32,
-        vp3d_stream_pack_detections' table) | per push end, count | per push start."""
+        vp3d_stream_pack_detections' table) | per push end, count | per push start, and for a
+        provisional request the held counts (int32, S) in the last 4 S bytes."""
         S, n = len(self.slots), len(self.pushes)
         tab = np.concatenate([self.slots.reshape(-1), self.records.reshape(-1)]).astype(np.int32)
         head = -(-tab.nbytes // 8) * 8
-        host = np.zeros(head + 8 * S * n + -(-S * n // 8) * 8, np.uint8)
+        tail = 4 * S if self.prov_frames is not None else 0
+        host = np.zeros(head + 8 * S * n + -(-S * n // 8) * 8 + tail, np.uint8)
+        if tail:
+            host[-tail:] = self.held.view(np.uint8)
         host[:tab.nbytes] = tab.view(np.uint8)
         offsets = []
         for i, p in enumerate(self.pushes):
@@ -268,7 +307,12 @@ class DetectionBook:
     or finish(); with max_gap = G, a (G + 1)-th pending frame after a detection releases the oldest
     one held.  A video without detections releases nothing.  Pure host code: the CPU tests drive
     it, and the session turns each DetectionCall into one table copy, one pack launch and its
-    pushes."""
+    pushes.
+
+    Every call reports each slot's pending held count P = seen - released of an open video with a
+    detection (0 otherwise: finish() releases nothing before a first detection), at most G.  A
+    provisional call (max_gap given) also numbers the la + G rows finish() would return right
+    after it: the released frames' look-ahead, then the P pending ones."""
 
     def __init__(self, streams, max_frames, max_gap=None, lookahead=0):
         self.streams, self.max_frames = int(streams), int(max_frames)
@@ -331,8 +375,12 @@ class DetectionBook:
             res[s] = (w, h)
         return detected, start, end, res
 
-    def push(self, detected, start=None, end=None, resolution=None):
-        """Plan one push_detections call (k = detected.shape[1] video frames per slot)."""
+    def push(self, detected, start=None, end=None, resolution=None, provisional=False):
+        """Plan one push_detections call (k = detected.shape[1] video frames per slot);
+        provisional=True also plans the provisional rows of its last push (needs max_gap)."""
+        if provisional and self.max_gap is None:
+            raise ValueError("provisional rows need max_gap: with max_gap=None the frames after a "
+                             "slot's last detection may wait without bound")
         detected, start, end, res = self.check(detected, start, end, resolution)
         S, k = detected.shape
         rel = [[] for _ in range(S)]       # per slot: (t, left, right, num, den)
@@ -372,7 +420,8 @@ class DetectionBook:
                     self.released[s] = self.seen[s]
                 self.open[s] = False
                 ending[s] = True
-        return self._plan(k, rel, keep, drop, ending)
+        pending = np.where(self.open & (self.last >= 0), self.seen - self.released, 0)
+        return self._plan(k, rel, keep, drop, ending, pending.astype(np.int32), provisional)
 
     def finish(self):
         """Plan the pushes finish() makes before the device finish: every open video's pending
@@ -383,14 +432,15 @@ class DetectionBook:
             rel[s] = [(u, -1, -1, 0, 0) for u in range(int(self.released[s]), int(self.seen[s]))]
             self.released[s] = self.seen[s]
         none = np.zeros(S, bool)
-        call = self._plan(0, rel, np.full(S, -1, np.int64), none, none)
+        call = self._plan(0, rel, np.full(S, -1, np.int64), none, none, np.zeros(S, np.int32))
         self.open[:] = False
         self.on_device[:] = False
-        self.device.finish()
+        call.out = np.concatenate([call.out, self.device.finish()], 1)
         return call
 
-    def _plan(self, k, rel, keep, drop, ending):
-        """Split the released frames into pushes of at most max_frames, k rows in all at least."""
+    def _plan(self, k, rel, keep, drop, ending, pending, provisional=False):
+        """Split the released frames into pushes of at most max_frames, k rows in all at least;
+        with provisional, the last push also numbers the provisional rows (pending: P per slot)."""
         S, K = self.streams, self.max_frames
         n = np.array([len(r) for r in rel], np.int64)
         total = max(k, int(n.max()))
@@ -419,14 +469,19 @@ class DetectionBook:
                 pushes[i]["end"][s] = pushes[i]["count"][s]
                 end_push[s] = i
                 self.on_device[s] = False
-        realigned = []
+        realigned, out, prov = [], [np.zeros((S, 0), np.int64)], None
         for i, p in enumerate(pushes):
             # count is read for a slot whose open sequence does not end in this push
             held = [s for s in range(S) if open_dev[s] and i < end_push[s]
                     and p["count"][s] < p["k"]]
             p["counted"] = bool(held)
             realigned += [(s, i) for s in held]
-            self.device.push(p["k"], p["start"], p["end"], p["count"] if held else None)
+            fr = self.device.push(p["k"], p["start"], p["end"], p["count"] if held else None,
+                                  provisional and i == len(pushes) - 1, pending,
+                                  self.device.lookahead + (self.max_gap or 0))
+            if provisional and i == len(pushes) - 1:
+                fr, prov = fr
+            out.append(fr)
         records = np.zeros((int(offs[-1]) * S, 5), np.int32)
         r = 0
         for i, kk in enumerate(ks):
@@ -442,7 +497,8 @@ class DetectionBook:
         slots[:, :2] = self.resolution
         slots[:, 2] = keep
         frames = [[u[0] for u in r] for r in rel]
-        return DetectionCall(pushes, records, slots, frames, realigned)
+        return DetectionCall(pushes, records, slots, frames, realigned, np.concatenate(out, 1),
+                             pending, prov)
 
 
 def predict_schedule(lengths, streams, max_frames, lookahead):
@@ -566,9 +622,16 @@ class StreamingSession:
             if model.in_features != 2:
                 raise ValueError(f"detections=True takes 2-D keypoints (in_features == 2); this "
                                  f"model has in_features = {model.in_features}")
-            if provisional:
-                raise NotImplementedError("provisional=True with detections=True is not supported")
             DetectionBook(streams, max_frames, max_gap)   # (checks max_gap)
+            if provisional and max_gap is None:
+                raise NotImplementedError(
+                    "provisional=True with detections=True needs max_gap = G (an int >= 0): the "
+                    "provisional rows cover the look-ahead and the at most G frames waiting after "
+                    "a slot's last detection, which max_gap=None leaves unbounded")
+            if provisional and lookahead(model) == 0 and max_gap == 0:
+                raise ValueError("provisional=True on a causal model with max_gap = 0 has nothing "
+                                 "provisional: every output is final and no frame waits (give "
+                                 "max_gap >= 1)")
         elif max_gap is not None:
             raise ValueError("max_gap is only used with detections=True")
         self.max_gap = max_gap
@@ -577,11 +640,13 @@ class StreamingSession:
                                                        joints_left, joints_right)
         self.augment = bool(augment)
         self.provisional = bool(provisional)
-        if self.provisional and lookahead(model) == 0:
+        if self.provisional and not self.detections and lookahead(model) == 0:
             raise ValueError("provisional=True needs a non-causal model: a causal model has no "
                              "look-ahead, every output of a push is already final")
+        # a detections session's provisional rows also cover held frames: HELD rings
+        prov_flag = _capi.VP3D_STREAM_HELD if self.detections else _capi.VP3D_STREAM_PROVISIONAL
         self._flags = (_capi.VP3D_STREAM_AUGMENT if self.augment else 0) | \
-            (_capi.VP3D_STREAM_PROVISIONAL if self.provisional else 0) | \
+            (prov_flag if self.provisional else 0) | \
             (_capi.VP3D_STREAM_INT8 if self.int8 else 0)
         device = model.expand_conv.weight.device
         if device.type != "cuda":
@@ -625,6 +690,7 @@ class StreamingSession:
         self.last_call_pushes = 0        # internal pushes of the last push_detections / finish
         self.last_call_launches = 0      # kernels it launched
         self.last_call_realigned = 0     # (slot, push) pairs of it that took the realign path
+        self.last_call_prov_rows = 0     # provisional tail rows it computed
         return self
 
     def _prepare(self):
@@ -828,7 +894,8 @@ class StreamingSession:
         offset = np.concatenate([[0], np.cumsum(lengths)])
         return [y[int(offset[i]):int(offset[i + 1])] for i in range(len(seqs))]
 
-    def push_detections(self, kps_px, detected, start=None, end=None, resolution=None):
+    def push_detections(self, kps_px, detected, start=None, end=None, resolution=None,
+                        provisional=False):
         """Push k video frames per slot straight from a 2-D detector (a session made with
         detections=True); returns (y (S, n, J_out, 3), frame (S, n) int64), n >= k.
 
@@ -848,10 +915,22 @@ class StreamingSession:
         with max_gap = G at most G missed frames wait for the next detection (DetectionBook).
         A video without any detection releases nothing.  `frame` numbers the video's frames from
         its start, -1 for rows that are no frame.  A call that releases more than max_frames
-        frames for a slot runs several pushes and returns their rows concatenated."""
+        frames for a slot runs several pushes and returns their rows concatenated.
+
+        provisional (a session made with provisional=True and max_gap = G): also return y_prov
+        (S, lookahead + G, J_out, 3) and frame_prov (S, lookahead + G) int64, what finish() would
+        return right after this call, bit for bit: row j of slot s is frame c - lookahead + j (c =
+        its released frames) for j < lookahead + P (P = its pending frames after its last
+        detection), under push's rules for ended, draining and idle slots; other rows have frame -1.
+        Nothing of it persists.  The tail rides in the call's last push; last_call_prov_rows says
+        how many rows it computed, min(lookahead + max P, receptive_field - 1)."""
         if not self.detections:
             raise RuntimeError("push_detections needs a session made with "
                                "model.streaming(..., detections=True)")
+        if provisional and not self.provisional:
+            raise RuntimeError("push_detections(provisional=True) needs a session made with "
+                               "model.streaming(..., detections=True, provisional=True, "
+                               "max_gap=G)")
         J = self.model.num_joints_in
         k = check_push_input(kps_px, self.streams, self.max_frames, J, 2)
         if kps_px.device != self.device:
@@ -860,16 +939,18 @@ class StreamingSession:
         if det.shape != (self.streams, k):
             raise ValueError(f"detected must have shape ({self.streams}, {k}) like kps_px's first "
                              f"two dimensions, got {det.shape}")
-        call = self._book.push(det, start, end, resolution)
+        call = self._book.push(det, start, end, resolution, provisional)
         return self._run_detections(call, kps_px.contiguous(), k)
 
     def _run_detections(self, call, kps, k):
-        """One table copy, one pack launch and the pushes of a DetectionCall."""
+        """One table copy, one pack launch and the pushes of a DetectionCall; the last one asks for
+        the provisional rows of a provisional call."""
         S, J = self.streams, self.model.num_joints_in
         pushes = call.pushes
         self.last_call_pushes = len(pushes)
         self.last_call_realigned = len(call.realigned)
         self.last_call_launches = 0
+        self.last_call_prov_rows = 0
         outs = []
         if not pushes:
             return None
@@ -894,17 +975,32 @@ class StreamingSession:
                                 device=self.device)
                 frame = torch.empty((S, kk), dtype=torch.int64, device=self.device)
                 e, c, st = (base + o for o in offsets[i])
-                _capi.check(lib.vp3d_stream_push_counts(
-                    self._plan, self._state.data_ptr(), xs[row:row + S * kk].data_ptr(), kk,
-                    st if p["start"].any() else None, e if (p["end"] >= 0).any() else None, None,
-                    None, y.data_ptr(), frame.data_ptr(), c if p["counted"] else None, stream),
-                    "vp3d_stream_push_counts")
+                args = (self._plan, self._state.data_ptr(), xs[row:row + S * kk].data_ptr(), kk,
+                        st if p["start"].any() else None, e if (p["end"] >= 0).any() else None)
+                if call.prov_frames is not None and i == len(pushes) - 1:
+                    max_held = int(call.held.max())
+                    rows = call.prov_frames.shape[1]
+                    prov = (torch.empty((S, rows, self.model.num_joints_out, 3),
+                                        dtype=torch.float32, device=self.device),
+                            torch.empty((S, rows), dtype=torch.int64, device=self.device))
+                    _capi.check(lib.vp3d_stream_push_held(
+                        *args, c if p["counted"] else None, base + host.nbytes - 4 * S, max_held,
+                        rows, y.data_ptr(), frame.data_ptr(), prov[0].data_ptr(),
+                        prov[1].data_ptr(), stream), "vp3d_stream_push_held")
+                    self.last_call_prov_rows = min(self.lookahead + max_held,
+                                                   self.model.receptive_field() - 1)
+                else:
+                    _capi.check(lib.vp3d_stream_push_counts(
+                        *args, None, None, y.data_ptr(), frame.data_ptr(),
+                        c if p["counted"] else None, stream), "vp3d_stream_push_counts")
                 self.last_call_launches += lib.vp3d_last_launch_count(self._plan)
                 outs.append((y, frame))
                 row += S * kk
         if len(outs) == 1:
-            return outs[0]
-        return torch.cat([o[0] for o in outs], 1), torch.cat([o[1] for o in outs], 1)
+            y, frame = outs[0]
+        else:
+            y, frame = torch.cat([o[0] for o in outs], 1), torch.cat([o[1] for o in outs], 1)
+        return (y, frame) if call.prov_frames is None else (y, frame) + prov
 
     def finish(self):
         """Emit the last `lookahead` frames of every slot (its last frame repeated, as the
