@@ -834,6 +834,56 @@ int vp3d_stream_push_held(vp3d_plan* plan, void* state, const float* x, int k,
                           float* y_prov, int64_t* frame_prov, void* stream);
 int vp3d_stream_finish(vp3d_plan* plan, void* state, float* y, int64_t* frame, void* stream);
 
+/* Moving slots between sessions (streaming.StreamSlots).  A slot's sequence is the reference's
+ * padded forward (run.py:186-193, common/generators.py:216-238) wherever its pushes run: export
+ * copies what a later push reads of the listed slots into a DEVICE blob, import puts it into slots of
+ * another compatible session, and each imported slot then continues its sequence -- frame numbers,
+ * `end`, draining tail and outputs -- bit for bit as if every push had gone to the session it came
+ * from (the offline forward on its padded sequence).  What a slot carries: per physical row (two
+ * with AUGMENT) and ring l, the H_l newest history positions of every plane (and of the u8 plane of
+ * rings 1..nb with INT8), by rank, plus its frame bookkeeping; nothing else persists between pushes.
+ * The blob stores frame ranks, not ring positions, so S, K, the PROVISIONAL / HELD sizing and the
+ * device of the two sessions may differ.
+ *
+ * vp3d_stream_slot_bytes: bytes of one slot's record for a session of `flags` (AUGMENT and INT8
+ *   shape it; 0 for a null plan, unknown flags or INT8 on a plan that is not int8).  At arc
+ *   3,3,3,3,3, C = 1024, fp16: 32 + 2 * 64 * 2 + 240 * 1024 * 2 bytes, about 0.49 MB.
+ * vp3d_stream_export: copies slots[0..n) (HOST int32, each in [0, S), repeats allowed) of `state`
+ *   into `blob` (DEVICE, 16-byte aligned, blob_bytes >= n * slot_bytes) record after record, and
+ *   fills the HOST `header` with what import checks without reading the device: the configuration,
+ *   ring geometry, the AUGMENT / INT8 flags and the session's int8 snapshot (block mask and
+ *   activation scales of its history).  The session is not changed; idle, open and draining slots
+ *   export alike.
+ * vp3d_stream_import: replaces slots[0..n) (HOST int32, distinct, in [0, S)) of `state` with the n
+ *   records of a blob exported with `header`, as a start replaces a sequence; the other slots are
+ *   not disturbed.  The header must match this session: n, configuration (precision included),
+ *   geometry and flags, and with an int8 snapshot the plan's current block mask and scales and the
+ *   session's own snapshot, if it has one (it records the blob's otherwise); VP3D_ERR_STATE
+ *   otherwise.  The weights and the AUGMENT mirror maps live on the device and are the caller's to
+ *   match (streaming.StreamSlots fingerprints them).
+ * Both return argument errors (null pointers, n < 1, a misaligned or too small blob, a slot out of
+ * range, a repeated import slot) and header mismatches before any device work, under their own
+ * names.  Each runs one launch per 1024 listed slots on `stream`, in order with the pushes, and no
+ * host synchronisation. */
+#define VP3D_STREAM_SLOTS_VERSION 1
+typedef struct {
+  int32_t version;          /* VP3D_STREAM_SLOTS_VERSION */
+  int32_t n;                /* slot records in the blob */
+  vp3d_config cfg;          /* the exporting plan's configuration */
+  int32_t flags;            /* the exporting session's AUGMENT | INT8 bits */
+  int32_t rings, planes, f16, lookahead;
+  int32_t H[VP3D_MAX_WIDTHS], ld[VP3D_MAX_WIDTHS];   /* per ring: history positions, row values */
+  int32_t int8_snap;        /* 1: the history holds the quantisation below */
+  uint32_t int8_mask;
+  float act_scale[VP3D_MAX_LAYERS];
+  int64_t slot_bytes;       /* bytes of one record */
+} vp3d_stream_slots_header;
+size_t vp3d_stream_slot_bytes(const vp3d_plan* plan, int flags);
+int vp3d_stream_export(vp3d_plan* plan, void* state, const int32_t* slots, int n, void* blob,
+                       size_t blob_bytes, vp3d_stream_slots_header* header, void* stream);
+int vp3d_stream_import(vp3d_plan* plan, void* state, const int32_t* slots, int n, const void* blob,
+                       size_t blob_bytes, const vp3d_stream_slots_header* header, void* stream);
+
 /* Detector input (streaming.StreamingSession.push_detections): the input rows of the pushes one
  * call makes, from a 2-D detector's pixel keypoints, as the reference's in-the-wild pipeline
  * prepares them.  It replaces, per released frame, joint and coordinate:

@@ -196,6 +196,26 @@ class WgradDesc(ctypes.Structure):
     ]
 
 
+class StreamSlotsHeader(ctypes.Structure):
+    """vp3d_stream_slots_header: what vp3d_stream_import checks of a slot blob on the host."""
+    _fields_ = [
+        ("version", ctypes.c_int32),
+        ("n", ctypes.c_int32),
+        ("cfg", Config),
+        ("flags", ctypes.c_int32),
+        ("rings", ctypes.c_int32),
+        ("planes", ctypes.c_int32),
+        ("f16", ctypes.c_int32),
+        ("lookahead", ctypes.c_int32),
+        ("H", ctypes.c_int32 * VP3D_MAX_WIDTHS),
+        ("ld", ctypes.c_int32 * VP3D_MAX_WIDTHS),
+        ("int8_snap", ctypes.c_int32),
+        ("int8_mask", ctypes.c_uint32),
+        ("act_scale", ctypes.c_float * VP3D_MAX_LAYERS),
+        ("slot_bytes", ctypes.c_int64),
+    ]
+
+
 _P, _I, _LL, _F, _SZ = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_size_t
 
 # name -> (restype, argtypes); also the list the CPU test checks against include/vp3d_b200.h
@@ -344,6 +364,13 @@ SIGNATURES = {
     "vp3d_stream_finish": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "vp3d_stream_release": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "vp3d_stream_slot_bytes": (ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int]),
+    "vp3d_stream_export": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                          ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                          ctypes.POINTER(StreamSlotsHeader), ctypes.c_void_p]),
+    "vp3d_stream_import": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                          ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                          ctypes.POINTER(StreamSlotsHeader), ctypes.c_void_p]),
     "vp3d_stream_pack_detections": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_int, ctypes.c_void_p, ctypes.c_int64,
                                                    ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,

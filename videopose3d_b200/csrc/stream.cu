@@ -99,6 +99,24 @@
 // (mirror halves, tail residues, the two realign phases) is about positions, not planes, so it
 // holds for each plane: the u8 plane is written and read at exactly the positions of the 16-bit
 // planes, by the same kernels in the same order.  H is stored as u8 in `h`, as offline.
+//
+// Moving slots (vp3d_stream_export / vp3d_stream_import).  Everything a later push reads of logical
+// slot s is, per physical row of it and ring l, the H_l history positions [q - H_l, q) of every
+// plane (u8 planes too), plus its bookkeeping in buffer `parity`; h, xlast, ybuf and the v vectors
+// are rebuilt by every push.  The blob stores them by their rank j = t - (q - H_l) in that window,
+// not by ring position, so R, K, S and the tail sizing of the two sessions may differ.
+//   Export reads the copy the last writer wrote.  After a push of prev_k frames from window start
+//   prev_w0, positions [q - H, q) are the last H positions of that push's window: window index
+//   prev_w0 + prev_k + j.  The newest prev_k of them exist in rings 1..nb only at that index (their
+//   mirror copy is the next input kernel's job); the older ones were mirrored by the input kernel of
+//   the last push, ring 0 and broadcast rows were written twice, and a realigned row had both
+//   copies rewritten by its two phases.  So the window index holds frame t whatever wrote it.
+//   Import writes both copies, w0' + j and its mirror (w0' = (q' - H) mod R'), of every history
+//   position of the destination, and the bookkeeping into buffer parity'.  The destination's own
+//   pending mirror copy (the rows [prev_w0' + H, + prev_k') of its last push, which overlap
+//   [q' - H, q')) then copies imported values onto equal imported values, whichever half it reads.
+//   Neither touches a tail residue or another slot's rows, and both are ordered with the pushes on
+//   the caller's stream.
 #include "internal.cuh"
 #include "launch.cuh"
 
@@ -586,6 +604,110 @@ __global__ void __launch_bounds__(256) stream_output_kernel(const float* ybuf, f
   }
 }
 
+// Slot transfer (header comment, moving slots).  One blob record per listed slot: two bookkeeping
+// vectors {count, length} {active, 0} (int64), then per physical row of the slot (row s, AUGMENT
+// also S + s) its history, ring by ring: the 16-bit planes [plane][j < H][ld], then with INT8 the u8
+// plane [j < H][ld] of rings 1..nb.  A launch takes at most kSlotChunk slots, listed in parameter
+// space.
+constexpr int kSlotChunk = 1024;
+constexpr int kSlotBookVecs = 2;
+
+struct SlotArgs {
+  StreamRing ring[kMaxRings];   // q: the u8 plane of every ring >= 1 with INT8
+  int rings, planes, S, phys;   // phys: physical rows per slot (2 with AUGMENT)
+  int P, row_vecs;              // row_vecs: 16-byte vectors of one physical row's history
+  long long slot_vecs;          // kSlotBookVecs + phys * row_vecs
+  long long* count;             // bookkeeping buffer `parity` (S each)
+  uint8_t* active;
+  long long* length;
+  uint4* blob;
+  int n;
+  int slot[kSlotChunk];
+};
+
+// Vector `rem` (< row_vecs) of physical row r's history: its address in the source window (export:
+// the copy the last push wrote, window index prev_w0 + prev_k + j) or the two copies of the
+// destination position (import: w0 + j and its mirror).
+__device__ __forceinline__ void slot_hist_vec(const SlotArgs& a, int r, int rem, bool import,
+                                              uint4** p0, uint4** p1) {
+#pragma unroll
+  for (int l = 0; l < kMaxRings; ++l) {   // (unrolled: the ring table stays in parameter space)
+    if (l >= a.rings) break;
+    const StreamRing& g = a.ring[l];
+    const int vec = g.ld / 8;
+    const int m = a.planes * g.H * vec;
+    const int m_all = m + (g.q ? g.H * (g.ld / 16) : 0);
+    if (rem >= m_all) {
+      rem -= m_all;
+      continue;
+    }
+    const bool u8 = rem >= m;
+    const int vr = u8 ? g.ld / 16 : vec;
+    if (u8) rem -= m;
+    const int e = rem % vr, q = rem / vr;
+    const int j = q % g.H, pl = q / g.H;
+    const int row_bytes = u8 ? g.ld : 2 * g.ld;
+    uint8_t* pb = u8 ? g.q : reinterpret_cast<uint8_t*>(g.base + pl * g.plane);
+    const int pos = import ? g.w0 + j : g.prev_w0 + g.prev_k + j;   // < 2R
+    *p0 = reinterpret_cast<uint4*>(pb + ((long long)pos * a.P + r) * row_bytes) + e;
+    *p1 = reinterpret_cast<uint4*>(pb + ((long long)mirror_pos(pos, g.R) * a.P + r) * row_bytes) + e;
+    return;
+  }
+}
+
+__global__ void __launch_bounds__(256) stream_export_kernel(const SlotArgs a) {
+  const long long total = (long long)a.n * a.slot_vecs;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int at = (int)(i / a.slot_vecs);
+    long long rem = i - (long long)at * a.slot_vecs;
+    const int s = a.slot[at];
+    uint4 v;
+    if (rem < kSlotBookVecs) {
+      const long long w0 = rem == 0 ? a.count[s] : (long long)a.active[s];
+      const long long w1 = rem == 0 ? a.length[s] : 0;
+      v = make_uint4((unsigned)w0, (unsigned)(w0 >> 32), (unsigned)w1, (unsigned)(w1 >> 32));
+    } else {
+      rem -= kSlotBookVecs;
+      const int pr = (int)(rem / a.row_vecs);
+      uint4 *src, *unused;
+      slot_hist_vec(a, pr == 0 ? s : a.S + s, (int)(rem - (long long)pr * a.row_vecs), false, &src,
+                    &unused);
+      v = *src;
+    }
+    a.blob[i] = v;
+  }
+}
+
+__global__ void __launch_bounds__(256) stream_import_kernel(const SlotArgs a) {
+  const long long total = (long long)a.n * a.slot_vecs;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int at = (int)(i / a.slot_vecs);
+    long long rem = i - (long long)at * a.slot_vecs;
+    const int s = a.slot[at];
+    const uint4 v = a.blob[i];
+    if (rem < kSlotBookVecs) {
+      const long long w0 = (long long)(((unsigned long long)v.y << 32) | v.x);
+      const long long w1 = (long long)(((unsigned long long)v.w << 32) | v.z);
+      if (rem == 0) {
+        a.count[s] = w0;
+        a.length[s] = w1;
+      } else {
+        a.active[s] = (uint8_t)w0;
+      }
+    } else {
+      rem -= kSlotBookVecs;
+      const int pr = (int)(rem / a.row_vecs);
+      uint4 *d0, *d1;
+      slot_hist_vec(a, pr == 0 ? s : a.S + s, (int)(rem - (long long)pr * a.row_vecs), true, &d0,
+                    &d1);
+      *d0 = v;
+      *d1 = v;
+    }
+  }
+}
+
 inline int grid_for(long long work) {
   long long b = (work + 255) / 256;
   if (b < 1) b = 1;
@@ -1000,6 +1122,93 @@ static int stream_lookup(vp3d_plan* p, void* state, const char* what, StreamHost
   return VP3D_OK;
 }
 
+// 16-byte vectors of one physical row's history in a slot blob (SlotArgs)
+static int slot_row_vecs(const vp3d_plan* p, int flags) {
+  int v = 0;
+  for (int l = 0; l <= p->nb; ++l) {
+    const int H = 2 * p->pad[l], ld = l == 0 ? p->c_in_pad : p->C;
+    v += p->planes * H * ld / 8 + ((flags & VP3D_STREAM_INT8) && l > 0 ? H * ld / 16 : 0);
+  }
+  return v;
+}
+
+static long long slot_vecs(const vp3d_plan* p, int flags) {
+  return kSlotBookVecs + (long long)(flags & VP3D_STREAM_AUGMENT ? 2 : 1) * slot_row_vecs(p, flags);
+}
+
+// The checks both transfer entries make before any device work (argument errors under `what`, then
+// the session's slots), and the kernel arguments of the session's current position.
+static int slot_transfer_args(const char* what, vp3d_plan* p, void* state, const int32_t* slots,
+                              int n, const void* blob, size_t blob_bytes, const void* header,
+                              bool import, StreamHost** hp, SlotArgs* a) {
+  if (!state) return fail(VP3D_ERR_INVALID, "%s: null state", what);
+  if (!p) return fail(VP3D_ERR_INVALID, "%s: null plan", what);
+  if (n < 1) return fail(VP3D_ERR_INVALID, "%s: n must be >= 1 (got %d)", what, n);
+  if (!slots || !blob || !header) return fail(VP3D_ERR_INVALID, "%s: null slots, blob or header", what);
+  if (reinterpret_cast<uintptr_t>(blob) % 16)
+    return fail(VP3D_ERR_INVALID, "%s: blob is not 16-byte aligned", what);
+  VP3D_TRY(stream_lookup(p, state, what, hp));
+  const StreamHost& h = **hp;
+  for (int i = 0; i < n; ++i) {
+    if (slots[i] < 0 || slots[i] >= h.S)
+      return fail(VP3D_ERR_INVALID, "%s: slots[%d] = %d is not a slot in [0, %d)", what, i, slots[i],
+                  h.S);
+    if (import)
+      for (int j = 0; j < i; ++j)
+        if (slots[j] == slots[i])
+          return fail(VP3D_ERR_INVALID, "%s: slot %d is listed twice (slots[%d], slots[%d])", what,
+                      slots[i], j, i);
+  }
+  const long long need = (long long)n * slot_vecs(p, h.flags) * 16;
+  if ((long long)blob_bytes < need)
+    return fail(VP3D_ERR_WORKSPACE, "%s: blob too small: %zu < %lld bytes for %d slots", what,
+                blob_bytes, need, n);
+  const StreamLayout L = stream_layout(p, h.S, h.K, h.flags);
+  uint8_t* base = ws_base(state);
+  memset(a, 0, sizeof(*a));
+  a->rings = L.rings;
+  a->planes = p->planes;
+  a->S = h.S;
+  a->phys = h.flags & VP3D_STREAM_AUGMENT ? 2 : 1;
+  a->P = physical_rows(h.S, h.flags);
+  a->row_vecs = slot_row_vecs(p, h.flags);
+  a->slot_vecs = slot_vecs(p, h.flags);
+  for (int l = 0; l < L.rings; ++l) {
+    StreamRing& r = a->ring[l];
+    r.base = reinterpret_cast<__nv_bfloat16*>(base + L.ring[l]);
+    r.plane = L.plane[l];
+    r.q = (h.flags & VP3D_STREAM_INT8) && l > 0 ? base + L.q[l] : nullptr;
+    r.ld = L.ld[l];
+    r.H = L.H[l];
+    r.R = L.R[l];
+    r.w0 = pos_mod(h.q - r.H, r.R);
+    r.prev_w0 = pos_mod(h.prev_q - r.H, r.R);
+    r.prev_k = h.prev_k;
+  }
+  a->count = reinterpret_cast<long long*>(base + L.count) + (size_t)h.parity * h.S;
+  a->active = base + L.active + (size_t)h.parity * h.S;
+  a->length = reinterpret_cast<long long*>(base + L.length) + (size_t)h.parity * h.S;
+  return VP3D_OK;
+}
+
+// One launch per kSlotChunk listed slots; the blob record of slots[i] starts at vector
+// i * slot_vecs.
+template <typename Kernel>
+static int slot_transfer_launch(Kernel kernel, vp3d_plan* p, SlotArgs& a, const int32_t* slots,
+                                int n, void* blob, cudaStream_t stream) {
+  int launches = 0;
+  for (int i0 = 0; i0 < n; i0 += kSlotChunk) {
+    a.n = n - i0 < kSlotChunk ? n - i0 : kSlotChunk;
+    memcpy(a.slot, slots + i0, sizeof(int) * a.n);
+    a.blob = reinterpret_cast<uint4*>(blob) + (long long)i0 * a.slot_vecs;
+    kernel<<<grid_for((long long)a.n * a.slot_vecs), 256, 0, stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    ++launches;
+  }
+  p->last_launches = launches;
+  return VP3D_OK;
+}
+
 static int stream_push(const char* what, vp3d_plan* p, void* state, const float* x, int k,
                        const uint8_t* start_mask, const int32_t* end, const int32_t* count,
                        const int64_t* x_rows, const int64_t* y_rows, float* y, int64_t* frame,
@@ -1115,5 +1324,93 @@ VP3D_EXPORT int vp3d_stream_finish(vp3d_plan* p, void* state, float* y, int64_t*
   CUDA_TRY(cudaMemsetAsync(base + stream_layout(p, h->S, h->K, h->flags).active +
                                (size_t)h->parity * h->S, 0, h->S, s));
   p->last_launches = launches;
+  return VP3D_OK;
+}
+
+// Bytes of one slot's record in a slot blob (the `flags` of its session; AUGMENT and INT8 shape it).
+VP3D_EXPORT size_t vp3d_stream_slot_bytes(const vp3d_plan* p, int flags) {
+  if (!p || (flags & ~kStreamFlags) || ((flags & VP3D_STREAM_INT8) && !p->int8)) return 0;
+  return (size_t)slot_vecs(p, flags) * 16;
+}
+
+VP3D_EXPORT int vp3d_stream_export(vp3d_plan* p, void* state, const int32_t* slots, int n,
+                                   void* blob, size_t blob_bytes,
+                                   vp3d_stream_slots_header* header, void* stream) {
+  const char* what = "stream_export";
+  StreamHost* h = nullptr;
+  SlotArgs a;
+  VP3D_TRY(slot_transfer_args(what, p, state, slots, n, blob, blob_bytes, header, false, &h, &a));
+  memset(header, 0, sizeof(*header));
+  header->version = VP3D_STREAM_SLOTS_VERSION;
+  header->n = n;
+  header->cfg = p->cfg;
+  header->flags = h->flags & (VP3D_STREAM_AUGMENT | VP3D_STREAM_INT8);
+  header->rings = a.rings;
+  header->planes = p->planes;
+  header->f16 = p->f16;
+  header->lookahead = stream_lookahead(p);
+  for (int l = 0; l < a.rings; ++l) {
+    header->H[l] = a.ring[l].H;
+    header->ld[l] = a.ring[l].ld;
+  }
+  header->int8_snap = h->int8_snap;
+  header->int8_mask = h->int8_mask;
+  memcpy(header->act_scale, h->act_scale, sizeof(header->act_scale));
+  header->slot_bytes = a.slot_vecs * 16;
+  return slot_transfer_launch(stream_export_kernel, p, a, slots, n, blob,
+                              static_cast<cudaStream_t>(stream));
+}
+
+VP3D_EXPORT int vp3d_stream_import(vp3d_plan* p, void* state, const int32_t* slots, int n,
+                                   const void* blob, size_t blob_bytes,
+                                   const vp3d_stream_slots_header* header, void* stream) {
+  const char* what = "stream_import";
+  StreamHost* h = nullptr;
+  SlotArgs a;
+  VP3D_TRY(slot_transfer_args(what, p, state, slots, n, blob, blob_bytes, header, true, &h, &a));
+  if (header->version != VP3D_STREAM_SLOTS_VERSION)
+    return fail(VP3D_ERR_STATE, "%s: header version %d, expected %d", what, header->version,
+                VP3D_STREAM_SLOTS_VERSION);
+  if (header->n != n)
+    return fail(VP3D_ERR_STATE, "%s: the blob holds %d slots, %d listed", what, header->n, n);
+  const vp3d_config &c0 = header->cfg, &c1 = p->cfg;
+  bool same = c0.num_joints_in == c1.num_joints_in && c0.in_features == c1.in_features &&
+              c0.num_joints_out == c1.num_joints_out && c0.num_widths == c1.num_widths &&
+              c0.causal == c1.causal && c0.channels == c1.channels && c0.dense == c1.dense &&
+              c0.variant == c1.variant && c0.precision == c1.precision;
+  for (int i = 0; same && i < c1.num_widths && i < VP3D_MAX_WIDTHS; ++i)
+    same = c0.filter_widths[i] == c1.filter_widths[i];
+  if (!same)
+    return fail(VP3D_ERR_STATE, "%s: the blob comes from another model configuration or precision",
+                what);
+  const int shape = VP3D_STREAM_AUGMENT | VP3D_STREAM_INT8;
+  if (header->flags != (h->flags & shape))
+    return fail(VP3D_ERR_STATE, "%s: the blob has flags 0x%x (AUGMENT | INT8), the session 0x%x", what,
+                (unsigned)header->flags, (unsigned)(h->flags & shape));
+  bool geometry = header->rings == a.rings && header->planes == p->planes &&
+                  header->f16 == p->f16 && header->lookahead == stream_lookahead(p) &&
+                  header->slot_bytes == a.slot_vecs * 16;
+  for (int l = 0; geometry && l < a.rings; ++l)
+    geometry = header->H[l] == a.ring[l].H && header->ld[l] == a.ring[l].ld;
+  if (!geometry)
+    return fail(VP3D_ERR_STATE, "%s: the blob's ring geometry differs from the session's", what);
+  if (header->int8_snap) {
+    // the imported history holds this quantisation: the plan's and the session's must be it
+    const size_t scale_bytes = sizeof(float) * 2 * p->nb;
+    if (header->int8_mask != p->int8_mask || memcmp(header->act_scale, p->act_scale, scale_bytes))
+      return fail(VP3D_ERR_STATE, "%s: the blob's int8 blocks or activation scales differ from the "
+                  "plan's", what);
+    if (h->int8_snap &&
+        (h->int8_mask != header->int8_mask || memcmp(h->act_scale, header->act_scale, scale_bytes)))
+      return fail(VP3D_ERR_STATE, "%s: the blob's int8 blocks or activation scales differ from the "
+                  "session's", what);
+  }
+  VP3D_TRY(slot_transfer_launch(stream_import_kernel, p, a, slots, n, const_cast<void*>(blob),
+                                static_cast<cudaStream_t>(stream)));
+  if (header->int8_snap && !h->int8_snap) {
+    h->int8_snap = true;
+    h->int8_mask = header->int8_mask;
+    memcpy(h->act_scale, header->act_scale, sizeof(h->act_scale));
+  }
   return VP3D_OK;
 }

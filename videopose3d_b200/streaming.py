@@ -84,7 +84,19 @@ then the look-ahead tail.  Causal models are accepted with G >= 1 (their provisi
 pending frames alone).  A push computes at most receptive_field - 1 tail rows however long the gap
 (past that every row is a copy), and the rings hold that many positions more
 (``ring_bytes_per_stream(..., held=True)``).
+
+A slot's state can move to another session, of any streams / max_frames / provisional sizing, on
+any device, as long as the model, precision, weights, int8 calibration, augmentation and detector
+settings are the same:
+
+    state = old.export_slots(range(S))        # StreamSlots; .to(device), torch.save / torch.load
+    new = model.streaming(streams=2 * S, max_frames=K2)
+    new.import_slots(state, range(S))          # each camera goes on as if it had never moved
+
+Every imported slot continues bit for bit as the uninterrupted stream.  To move a camera rather than
+copy it, free the old slot at its next push with start=True, end=0.
 """
+import hashlib
 import weakref
 
 import numpy as np
@@ -242,6 +254,23 @@ class FrameBook:
             np.zeros((len(self.count), 0), np.int64)
         self.active[:] = False
         return frame
+
+    def export_slots(self, slots):
+        """The bookkeeping rows of `slots` (what vp3d_stream_export copies of them on the device)."""
+        i = np.asarray(slots, np.int64)
+        return dict(lookahead=self.lookahead, count=torch.from_numpy(self.count[i].copy()),
+                    active=torch.from_numpy(self.active[i].copy()),
+                    length=torch.from_numpy(self.length[i].copy()))
+
+    def import_slots(self, rows, slots):
+        """Replace the rows of `slots` with those export_slots returned (the same look-ahead)."""
+        if rows["lookahead"] != self.lookahead:
+            raise ValueError(f"the slots come from a book with lookahead {rows['lookahead']}, this "
+                             f"one has {self.lookahead}")
+        i = np.asarray(slots, np.int64)
+        self.count[i] = rows["count"].numpy()
+        self.active[i] = rows["active"].numpy()
+        self.length[i] = rows["length"].numpy()
 
 
 class DetectionCall:
@@ -438,6 +467,27 @@ class DetectionBook:
         call.out = np.concatenate([call.out, self.device.finish()], 1)
         return call
 
+    _SLOT_FIELDS = ("open", "seen", "last", "released", "on_device", "resolution")
+
+    def export_slots(self, slots):
+        """Everything the book keeps of `slots`, its FrameBook rows included, for import_slots of
+        another book with the same max_gap and look-ahead (max_frames and streams may differ)."""
+        i = np.asarray(slots, np.int64)
+        rows = {f: torch.from_numpy(getattr(self, f)[i].copy()) for f in self._SLOT_FIELDS}
+        rows.update(max_gap=self.max_gap, device=self.device.export_slots(i))
+        return rows
+
+    def import_slots(self, rows, slots):
+        """Replace what `slots` hold with the rows export_slots returned: each video goes on as in
+        the book it left (its frames, releases and pending ones)."""
+        if rows["max_gap"] != self.max_gap:
+            raise ValueError(f"the slots come from a book with max_gap {rows['max_gap']}, this one "
+                             f"has {self.max_gap}")
+        i = np.asarray(slots, np.int64)
+        self.device.import_slots(rows["device"], i)
+        for f in self._SLOT_FIELDS:
+            getattr(self, f)[i] = rows[f].numpy()
+
     def _plan(self, k, rel, keep, drop, ending, pending, provisional=False):
         """Split the released frames into pushes of at most max_frames, k rows in all at least;
         with provisional, the last push also numbers the provisional rows (pending: P per slot)."""
@@ -582,6 +632,70 @@ def check_push_input(x, streams, max_frames, joints, features):
     if not 1 <= k <= max_frames:
         raise ValueError(f"push of {k} frames: k must be in [1, max_frames = {max_frames}]")
     return k
+
+
+def weights_fingerprint(model):
+    """A digest of the values of every tensor the eval forward reads (conv weights, BatchNorm
+    parameters and running statistics, shrink bias), whatever device they are on.  Taken once per
+    parameter version: the first call after a change reads the parameters back to the host."""
+    eng = model._engine
+    versions = model._versions()
+    cached = getattr(eng, "fingerprint", None)
+    if cached is not None and cached[0] == versions:
+        return cached[1]
+    conv, bn = model._param_tensors()
+    h = hashlib.sha256()
+    for t in conv + bn:
+        a = t.detach().to("cpu", torch.float32).contiguous().numpy()
+        h.update(repr(a.shape).encode())
+        h.update(a.tobytes())
+    eng.fingerprint = (versions, h.hexdigest())
+    return eng.fingerprint[1]
+
+
+def int8_fingerprint(model):
+    """A digest of an int8 model's calibration (activation amax per block conv) and block set."""
+    eng = model._engine
+    key = (model._int8, tuple(model.int8_blocks))
+    cached = getattr(eng, "int8_fingerprint", None)
+    if cached is not None and cached[0][0] is key[0] and cached[0][1] == key[1]:
+        return cached[1]
+    h = hashlib.sha256()
+    if model._int8 is not None:
+        h.update(model._int8[0].detach().to("cpu", torch.float32).contiguous().numpy().tobytes())
+    h.update(repr(key[1]).encode())
+    eng.int8_fingerprint = (key, h.hexdigest())
+    return eng.int8_fingerprint[1]
+
+
+class StreamSlots:
+    """Slots exported from a StreamingSession (export_slots), to be imported into slots of a
+    compatible session (import_slots), on this device or another one.
+
+    blob: the DEVICE (or CPU, after .to("cpu")) uint8 records of vp3d_stream_export, one per slot.
+    header: the vp3d_stream_slots_header bytes import checks on the host.  compat: what import
+    compares with the destination (architecture, precision, augmentation and its mirror maps, the
+    detector settings, look-ahead, and fingerprints of the weights and the int8 calibration).  book /
+    last: for a detector-fed session, the DetectionBook rows of the slots and their last detections
+    (n, J_in, 2).  Survives torch.save / torch.load (also with weights_only=True)."""
+
+    def __init__(self, blob, header, compat, book=None, last=None):
+        self.blob, self.header, self.compat, self.book, self.last = blob, header, compat, book, last
+
+    def __len__(self):
+        return _capi.StreamSlotsHeader.from_buffer_copy(self.header.numpy().tobytes()).n
+
+    @property
+    def device(self):
+        return self.blob.device
+
+    def to(self, device):
+        """The same slots with the device tensors on `device` (a CUDA device or the CPU)."""
+        return StreamSlots(self.blob.to(device), self.header, self.compat, self.book,
+                           None if self.last is None else self.last.to(device))
+
+
+torch.serialization.add_safe_globals([StreamSlots])
 
 
 class StreamingSession:
@@ -1033,6 +1147,122 @@ class StreamingSession:
     def last_launch_count(self):
         """Kernels the last push (or finish) launched."""
         return _capi.load().vp3d_last_launch_count(self._plan)
+
+    def _slot_list(self, slots, distinct):
+        """The validated host list of slot indices of export_slots / import_slots."""
+        if isinstance(slots, torch.Tensor):
+            if slots.is_cuda:
+                raise TypeError("slots must be a host list (the indices are checked on the host)")
+            slots = slots.tolist()
+        out = []
+        for s in slots:
+            if isinstance(s, bool) or int(s) != s:
+                raise TypeError(f"slot indices must be ints, got {s!r}")
+            out.append(int(s))
+        if not out:
+            raise ValueError("no slots listed")
+        for s in out:
+            if not 0 <= s < self.streams:
+                raise ValueError(f"slot {s} is out of range for {self.streams} slots")
+        if distinct and len(set(out)) != len(out):
+            dup = next(s for s in out if out.count(s) > 1)
+            raise ValueError(f"slot {dup} is listed twice")
+        return out
+
+    def _compat(self):
+        """What a slot's state depends on besides S, K, provisional sizing and device."""
+        m = self.model
+        tup = lambda a: None if a is None else tuple(int(v) for v in a)  # noqa: E731
+        return dict(
+            architecture=(m.num_joints_in, m.in_features, m.num_joints_out,
+                          tuple(int(w) for w in m.filter_widths), int(m._channels),
+                          bool(m._causal), bool(m._dense)),
+            precision=self.precision, lookahead=self.lookahead, augment=self.augment,
+            kps_src=tup(self._kps_src), joints_src=tup(self._joints_src),
+            detections=self.detections, max_gap=self.max_gap,
+            weights=weights_fingerprint(m), int8=int8_fingerprint(m) if self.int8 else None)
+
+    def _unchanged_since_push(self):
+        """Raise if the parameters or the int8 quantisation changed under the session's history (as
+        the next push would)."""
+        m = self.model
+        if self._versions is not None and m._versions() != self._versions:
+            raise RuntimeError("the model's parameters changed since this session started; call "
+                               "reset() first (old and new weights never mix)")
+        if self._versions is not None and self.int8 and (
+                m._int8 is not self._quant[0] or m.int8_blocks != self._quant[1]):
+            raise RuntimeError("the model's int8 calibration or int8 blocks changed since this "
+                               "session started; call reset() first")
+
+    def _device_index(self, slots):
+        idx = torch.tensor(slots, dtype=torch.int64).pin_memory()
+        return idx.to(self.device, non_blocking=True)
+
+    def export_slots(self, slots):
+        """Copy the listed slots (host ints in [0, S), any state: idle, open or draining) into a
+        StreamSlots, for import_slots of a compatible session; the session is not changed.  One
+        launch (vp3d_stream_export) on the current stream, no host synchronisation once the weights'
+        fingerprint of this parameter version is known; a detector-fed session also copies the
+        slots' last detections."""
+        slots = self._slot_list(slots, distinct=False)
+        self._unchanged_since_push()
+        compat = self._compat()
+        lib = _capi.load()
+        nbytes = lib.vp3d_stream_slot_bytes(self._plan, self._flags)
+        header = _capi.StreamSlotsHeader()
+        idx = np.asarray(slots, np.int32)
+        book = last = None
+        with torch.cuda.device(self.device):
+            blob = torch.empty(len(slots) * nbytes, dtype=torch.uint8, device=self.device)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _capi.check(lib.vp3d_stream_export(self._plan, self._state.data_ptr(), idx.ctypes.data,
+                                               len(slots), blob.data_ptr(), blob.numel(),
+                                               _capi.ctypes.byref(header), stream),
+                        "vp3d_stream_export")
+            if self.detections:
+                book = self._book.export_slots(slots)
+                last = self._last[self._parity].index_select(0, self._device_index(slots))
+        raw = torch.frombuffer(bytearray(bytes(header)), dtype=torch.uint8)
+        return StreamSlots(blob, raw, compat, book, last)
+
+    def import_slots(self, state, slots):
+        """Replace what the listed slots (distinct host ints in [0, S), one per exported slot, in
+        order) hold with the exported ones, as a start replaces a sequence; the other slots are not
+        disturbed.  Each imported slot continues as if every push had gone to the session it came
+        from: its frame numbers, end, draining tail, provisional rows and detection gaps, bit for
+        bit.  The sessions must be compatible: the same architecture, precision, weights, int8
+        calibration and blocks, augment and mirror maps, detections and max_gap (streams,
+        max_frames, provisional and device may differ); anything else raises before any device
+        work.  One launch (vp3d_stream_import), no host synchronisation once the weights'
+        fingerprint of this parameter version is known."""
+        if not isinstance(state, StreamSlots):
+            raise TypeError(f"import_slots takes the StreamSlots of export_slots, got "
+                            f"{type(state).__name__}")
+        slots = self._slot_list(slots, distinct=True)
+        if len(slots) != len(state):
+            raise ValueError(f"{len(slots)} slots listed for {len(state)} exported ones")
+        if state.device != self.device:
+            raise RuntimeError(f"the exported slots are on {state.device}, the session on "
+                               f"{self.device}: call .to({str(self.device)!r}) first")
+        self._unchanged_since_push()
+        mine = self._compat()
+        for key, value in mine.items():
+            if state.compat.get(key) != value:
+                raise ValueError(f"the exported slots come from an incompatible session: {key} "
+                                 f"differs ({state.compat.get(key)!r} there, {value!r} here)")
+        header = _capi.StreamSlotsHeader.from_buffer_copy(state.header.numpy().tobytes())
+        idx = np.asarray(slots, np.int32)
+        lib = _capi.load()
+        with torch.cuda.device(self.device):
+            stream = self._prepare()
+            _capi.check(lib.vp3d_stream_import(self._plan, self._state.data_ptr(), idx.ctypes.data,
+                                               len(slots), state.blob.data_ptr(),
+                                               state.blob.numel(), _capi.ctypes.byref(header),
+                                               stream), "vp3d_stream_import")
+            if self.detections:
+                self._last[self._parity].index_copy_(0, self._device_index(slots), state.last)
+                self._book.import_slots(state.book, slots)
+        return self
 
 
 def _release(plan, state_ptr, engine):
